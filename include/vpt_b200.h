@@ -118,6 +118,38 @@ int  vpt_comm_p2p_status(vpt_context* ctx, unsigned long long* abandoned_waits);
 int  vpt_render_pass(vpt_context* ctx, void* const params[VPT_NUM_ARGS], void* stream);
 int  vpt_render_passes(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsigned n_passes, void* stream);
 
+/* ---- adaptive sampling: converged pixels stop early --------------------------------------------------
+ * vpt_render_adaptive renders ONE new frame (Kernel_params.iteration must be 0; pass k of the frame is the reference launch with
+ * iteration k) of at most min(max_passes, max_interactions) passes, and lets each pixel stop once it and its neighbours have converged.
+ *
+ *   Statistic.  Every pass a pixel takes updates a float32 Welford state of the luminance Y = 0.2126 r + 0.7152 g + 0.0722 b of its
+ *     sample, taken exactly as the sample enters the running mean (after the NaN / Inf guard and the viz_dof tint):
+ *         n += 1;  d = Y - mean;  mean += d / n;  M2 += d * (Y - mean)
+ *     and its relative error is err = sqrt(M2 / (n (n-1))) / max(mean, 1e-3)  (the floor keeps dark pixels from never converging).
+ *   Tests.  After min_passes passes, then every check_interval passes, a pixel that is still active stops if the largest err over its
+ *     3x3 neighbourhood (clipped at the frame edge) is strictly below `threshold`; a neighbour that has already stopped counts with the
+ *     last err it had.  threshold = 0: no pixel ever stops; threshold = FLT_MAX: every pixel stops at the first test.
+ *   Outputs.  d_pass_count[p] (W*H unsigned, device, required) = the passes pixel p took, and accum, depth, cost, raw and display of p
+ *     are bit for bit what vpt_render_passes(d_pass_count[p]) would leave there: the Philox stream is keyed by (pixel, iteration) and
+ *     the jitter of a pass does not depend on which pixels sample it.  d_rel_error (W*H float, device, may be NULL) = each pixel's last
+ *     err, a noise map of the frame.  *passes_run (host, may be NULL) = the passes issued: min(max_passes, max_interactions), or fewer
+ *     when every pixel stopped earlier; the blue-noise buffer is advanced exactly that many times.
+ *   Synchronisation.  The call synchronises `stream` once per convergence test, to read back how many 32x4 pixel tiles are still
+ *     active; everything else is enqueued asynchronously like vpt_render_passes.
+ *   An adaptive frame is final.  vpt_render_passes with iteration > 0 on the accum_buffer of the context's last adaptive frame fails
+ *     with VPT_ERR_INVALID; a call with iteration == 0 on it starts a new frame as usual.
+ *   Refused: render == 0, max_interactions < 2, min_passes < 2, check_interval == 0, a negative threshold, max_passes == 0
+ *     (VPT_ERR_INVALID); a partitioned context -- vpt_set_partition with n_ranks > 1, NCCL or peer exchange -- (VPT_ERR_UNSUPPORTED:
+ *     the 3x3 test reads across stripes).  Brick mode and cell mode work.  opt == NULL takes the defaults. */
+typedef struct vpt_adaptive_options {
+    unsigned min_passes;       /* passes every pixel takes before it may stop; >= 2 (default 16) */
+    unsigned check_interval;   /* passes between two convergence tests; >= 1 (default 16) */
+    float    threshold;        /* stop when the relative error of the pixel and of its 8 neighbours is below this (default 0.01) */
+} vpt_adaptive_options;
+void vpt_adaptive_options_defaults(vpt_adaptive_options* opt);
+int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsigned max_passes, const vpt_adaptive_options* opt,
+                         unsigned* d_pass_count, float* d_rel_error, unsigned* passes_run, void* stream);
+
 /* The flattened scene tables are cached per (volumes pointer, octree root pointer, build generation of a vpt_octree_build
  * octree) and refreshed whenever a call arrives with Kernel_params.iteration == 0 (the reference application resets the
  * iteration on every scene edit, main.cpp:1667-1780).  Call this only if the GPU_VDB[] array or a foreign octree was
@@ -131,7 +163,8 @@ int  vpt_get_stats(vpt_context* ctx, unsigned long long* kernel_launches_total, 
 /* Instrumentation.  Option "count_stats" = 1 makes the trace kernel accumulate out[0] volume lookups,
  * out[1] lane-steps, out[2] warp step-loop iterations, out[3] rays serviced, out[4] warp service rounds, out[5] rays
  * fetched from the queue, out[6] bricks staged by TMA (brick mode) (SIMT efficiency of the step loop = out[1] / (32 * out[2])).  Option "profile" = 1 brackets every kernel with
- * CUDA events: ms/n[0..3] = generate, trace, resolve, blue-noise advance.  Both calls synchronise the device. */
+ * CUDA events: ms/n[0..3] = generate, trace, resolve, blue-noise advance (in adaptive frames the convergence tests count as resolve).
+ * Both calls synchronise the device. */
 int  vpt_get_counters(vpt_context* ctx, unsigned long long out[8], int reset);
 int  vpt_get_kernel_times(vpt_context* ctx, float ms[4], int n[4]);
 

@@ -158,6 +158,7 @@ EXPORTED_SYMBOLS = [
     "vpt_texture_read_f4", "vpt_debug_texture_sample",
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
+    "vpt_adaptive_options_defaults", "vpt_render_adaptive",
 ]
 
 # ---- prototypes ------------------------------------------------------------------------------------
@@ -174,6 +175,15 @@ lib.vpt_unpermute.argtypes = [_vp, _vp, _vp, C.c_uint, C.c_uint, C.c_int, _vp]; 
 lib.vpt_render_pass.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_render_pass.restype = C.c_int
 lib.vpt_render_passes.argtypes = [_vp, C.POINTER(_vp), C.c_uint, _vp]; lib.vpt_render_passes.restype = C.c_int
 lib.vpt_invalidate_scene.argtypes = [_vp]; lib.vpt_invalidate_scene.restype = C.c_int
+
+
+class adaptive_options(C.Structure):
+    _fields_ = [("min_passes", C.c_uint), ("check_interval", C.c_uint), ("threshold", C.c_float)]
+
+
+lib.vpt_adaptive_options_defaults.argtypes = [C.POINTER(adaptive_options)]; lib.vpt_adaptive_options_defaults.restype = None
+lib.vpt_render_adaptive.argtypes = [_vp, C.POINTER(_vp), C.c_uint, C.POINTER(adaptive_options), _vp, _vp, C.POINTER(C.c_uint), _vp]
+lib.vpt_render_adaptive.restype = C.c_int
 lib.vpt_get_stats.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.POINTER(C.c_uint)]; lib.vpt_get_stats.restype = C.c_int
 lib.vpt_get_counters.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.c_int]; lib.vpt_get_counters.restype = C.c_int
 lib.vpt_get_kernel_times.argtypes = [_vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]; lib.vpt_get_kernel_times.restype = C.c_int

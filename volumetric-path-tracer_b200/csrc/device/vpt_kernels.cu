@@ -11,6 +11,8 @@
 //   k_resolve<S>    : per pixel, passes in order: environment term (S = 0 HDRI, 1 / 2 precomputed sky: vpt_atmosphere.cuh),
 //                     NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference kernel)
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
+//   k_generate_adaptive, k_resolve_adaptive<S>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
+//                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -93,8 +95,10 @@ __global__ void k_prepare_scene(const vpt_gpu_vdb* __restrict__ vols, const vpt_
 // =====================================================================================================
 // k_generate
 // =====================================================================================================
-__global__ void __launch_bounds__(128)
-k_generate(const FrameArgs fa)
+// kAdaptive: the grid runs over the active tiles of `ad` instead of all tiles, and a lane whose pixel has stopped samples nothing (no
+// plane record, no ray).  Two kernels (k_generate, k_generate_adaptive) so the fixed-count one is the very same machine code as before.
+template <bool kAdaptive>
+__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad)
 {
     __shared__ FrameShared fs;
     __shared__ float vdc2[101], vdc3[101];                     // radical inverses of 0..100 in bases 2 and 3
@@ -112,13 +116,15 @@ k_generate(const FrameArgs fa)
     // one block = a run of 32x4 pixel tiles x a run of passes: enough (tile, pass) pairs per block to amortise the octree / table staging
     // above -- many passes of one tile when passes are fused, several tiles when the caller renders pass by pass; a small local frame
     // (multi-GPU shard, low resolution) splits the chunk's passes over blockIdx.z instead: see launch_generate
-    const int tiles_x = (g.width + 31) / 32, n_tiles = tiles_x * ((g.local_rows + 3) / 4);
-    for (int tile = blockIdx.x * fa.tiles_per_block; tile < min(n_tiles, (int)(blockIdx.x + 1) * fa.tiles_per_block); ++tile) {
+    const int tiles_x = (g.width + 31) / 32, n_tiles = kAdaptive ? ad->n_tiles : tiles_x * ((g.local_rows + 3) / 4);
+    for (int ti = blockIdx.x * fa.tiles_per_block; ti < min(n_tiles, (int)(blockIdx.x + 1) * fa.tiles_per_block); ++ti) {
+    const int tile = kAdaptive ? (int)__ldg(ad->tiles + ti) : ti;
     const int tile_y = tile / tiles_x, tile_x = tile - tile_y * tiles_x;
     const int x = tile_x * 32 + warp * 8 + (lane & 7);
     const int lr = tile_y * 4 + (lane >> 3);
     const int y = global_row(g, lr);
-    const bool valid = (x < g.width) && (lr < g.local_rows) && (y < g.height);
+    bool valid = (x < g.width) && (lr < g.local_rows) && (y < g.height);
+    if constexpr (kAdaptive) { if (valid && ad->stopped[(size_t)lr * g.width + x]) valid = false; }
 
     const int pass_begin = blockIdx.z * fa.passes_per_block;
     const int pass_end = min(fa.n_passes, pass_begin + fa.passes_per_block);
@@ -239,6 +245,12 @@ k_generate(const FrameArgs fa)
     }   // tile loop
 }
 
+__global__ void __launch_bounds__(128)
+k_generate(const FrameArgs fa) { generate_body<false>(fa, nullptr); }
+
+__global__ void __launch_bounds__(128)
+k_generate_adaptive(const FrameArgs fa, const AdaptArgs ad) { generate_body<true>(fa, &ad); }
+
 
 // =====================================================================================================
 // k_resolve
@@ -249,19 +261,18 @@ k_generate(const FrameArgs fa)
 struct NoSky { int pad[4]; };
 struct PeerFlagPtrs { unsigned long long* p[kMaxPeers]; };
 
-template <int kSky>
-__global__ void __launch_bounds__(256)
-k_resolve(const FrameArgs fa, const typename std::conditional<kSky != 0, vpt_atmosphere, NoSky>::type atmo,
-          const int n_passes, const int sampled, const int write_display, const PeerFrames peers)
+template <int kSky> using SkyArg = typename std::conditional<kSky != 0, vpt_atmosphere, NoSky>::type;
+
+// One pixel of k_resolve (local pixel lp, local row lr, global row y).  kAdaptive (k_resolve_adaptive): the same running mean, plus the
+// pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.
+template <int kSky, bool kAdaptive>
+__device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
+                                              const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
+                                              const AdaptArgs* ad)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
     const vpt_camera& cam = fa.cam;
-    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
-    if (lp >= (uint32_t)g.n_local) return;
-    const int lr = lp / g.width;
-    const int y = global_row(g, lr);
-    if (y >= g.height) return;
 
     float3* accum_buf = reinterpret_cast<float3*>(kp.accum_buffer);
     float3* cost_buf = reinterpret_cast<float3*>(kp.cost_buffer);
@@ -272,6 +283,9 @@ k_resolve(const FrameArgs fa, const typename std::conditional<kSky != 0, vpt_atm
     if (have_prev || !sampled) { accum = accum_buf[lp]; costv = cost_buf[lp]; depthv = depth_buf[lp]; }
     float tr = .0f;
 
+    // adaptive: Welford state {n, mean, M2} of the luminance of every sample of this pixel
+    float wn = 0.f, wmean = 0.f, wm2 = 0.f;
+    if constexpr (kAdaptive) { if (have_prev) { const float4 st = ad->stat[lp]; wn = st.x; wmean = st.y; wm2 = st.z; } }
     // one pass of the running mean; A (and B, C for a hit sample) are the pass's plane records, loaded by the caller
     auto one_pass = [&](const int p, const float4 A, const float4 B, const float4 C) {
         const uint32_t iteration = kp.iteration + (uint32_t)p;
@@ -320,6 +334,13 @@ k_resolve(const FrameArgs fa, const typename std::conditional<kSky != 0, vpt_atm
             costv = costv + (f3(0.f) - costv) / (float)(iteration + 1);
             depthv = depthv + (depth - depthv) / (float)(iteration + 1);
         }
+        if constexpr (kAdaptive) {                              // the sample as it entered the mean (after the NaN guard and the tint)
+            const float lum = 0.2126f * value.x + 0.7152f * value.y + 0.0722f * value.z;
+            wn += 1.0f;
+            const float d = lum - wmean;
+            wmean += d / wn;
+            wm2 += d * (lum - wmean);
+        }
     };
     const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
     {
@@ -334,6 +355,12 @@ k_resolve(const FrameArgs fa, const typename std::conditional<kSky != 0, vpt_atm
         }
     }
     accum_buf[lp] = accum; cost_buf[lp] = costv; depth_buf[lp] = depthv;
+    if constexpr (kAdaptive) {
+        const float err = wn >= 2.0f ? sqrtf(wm2 / (wn * (wn - 1.0f))) / fmaxf(wmean, kAdaptMeanFloor) : INFINITY;
+        ad->stat[lp] = make_float4(wn, wmean, wm2, err);
+        ad->pass_count[lp] = kp.iteration + (uint32_t)n_passes;
+        if (ad->rel_error) ad->rel_error[lp] = err;
+    }
 
     if (write_display) {
         const float aces_in[9]  = { 0.59719f, 0.35458f, 0.04823f, 0.07600f, 0.90834f, 0.01566f, 0.02840f, 0.13383f, 0.83777f };
@@ -358,6 +385,81 @@ k_resolve(const FrameArgs fa, const typename std::conditional<kSky != 0, vpt_atm
         const size_t gp = (size_t)y * g.width + (lp - (uint32_t)lr * (uint32_t)g.width);
         #pragma unroll
         for (int p = 0; p < kMaxPeers; ++p) if (p < peers.n) { float* a = peers.accum[p] + 3 * gp; a[0] = accum.x; a[1] = accum.y; a[2] = accum.z; }
+    }
+}
+
+template <int kSky>
+__global__ void __launch_bounds__(256)
+k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers)
+{
+    const FrameGeom& g = fa.geom;
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= (uint32_t)g.n_local) return;
+    const int lr = lp / g.width;
+    const int y = global_row(g, lr);
+    if (y >= g.height) return;
+    resolve_pixel<kSky, false>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr);
+}
+
+// 32x4 pixel tile and the lane's pixel in it, for the per-tile adaptive kernels (a warp covers one row of 32 pixels)
+struct TilePixel { int x, lr; bool inside; };
+__device__ __forceinline__ TilePixel tile_pixel(const FrameGeom& g, const int tile)
+{
+    const int tiles_x = (g.width + 31) / 32;
+    const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
+    TilePixel t; t.x = tx * 32 + (int)(threadIdx.x & 31); t.lr = ty * 4 + (int)(threadIdx.x >> 5);
+    t.inside = t.x < g.width && t.lr < g.local_rows && global_row(g, t.lr) < g.height;
+    return t;
+}
+
+// One block of 128 per active tile: the running mean of the pixels that have not stopped, every pass of the chunk sampled; at the end of the
+// chunk their display / raw words, pass count and relative error (so a pixel keeps those of the last pass it took).
+template <int kSky>
+__global__ void __launch_bounds__(128)
+k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad)
+{
+    const FrameGeom& g = fa.geom;
+    const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
+    if (!t.inside) return;
+    const uint32_t lp = (uint32_t)t.lr * (uint32_t)g.width + (uint32_t)t.x;
+    if (ad.stopped[lp]) return;
+    resolve_pixel<kSky, true>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad);
+}
+
+// Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (clipped at
+// the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A tile with a pixel still
+// active is appended to the next list (one atomic per tile).
+__global__ void __launch_bounds__(128)
+k_adapt(const FrameGeom g, const AdaptArgs ad)
+{
+    const int tile = (int)__ldg(ad.tiles + blockIdx.x);
+    const TilePixel t = tile_pixel(g, tile);
+    bool active = false;
+    if (t.inside) {
+        const size_t lp = (size_t)t.lr * g.width + t.x;
+        if (!ad.stopped[lp]) {
+            float worst = 0.0f;
+            for (int dy = -1; dy <= 1; ++dy) {
+                const int r = t.lr + dy;
+                if (r < 0 || r >= g.local_rows) continue;
+                for (int dx = -1; dx <= 1; ++dx) {
+                    const int c = t.x + dx;
+                    if (c < 0 || c >= g.width) continue;
+                    worst = fmaxf(worst, ad.stat[(size_t)r * g.width + c].w);
+                }
+            }
+            if (worst < ad.threshold) ad.stopped[lp] = 1;
+            else active = true;
+        }
+    }
+    if (__syncthreads_or(active) && threadIdx.x == 0) ad.next_tiles[atomicAdd(ad.next_count, 1u)] = (unsigned)tile;
+}
+
+__global__ void k_adapt_init(uint8_t* stopped, unsigned* tiles, int n_local, int n_tiles)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(n_local, n_tiles); i += gridDim.x * blockDim.x) {
+        if (i < n_local) stopped[i] = 0;
+        if (i < n_tiles) tiles[i] = (unsigned)i;
     }
 }
 
@@ -458,20 +560,35 @@ cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& h
     return cudaGetLastError();
 }
 
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s)
+// one block = a run of 32x4 pixel tiles x a run of passes.  Keep >= ~8 waves of blocks (H100 SXM: 132 SMs x 7 resident blocks) so the tail of the
+// grid does not idle the SMs when the local frame is small; never fewer than 4 (tile, pass) pairs per block (amortises the table
+// staging: one pass per call used to spend half of this kernel on it).
+static dim3 generate_grid(FrameArgs& a, long long tiles, int n_passes)
 {
-    FrameArgs a = fa; a.n_passes = n_passes;
-    // one block = a run of 32x4 pixel tiles x a run of passes.  Keep >= ~8 waves of blocks (H100 SXM: 132 SMs x 7 resident blocks) so the tail of the
-    // grid does not idle the SMs when the local frame is small; never fewer than 4 (tile, pass) pairs per block (amortises the table
-    // staging: one pass per call used to spend half of this kernel on it).
+    a.n_passes = n_passes;
     int ppb = n_passes;
-    const long long tiles = (long long)((fa.geom.width + 31) / 32) * ((fa.geom.local_rows + 3) / 4);
     while (ppb > 4 && tiles * ((n_passes + ppb - 1) / ppb) < 7392) ppb = (ppb + 1) / 2;
     int tpb = 1;
     while (ppb * tpb < 4 && tiles / (tpb * 2) >= 2112) tpb *= 2;
     a.passes_per_block = ppb; a.tiles_per_block = tpb;
-    dim3 grid((unsigned)((tiles + tpb - 1) / tpb), 1, (unsigned)((n_passes + ppb - 1) / ppb));
+    return dim3((unsigned)((tiles + tpb - 1) / tpb), 1, (unsigned)((n_passes + ppb - 1) / ppb));
+}
+
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s)
+{
+    FrameArgs a = fa;
+    const long long tiles = (long long)((fa.geom.width + 31) / 32) * ((fa.geom.local_rows + 3) / 4);
+    const dim3 grid = generate_grid(a, tiles, n_passes);
     k_generate<<<grid, 128, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s)
+{
+    if (ad.n_tiles <= 0) return cudaSuccess;
+    FrameArgs a = fa;
+    const dim3 grid = generate_grid(a, ad.n_tiles, n_passes);
+    k_generate_adaptive<<<grid, 128, 0, s>>>(a, ad);
     return cudaGetLastError();
 }
 
@@ -555,6 +672,28 @@ cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n
     if (sky && fa.kp.integrator != 0) k_resolve<2><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
     else if (sky)                     k_resolve<1><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
     else                              k_resolve<0><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, cudaStream_t s)
+{
+    if (ad.n_tiles <= 0) return cudaSuccess;
+    if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
+    else if (sky)                     k_resolve_adaptive<1><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
+    else                              k_resolve_adaptive<0><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, cudaStream_t s)
+{
+    if (ad.n_tiles <= 0) return cudaSuccess;
+    k_adapt<<<ad.n_tiles, 128, 0, s>>>(g, ad);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, int n_tiles, cudaStream_t s)
+{
+    k_adapt_init<<<1184, 256, 0, s>>>(stopped, tiles, g.n_local, n_tiles);
     return cudaGetLastError();
 }
 

@@ -52,6 +52,21 @@ struct FrameArgs {
     int       tiles_per_block;     // k_generate: consecutive 32x4 tiles handled by one block (blockIdx.x selects the run)
 };
 
+// Adaptive sampling (vpt_render_adaptive): pixels are grouped in the 32x4 tiles k_generate works on; a chunk only visits the tiles that
+// still hold an active pixel.  Per pixel the context keeps a float32 Welford state of the sample luminance {n, mean, M2, err}.
+constexpr float kAdaptMeanFloor = 1e-3f;   // err = sqrt(M2 / (n (n-1))) / max(mean, kAdaptMeanFloor): dark pixels are judged on absolute error
+struct AdaptArgs {
+    const unsigned* tiles;         // active tiles of this chunk (tile = tile_y * tiles_x + tile_x), `n_tiles` entries
+    int       n_tiles;
+    uint8_t*  stopped;             // [local pixel] 1 once the pixel has stopped
+    float4*   stat;                // [local pixel] n, mean, M2, err
+    unsigned* pass_count;          // [local pixel] passes taken (the caller's buffer)
+    float*    rel_error;           // [local pixel] last err (the caller's buffer, may be null)
+    unsigned* next_tiles;          // k_adapt: tiles still active after the test, appended in any order
+    unsigned* next_count;          //          their number (zeroed by the host before the launch)
+    float     threshold;
+};
+
 cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* root, SceneTables* out, OctInternal* internal,
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
@@ -82,5 +97,13 @@ constexpr int kPeerFlagStride = 16;                   // u64 slots per flag arra
 cudaError_t launch_bn_prepare(void* bn, float2* table, int np, int limit, unsigned* queue_counters, cudaStream_t s);   // also zeroes queue_counters[0..1]
 cudaError_t launch_bn_advance(void* bn, int n, int limit, cudaStream_t s);
 cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& g, int elem_bytes, cudaStream_t s);
+// adaptive frame: k_generate / k_resolve over the tiles of ad.tiles only (stopped pixels sample nothing and keep their buffers); the resolve
+// also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
+cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s);
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, cudaStream_t s);
+// convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood has err < threshold, lists the tiles still active
+cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, cudaStream_t s);
+// start of an adaptive frame: no pixel stopped, tile list = every tile
+cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, int n_tiles, cudaStream_t s);
 
 } // namespace vpt

@@ -7,6 +7,8 @@
 //        memset(queue counters) -> k_bn_prepare -> k_generate -> k_trace<integrator, lean> (persistent) -> k_resolve<env>
 //   passes beyond max_interactions / render == false: k_resolve (re-tonemap) + k_bn_advance
 // which leaves every buffer named by Kernel_params in the state n reference launches would.
+// vpt_render_adaptive runs the same rounds over the tiles that still hold an active pixel (k_generate_adaptive, k_resolve_adaptive),
+// with k_adapt and one stream synchronisation at every convergence test.
 #include "vpt_host.h"
 #include "vdb_reader.h"
 #include "image_io.h"
@@ -77,6 +79,7 @@ static void free_context(vpt_context* c) {
     for (auto& e : c->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     cudaFree(c->d_queue_id); cudaFree(c->d_queue_org); cudaFree(c->d_bn_table);
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
+    cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
     delete c;
 }
 
@@ -182,13 +185,36 @@ static int ensure_frame_buffers(vpt_context* c, size_t n_samples, bool need_plan
     return VPT_OK;
 }
 
-int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned n_passes, void* stream_) {
-    if (!c || !params) return fail(c, VPT_ERR_INVALID, "vpt_render_passes: null argument");
-    for (int i = 0; i < VPT_NUM_ARGS; ++i) if (!params[i]) return fail(c, VPT_ERR_INVALID, "vpt_render_passes: params[" + std::to_string(i) + "] is null");
-    if (n_passes == 0) return VPT_OK;
-    cudaStream_t stream = (cudaStream_t)stream_;
+} // extern "C"
 
+namespace {
+// What one render call works with once the parameter block is unpacked: vpt_render_passes and vpt_render_adaptive share it (frame_setup).
+struct FramePlan {
     vpt::FrameArgs fa;
+    vpt_atmosphere atmo;                  // the caller's AtmosphereParameters
+    const vpt_atmosphere* sky = nullptr;  // &atmo when the frame ends on the precomputed sky (environment_type == 0 or integrator != 0)
+    bool vol_integ = false, lean = false;
+    int trace_ctas = 0, slots = 3, chunk = 1, bn_limit = 0;
+    unsigned n_sampled = 0;               // how many of the requested passes sample (the rest only re-tonemap)
+};
+
+// Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
+template <class F>
+cudaError_t timed(vpt_context* c, cudaStream_t stream, int kind, F&& fn) {
+    if (!c->profile) return fn();
+    vpt_context::Ev ev; ev.kind = kind;
+    cudaEventCreate(&ev.a); cudaEventCreate(&ev.b);
+    cudaEventRecord(ev.a, stream);
+    cudaError_t e = fn();
+    cudaEventRecord(ev.b, stream);
+    c->events.push_back(ev);
+    return e;
+}
+} // namespace
+
+// The preamble of a render call of n_passes passes: validation, scene-table refresh, trace-kernel choice, chunk size and scratch buffers.
+static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned n_passes, cudaStream_t stream, FramePlan& plan) {
+    vpt::FrameArgs& fa = plan.fa;
     memcpy(&fa.cam, params[VPT_ARG_CAMERA], sizeof(vpt_camera));
     memcpy(&fa.lights, params[VPT_ARG_LIGHTS], sizeof(vpt_light_list));
     memcpy(&fa.kp, params[VPT_ARG_KERNEL_PARAMS], sizeof(vpt_kernel_params));
@@ -199,7 +225,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
     const vpt_kernel_params& kp = fa.kp;
 
     // environment_type == 0: the caller's AtmosphereParameters (scalars + the four precomputed look-up textures)
-    vpt_atmosphere atmo;
+    vpt_atmosphere& atmo = plan.atmo;
     memcpy(&atmo, params[VPT_ARG_ATMOSPHERE], sizeof(vpt_atmosphere));
     if (c->n_ranks > 1 && (kp.resolution.x > 65535u || kp.resolution.y > 65535u)) return fail(c, VPT_ERR_UNSUPPORTED, "a partitioned frame is limited to 65535 x 65535 pixels");
     const bool vol_integ = (kp.integrator != 0);             // vol_integrator always ends on the precomputed sky (:1752)
@@ -213,7 +239,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         return fail(c, VPT_ERR_INVALID, "integrator != 0 with environment_type == 0 needs the env sampling tables (env_*_tex, env_sample_tex_res) in Kernel_params");
     if (vol_integ && samples && kp.environment_type != 0 && !kp.env_tex)
         return fail(c, VPT_ERR_INVALID, "environment_type != 0 needs Kernel_params.env_tex");
-    const vpt_atmosphere* sky = sky_env ? &atmo : nullptr;
+    plan.sky = sky_env ? &atmo : nullptr;
     if (!d_volumes || !d_sphere || !d_root) return fail(c, VPT_ERR_INVALID, "volumes / sphere / octree device pointer is null");
     if (!kp.accum_buffer || !kp.depth_buffer || !kp.cost_buffer || !kp.display_buffer || !kp.raw_buffer || !kp.blue_noise_buffer)
         return fail(c, VPT_ERR_INVALID, "Kernel_params output buffer pointer is null");
@@ -330,39 +356,63 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
     fa.sched_min_lanes = c->sched_min_lanes > 0 ? c->sched_min_lanes : ((lean && slots == 3 && !vol_integ && !c->brick_pool && !c->cell_table) ? 26 : 20);
     int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm : c->max_ctas[c->brick_pool ? 3 : c->cell_table ? 6 : vol_integ ? 2 : (slots == 2 ? (lean ? 5 : 4) : (lean ? 1 : 0))];
     if (ctas_per_sm < 1) ctas_per_sm = 1;
-    const int trace_ctas = c->num_sms * ctas_per_sm;
 
     fa.counters = c->count_stats ? c->d_stats : nullptr;
     fa.cell_table = c->cell_table; fa.cell_nx = c->cell_dims[0]; fa.cell_ny = c->cell_dims[1]; fa.cell_nz = c->cell_dims[2];
-    auto timed = [&](int kind, auto&& fn) -> cudaError_t {
-        if (!c->profile) return fn();
-        vpt_context::Ev ev; ev.kind = kind;
-        cudaEventCreate(&ev.a); cudaEventCreate(&ev.b);
-        cudaEventRecord(ev.a, stream);
-        cudaError_t e = fn();
-        cudaEventRecord(ev.b, stream);
-        c->events.push_back(ev);
-        return e;
-    };
+    const unsigned long long frame_px = (unsigned long long)kp.resolution.x * kp.resolution.y;
+    plan.vol_integ = vol_integ; plan.lean = lean; plan.slots = slots; plan.trace_ctas = c->num_sms * ctas_per_sm;
+    plan.chunk = chunk; plan.n_sampled = n_sampled;
+    plan.bn_limit = frame_px < 65536ull ? (int)frame_px : 65536;
+    return VPT_OK;
+}
+
+// k_trace (or k_trace_brick in brick mode) over whatever k_generate queued
+static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, cudaStream_t stream) {
+    if (c->brick_pool) return vpt::launch_trace_brick(plan.fa, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
+    return vpt::launch_trace(plan.fa, plan.vol_integ ? &plan.atmo : nullptr, plan.lean, plan.slots, plan.trace_ctas, stream);
+}
+
+extern "C" {
+
+int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned n_passes, void* stream_) {
+    if (!c || !params) return fail(c, VPT_ERR_INVALID, "vpt_render_passes: null argument");
+    for (int i = 0; i < VPT_NUM_ARGS; ++i) if (!params[i]) return fail(c, VPT_ERR_INVALID, "vpt_render_passes: params[" + std::to_string(i) + "] is null");
+    if (n_passes == 0) return VPT_OK;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    {
+        // an adaptive frame is final: its pixels hold different sample counts, so no later pass can continue it
+        vpt_kernel_params kp0;
+        memcpy(&kp0, params[VPT_ARG_KERNEL_PARAMS], sizeof(vpt_kernel_params));
+        if (c->adaptive_accum && kp0.accum_buffer == c->adaptive_accum) {
+            if (kp0.iteration > 0)
+                return fail(c, VPT_ERR_INVALID, "vpt_render_passes: accum_buffer holds a finished adaptive frame (vpt_render_adaptive), which cannot be "
+                                                "continued; start a new frame with iteration == 0");
+            c->adaptive_accum = 0;
+        }
+    }
+
+    FramePlan plan;
+    { int rc = frame_setup(c, params, n_passes, stream, plan); if (rc != VPT_OK) return rc; }
+    vpt::FrameArgs& fa = plan.fa;
+    const vpt_kernel_params& kp = fa.kp;
+    const unsigned n_sampled = plan.n_sampled;
+    const int chunk = plan.chunk, bn_limit = plan.bn_limit;
     if (c->p2p_on && ((int)kp.resolution.x != c->p2p_w || (int)kp.resolution.y != c->p2p_h))
         return fail(c, VPT_ERR_INVALID, "the peer exchange block was exported for another frame size (vpt_comm_p2p_export)");
     { int rc = vpt::comm_p2p_begin(c, stream); if (rc != VPT_OK) return rc; }      // multi-GPU peer exchange: this rank's frame may be overwritten from here on
     const uint32_t it0 = kp.iteration;
-    const unsigned long long frame_px = (unsigned long long)kp.resolution.x * kp.resolution.y;
-    const int bn_limit = frame_px < 65536ull ? (int)frame_px : 65536;
     unsigned done = 0;
     while (done < n_sampled) {
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
         fa.kp.iteration = it0 + done;
-        VPT_CUDA(c, timed(3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
-        VPT_CUDA(c, timed(0, [&] { return vpt::launch_generate(fa, (int)np, stream); }));
-        if (c->brick_pool) VPT_CUDA(c, timed(1, [&] { return vpt::launch_trace_brick(fa, c->brick_pool, c->brick_dims, trace_ctas, stream); }));
-        else VPT_CUDA(c, timed(1, [&] { return vpt::launch_trace(fa, vol_integ ? &atmo : nullptr, lean, slots, trace_ctas, stream); }));
+        VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate(fa, (int)np, stream); }));
+        VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, timed(2, [&] { return vpt::launch_resolve(fa, sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, stream); }));
+        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, stream); }));
         c->launches += 4;
         done += np;
     }
@@ -372,7 +422,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, vpt::launch_resolve(fa, sky, (int)(n_passes - n_sampled), 0, 1, &peers, stream));
+        VPT_CUDA(c, vpt::launch_resolve(fa, plan.sky, (int)(n_passes - n_sampled), 0, 1, &peers, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2;
     }
@@ -383,6 +433,96 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         int rc = vpt::comm_gather_frame(c, fa.geom, (const void*)kp.accum_buffer, (const void*)kp.display_buffer, stream);
         if (rc != VPT_OK) return rc;
     }
+    return VPT_OK;
+}
+
+void vpt_adaptive_options_defaults(vpt_adaptive_options* opt) {
+    if (!opt) return;
+    opt->min_passes = 16; opt->check_interval = 16; opt->threshold = 0.01f;
+}
+
+// Adaptive frame.  Chunks end at every test point (min_passes, then every check_interval passes); after the resolve of a test chunk
+// k_adapt stops the converged pixels and lists the tiles still active, whose number the host reads back (one stream synchronisation per
+// test) to size the next chunk's grids.  Per pixel the work is that of vpt_render_passes: same Philox streams, same blue-noise table of
+// each pass, same running mean in pass order.
+int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned max_passes, const vpt_adaptive_options* opt,
+                        unsigned* d_pass_count, float* d_rel_error, unsigned* passes_run, void* stream_) {
+    if (!c || !params) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: null argument");
+    for (int i = 0; i < VPT_NUM_ARGS; ++i) if (!params[i]) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: params[" + std::to_string(i) + "] is null");
+    if (!d_pass_count) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: d_pass_count is required (one unsigned per pixel)");
+    vpt_adaptive_options o;
+    vpt_adaptive_options_defaults(&o);
+    if (opt) o = *opt;
+    if (o.min_passes < 2) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: min_passes must be >= 2 (the error estimate needs two samples)");
+    if (o.check_interval < 1) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: check_interval must be >= 1");
+    if (!(o.threshold >= 0.0f)) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: threshold must be >= 0");
+    if (max_passes == 0) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: max_passes must be >= 1");
+    if (c->n_ranks > 1 || c->nccl_comm || c->p2p_on)
+        return fail(c, VPT_ERR_UNSUPPORTED, "vpt_render_adaptive: a partitioned context (vpt_set_partition / vpt_comm_*) is not supported: "
+                                            "the 3x3 convergence test reads across stripe boundaries");
+    vpt_kernel_params kp0;
+    memcpy(&kp0, params[VPT_ARG_KERNEL_PARAMS], sizeof(vpt_kernel_params));
+    if (kp0.iteration != 0) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: Kernel_params.iteration must be 0 (an adaptive frame is a new frame)");
+    if (!kp0.render) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: Kernel_params.render is 0, nothing would be sampled");
+    if (kp0.max_interactions < 2) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: Kernel_params.max_interactions must be >= 2");
+    const unsigned n_total = max_passes < kp0.max_interactions ? max_passes : kp0.max_interactions;
+    cudaStream_t stream = (cudaStream_t)stream_;
+
+    FramePlan plan;
+    { int rc = frame_setup(c, params, n_total, stream, plan); if (rc != VPT_OK) return rc; }
+    vpt::FrameArgs& fa = plan.fa;
+    const vpt::FrameGeom& g = fa.geom;
+    const int n_tiles = ((g.width + 31) / 32) * ((g.local_rows + 3) / 4);
+
+    // per-pixel state and the two tile lists, grown on demand and kept for later frames
+    if ((size_t)g.n_local > c->cap_adapt_px) {
+        cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); c->d_adapt_stat = nullptr; c->d_adapt_stopped = nullptr; c->cap_adapt_px = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_adapt_stat, sizeof(float4) * (size_t)g.n_local));
+        VPT_CUDA(c, cudaMalloc(&c->d_adapt_stopped, (size_t)g.n_local));
+        c->cap_adapt_px = (size_t)g.n_local;
+    }
+    if ((size_t)n_tiles > c->cap_adapt_tiles) {
+        cudaFree(c->d_adapt_tiles); c->d_adapt_tiles = nullptr; c->cap_adapt_tiles = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_adapt_tiles, sizeof(unsigned) * (2 * (size_t)n_tiles + 1)));     // two lists + the count of the next one
+        c->cap_adapt_tiles = (size_t)n_tiles;
+    }
+    unsigned* lists[2] = { c->d_adapt_tiles, c->d_adapt_tiles + n_tiles };
+    unsigned* d_next_count = c->d_adapt_tiles + 2 * (size_t)n_tiles;
+
+    vpt::AdaptArgs ad;
+    ad.tiles = lists[0]; ad.n_tiles = n_tiles; ad.stopped = c->d_adapt_stopped; ad.stat = c->d_adapt_stat;
+    ad.pass_count = d_pass_count; ad.rel_error = d_rel_error;
+    ad.next_tiles = lists[1]; ad.next_count = d_next_count; ad.threshold = o.threshold;
+
+    c->adaptive_accum = kp0.accum_buffer;        // from here on the buffers hold an adaptive frame
+    VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt_init(g, c->d_adapt_stopped, lists[0], n_tiles, stream); }));
+    c->launches++;
+    const void* bn = (const void*)(uintptr_t)kp0.blue_noise_buffer;
+    unsigned done = 0, next_test = o.min_passes;
+    int cur = 0;
+    while (done < n_total && ad.n_tiles > 0) {
+        // a chunk never crosses a test point
+        const unsigned boundary = next_test < n_total ? next_test : n_total;
+        const unsigned np = (boundary - done) < (unsigned)plan.chunk ? (boundary - done) : (unsigned)plan.chunk;
+        fa.kp.iteration = done;
+        VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)bn, c->d_bn_table, (int)np, plan.bn_limit, c->d_counters, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
+        VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, stream); }));
+        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, stream); }));
+        c->launches += 4;
+        done += np;
+        if (done == next_test && done < n_total) {
+            VPT_CUDA(c, cudaMemsetAsync(d_next_count, 0, sizeof(unsigned), stream));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt(g, ad, stream); }));
+            VPT_CUDA(c, cudaMemcpyAsync(c->h_pinned, d_next_count, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+            VPT_CUDA(c, cudaStreamSynchronize(stream));
+            c->launches++;
+            cur ^= 1;
+            ad.tiles = lists[cur]; ad.next_tiles = lists[cur ^ 1]; ad.n_tiles = c->h_pinned[0];
+            next_test = o.check_interval > 0xffffffffu - next_test ? 0xffffffffu : next_test + o.check_interval;
+        }
+    }
+    if (passes_run) *passes_run = done;
     return VPT_OK;
 }
 

@@ -66,6 +66,12 @@ struct vpt_context {
     bool   gather_pending = false;
     size_t max_scratch_bytes = (size_t)12 << 30;                // cap of the per-chunk ray queue + sample planes
     int    chunk_auto = 1;                                      // passes_per_chunk not set by the caller: pick by local frame size
+    // adaptive frames (vpt_render_adaptive), allocated on first use
+    float4*   d_adapt_stat = nullptr;                           // [pixel] Welford state n, mean, M2, err of the sample luminance
+    uint8_t*  d_adapt_stopped = nullptr;                        // [pixel] 1 once stopped
+    unsigned* d_adapt_tiles = nullptr;                          // two active-tile lists + the count of the next one
+    size_t    cap_adapt_px = 0, cap_adapt_tiles = 0;
+    vpt_devptr_t adaptive_accum = 0;                            // accum_buffer of the last adaptive frame: vpt_render_passes may not continue it
 };
 
 

@@ -88,6 +88,23 @@ class Renderer:
         check(lib.vpt_render_passes(self.ctx, self.params.array, int(n_passes), C.c_void_p(stream or 0)), self.ctx, "vpt_render_passes")
         self.kp.iteration += int(n_passes)
 
+    def render_adaptive(self, max_passes, threshold=0.01, min_passes=16, check_interval=16, error_map=False, stream=None):
+        """One new frame (kp.iteration must be 0) of at most `max_passes` passes in which converged pixels stop early
+        (vpt_render_adaptive).  Returns (passes_run, counts) or, with error_map=True, (passes_run, counts, rel_error): counts is the
+        (H, W) int32 number of passes each pixel took, rel_error the (H, W) float32 relative error each pixel stopped with.  Every pixel
+        holds what render(counts[pixel]) would have left in it.  The frame is final: render() cannot continue it."""
+        opt = N.adaptive_options(int(min_passes), int(check_interval), float(threshold))
+        dev = self.buffers.accum.device
+        counts = torch.empty(self.n_local, dtype=torch.int32, device=dev)
+        err = torch.empty(self.n_local, dtype=torch.float32, device=dev) if error_map else None
+        run = C.c_uint(0)
+        check(lib.vpt_render_adaptive(self.ctx, self.params.array, int(max_passes), C.byref(opt), C.c_void_p(counts.data_ptr()),
+                                      C.c_void_p(err.data_ptr()) if err is not None else None, C.byref(run), C.c_void_p(stream or 0)),
+              self.ctx, "vpt_render_adaptive")
+        self.kp.iteration += int(run.value)
+        counts = counts.view(self.height, self.width)
+        return (int(run.value), counts, err.view(self.height, self.width)) if error_map else (int(run.value), counts)
+
     def reset(self):
         self.kp.iteration = 0
         self.buffers.zero_()
