@@ -103,6 +103,9 @@ int  vpt_comm_p2p_import(vpt_context* ctx, const unsigned char* handles /* n_ran
 int  vpt_comm_p2p_block(vpt_context* ctx, vpt_devptr_t* d_block);
 int  vpt_comm_p2p_import_local(vpt_context* ctx, const vpt_devptr_t* blocks /* n_ranks addresses, rank order */);
 int  vpt_comm_p2p_frame(vpt_context* ctx, vpt_devptr_t* d_full_accum_f3, vpt_devptr_t* d_full_display_u32);
+/* Full-frame planes [H][W] of the block that a sharded vpt_render_adaptive fills on every rank: unsigned pass counts and float relative
+ * errors, at global pixels.  A fixed-count call leaves them untouched.  Either output pointer may be NULL. */
+int  vpt_comm_p2p_adaptive_frame(vpt_context* ctx, vpt_devptr_t* d_full_pass_count_u32, vpt_devptr_t* d_full_rel_error_f32);
 int  vpt_comm_p2p_enable(vpt_context* ctx, int on);
 int  vpt_comm_p2p_status(vpt_context* ctx, unsigned long long* abandoned_waits);
 
@@ -138,9 +141,20 @@ int  vpt_render_passes(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsig
  *     active; everything else is enqueued asynchronously like vpt_render_passes.
  *   An adaptive frame is final.  vpt_render_passes with iteration > 0 on the accum_buffer of the context's last adaptive frame fails
  *     with VPT_ERR_INVALID; a call with iteration == 0 on it starts a new frame as usual.
- *   Refused: render == 0, max_interactions < 2, min_passes < 2, check_interval == 0, a negative threshold, max_passes == 0
- *     (VPT_ERR_INVALID); a partitioned context -- vpt_set_partition with n_ranks > 1, NCCL or peer exchange -- (VPT_ERR_UNSUPPORTED:
- *     the 3x3 test reads across stripes).  Brick mode and cell mode work.  opt == NULL takes the defaults. */
+ *   Multi-GPU.  A partitioned context renders its share of the frame when its peer-memory exchange is active (vpt_comm_p2p_export, then
+ *     vpt_comm_p2p_import or vpt_comm_p2p_import_local, not suspended by vpt_comm_p2p_enable(ctx, 0)).  Every rank makes the same call
+ *     with the same options, and the frame is exactly the single-context adaptive frame of the whole image: the 3x3 neighbourhood is taken
+ *     over global rows (clipped at the global frame edge), the same passes and tests are issued, every rank returns the same *passes_run
+ *     and advances its blue-noise replica that many times, also when all of its own pixels have stopped.  d_pass_count / d_rel_error hold
+ *     vpt_local_pixels() entries in rank-local order like the Kernel_params buffers; entries of padding rows (global row >= H) are 0.
+ *     When the call returns, every rank's exchange block holds the whole frame: accumulators and display words (vpt_comm_p2p_frame),
+ *     pass counts and relative errors (vpt_comm_p2p_adaptive_frame).  Every convergence test waits for all peers, so each rank's call
+ *     must be issued by its own host thread or process.  If a peer flag wait gives up (about 10 s), the call issues no further passes and
+ *     fails with VPT_ERR_CUDA naming the barrier; the exchange is then out of step and must be set up again.
+ *   Refused: render == 0, max_interactions < 2, min_passes < 2, check_interval == 0, a negative threshold, max_passes == 0, a frame size
+ *     other than the exported one (VPT_ERR_INVALID); a partitioned context without an active peer exchange -- vpt_set_partition alone, a
+ *     suspended exchange -- and the NCCL exchange, whose adaptive frames are not built (VPT_ERR_UNSUPPORTED).  Brick mode and cell mode
+ *     work.  opt == NULL takes the defaults. */
 typedef struct vpt_adaptive_options {
     unsigned min_passes;       /* passes every pixel takes before it may stop; >= 2 (default 16) */
     unsigned check_interval;   /* passes between two convergence tests; >= 1 (default 16) */

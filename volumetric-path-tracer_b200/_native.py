@@ -158,7 +158,7 @@ EXPORTED_SYMBOLS = [
     "vpt_texture_read_f4", "vpt_debug_texture_sample",
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
-    "vpt_adaptive_options_defaults", "vpt_render_adaptive",
+    "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
 ]
 
 # ---- prototypes ------------------------------------------------------------------------------------
@@ -211,6 +211,7 @@ lib.vpt_comm_p2p_import.argtypes = [_vp, C.POINTER(C.c_ubyte)]; lib.vpt_comm_p2p
 lib.vpt_comm_p2p_import_local.argtypes = [_vp, C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_import_local.restype = C.c_int
 lib.vpt_comm_p2p_block.argtypes = [_vp, C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_block.restype = C.c_int
 lib.vpt_comm_p2p_frame.argtypes = [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_frame.restype = C.c_int
+lib.vpt_comm_p2p_adaptive_frame.argtypes = [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_adaptive_frame.restype = C.c_int
 lib.vpt_comm_p2p_enable.argtypes = [_vp, C.c_int]; lib.vpt_comm_p2p_enable.restype = C.c_int
 lib.vpt_comm_p2p_status.argtypes = [_vp, C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_status.restype = C.c_int
 

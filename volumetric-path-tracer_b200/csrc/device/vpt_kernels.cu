@@ -13,6 +13,8 @@
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
 //   k_generate_adaptive, k_resolve_adaptive<S>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
+//   k_adapt_halo, k_adapt_count_publish, k_adapt_tally, k_adapt_publish : the same frame sharded over the peer-memory exchange -- stripe-edge
+//                     errors, the agreement on when to stop, and the final full-frame stores
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -426,11 +428,13 @@ k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_pass
     resolve_pixel<kSky, true>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad);
 }
 
-// Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (clipped at
-// the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A tile with a pixel still
-// active is appended to the next list (one atomic per tile).
+// Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
+// clipped at the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A neighbour row this
+// rank owns is read from ad.stat, a row of another rank from `halo` (the local exchange block's full-frame err plane, which k_adapt_halo of
+// every rank filled before the barrier ahead of this launch).  One rank owns every row: the neighbour set is the local one.  A tile with a
+// pixel still active is appended to the next list (one atomic per tile).
 __global__ void __launch_bounds__(128)
-k_adapt(const FrameGeom g, const AdaptArgs ad)
+k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo)
 {
     const int tile = (int)__ldg(ad.tiles + blockIdx.x);
     const TilePixel t = tile_pixel(g, tile);
@@ -439,13 +443,20 @@ k_adapt(const FrameGeom g, const AdaptArgs ad)
         const size_t lp = (size_t)t.lr * g.width + t.x;
         if (!ad.stopped[lp]) {
             float worst = 0.0f;
+            const int y = g.n_ranks > 1 ? global_row(g, t.lr) : t.lr;
             for (int dy = -1; dy <= 1; ++dy) {
-                const int r = t.lr + dy;
-                if (r < 0 || r >= g.local_rows) continue;
+                const int gy = y + dy;
+                if (gy < 0 || gy >= g.height) continue;
+                int r = gy; bool own = true;                           // r: local row of gy when this rank owns it
+                if (g.n_ranks > 1) {
+                    const int s = gy / g.stripe_h;
+                    own = s % g.n_ranks == g.rank;
+                    r = (s / g.n_ranks) * g.stripe_h + (gy - s * g.stripe_h);
+                }
                 for (int dx = -1; dx <= 1; ++dx) {
                     const int c = t.x + dx;
                     if (c < 0 || c >= g.width) continue;
-                    worst = fmaxf(worst, ad.stat[(size_t)r * g.width + c].w);
+                    worst = fmaxf(worst, own ? ad.stat[(size_t)r * g.width + c].w : halo[(size_t)gy * g.width + c]);
                 }
             }
             if (worst < ad.threshold) ad.stopped[lp] = 1;
@@ -460,6 +471,68 @@ __global__ void k_adapt_init(uint8_t* stopped, unsigned* tiles, int n_local, int
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(n_local, n_tiles); i += gridDim.x * blockDim.x) {
         if (i < n_local) stopped[i] = 0;
         if (i < n_tiles) tiles[i] = (unsigned)i;
+    }
+}
+
+// ---- sharded adaptive frames (peer-memory exchange) ---------------------------------------------------------------------------------
+// Halo, one block of 128 per active tile, after the resolve of a test chunk: a pixel that has not stopped and whose global row has a
+// neighbour row of another rank (first / last row of its stripe, inside the frame) stores its err at its global position in every rank's
+// err plane.  A stopped pixel's last store stays there, which is what the rule reads for a stopped neighbour.
+__global__ void __launch_bounds__(128)
+k_adapt_halo(const FrameGeom g, const AdaptArgs ad, const AdaptPeers pp)
+{
+    const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
+    if (!t.inside || g.n_ranks < 2) return;
+    const int y = global_row(g, t.lr);
+    const int off = y % g.stripe_h;
+    if (!((off == 0 && y > 0) || (off == g.stripe_h - 1 && y + 1 < g.height))) return;
+    const size_t lp = (size_t)t.lr * g.width + t.x;
+    if (ad.stopped[lp]) return;
+    const float e = ad.stat[lp].w;
+    const size_t gp = (size_t)y * g.width + t.x;
+    #pragma unroll
+    for (int p = 0; p < kMaxPeers; ++p) if (p < pp.n) pp.err[p][gp] = e;
+}
+
+// Count publish (lane p -> rank p's block) and the snapshot of the error word taken before the count barrier.
+__global__ void k_adapt_count_publish(const AdaptPeers pp, int rank, const unsigned* next_count, const unsigned long long* err_word, unsigned* out)
+{
+    const int p = threadIdx.x;
+    if (p == 0) out[2] = (unsigned)*reinterpret_cast<const volatile unsigned long long*>(err_word);
+    if (p < pp.n) pp.tiles[p][rank] = *next_count;
+}
+
+__global__ void k_adapt_tally(const unsigned* slots, int n, const unsigned long long* err_word, unsigned* out, int at)
+{
+    if (threadIdx.x != 0) return;
+    if (n > 0) {
+        unsigned s = 0;
+        for (int p = 0; p < n; ++p) s += reinterpret_cast<const volatile unsigned*>(slots)[p];   // stored by the peers before their flag
+        out[1] = s;
+    }
+    out[at] = (unsigned)*reinterpret_cast<const volatile unsigned long long*>(err_word);
+}
+
+// Final publish, one thread per local pixel: the finished pixel at its global position in every rank's planes.
+__global__ void __launch_bounds__(256)
+k_adapt_publish(const FrameGeom g, const float3* __restrict__ accum, const unsigned* __restrict__ display, unsigned* pass_count, float* rel_error,
+                const float4* __restrict__ stat, const AdaptPeers pp)
+{
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= (uint32_t)g.n_local) return;
+    const int lr = lp / g.width;
+    const int y = global_row(g, lr);
+    if (y >= g.height) { pass_count[lp] = 0u; if (rel_error) rel_error[lp] = 0.0f; return; }
+    const size_t gp = (size_t)y * g.width + (lp - (uint32_t)lr * (uint32_t)g.width);
+    const float3 a = accum[lp];
+    const unsigned n = pass_count[lp];
+    const float e = stat[lp].w;
+    const unsigned d = pp.display[0] ? display[lp] : 0u;
+    #pragma unroll
+    for (int p = 0; p < kMaxPeers; ++p) if (p < pp.n) {
+        float* q = pp.accum[p] + 3 * gp; q[0] = a.x; q[1] = a.y; q[2] = a.z;
+        if (pp.display[p]) pp.display[p][gp] = d;
+        pp.count[p][gp] = n; pp.err[p][gp] = e;
     }
 }
 
@@ -627,6 +700,27 @@ static cudaError_t trace_init_t(int* max_ctas)
 
 static size_t brick_smem_bytes() { return (size_t)kBrickThreads * kBrickBytes; }
 
+// Under lazy module loading (the CUDA 12 default) the first launch of a kernel loads it, and loading may wait for the device's running
+// kernels.  With a peer exchange, a rank's k_peer_wait spins until the other ranks' kernels have run, so a first launch on one rank
+// can wait behind that spin until the wait gives up.  The exchange therefore loads every kernel it may issue up front.
+cudaError_t exchange_kernels_preload()
+{
+    const void* fns[] = {
+        (const void*)k_bn_prepare, (const void*)k_bn_advance, (const void*)k_generate, (const void*)k_generate_adaptive,
+        (const void*)k_trace<0, false, 3>, (const void*)k_trace<0, true, 3>, (const void*)k_trace<1, false, 3>,
+        (const void*)k_trace<0, false, 2>, (const void*)k_trace<0, true, 2>, (const void*)k_trace<0, true, 2, true>, (const void*)k_trace_brick,
+        (const void*)k_resolve<0>, (const void*)k_resolve<1>, (const void*)k_resolve<2>,
+        (const void*)k_resolve_adaptive<0>, (const void*)k_resolve_adaptive<1>, (const void*)k_resolve_adaptive<2>,
+        (const void*)k_adapt_init, (const void*)k_adapt, (const void*)k_adapt_halo, (const void*)k_adapt_count_publish, (const void*)k_adapt_tally,
+        (const void*)k_adapt_publish, (const void*)k_peer_signal, (const void*)k_peer_wait };
+    for (const void* f : fns) {
+        cudaFuncAttributes a;
+        const cudaError_t e = cudaFuncGetAttributes(&a, f);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
 cudaError_t trace_kernels_init(int max_ctas[7])
 {
     {
@@ -684,10 +778,38 @@ cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* s
     return cudaGetLastError();
 }
 
-cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, cudaStream_t s)
+cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
-    k_adapt<<<ad.n_tiles, 128, 0, s>>>(g, ad);
+    k_adapt<<<ad.n_tiles, 128, 0, s>>>(g, ad, halo);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_halo(const FrameGeom& g, const AdaptArgs& ad, const AdaptPeers& pp, cudaStream_t s)
+{
+    if (ad.n_tiles <= 0 || g.n_ranks < 2) return cudaSuccess;
+    k_adapt_halo<<<ad.n_tiles, 128, 0, s>>>(g, ad, pp);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_count_publish(const AdaptPeers& pp, int rank, const unsigned* next_count, const unsigned long long* err_word,
+                                       unsigned* out, cudaStream_t s)
+{
+    k_adapt_count_publish<<<1, 32, 0, s>>>(pp, rank, next_count, err_word, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_tally(const unsigned* slots, int n, const unsigned long long* err_word, unsigned* out, int at, cudaStream_t s)
+{
+    k_adapt_tally<<<1, 32, 0, s>>>(slots, n, err_word, out, at);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_publish(const FrameGeom& g, const vpt_kernel_params& kp, const AdaptArgs& ad, const AdaptPeers& pp, cudaStream_t s)
+{
+    if (g.n_local <= 0) return cudaSuccess;
+    k_adapt_publish<<<(g.n_local + 255) / 256, 256, 0, s>>>(g, reinterpret_cast<const float3*>(kp.accum_buffer),
+                                                            reinterpret_cast<const unsigned*>(kp.display_buffer), ad.pass_count, ad.rel_error, ad.stat, pp);
     return cudaGetLastError();
 }
 

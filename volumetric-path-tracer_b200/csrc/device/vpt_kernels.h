@@ -92,7 +92,10 @@ cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
 cudaError_t launch_peer_wait(unsigned long long* local_flags, int n, int which, unsigned long long epoch, cudaStream_t s);
-constexpr int kPeerFlagStride = 16;                   // u64 slots per flag array; layout of a block header: ready[16] done[16] error[1]
+// loads every kernel a render call may issue (lazy module loading): no first launch may have to wait behind a peer's spinning flag wait
+cudaError_t exchange_kernels_preload();
+constexpr int kPeerFlagStride = 16;                   // u64 slots per flag array; layout of a block header: ready[16] done[16] error[1] (+15 unused) adapt[16]
+constexpr int kPeerFlagsAdapt = 3;                    // flag array of the two barriers of every convergence test of a sharded adaptive frame
 // limit = min(W*H, 65536) entries are advanced (the reference updates entry y*W + x from pixel (x, y))
 cudaError_t launch_bn_prepare(void* bn, float2* table, int np, int limit, unsigned* queue_counters, cudaStream_t s);   // also zeroes queue_counters[0..1]
 cudaError_t launch_bn_advance(void* bn, int n, int limit, cudaStream_t s);
@@ -101,9 +104,27 @@ cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& 
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, cudaStream_t s);
-// convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood has err < threshold, lists the tiles still active
-cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, cudaStream_t s);
+// convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
+// active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
+cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);
 // start of an adaptive frame: no pixel stopped, tile list = every tile
 cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, int n_tiles, cudaStream_t s);
+
+// Sharded adaptive frame over the peer-memory exchange: every rank's block as mapped here, full-frame planes [H][W] at global pixels.
+struct AdaptPeers {
+    int n = 0;
+    float* accum[kMaxPeers] = {}; unsigned int* display[kMaxPeers] = {};   // display null when the block was exported without it
+    unsigned* count[kMaxPeers] = {}; float* err[kMaxPeers] = {};           // pass counts, relative errors (err doubles as the 3x3 halo)
+    unsigned* tiles[kMaxPeers] = {};                                       // [rank] active-tile count of every rank after a test
+};
+// at a test chunk: the err of every active pixel whose global row borders another rank's stripe, into every rank's err plane
+cudaError_t launch_adapt_halo(const FrameGeom& g, const AdaptArgs& ad, const AdaptPeers& pp, cudaStream_t s);
+// after k_adapt: this rank's active-tile count (*next_count) into slot `rank` of every rank's count array; out[2] = the local error word
+cudaError_t launch_adapt_count_publish(const AdaptPeers& pp, int rank, const unsigned* next_count, const unsigned long long* err_word,
+                                       unsigned* out, cudaStream_t s);
+// out[1] = sum of the n local count slots (n > 0), out[at] = the local error word (abandoned flag waits so far)
+cudaError_t launch_adapt_tally(const unsigned* slots, int n, const unsigned long long* err_word, unsigned* out, int at, cudaStream_t s);
+// end of the frame: accum, display, pass count and err of every local pixel into every rank's planes; padding rows get count 0 / err 0
+cudaError_t launch_adapt_publish(const FrameGeom& g, const vpt_kernel_params& kp, const AdaptArgs& ad, const AdaptPeers& pp, cudaStream_t s);
 
 } // namespace vpt

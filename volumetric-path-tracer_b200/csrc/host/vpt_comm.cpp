@@ -104,8 +104,16 @@ int comm_gather_frame(vpt_context* c, const FrameGeom& g, const void* d_local_ac
 }
 
 // ---- peer-memory exchange ---------------------------------------------------------------------------------------------------------
-static constexpr size_t kP2pHeader = 512;                      // ready[16] done[16] error[1] as u64
-static size_t p2p_accum_bytes(const vpt_context* c) { return (((size_t)c->p2p_w * c->p2p_h * 12) + 255) & ~(size_t)255; }
+// Block layout: header (u64 flag arrays: ready[16] done[16] error[1], adapt[16] at kPeerFlagsAdapt) | float3 accum [H][W] | u32 display
+// [H][W] (exported with display only) | u32 pass counts [H][W] | f32 relative errors [H][W] | u32 active-tile count per rank [16].
+// The last three serve vpt_render_adaptive; each part starts on a 256-byte boundary.
+static constexpr size_t kP2pHeader = 512;
+static size_t p2p_round(size_t b) { return (b + 255) & ~(size_t)255; }
+static size_t p2p_accum_bytes(const vpt_context* c) { return p2p_round((size_t)c->p2p_w * c->p2p_h * 12); }
+static size_t p2p_plane_bytes(const vpt_context* c) { return p2p_round((size_t)c->p2p_w * c->p2p_h * 4); }
+static size_t p2p_count_offset(const vpt_context* c) { return kP2pHeader + p2p_accum_bytes(c) + (c->p2p_display ? p2p_plane_bytes(c) : 0); }
+static size_t p2p_err_offset(const vpt_context* c) { return p2p_count_offset(c) + p2p_plane_bytes(c); }
+static size_t p2p_tiles_offset(const vpt_context* c) { return p2p_err_offset(c) + p2p_plane_bytes(c); }
 static unsigned long long* p2p_flags(void* block) { return reinterpret_cast<unsigned long long*>(block); }
 
 int comm_p2p_begin(vpt_context* c, cudaStream_t stream) {
@@ -142,6 +150,33 @@ int comm_p2p_end(vpt_context* c, cudaStream_t stream) {
     return VPT_OK;
 }
 
+void comm_p2p_adapt_views(vpt_context* c, AdaptPeers* out, P2pAdaptLocal* local) {
+    *out = AdaptPeers{};
+    out->n = c->p2p_n;
+    for (int p = 0; p < c->p2p_n; ++p) {
+        char* base = reinterpret_cast<char*>(c->p2p_peer[p]);
+        out->accum[p] = reinterpret_cast<float*>(base + kP2pHeader);
+        out->display[p] = c->p2p_display ? reinterpret_cast<unsigned int*>(base + kP2pHeader + p2p_accum_bytes(c)) : nullptr;
+        out->count[p] = reinterpret_cast<unsigned*>(base + p2p_count_offset(c));
+        out->err[p] = reinterpret_cast<float*>(base + p2p_err_offset(c));
+        out->tiles[p] = reinterpret_cast<unsigned*>(base + p2p_tiles_offset(c));
+    }
+    char* own = reinterpret_cast<char*>(c->p2p_block);
+    local->halo = reinterpret_cast<const float*>(own + p2p_err_offset(c));
+    local->tiles = reinterpret_cast<const unsigned*>(own + p2p_tiles_offset(c));
+    local->error_word = p2p_flags(c->p2p_block) + 2 * kPeerFlagStride;
+}
+
+int comm_p2p_adapt_barrier(vpt_context* c, cudaStream_t stream) {
+    ++c->p2p_adapt_epoch;
+    unsigned long long* fl[kMaxPeers];
+    for (int p = 0; p < kMaxPeers; ++p) fl[p] = p < c->p2p_n ? p2p_flags(c->p2p_peer[p]) : nullptr;
+    VPT_CU(c, launch_peer_signal(fl, c->p2p_n, c->rank, kPeerFlagsAdapt, c->p2p_adapt_epoch, stream));
+    VPT_CU(c, launch_peer_wait(p2p_flags(c->p2p_block), c->p2p_n, kPeerFlagsAdapt, c->p2p_adapt_epoch, stream));
+    c->launches += 2;
+    return VPT_OK;
+}
+
 } // namespace vpt
 
 extern "C" {
@@ -155,8 +190,9 @@ int vpt_comm_p2p_export(vpt_context* c, int rank, int n_ranks, int stripe_rows, 
     VPT_CU(c, cudaSetDevice(c->device));
     int rc = vpt_set_partition(c, rank, n_ranks, stripe_rows);
     if (rc != VPT_OK) return rc;
+    VPT_CU(c, vpt::exchange_kernels_preload());
     c->p2p_w = (int)width; c->p2p_h = (int)height; c->p2p_display = with_display != 0; c->p2p_n = n_ranks;
-    c->p2p_bytes = vpt::kP2pHeader + vpt::p2p_accum_bytes(c) + (with_display ? (size_t)width * height * 4 : 0);
+    c->p2p_bytes = vpt::p2p_tiles_offset(c) + sizeof(unsigned) * vpt::kPeerFlagStride;
     VPT_CU(c, cudaMalloc(&c->p2p_block, c->p2p_bytes));
     VPT_CU(c, cudaMemset(c->p2p_block, 0, c->p2p_bytes));
     VPT_CU(c, cudaDeviceSynchronize());
@@ -173,7 +209,7 @@ int vpt_comm_p2p_import(vpt_context* c, const unsigned char* handles) {
         cudaIpcMemHandle_t h; memcpy(&h, handles + (size_t)p * VPT_P2P_HANDLE_BYTES, sizeof(h));
         VPT_CU(c, cudaIpcOpenMemHandle(&c->p2p_peer[p], h, cudaIpcMemLazyEnablePeerAccess));
     }
-    c->p2p_on = true; c->p2p_epoch = 0;
+    c->p2p_on = true; c->p2p_epoch = 0; c->p2p_adapt_epoch = 0;
     return VPT_OK;
 }
 
@@ -183,7 +219,7 @@ int vpt_comm_p2p_import_local(vpt_context* c, const vpt_devptr_t* blocks) {
         if (p != c->rank && !blocks[p]) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_import_local: null block");
         c->p2p_peer[p] = p == c->rank ? c->p2p_block : reinterpret_cast<void*>(blocks[p]);
     }
-    c->p2p_local = true; c->p2p_on = true; c->p2p_epoch = 0;
+    c->p2p_local = true; c->p2p_on = true; c->p2p_epoch = 0; c->p2p_adapt_epoch = 0;
     return VPT_OK;
 }
 
@@ -198,6 +234,14 @@ int vpt_comm_p2p_frame(vpt_context* c, vpt_devptr_t* d_full_accum, vpt_devptr_t*
     char* base = reinterpret_cast<char*>(c->p2p_block);
     if (d_full_accum) *d_full_accum = (vpt_devptr_t)(base + vpt::kP2pHeader);
     if (d_full_display) *d_full_display = c->p2p_display ? (vpt_devptr_t)(base + vpt::kP2pHeader + vpt::p2p_accum_bytes(c)) : 0;
+    return VPT_OK;
+}
+
+int vpt_comm_p2p_adaptive_frame(vpt_context* c, vpt_devptr_t* d_full_pass_count, vpt_devptr_t* d_full_rel_error) {
+    if (!c || !c->p2p_block) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_adaptive_frame: no exchange block");
+    char* base = reinterpret_cast<char*>(c->p2p_block);
+    if (d_full_pass_count) *d_full_pass_count = (vpt_devptr_t)(base + vpt::p2p_count_offset(c));
+    if (d_full_rel_error) *d_full_rel_error = (vpt_devptr_t)(base + vpt::p2p_err_offset(c));
     return VPT_OK;
 }
 

@@ -104,7 +104,7 @@ int vpt_create(vpt_context** out) {
     VPT_CREATE(cudaMalloc(&c->d_counters, sizeof(unsigned) * 4));
     VPT_CREATE(cudaMalloc(&c->d_stats, sizeof(unsigned long long) * 8));
     VPT_CREATE(cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 8));
-    VPT_CREATE(cudaHostAlloc((void**)&c->h_pinned, sizeof(int) * 4, cudaHostAllocDefault));
+    VPT_CREATE(cudaHostAlloc((void**)&c->h_pinned, sizeof(int) * 8, cudaHostAllocDefault));
     // per-DEVICE kernel attributes (dynamic shared memory opt-in) and the occupancy the persistent grid is sized with
     VPT_CREATE(vpt::trace_kernels_init(c->max_ctas));
 #undef VPT_CREATE
@@ -444,7 +444,8 @@ void vpt_adaptive_options_defaults(vpt_adaptive_options* opt) {
 // Adaptive frame.  Chunks end at every test point (min_passes, then every check_interval passes); after the resolve of a test chunk
 // k_adapt stops the converged pixels and lists the tiles still active, whose number the host reads back (one stream synchronisation per
 // test) to size the next chunk's grids.  Per pixel the work is that of vpt_render_passes: same Philox streams, same blue-noise table of
-// each pass, same running mean in pass order.
+// each pass, same running mean in pass order.  A partitioned context with an active peer-memory exchange renders its share of the same
+// frame: halo, agreement on when to stop and the final publish go through the exchange blocks (DESIGN.md section 8a).
 int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned max_passes, const vpt_adaptive_options* opt,
                         unsigned* d_pass_count, float* d_rel_error, unsigned* passes_run, void* stream_) {
     if (!c || !params) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: null argument");
@@ -457,11 +458,15 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
     if (o.check_interval < 1) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: check_interval must be >= 1");
     if (!(o.threshold >= 0.0f)) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: threshold must be >= 0");
     if (max_passes == 0) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: max_passes must be >= 1");
-    if (c->n_ranks > 1 || c->nccl_comm || c->p2p_on)
-        return fail(c, VPT_ERR_UNSUPPORTED, "vpt_render_adaptive: a partitioned context (vpt_set_partition / vpt_comm_*) is not supported: "
-                                            "the 3x3 convergence test reads across stripe boundaries");
+    // a partitioned frame needs the peer-memory exchange: the 3x3 test reads across stripe boundaries and the ranks must agree on when to stop
+    if (c->nccl_comm || (c->p2p_block && !c->p2p_on) || (c->n_ranks > 1 && !c->p2p_on))
+        return fail(c, VPT_ERR_UNSUPPORTED, "vpt_render_adaptive: a partitioned context is supported only with an active peer-memory exchange "
+                                            "(vpt_comm_p2p_export + import); vpt_set_partition alone, a suspended exchange and NCCL are not");
+    const bool sharded = c->p2p_on;
     vpt_kernel_params kp0;
     memcpy(&kp0, params[VPT_ARG_KERNEL_PARAMS], sizeof(vpt_kernel_params));
+    if (sharded && ((int)kp0.resolution.x != c->p2p_w || (int)kp0.resolution.y != c->p2p_h))
+        return fail(c, VPT_ERR_INVALID, "the peer exchange block was exported for another frame size (vpt_comm_p2p_export)");
     if (kp0.iteration != 0) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: Kernel_params.iteration must be 0 (an adaptive frame is a new frame)");
     if (!kp0.render) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: Kernel_params.render is 0, nothing would be sampled");
     if (kp0.max_interactions < 2) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: Kernel_params.max_interactions must be >= 2");
@@ -483,10 +488,12 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
     }
     if ((size_t)n_tiles > c->cap_adapt_tiles) {
         cudaFree(c->d_adapt_tiles); c->d_adapt_tiles = nullptr; c->cap_adapt_tiles = 0;
-        VPT_CUDA(c, cudaMalloc(&c->d_adapt_tiles, sizeof(unsigned) * (2 * (size_t)n_tiles + 1)));     // two lists + the count of the next one
+        VPT_CUDA(c, cudaMalloc(&c->d_adapt_tiles, sizeof(unsigned) * (2 * (size_t)n_tiles + 5)));     // two lists + the read-back words below
         c->cap_adapt_tiles = (size_t)n_tiles;
     }
     unsigned* lists[2] = { c->d_adapt_tiles, c->d_adapt_tiles + n_tiles };
+    // read back after a test: [0] tiles still active here (k_adapt's count of the next list); sharded frames also [1] tiles still active on
+    // all ranks, [2] / [3] the error word after the halo / count barrier, [4] the error word when the call began
     unsigned* d_next_count = c->d_adapt_tiles + 2 * (size_t)n_tiles;
 
     vpt::AdaptArgs ad;
@@ -497,30 +504,79 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
     c->adaptive_accum = kp0.accum_buffer;        // from here on the buffers hold an adaptive frame
     VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt_init(g, c->d_adapt_stopped, lists[0], n_tiles, stream); }));
     c->launches++;
+
+    // Sharded frame (peer-memory exchange): at every test the stripe-edge errors travel through the err planes of the blocks (halo), and
+    // the ranks agree on the number of tiles still active anywhere; the frame goes on while that is > 0, so every rank issues the same
+    // passes.  Two barriers per test on the adapt flags; ordering argument in DESIGN.md section 8a.
+    vpt::AdaptPeers peers;
+    vpt::P2pAdaptLocal own;
+    bool entered = false;                        // every peer has entered this call: stores into their blocks are allowed
+    auto await_peers = [&]() -> int {
+        if (entered) return VPT_OK;
+        entered = true;
+        vpt::PeerFrames unused;
+        return vpt::comm_p2p_peers(c, stream, &unused);
+    };
+    if (sharded) {
+        vpt::comm_p2p_adapt_views(c, &peers, &own);
+        { int rc = vpt::comm_p2p_begin(c, stream); if (rc != VPT_OK) return rc; }
+        VPT_CUDA(c, vpt::launch_adapt_tally(nullptr, 0, own.error_word, d_next_count, 4, stream));
+        c->launches++;
+    }
     const void* bn = (const void*)(uintptr_t)kp0.blue_noise_buffer;
     unsigned done = 0, next_test = o.min_passes;
+    unsigned active_anywhere = (unsigned)n_tiles;      // sharded: tiles still active on any rank (a rank may have none left of its own)
     int cur = 0;
-    while (done < n_total && ad.n_tiles > 0) {
+    while (done < n_total && active_anywhere > 0) {
         // a chunk never crosses a test point
         const unsigned boundary = next_test < n_total ? next_test : n_total;
         const unsigned np = (boundary - done) < (unsigned)plan.chunk ? (boundary - done) : (unsigned)plan.chunk;
         fa.kp.iteration = done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)bn, c->d_bn_table, (int)np, plan.bn_limit, c->d_counters, stream); }));
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
-        VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, stream); }));
-        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, stream); }));
-        c->launches += 4;
+        c->launches++;
+        if (ad.n_tiles > 0) {
+            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
+            VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, stream); }));
+            c->launches += 3;
+        }
         done += np;
         if (done == next_test && done < n_total) {
             VPT_CUDA(c, cudaMemsetAsync(d_next_count, 0, sizeof(unsigned), stream));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt(g, ad, stream); }));
-            VPT_CUDA(c, cudaMemcpyAsync(c->h_pinned, d_next_count, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
-            VPT_CUDA(c, cudaStreamSynchronize(stream));
+            if (sharded) {
+                { int rc = await_peers(); if (rc != VPT_OK) return rc; }
+                VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt_halo(g, ad, peers, stream); }));
+                { int rc = vpt::comm_p2p_adapt_barrier(c, stream); if (rc != VPT_OK) return rc; }         // halo barrier
+            }
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt(g, ad, own.halo, stream); }));
             c->launches++;
+            if (sharded) {
+                VPT_CUDA(c, vpt::launch_adapt_count_publish(peers, c->rank, d_next_count, own.error_word, d_next_count, stream));
+                { int rc = vpt::comm_p2p_adapt_barrier(c, stream); if (rc != VPT_OK) return rc; }         // count barrier
+                VPT_CUDA(c, vpt::launch_adapt_tally(own.tiles, c->p2p_n, own.error_word, d_next_count, 3, stream));
+                VPT_CUDA(c, cudaMemcpyAsync(c->h_pinned, d_next_count, 5 * sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+                c->launches += 3;
+            } else {
+                VPT_CUDA(c, cudaMemcpyAsync(c->h_pinned, d_next_count, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+            }
+            VPT_CUDA(c, cudaStreamSynchronize(stream));
+            const unsigned* h = reinterpret_cast<const unsigned*>(c->h_pinned);
+            if (sharded && h[3] != h[4])                 // a flag wait gave up (a rank is gone or made other calls): stop, do not trust the counts
+                return fail(c, VPT_ERR_CUDA, std::string("vpt_render_adaptive: a peer flag wait was abandoned at the ") +
+                                             (h[2] != h[4] ? "halo barrier (or the wait for the peers to enter the call)" : "count barrier") +
+                                             " of the convergence test after " + std::to_string(done) + " passes; the exchange is no longer in step");
             cur ^= 1;
-            ad.tiles = lists[cur]; ad.next_tiles = lists[cur ^ 1]; ad.n_tiles = c->h_pinned[0];
+            ad.tiles = lists[cur]; ad.next_tiles = lists[cur ^ 1]; ad.n_tiles = (int)h[0];
+            active_anywhere = sharded ? h[1] : h[0];
             next_test = o.check_interval > 0xffffffffu - next_test ? 0xffffffffu : next_test + o.check_interval;
         }
+    }
+    if (sharded) {
+        // every local pixel, finished, into every rank's full-frame planes; then publish and wait until every peer has done the same
+        { int rc = await_peers(); if (rc != VPT_OK) return rc; }
+        VPT_CUDA(c, vpt::launch_adapt_publish(g, fa.kp, ad, peers, stream));
+        c->launches++;
+        { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }
     if (passes_run) *passes_run = done;
     return VPT_OK;

@@ -23,7 +23,7 @@ struct vpt_context {
     unsigned long long cached_generation = 0;
     bool   scene_single_volume = false;
     size_t cap_vrec = 0;              // VolumeRec capacity (grows with the instance count)
-    int*   h_pinned = nullptr;        // one pinned word for the 4-byte read-back a foreign octree needs
+    int*   h_pinned = nullptr;        // eight pinned words: the read-back a foreign octree needs, the tile counts of an adaptive test
     int    max_ctas[7] = {0, 0, 0, 0, 0, 0, 0};   // trace kernel occupancy: [0] generic, [1] lean, [2] volumetric path, [3] brick mode, [4] generic / [5] lean at 2 rays per lane, [6] lean + cell table
     size_t l2_fetch_default = 0; int l2_sector_fetch = 0;     // option "l2_sector_fetch" (cell mode)
     const float4* cell_table = nullptr; int cell_dims[3] = {0, 0, 0};   // vpt_set_cell_volume
@@ -62,6 +62,7 @@ struct vpt_context {
     void*  p2p_block = nullptr; size_t p2p_bytes = 0; int p2p_w = 0, p2p_h = 0;
     void*  p2p_peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [rank] -> that rank's block as mapped here (own: p2p_block)
     int    p2p_n = 0; bool p2p_on = false, p2p_display = false, p2p_local = false; unsigned long long p2p_epoch = 0;
+    unsigned long long p2p_adapt_epoch = 0;                     // barriers of the convergence tests of sharded adaptive frames (flag array kPeerFlagsAdapt)
     int    gather_async = 0;                                    // option "gather_async": gather on the side stream (see vpt_comm_wait)
     bool   gather_pending = false;
     size_t max_scratch_bytes = (size_t)12 << 30;                // cap of the per-chunk ray queue + sample planes
@@ -114,6 +115,10 @@ FrameGeom make_frame_geom(const vpt_context* c, unsigned w, unsigned h);
 int  comm_p2p_begin(vpt_context* c, cudaStream_t stream);                                        // call start: tell the peers this rank's frame may be overwritten
 int  comm_p2p_peers(vpt_context* c, cudaStream_t stream, PeerFrames* out);                       // before the call's last resolve: wait for the peers, hand out their frames
 int  comm_p2p_end(vpt_context* c, cudaStream_t stream);                                          // after it: publish, and wait until every peer has published
+// sharded adaptive frames: every rank's planes as mapped here, and the local block's halo (err plane), count slots and error word
+struct P2pAdaptLocal { const float* halo = nullptr; const unsigned* tiles = nullptr; const unsigned long long* error_word = nullptr; };
+void comm_p2p_adapt_views(vpt_context* c, AdaptPeers* out, P2pAdaptLocal* local);
+int  comm_p2p_adapt_barrier(vpt_context* c, cudaStream_t stream);                                // signal + wait on the adapt flags (own epoch)
 int  comm_gather_frame(vpt_context* c, const FrameGeom& g, const void* d_local_accum, const void* d_local_display, cudaStream_t stream);
 int  comm_before_accum_write(vpt_context* c, cudaStream_t stream);   // async mode: the previous gather must have read accum
 

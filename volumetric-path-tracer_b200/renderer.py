@@ -92,7 +92,9 @@ class Renderer:
         """One new frame (kp.iteration must be 0) of at most `max_passes` passes in which converged pixels stop early
         (vpt_render_adaptive).  Returns (passes_run, counts) or, with error_map=True, (passes_run, counts, rel_error): counts is the
         (H, W) int32 number of passes each pixel took, rel_error the (H, W) float32 relative error each pixel stopped with.  Every pixel
-        holds what render(counts[pixel]) would have left in it.  The frame is final: render() cannot continue it."""
+        holds what render(counts[pixel]) would have left in it.  The frame is final: render() cannot continue it.
+        Partitioned (n_ranks > 1, peer-memory exchange active): this rank's share of the frame, counts and rel_error shaped
+        (local_rows, W) in rank-local order (padding rows 0); every rank must make the same call, each from its own thread or process."""
         opt = N.adaptive_options(int(min_passes), int(check_interval), float(threshold))
         dev = self.buffers.accum.device
         counts = torch.empty(self.n_local, dtype=torch.int32, device=dev)
@@ -102,8 +104,9 @@ class Renderer:
                                       C.c_void_p(err.data_ptr()) if err is not None else None, C.byref(run), C.c_void_p(stream or 0)),
               self.ctx, "vpt_render_adaptive")
         self.kp.iteration += int(run.value)
-        counts = counts.view(self.height, self.width)
-        return (int(run.value), counts, err.view(self.height, self.width)) if error_map else (int(run.value), counts)
+        rows = self.n_local // self.width
+        counts = counts.view(rows, self.width)
+        return (int(run.value), counts, err.view(rows, self.width)) if error_map else (int(run.value), counts)
 
     def reset(self):
         self.kp.iteration = 0
@@ -243,6 +246,29 @@ class DistributedRenderer:
         if self.world == 1:
             self.full.copy_(self.r.buffers.accum)
             if self.full_display is not None: self.full_display.copy_(self.r.buffers.display)
+
+    def render_adaptive(self, max_passes, threshold=0.01, min_passes=16, check_interval=16, error_map=False, stream=None):
+        """One adaptive frame of the whole image (Renderer.render_adaptive), sharded over the ranks; every rank makes the same call.
+        Returns (passes_run, counts) or, with error_map=True, (passes_run, counts, rel_error), full-frame (H, W) tensors -- with more
+        than one rank, views of this rank's exchange block that the next render call overwrites.  full_accum() then holds the frame.
+        Needs the peer-memory exchange: with exchange="nccl" it raises VptError."""
+        if self.world > 1 and self.exchange != "p2p":
+            raise N.VptError("DistributedRenderer.render_adaptive: adaptive frames need the peer-memory exchange (exchange='p2p'); "
+                             "the NCCL exchange does not support them")
+        out = self.r.render_adaptive(max_passes, threshold=threshold, min_passes=min_passes, check_interval=check_interval,
+                                     error_map=error_map, stream=stream)
+        H, W = self.r.height, self.r.width
+        if self.world == 1:
+            self.full.copy_(self.r.buffers.accum)
+            if self.full_display is not None: self.full_display.copy_(self.r.buffers.display)
+            return out
+        pc, pe = C.c_uint64(0), C.c_uint64(0)
+        check(lib.vpt_comm_p2p_adaptive_frame(self.r.ctx, C.byref(pc), C.byref(pe)), self.r.ctx, "vpt_comm_p2p_adaptive_frame")
+        dev = self.full.device
+        counts = torch.as_tensor(_DeviceView(pc.value, (H, W), "<i4"), device=dev)
+        if not error_map:
+            return out[0], counts
+        return out[0], counts, torch.as_tensor(_DeviceView(pe.value, (H, W), "<f4"), device=dev)
 
     def set_gather(self, enabled: bool):
         """Switch the per-call exchange off (rank-local work only: profiling runs that not every rank takes part in) or back on."""
