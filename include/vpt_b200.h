@@ -164,6 +164,47 @@ void vpt_adaptive_options_defaults(vpt_adaptive_options* opt);
 int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsigned max_passes, const vpt_adaptive_options* opt,
                          unsigned* d_pass_count, float* d_rel_error, unsigned* passes_run, void* stream);
 
+/* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
+ * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
+ * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.
+ *
+ *   Noise.  Y = 0.2126 r + 0.7152 g + 0.0722 b.  With d_rel_error (vpt_render_adaptive's error map; threshold 0 gives a fixed-count frame
+ *     with one) the variance of the pixel's mean luminance is v = (err * max(Y, 1e-3))^2, which inverts err = sigma / max(mean, 1e-3) with
+ *     the colour's Y for the mean; an err that is NaN or <= 0 gives v = 0, +inf stays +inf.  Without it, v is the population variance of
+ *     Y over the 5x5 window (clipped at the frame edge).
+ *   Levels.  Level i = 0 .. iterations-1 has step s = 2^i.  g = the 3x3 Gaussian (1/4, 1/2, 1/4)^2 of the current v (renormalised at the
+ *     frame edge); a pixel with g == 0 keeps its colour and variance bit for bit.  Otherwise its taps q at s * (-2..2)^2 with the B3-spline
+ *     weights h = (1/16, 1/4, 3/8, 1/4, 1/16)^2 (taps outside the frame drop out) weigh
+ *         w = exp(-|Y_p - Y_q| / (sigma_luminance sqrt(g) + 1e-10) - |z_p - z_q| / (sigma_depth max(|z_p|, |z_q|) + 1e-6))
+ *     (no depth term when d_depth is NULL; the centre tap weighs 1), and c' = sum(h w c_q) / sum(h w), v' = sum((h w)^2 v_q) / sum(h w)^2.
+ *   Non-finite pixels.  A pixel whose colour (or luminance) is not finite is copied unchanged and has weight 0 as a neighbour.
+ *   Outputs.  The last level writes d_out_f3 and, if d_out_display is given, the display word of each pixel exactly as k_resolve packs it
+ *     (ACES, exposure_scale, gamma 2.2, BGRA).  A zero error map therefore reproduces the colour and k_resolve's display words bit for bit.
+ *   Contract.  The work is enqueued asynchronously on `stream` (a cudaStream_t), with no synchronisation.  All buffers are full row-major
+ *     [H][W] frames in device memory; on a partitioned context pass the full frame of the exchange block (vpt_comm_p2p_frame,
+ *     vpt_comm_p2p_adaptive_frame), not the rank-local Kernel_params buffers.  Deterministic: no atomics, the same inputs give the same
+ *     bits.  d_out_f3 may EQUAL d_color_f3 (in place, as the reference's Denoise button); any partial overlap of an output with an input,
+ *     and any overlap of the two outputs, is refused.  The scratch planes (48 B per pixel, allocated on first use) belong to the context,
+ *     so calls on one context must be ordered on one stream.  The filter touches no render state: accumulating further passes onto an
+ *     accumulator denoised in place continues from the filtered mean.
+ *   Refused (VPT_ERR_INVALID): a NULL ctx, colour or output; width or height 0 or above 65535; iterations outside 1..10; a sigma that is
+ *     not finite and > 0; the overlaps above.  opt == NULL takes the defaults. */
+typedef struct vpt_denoise_options {
+    unsigned iterations;       /* a-trous levels, step 2^i for level i; 1..10 (default 5: steps 1..16) */
+    float    sigma_luminance;  /* luminance edge-stopping, in units of the pixel's noise sigma; > 0 (default 4) */
+    float    sigma_depth;      /* relative depth edge-stopping; > 0 (default 0.2) */
+} vpt_denoise_options;
+void vpt_denoise_options_defaults(vpt_denoise_options* opt);
+int  vpt_denoise(vpt_context* ctx, unsigned width, unsigned height,
+                 const float* d_color_f3,         /* [H][W] float3 HDR, e.g. accum_buffer or vpt_comm_p2p_frame's accumulators */
+                 const float* d_depth,            /* [H][W] float, may be NULL: no depth term */
+                 const float* d_rel_error,        /* [H][W] float, vpt_render_adaptive's error map, may be NULL: spatial estimate */
+                 const vpt_denoise_options* opt,  /* NULL = defaults */
+                 float exposure_scale,            /* only read when d_out_display != NULL */
+                 float* d_out_f3,                 /* [H][W] float3; may EQUAL d_color_f3 */
+                 unsigned* d_out_display,         /* [H][W] BGRA words as k_resolve writes them, may be NULL */
+                 void* stream);
+
 /* The flattened scene tables are cached per (volumes pointer, octree root pointer, build generation of a vpt_octree_build
  * octree) and refreshed whenever a call arrives with Kernel_params.iteration == 0 (the reference application resets the
  * iteration on every scene edit, main.cpp:1667-1780).  Call this only if the GPU_VDB[] array or a foreign octree was

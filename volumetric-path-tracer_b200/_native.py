@@ -159,6 +159,7 @@ EXPORTED_SYMBOLS = [
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
     "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
+    "vpt_denoise_options_defaults", "vpt_denoise",
 ]
 
 # ---- prototypes ------------------------------------------------------------------------------------
@@ -184,6 +185,15 @@ class adaptive_options(C.Structure):
 lib.vpt_adaptive_options_defaults.argtypes = [C.POINTER(adaptive_options)]; lib.vpt_adaptive_options_defaults.restype = None
 lib.vpt_render_adaptive.argtypes = [_vp, C.POINTER(_vp), C.c_uint, C.POINTER(adaptive_options), _vp, _vp, C.POINTER(C.c_uint), _vp]
 lib.vpt_render_adaptive.restype = C.c_int
+
+
+class denoise_options(C.Structure):
+    _fields_ = [("iterations", C.c_uint), ("sigma_luminance", C.c_float), ("sigma_depth", C.c_float)]
+
+
+lib.vpt_denoise_options_defaults.argtypes = [C.POINTER(denoise_options)]; lib.vpt_denoise_options_defaults.restype = None
+lib.vpt_denoise.argtypes = [_vp, C.c_uint, C.c_uint, _vp, _vp, _vp, C.POINTER(denoise_options), C.c_float, _vp, _vp, _vp]
+lib.vpt_denoise.restype = C.c_int
 lib.vpt_get_stats.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.POINTER(C.c_uint)]; lib.vpt_get_stats.restype = C.c_int
 lib.vpt_get_counters.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.c_int]; lib.vpt_get_counters.restype = C.c_int
 lib.vpt_get_kernel_times.argtypes = [_vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]; lib.vpt_get_kernel_times.restype = C.c_int

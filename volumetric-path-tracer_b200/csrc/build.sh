@@ -9,6 +9,8 @@ NVCC="${NVCC:-nvcc}"
 # kernels: the reference's numeric flags (--use_fast_math) so per-seed parity is reachable
 $NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC ${VPT_KERNEL_DEFS:-} -c "$HERE/device/vpt_kernels.cu" -o "$HERE/_obj/vpt_kernels.o"
 $NVCC $ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_bricks.cu" -o "$HERE/_obj/vpt_bricks.o"
+# denoiser: the same flags as vpt_kernels.cu, so its display words come out of the very same tonemap code as k_resolve's
+$NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_denoise.cu" -o "$HERE/_obj/vpt_denoise.o"
 $NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_bruneton.cu" -o "$HERE/_obj/vpt_bruneton.o"
 # octree build: plain IEEE flags, as the reference's bvh object
 $NVCC $ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-ffp-contract=off -c "$HERE/device/vpt_octree.cu" -o "$HERE/_obj/vpt_octree.o"

@@ -7,6 +7,7 @@
 #include "vpt_walk.cuh"
 #include "vpt_atmosphere.cuh"
 #include "vpt_kernels.h"
+#include "vpt_tonemap.cuh"
 
 namespace vpt {
 
@@ -120,16 +121,6 @@ VPT_DEV float van_der_corput(Rng& rng) {
         n *= invBase;
     }
     return rand_int;
-}
-
-VPT_DEV float3 aces_fit(float3 v) {                           // reference rtt_and_odt_fit, :2208-2213
-    float3 a = v * (v + f3(0.0245786f)) - f3(0.000090537f);
-    float3 b = v * (0.983729f * v + f3(0.4329510f)) + f3(0.238081f);
-    return a / b;
-}
-
-VPT_DEV float3 mat3_mul(const float m[9], float3 v) {
-    return f3(m[0] * v.x + m[1] * v.y + m[2] * v.z, m[3] * v.x + m[4] * v.y + m[5] * v.z, m[6] * v.x + m[7] * v.y + m[8] * v.z);
 }
 
 #include "vpt_texfilter.cuh"

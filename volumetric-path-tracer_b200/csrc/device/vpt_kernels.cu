@@ -365,17 +365,10 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     }
 
     if (write_display) {
-        const float aces_in[9]  = { 0.59719f, 0.35458f, 0.04823f, 0.07600f, 0.90834f, 0.01566f, 0.02840f, 0.13383f, 0.83777f };
-        const float aces_out[9] = { 1.60475f, -0.53108f, -0.07367f, -0.10208f, 1.10813f, -0.00605f, -0.00327f, -0.07276f, 1.07602f };
-        float3 val = mat3_mul(aces_in, accum);
-        val = aces_fit(val);
-        val = mat3_mul(aces_out, val) * kp.exposure_scale;
-        const unsigned int r = (unsigned int)(255.0f * fminf(powf(fmaxf(val.x, 0.0f), (float)(1.0 / 2.2)), 1.0f));
-        const unsigned int gg = (unsigned int)(255.0f * fminf(powf(fmaxf(val.y, 0.0f), (float)(1.0 / 2.2)), 1.0f));
-        const unsigned int b = (unsigned int)(255.0f * fminf(powf(fmaxf(val.z, 0.0f), (float)(1.0 / 2.2)), 1.0f));
-        const unsigned int word = 0xff000000 | (r << 16) | (gg << 8) | b;
+        const Tonemapped tm = tonemap_display(accum, kp.exposure_scale);
+        const unsigned int word = tm.word;
         reinterpret_cast<unsigned int*>(kp.display_buffer)[lp] = word;
-        reinterpret_cast<float4*>(kp.raw_buffer)[lp] = make_float4(val.x, val.y, val.z, tr);
+        reinterpret_cast<float4*>(kp.raw_buffer)[lp] = make_float4(tm.val.x, tm.val.y, tm.val.z, tr);
         if (peers.n > 0 && peers.display[0]) {
             const size_t gp = (size_t)y * g.width + (lp - (uint32_t)lr * (uint32_t)g.width);
             #pragma unroll

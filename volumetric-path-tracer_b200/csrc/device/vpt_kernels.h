@@ -127,4 +127,19 @@ cudaError_t launch_adapt_tally(const unsigned* slots, int n, const unsigned long
 // end of the frame: accum, display, pass count and err of every local pixel into every rank's planes; padding rows get count 0 / err 0
 cudaError_t launch_adapt_publish(const FrameGeom& g, const vpt_kernel_params& kp, const AdaptArgs& ad, const AdaptPeers& pp, cudaStream_t s);
 
+// Denoiser (vpt_denoise, csrc/device/vpt_denoise.cu): k_denoise_prep fills plane pair 0, then one k_denoise_atrous per level ping-pongs
+// the pairs; the last level reads the planes only and writes out_f3 / out_display, so out_f3 may be the colour input itself.
+struct DenoiseArgs {
+    int          width, height, iterations;
+    float        sigma_l, sigma_z, exposure_scale;
+    const float* color;                  // [H][W] float3
+    const float* depth;                  // [H][W], null: no depth term
+    const float* rel_error;              // [H][W], null: spatial variance estimate
+    float*       out_f3;                 // [H][W] float3
+    unsigned*    out_display;            // [H][W], may be null
+    float4*      cv[2];                  // scratch planes {r, g, b, v}, width * height each
+    float2*      yz[2];                  // scratch planes {Y, z}
+};
+cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t s);
+
 } // namespace vpt

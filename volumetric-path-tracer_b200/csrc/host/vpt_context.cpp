@@ -80,6 +80,7 @@ static void free_context(vpt_context* c) {
     cudaFree(c->d_queue_id); cudaFree(c->d_queue_org); cudaFree(c->d_bn_table);
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
     cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
+    cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz);
     delete c;
 }
 
@@ -579,6 +580,57 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }
     if (passes_run) *passes_run = done;
+    return VPT_OK;
+}
+
+void vpt_denoise_options_defaults(vpt_denoise_options* opt) {
+    if (!opt) return;
+    opt->iterations = 5; opt->sigma_luminance = 4.0f; opt->sigma_depth = 0.2f;
+}
+
+static bool byte_ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    if (!a || !b) return false;
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + nb && y < x + na;
+}
+
+// Denoiser: prep + one a-trous launch per level on `stream` (csrc/device/vpt_denoise.cu), no synchronisation.  The scratch planes are the
+// context's; the last level reads only them, which is what makes d_out_f3 == d_color_f3 safe.
+int vpt_denoise(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_depth, const float* d_rel_error,
+                const vpt_denoise_options* opt, float exposure_scale, float* d_out, unsigned* d_out_display, void* stream) {
+    if (!c || !d_color || !d_out) return fail(c, VPT_ERR_INVALID, "vpt_denoise: null context, colour or output");
+    if (width == 0 || height == 0) return fail(c, VPT_ERR_INVALID, "vpt_denoise: width and height must be >= 1");
+    if (width > 65535 || height > 65535) return fail(c, VPT_ERR_INVALID, "vpt_denoise: width and height must be <= 65535");
+    vpt_denoise_options o;
+    vpt_denoise_options_defaults(&o);
+    if (opt) o = *opt;
+    if (o.iterations < 1 || o.iterations > 10) return fail(c, VPT_ERR_INVALID, "vpt_denoise: iterations must be 1..10");
+    if (!(std::isfinite(o.sigma_luminance) && o.sigma_luminance > 0.0f))
+        return fail(c, VPT_ERR_INVALID, "vpt_denoise: sigma_luminance must be finite and > 0");
+    if (!(std::isfinite(o.sigma_depth) && o.sigma_depth > 0.0f)) return fail(c, VPT_ERR_INVALID, "vpt_denoise: sigma_depth must be finite and > 0");
+    const size_t px = (size_t)width * height;
+    const size_t b3 = 3 * sizeof(float) * px, b1 = sizeof(float) * px;
+    if (d_out != d_color && byte_ranges_overlap(d_out, b3, d_color, b3))
+        return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_f3 partially overlaps d_color_f3 (it may only be the very same buffer)");
+    if (byte_ranges_overlap(d_out, b3, d_depth, b1) || byte_ranges_overlap(d_out, b3, d_rel_error, b1))
+        return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_f3 overlaps d_depth or d_rel_error");
+    if (byte_ranges_overlap(d_out_display, b1, d_color, b3) || byte_ranges_overlap(d_out_display, b1, d_depth, b1) ||
+        byte_ranges_overlap(d_out_display, b1, d_rel_error, b1))
+        return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_display overlaps an input");
+    if (byte_ranges_overlap(d_out_display, b1, d_out, b3)) return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_display overlaps d_out_f3");
+    if (px > c->cap_dn_px) {
+        cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz); c->d_dn_cv = nullptr; c->d_dn_yz = nullptr; c->cap_dn_px = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_dn_cv, 2 * px * sizeof(float4)));
+        VPT_CUDA(c, cudaMalloc(&c->d_dn_yz, 2 * px * sizeof(float2)));
+        c->cap_dn_px = px;
+    }
+    vpt::DenoiseArgs a;
+    a.width = (int)width; a.height = (int)height; a.iterations = (int)o.iterations;
+    a.sigma_l = o.sigma_luminance; a.sigma_z = o.sigma_depth; a.exposure_scale = exposure_scale;
+    a.color = d_color; a.depth = d_depth; a.rel_error = d_rel_error; a.out_f3 = d_out; a.out_display = d_out_display;
+    a.cv[0] = c->d_dn_cv; a.cv[1] = c->d_dn_cv + px; a.yz[0] = c->d_dn_yz; a.yz[1] = c->d_dn_yz + px;
+    VPT_CUDA(c, vpt::launch_denoise(a, (cudaStream_t)stream));
+    c->launches += 1 + o.iterations;
     return VPT_OK;
 }
 

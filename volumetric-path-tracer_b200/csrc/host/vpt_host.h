@@ -73,6 +73,10 @@ struct vpt_context {
     unsigned* d_adapt_tiles = nullptr;                          // two active-tile lists + the count of the next one
     size_t    cap_adapt_px = 0, cap_adapt_tiles = 0;
     vpt_devptr_t adaptive_accum = 0;                            // accum_buffer of the last adaptive frame: vpt_render_passes may not continue it
+    // denoiser (vpt_denoise), allocated on first use: two ping-pong plane pairs {r, g, b, v} and {Y, z}
+    float4*   d_dn_cv = nullptr;                                // 2 * cap_dn_px
+    float2*   d_dn_yz = nullptr;                                // 2 * cap_dn_px
+    size_t    cap_dn_px = 0;
 };
 
 

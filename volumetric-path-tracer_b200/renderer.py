@@ -108,6 +108,36 @@ class Renderer:
         counts = counts.view(rows, self.width)
         return (int(run.value), counts, err.view(rows, self.width)) if error_map else (int(run.value), counts)
 
+    def denoise(self, color=None, depth=True, rel_error=None, out=None, display=False, iterations=5, sigma_luminance=4.0,
+                sigma_depth=0.2, stream=None):
+        """Edge-avoiding a-trous filter of a full frame (vpt_denoise), enqueued on `stream`.  Returns the (H, W, 3) float32 result, or
+        (result, display words (H, W) int32) with display=True, packed with kp.exposure_scale as k_resolve packs them.
+        color: (H, W, 3) float32 HDR frame; None = this renderer's accumulator.  depth: True = this renderer's depth buffer, None / False =
+        no depth term, or an (H, W) float32 tensor.  rel_error: the (H, W) error map of render_adaptive(..., error_map=True); None = the
+        spatial noise estimate.  out: None = a new tensor, or any (H, W, 3) float32 tensor -- `color` itself denoises in place.
+        On a partitioned renderer `color` must be given (a full frame, e.g. DistributedRenderer.full_accum()) and depth=True means none."""
+        H, W = self.height, self.width
+        if color is None:
+            if self.n_ranks > 1:
+                raise N.VptError("Renderer.denoise: a partitioned renderer holds no full frame; pass `color` (e.g. DistributedRenderer.full_accum())")
+            color = self.buffers.accum
+        if depth is True:
+            depth = self.buffers.depth if self.n_ranks == 1 else None
+        elif depth is False:
+            depth = None
+        dev = color.device
+        color = _frame_tensor(color, H * W * 3, "color", dev)
+        depth = _frame_tensor(depth, H * W, "depth", dev)
+        rel_error = _frame_tensor(rel_error, H * W, "rel_error", dev)
+        out = torch.empty(H, W, 3, dtype=torch.float32, device=dev) if out is None else _frame_tensor(out, H * W * 3, "out", dev)
+        words = torch.empty(H, W, dtype=torch.int32, device=dev) if display else None
+        opt = N.denoise_options(int(iterations), float(sigma_luminance), float(sigma_depth))
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        check(lib.vpt_denoise(self.ctx, W, H, ptr(color), ptr(depth), ptr(rel_error), C.byref(opt), float(self.kp.exposure_scale),
+                              ptr(out), ptr(words), C.c_void_p(stream or 0)), self.ctx, "vpt_denoise")
+        out = out.view(H, W, 3)
+        return (out, words) if display else out
+
     def reset(self):
         self.kp.iteration = 0
         self.buffers.zero_()
@@ -163,6 +193,16 @@ class Renderer:
     def close(self):
         if self.ctx:
             lib.vpt_destroy(self.ctx); self.ctx = C.c_void_p(0)
+
+
+def _frame_tensor(t, numel, name, device):
+    """A full-frame float32 operand of vpt_denoise: contiguous, on `device`, `numel` elements (None passes through)."""
+    if t is None:
+        return None
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.device != device or t.numel() != numel:
+        raise N.VptError(f"Renderer.denoise: `{name}` must be a contiguous float32 tensor of {numel} elements on {device} "
+                         f"(got {t.dtype}, {tuple(t.shape)}, contiguous={t.is_contiguous()}, {t.device})")
+    return t
 
 
 class _DeviceView:
