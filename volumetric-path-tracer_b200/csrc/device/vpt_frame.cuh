@@ -123,6 +123,21 @@ VPT_DEV float van_der_corput(Rng& rng) {
     return rand_int;
 }
 
+// Radiance of a finished sample under the HDRI environment (reference :1838-1850): L + env(dir) * sky_color * beta / (4 pi).  A lean
+// k_trace finishes its rays with it, k_resolve<0> its misses (L = 0, beta = 1) and the hits of wide records.  nvcc contracts this
+// expression per call site, so the order is pinned to the one the end-of-path site compiles to: u = fma(atan2, 1/(2 pi), 0.5),
+// v = acos * 1/pi, L + ((env * sky) * beta) / (4 pi) as one fma.  Every caller then gives the same bits.
+VPT_DEV float3 hdri_radiance(const cudaTextureObject_t env, const float3 sky_color, const float3 dir, const float3 L, const float3 beta)
+{
+    const float4 e = tex2D<float4>(env,
+        pfma(atan2f(dir.z, dir.x), (float)(0.5 / 3.14159265358979323846), 0.5f),
+        pmul(acosf(fmaxf(fminf(dir.y, 1.0f), -1.0f)), (float)(1.0 / 3.14159265358979323846)));
+    const float c = 1.0f / (4.0f * VPT_PI_F);                   // isotropic() returns the folded constant
+    return f3(pfma(pmul(pmul(e.x, sky_color.x), beta.x), c, L.x),
+              pfma(pmul(pmul(e.y, sky_color.y), beta.y), c, L.y),
+              pfma(pmul(pmul(e.z, sky_color.z), beta.z), c, L.z));
+}
+
 #include "vpt_texfilter.cuh"
 #include "vpt_trace.cuh"
 #ifndef VPT_LEVEL_A_MODULE          // the level (A) cubin exports exactly one entry: no wavefront kernels in it

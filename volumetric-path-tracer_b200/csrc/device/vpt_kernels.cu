@@ -8,8 +8,8 @@
 //                     record, the rest are pushed into a warp-compacted ray queue (one atomic per warp)
 //   k_trace<I, L>   : persistent; every lane owns three rays parked in shared memory (vpt_trace.cuh); I = integrator
 //                     (0 direct, 1 volumetric path: vpt_trace_vol.cuh), L = lean instantiation for the common scene
-//   k_resolve<S>    : per pixel, passes in order: environment term (S = 0 HDRI, 1 / 2 precomputed sky: vpt_atmosphere.cuh),
-//                     NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference kernel)
+//   k_resolve<S>    : per pixel, passes in order: environment term (S = 0 HDRI: with compact records for misses only; 1 / 2 precomputed
+//                     sky: vpt_atmosphere.cuh), NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference kernel)
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
 //   k_generate_adaptive, k_resolve_adaptive<S>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
@@ -288,7 +288,10 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     // adaptive: Welford state {n, mean, M2} of the luminance of every sample of this pixel
     float wn = 0.f, wmean = 0.f, wm2 = 0.f;
     if constexpr (kAdaptive) { if (have_prev) { const float4 st = ad->stat[lp]; wn = st.x; wmean = st.y; wm2 = st.z; } }
-    // one pass of the running mean; A (and B, C for a hit sample) are the pass's plane records, loaded by the caller
+    // compact records (HDRI frames traced by a lean kernel, planeB null): one float4 per sample
+    const bool compact = kSky == 0 && !fa.planeB;
+    // one pass of the running mean; A (and B, C for a hit sample) are the pass's plane records, loaded by the caller.  Compact records:
+    // B.x carries tr of a hit sample of the chunk's last pass when the display / raw words are written, C is unused.
     auto one_pass = [&](const int p, const float4 A, const float4 B, const float4 C) {
         const uint32_t iteration = kp.iteration + (uint32_t)p;
         float3 value = f3(1.0f);                                // WHITE when nothing is sampled (:2248)
@@ -298,22 +301,24 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             const size_t s = (size_t)p * g.n_local + lp;
             const float3 ray_dir = f3(A.x, A.y, A.z);
             float3 beta = f3(1.0f), L = f3(0.0f);
-            if (__float_as_uint(A.w) != kMissSentinel) {          // hit sample: the trace kernel wrote all three planes
+            const bool hit = __float_as_uint(A.w) != kMissSentinel;
+            if (compact) {
+                // the trace kernel finished a hit sample; a miss sees the environment along its direction
+                if (hit) { L = f3(A.x, A.y, A.z); depth = A.w; tr = B.x; }
+                else L = hdri_radiance((cudaTextureObject_t)kp.env_tex, ld3(kp.sky_color), ray_dir, L, beta);
+            } else if (hit) {                                    // hit sample: the trace kernel wrote planes A, B, C (and D)
                 beta = f3(C.x, C.y, C.z); L = f3(B.x, B.y, B.z);
                 depth = B.w; tr = A.w;
             }
-            if constexpr (kSky == 1) {
+            if constexpr (kSky == 0) {
+                if (!compact) L = hdri_radiance((cudaTextureObject_t)kp.env_tex, ld3(kp.sky_color), ray_dir, L, beta);
+            } else if constexpr (kSky == 1) {
                 // precomputed sky seen from env_pos along the final direction (:1838-1841)
                 const float4 D = fa.planeD[s];
                 L += sample_atmosphere(atmo, kp.azimuth, kp.elevation, f3(D.x, D.y, D.z), ray_dir) * beta * kp.sky_mult * ld3(kp.sky_color);
             } else if constexpr (kSky == 2) {
                 const float4 D = fa.planeD[s];                       // env_pos or the last path position (:1750-1752)
                 L += beta * sample_atmosphere(atmo, kp.azimuth, kp.elevation, f3(D.x, D.y, D.z), ray_dir);
-            } else {
-                const float4 texval = tex2D<float4>((cudaTextureObject_t)kp.env_tex,
-                    atan2f(ray_dir.z, ray_dir.x) * (float)(0.5 / 3.14159265358979323846) + 0.5f,
-                    acosf(fmaxf(fminf(ray_dir.y, 1.0f), -1.0f)) * (float)(1.0 / 3.14159265358979323846));
-                L += f3(texval.x, texval.y, texval.z) * ld3(kp.sky_color) * beta * (1.0f / (4.0f * VPT_PI_F));   // isotropic() returns the folded constant
             }
             tr = fminf(tr, 1.0f);
             value = L;
@@ -351,7 +356,10 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             if (sampled) {
                 const size_t s = (size_t)p * g.n_local + lp;
                 A = fa.planeA[s];
-                if (__float_as_uint(A.w) != kMissSentinel) { B = fa.planeB[s]; C = fa.planeC[s]; }
+                if (__float_as_uint(A.w) != kMissSentinel) {
+                    if (compact) { if (write_display && p == n_passes - 1) B.x = fa.plane_tr[lp]; }
+                    else { B = fa.planeB[s]; C = fa.planeC[s]; }
+                }
             }
             one_pass(p, A, B, C);
         }

@@ -36,20 +36,23 @@ struct FrameArgs {
     float4*   queue_aux;           // thin lens: per-ray origin; pre-stepped ray (pinhole only): position where stepping starts
     int       thin_lens;           // cam.lens_radius != 0
     const float2* bn_table;        // [pass][65536] blue-noise jitter of the chunk
-    int       n_passes;            // passes in this chunk (k_generate loops over them)
+    int       n_passes;            // passes in this chunk (k_generate loops over them; k_trace keeps tr of the last one)
     int       passes_per_block;    // k_generate: passes handled by one block (blockIdx.z selects the run)
     int       debug_flags;         // development switches (0 in production)
     int       sched_min_lanes;     // trace scheduler: lanes an operation must gather before it pre-empts stepping
     unsigned* queue_count;
     unsigned* queue_head;
-    // sample planes, [pass][local pixel]
-    float4 *planeA, *planeB, *planeC, *planeD;   // planeD (env_pos) only for environment_type == 0, else null
+    // sample planes, [pass][local pixel].  Wide records (the frame ends on the precomputed sky: k_resolve<1/2>): A = final direction + tr,
+    // B = L + depth, C = beta, D = env_pos.  Compact records (HDRI frames traced by a lean kernel; planeB/C/D null): A = the finished radiance
+    // + depth, and plane_tr (below) holds tr of the hit samples of the chunk's last pass.  A miss is always A = direction + kMissSentinel.
+    float4 *planeA, *planeB, *planeC, *planeD;
     // optional statistics: [0] volume lookups, [1] lane-steps, [2] warp step iterations, [3] lane transitions, [4] warp transition rounds
     unsigned long long* counters;
     // cell table of volume 0 (vpt_cells_create; null = texture path): per texel cell its eight corner values, 32 bytes = ONE sector per look-up
     const float4* cell_table;
     int       cell_nx, cell_ny, cell_nz;
     int       tiles_per_block;     // k_generate: consecutive 32x4 tiles handled by one block (blockIdx.x selects the run)
+    float*    plane_tr;            // compact records: [local pixel] tr of the hit samples of pass n_passes - 1 (k_resolve writes it to raw.w)
 };
 
 // Adaptive sampling (vpt_render_adaptive): pixels are grouped in the 32x4 tiles k_generate works on; a chunk only visits the tiles that

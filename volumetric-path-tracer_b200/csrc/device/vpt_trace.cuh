@@ -437,12 +437,21 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
 
 #include "vpt_trace_vol.cuh"
 
-template <int kInteg>
+// kLean: the instantiation may write compact records (the host allocates them for the lean kernels only, see frame_setup)
+template <int kInteg, bool kLean>
 VPT_DEV void write_sample(const PathState& st, const FrameArgs& fa)
 {
     uint32_t lp = st.lp;
     if (fa.geom.n_ranks > 1) lp = ray_local_pixel(fa.geom, st.lp);
     const size_t o = (size_t)st.pass * fa.geom.n_local + lp;
+    if (kLean && !fa.planeB) {
+        // compact record (HDRI environment): the finished radiance, so k_resolve<0> reads one float4 per sample; tr only reaches raw.w
+        // from the chunk's last pass.  A depth is never the sentinel: arithmetic NaNs are 0x7fffffff.
+        const float3 v = hdri_radiance((cudaTextureObject_t)fa.kp.env_tex, ld3(fa.kp.sky_color), st.dir, st.L, st.beta);
+        fa.planeA[o] = make_float4(v.x, v.y, v.z, st.depth);
+        if (st.pass == (uint32_t)fa.n_passes - 1u) fa.plane_tr[lp] = st.alpha;
+        return;
+    }
     fa.planeA[o] = make_float4(st.dir.x, st.dir.y, st.dir.z, st.alpha);                 // final direction, tr
     fa.planeB[o] = make_float4(st.L.x, st.L.y, st.L.z, st.depth);                       // L, depth
     fa.planeC[o] = make_float4(st.beta.x, st.beta.y, st.beta.z, 1.f);                   // beta
@@ -555,7 +564,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
                     else advance<kLean>(st, fs, fa, tc, sph);
                 }
                 if (st.op == OP_TRBEGIN) begin_ratio_walk(st, fs, tc, sph);
-                if (st.op == OP_FINISH) { write_sample<kInteg>(st, fa); st.op = OP_IDLE; }
+                if (st.op == OP_FINISH) { write_sample<kInteg, kLean>(st, fa); st.op = OP_IDLE; }
                 else store_ray(pv, j, st);
                 if (j == 0) tag0 = st.op; else if (j == 1) tag1 = st.op; else tag2 = st.op;
                 lane_ops++;

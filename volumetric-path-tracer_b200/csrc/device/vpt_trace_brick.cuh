@@ -249,7 +249,7 @@ k_trace_brick(const FrameArgs fa, const BrickArgs ba)
                 }
                 if (st.op == OP_GLUE) advance<true>(st, fs, fa, tc, sph);
                 if (st.op == OP_TRBEGIN) begin_ratio_walk(st, fs, tc, sph);
-                if (st.op == OP_FINISH) { write_sample<0>(st, fa); st.op = OP_IDLE; }
+                if (st.op == OP_FINISH) { write_sample<0, true>(st, fa); st.op = OP_IDLE; }
                 lane_ops++;
             }
             warp_ops++;

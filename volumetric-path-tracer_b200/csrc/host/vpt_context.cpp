@@ -79,6 +79,7 @@ static void free_context(vpt_context* c) {
     for (auto& e : c->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     cudaFree(c->d_queue_id); cudaFree(c->d_queue_org); cudaFree(c->d_bn_table);
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
+    cudaFree(c->d_plane_tr);
     cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
     cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz);
     delete c;
@@ -165,23 +166,29 @@ int vpt_get_stats(vpt_context* c, unsigned long long* launches, unsigned* last_q
     return VPT_OK;
 }
 
-static int ensure_frame_buffers(vpt_context* c, size_t n_samples, bool need_planeD) {
-    if (n_samples > c->cap_samples) {
+// Scratch of one round: the ray queue and plane A per sample, then either planes B, C (and D) per sample (wide records) or the tr plane
+// per pixel (compact records).  A change of record layout reallocates, so the scratch never holds another layout's planes.
+static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixels, bool wide, bool planeD) {
+    if (n_samples > c->cap_samples || wide != c->cap_wide || planeD != c->cap_planeD) {
         cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
         cudaFree(c->d_queue_id); cudaFree(c->d_queue_org);
         c->d_queue = c->d_planeA = c->d_planeB = c->d_planeC = c->d_planeD = c->d_queue_org = nullptr; c->d_queue_id = nullptr;
-        c->cap_samples = 0; c->cap_planeD = false;
+        c->cap_samples = 0;
         VPT_CUDA(c, cudaMalloc(&c->d_queue, n_samples * sizeof(float4)));
         VPT_CUDA(c, cudaMalloc(&c->d_queue_id, n_samples * sizeof(uint2)));
         VPT_CUDA(c, cudaMalloc(&c->d_queue_org, n_samples * sizeof(float4)));
         VPT_CUDA(c, cudaMalloc(&c->d_planeA, n_samples * sizeof(float4)));
-        VPT_CUDA(c, cudaMalloc(&c->d_planeB, n_samples * sizeof(float4)));
-        VPT_CUDA(c, cudaMalloc(&c->d_planeC, n_samples * sizeof(float4)));
-        c->cap_samples = n_samples;
+        if (wide) {
+            VPT_CUDA(c, cudaMalloc(&c->d_planeB, n_samples * sizeof(float4)));
+            VPT_CUDA(c, cudaMalloc(&c->d_planeC, n_samples * sizeof(float4)));
+        }
+        if (planeD) VPT_CUDA(c, cudaMalloc(&c->d_planeD, n_samples * sizeof(float4)));
+        c->cap_samples = n_samples; c->cap_wide = wide; c->cap_planeD = planeD;
     }
-    if (need_planeD && !c->cap_planeD) {
-        VPT_CUDA(c, cudaMalloc(&c->d_planeD, c->cap_samples * sizeof(float4)));
-        c->cap_planeD = true;
+    if (!wide && n_pixels > c->cap_tr) {
+        cudaFree(c->d_plane_tr); c->d_plane_tr = nullptr; c->cap_tr = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_plane_tr, n_pixels * sizeof(float)));
+        c->cap_tr = n_pixels;
     }
     return VPT_OK;
 }
@@ -317,18 +324,22 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
 
     // passes fused per generate/trace/resolve round: 32 by default; a small local frame (multi-GPU shard, low resolution)
     // takes up to 64 so the fixed per-round cost and the persistent kernel's tail are paid half as often; always capped so
-    // the per-round scratch (ray queue + sample planes, 88 B or 104 B per sample) stays under max_scratch_bytes
+    // the per-round scratch (ray queue + sample planes: 56 B per sample with compact records, 88 B or 104 B with wide ones) stays under
+    // max_scratch_bytes.  Compact records: an HDRI frame traced by a lean kernel, which then finishes each ray's environment term
+    // itself.  A frame that ends on the precomputed sky needs wide records and env_pos (plane D: k_resolve<1/2> evaluate the sky from
+    // them), and so does the generic kernel (the texture look-up in its service round cost it more than k_resolve<0> saved).
     const bool planeD = sky_env;
+    const bool wide = sky_env || !lean;
     int chunk = c->passes_per_chunk;
     if (c->chunk_auto) chunk = (size_t)fa.geom.n_local <= ((size_t)1 << 20) ? 64 : 32;
     {
-        const size_t per_sample = 88 + (planeD ? 16 : 0);
+        const size_t per_sample = wide ? 88 + (planeD ? 16 : 0) : 56;
         const size_t fit = c->max_scratch_bytes / (per_sample * (size_t)(fa.geom.n_local > 0 ? fa.geom.n_local : 1));
         if ((size_t)chunk > fit) chunk = fit < 1 ? 1 : (int)fit;
     }
     if (n_sampled) {
         const size_t per_chunk = (size_t)fa.geom.n_local * (size_t)(n_sampled < (unsigned)chunk ? n_sampled : (unsigned)chunk);
-        int rc = ensure_frame_buffers(c, per_chunk, planeD);
+        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD);
         if (rc != VPT_OK) return rc;
     }
     if (c->cap_chunk < chunk) {
@@ -339,7 +350,9 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     fa.queue_dir = c->d_queue; fa.queue_id = c->d_queue_id; fa.queue_aux = c->d_queue_org; fa.thin_lens = (fa.cam.lens_radius != 0.0f) ? 1 : 0;
     fa.bn_table = c->d_bn_table; fa.debug_flags = c->debug_flags;     // fa.sched_min_lanes: set below, once the trace kernel is chosen
     fa.queue_count = c->d_counters; fa.queue_head = c->d_counters + 1;
-    fa.planeA = c->d_planeA; fa.planeB = c->d_planeB; fa.planeC = c->d_planeC; fa.planeD = planeD ? c->d_planeD : nullptr;
+    fa.planeA = c->d_planeA;
+    fa.planeB = wide ? c->d_planeB : nullptr; fa.planeC = wide ? c->d_planeC : nullptr; fa.planeD = planeD ? c->d_planeD : nullptr;
+    fa.plane_tr = wide ? nullptr : c->d_plane_tr;
 
     // rays per lane: 3 by default; 2 (one more CTA per SM) when a look-up is a chain of cache misses -- a density grid that cannot live
     // in L2 (every look-up a DRAM round trip) or long per-leaf instance lists (dependent loads): warps in flight then matter more than
@@ -367,10 +380,12 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     return VPT_OK;
 }
 
-// k_trace (or k_trace_brick in brick mode) over whatever k_generate queued
-static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, cudaStream_t stream) {
-    if (c->brick_pool) return vpt::launch_trace_brick(plan.fa, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
-    return vpt::launch_trace(plan.fa, plan.vol_integ ? &plan.atmo : nullptr, plan.lean, plan.slots, plan.trace_ctas, stream);
+// k_trace (or k_trace_brick in brick mode) over whatever k_generate queued for a chunk of np passes
+static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, unsigned np, cudaStream_t stream) {
+    vpt::FrameArgs fa = plan.fa;
+    fa.n_passes = (int)np;
+    if (c->brick_pool) return vpt::launch_trace_brick(fa, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
+    return vpt::launch_trace(fa, plan.vol_integ ? &plan.atmo : nullptr, plan.lean, plan.slots, plan.trace_ctas, stream);
 }
 
 extern "C" {
@@ -408,7 +423,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         fa.kp.iteration = it0 + done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
         VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate(fa, (int)np, stream); }));
-        VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, stream); }));
+        VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
@@ -537,7 +552,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         c->launches++;
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
-            VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, stream); }));
+            VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, stream); }));
             c->launches += 3;
         }

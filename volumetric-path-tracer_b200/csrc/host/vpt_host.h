@@ -38,7 +38,10 @@ struct vpt_context {
     vpt::VolumeRec* d_vrec = nullptr;
     // frame buffers
     size_t cap_samples = 0;           // n_local * chunk
+    bool   cap_wide = false;          // planes B, C allocated (wide sample records) rather than the tr plane
     bool   cap_planeD = false;
+    size_t cap_tr = 0;                // pixels of d_plane_tr
+    float* d_plane_tr = nullptr;
     uint2* d_queue_id = nullptr; float4* d_queue_org = nullptr; float2* d_bn_table = nullptr; int cap_chunk = 0;
     int sched_min_lanes = 0;          // option "sched_min_lanes": 0 = by kernel (26 for the lean kernel at 3 rays per lane, else 20)
     int debug_flags = 0;
