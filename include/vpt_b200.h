@@ -164,6 +164,33 @@ void vpt_adaptive_options_defaults(vpt_adaptive_options* opt);
 int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsigned max_passes, const vpt_adaptive_options* opt,
                          unsigned* d_pass_count, float* d_rel_error, unsigned* passes_run, void* stream);
 
+/* ---- compositing AOVs: how much of each pixel is volume, and the volume's colour without the background ----------------------
+ * accum_buffer holds the volume over the environment.  With AOV buffers set, every render call also keeps, per pixel, two running
+ * means next to it, so the frame can be composited over another plate and the environment swapped or graded downstream.
+ *
+ *   Definition.  For each pass a pixel takes, let c = (depth > 0), where depth is the pass's depth sample (the one depth_buffer
+ *     averages) and a NaN depth counts as false: c is the reference's own decision that the camera ray's first walk collided in the
+ *     medium, or that the ray hit the sphere before the volume box.
+ *       alpha   sample: c ? 1 : 0.
+ *       volume  sample (float3): the sample exactly as it enters accum (after the NaN / Inf guard and the viz_dof tint) if c, +0 otherwise
+ *               (a select, not a product).  When the guard replaced the sample, the volume sample is the volume AOV's own mean so far,
+ *               as the guard uses accum's.
+ *     Both follow accum's rule and arithmetic: iteration == 0 assigns, iteration < max_interactions updates x + (s - x) / (iteration + 1),
+ *     later passes change nothing.  So per sample, beauty = volume + the transmitted background, and alpha estimates 1 - transmittance
+ *     along the camera ray under the reference's tracker; over a new plate P the frame is  volume + (1 - alpha) * P.
+ *   Sphere.  The sphere seen THROUGH the volume box without a collision counts as background (c is false there): that is the
+ *     reference's depth decision.
+ *   Buffers.  Caller-owned device memory of vpt_local_pixels() entries like the Kernel_params buffers (rank-local order on a partitioned
+ *     context): d_alpha float, d_volume_f3 float3.  Either may be NULL; both NULL turns the AOVs off at once.  Buffers registered here
+ *     become active at the next render call whose Kernel_params.iteration is 0; calls before that leave them untouched, so a viewer loop
+ *     that enables AOVs mid-frame never continues a mean from garbage (vpt_render_adaptive always starts at 0).
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active AOVs.  An adaptive frame's stopped pixels keep theirs, and every
+ *     pixel's AOVs are bit for bit what a fixed-count frame of its own pass count leaves there.  Level (A) (volume_rt_kernel) has none.
+ *     The NCCL and peer-memory exchanges do not carry AOVs: on a partitioned context they stay rank-local.
+ *   Refused at render time (VPT_ERR_INVALID, naming the buffer): an AOV buffer that overlaps accum, depth, cost, raw or display, and
+ *     the two AOV buffers overlapping each other. */
+int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
+
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
  * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.

@@ -10,6 +10,7 @@
 //                     (0 direct, 1 volumetric path: vpt_trace_vol.cuh), L = lean instantiation for the common scene
 //   k_resolve<S>    : per pixel, passes in order: environment term (S = 0 HDRI: with compact records for misses only; 1 / 2 precomputed
 //                     sky: vpt_atmosphere.cuh), NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference kernel)
+//   k_resolve<S, true>, k_resolve_adaptive<S, true> : the same, plus the running means of the compositing AOVs (alpha, volume colour)
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
 //   k_generate_adaptive, k_resolve_adaptive<S>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
@@ -266,11 +267,12 @@ struct PeerFlagPtrs { unsigned long long* p[kMaxPeers]; };
 template <int kSky> using SkyArg = typename std::conditional<kSky != 0, vpt_atmosphere, NoSky>::type;
 
 // One pixel of k_resolve (local pixel lp, local row lr, global row y).  kAdaptive (k_resolve_adaptive): the same running mean, plus the
-// pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.
-template <int kSky, bool kAdaptive>
+// pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.  kAov: also the running means of
+// the compositing AOVs in `aov` (DESIGN.md section 8c).
+template <int kSky, bool kAdaptive, bool kAov>
 __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                               const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
-                                              const AdaptArgs* ad)
+                                              const AdaptArgs* ad, const AovBuffers* aov)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
@@ -288,6 +290,11 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     // adaptive: Welford state {n, mean, M2} of the luminance of every sample of this pixel
     float wn = 0.f, wmean = 0.f, wm2 = 0.f;
     if constexpr (kAdaptive) { if (have_prev) { const float4 st = ad->stat[lp]; wn = st.x; wmean = st.y; wm2 = st.z; } }
+    // AOVs: alpha = mean of [depth > 0], volume = mean of the sample where depth > 0 and +0 elsewhere; read exactly when accum is
+    float alphav = 0.f; float3 volv = f3(0.f);
+    if constexpr (kAov) {
+        if (have_prev || !sampled) { if (aov->alpha) alphav = aov->alpha[lp]; if (aov->volume) volv = aov->volume[lp]; }
+    }
     // compact records (HDRI frames traced by a lean kernel, planeB null): one float4 per sample
     const bool compact = kSky == 0 && !fa.planeB;
     // one pass of the running mean; A (and B, C for a hit sample) are the pass's plane records, loaded by the caller.  Compact records:
@@ -324,6 +331,8 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             value = L;
         }
         // NaN / Inf guard (:2263-2264)
+        bool guarded = false;                                   // AOVs only, apart from the guard: the other instantiations keep their code
+        if constexpr (kAov) guarded = any_nan(value) || any_inf(value);
         if (any_nan(value) || any_inf(value)) value = accum;
         if (isnan(tr) || isinf(tr)) tr = 1.0f;
 
@@ -340,6 +349,18 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             accum = accum + (value - accum) / (float)(iteration + 1);
             costv = costv + (f3(0.f) - costv) / (float)(iteration + 1);
             depthv = depthv + (depth - depthv) / (float)(iteration + 1);
+        }
+        if constexpr (kAov) {
+            // the reference's collision decision of the camera ray (a NaN depth counts as none); selects, so a miss adds an exact +0.
+            // A sample the guard replaced leaves the volume mean where it is, as the guard leaves accum.
+            const bool c = depth > 0.0f;
+            const float as = c ? 1.0f : 0.0f;
+            const float3 vs = guarded ? volv : (c ? value : f3(0.f));
+            if (iteration == 0) { alphav = as; volv = vs; }
+            else if (iteration < kp.max_interactions) {
+                alphav = alphav + (as - alphav) / (float)(iteration + 1);
+                volv = volv + (vs - volv) / (float)(iteration + 1);
+            }
         }
         if constexpr (kAdaptive) {                              // the sample as it entered the mean (after the NaN guard and the tint)
             const float lum = 0.2126f * value.x + 0.7152f * value.y + 0.0722f * value.z;
@@ -365,6 +386,7 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         }
     }
     accum_buf[lp] = accum; cost_buf[lp] = costv; depth_buf[lp] = depthv;
+    if constexpr (kAov) { if (aov->alpha) aov->alpha[lp] = alphav; if (aov->volume) aov->volume[lp] = volv; }
     if constexpr (kAdaptive) {
         const float err = wn >= 2.0f ? sqrtf(wm2 / (wn * (wn - 1.0f))) / fmaxf(wmean, kAdaptMeanFloor) : INFINITY;
         ad->stat[lp] = make_float4(wn, wmean, wm2, err);
@@ -391,17 +413,25 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     }
 }
 
-template <int kSky>
+// kAov: the instantiations that also keep the compositing AOVs take the AovBuffers as one more argument (the pack `aov`, empty
+// otherwise), so the kernels without AOVs keep their parameter block.
+__device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a) { return &a; }
+
+template <int kSky, bool kAov = false, class... Aov>
 __global__ void __launch_bounds__(256)
-k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers)
+k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+          const Aov... aov)
 {
+    static_assert(sizeof...(Aov) == (kAov ? 1 : 0), "k_resolve<kSky, true> takes one AovBuffers, k_resolve<kSky> none");
     const FrameGeom& g = fa.geom;
     const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
     if (lp >= (uint32_t)g.n_local) return;
     const int lr = lp / g.width;
     const int y = global_row(g, lr);
     if (y >= g.height) return;
-    resolve_pixel<kSky, false>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr);
+    const AovBuffers* ap = nullptr;
+    if constexpr (kAov) ap = aov_of(aov...);
+    resolve_pixel<kSky, false, kAov>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap);
 }
 
 // 32x4 pixel tile and the lane's pixel in it, for the per-tile adaptive kernels (a warp covers one row of 32 pixels)
@@ -416,17 +446,20 @@ __device__ __forceinline__ TilePixel tile_pixel(const FrameGeom& g, const int ti
 }
 
 // One block of 128 per active tile: the running mean of the pixels that have not stopped, every pass of the chunk sampled; at the end of the
-// chunk their display / raw words, pass count and relative error (so a pixel keeps those of the last pass it took).
-template <int kSky>
+// chunk their display / raw words, pass count and relative error (so a pixel keeps those of the last pass it took).  kAov: as k_resolve.
+template <int kSky, bool kAov = false, class... Aov>
 __global__ void __launch_bounds__(128)
-k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad)
+k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Aov... aov)
 {
+    static_assert(sizeof...(Aov) == (kAov ? 1 : 0), "k_resolve_adaptive<kSky, true> takes one AovBuffers, k_resolve_adaptive<kSky> none");
     const FrameGeom& g = fa.geom;
     const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
     if (!t.inside) return;
     const uint32_t lp = (uint32_t)t.lr * (uint32_t)g.width + (uint32_t)t.x;
     if (ad.stopped[lp]) return;
-    resolve_pixel<kSky, true>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad);
+    const AovBuffers* ap = nullptr;
+    if constexpr (kAov) ap = aov_of(aov...);
+    resolve_pixel<kSky, true, kAov>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap);
 }
 
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
@@ -712,6 +745,9 @@ cudaError_t exchange_kernels_preload()
         (const void*)k_trace<0, false, 2>, (const void*)k_trace<0, true, 2>, (const void*)k_trace<0, true, 2, true>, (const void*)k_trace_brick,
         (const void*)k_resolve<0>, (const void*)k_resolve<1>, (const void*)k_resolve<2>,
         (const void*)k_resolve_adaptive<0>, (const void*)k_resolve_adaptive<1>, (const void*)k_resolve_adaptive<2>,
+        (const void*)k_resolve<0, true, AovBuffers>, (const void*)k_resolve<1, true, AovBuffers>, (const void*)k_resolve<2, true, AovBuffers>,
+        (const void*)k_resolve_adaptive<0, true, AovBuffers>, (const void*)k_resolve_adaptive<1, true, AovBuffers>,
+        (const void*)k_resolve_adaptive<2, true, AovBuffers>,
         (const void*)k_adapt_init, (const void*)k_adapt, (const void*)k_adapt_halo, (const void*)k_adapt_count_publish, (const void*)k_adapt_tally,
         (const void*)k_adapt_publish, (const void*)k_peer_signal, (const void*)k_peer_wait };
     for (const void* f : fns) {
@@ -757,25 +793,39 @@ cudaError_t launch_trace_brick(const FrameArgs& fa, const float* pool, const int
     return cudaGetLastError();
 }
 
-cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers, cudaStream_t s)
+static bool aov_on(const AovBuffers* aov) { return aov && (aov->alpha || aov->volume); }
+
+cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers,
+                           const AovBuffers* aov, cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
-    if (sky && fa.kp.integrator != 0) k_resolve<2><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
-    else if (sky)                     k_resolve<1><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
-    else                              k_resolve<0><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf);
+    if (aov_on(aov)) {
+        if (sky && fa.kp.integrator != 0) k_resolve<2, true><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf, *aov);
+        else if (sky)                     k_resolve<1, true><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf, *aov);
+        else                              k_resolve<0, true><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf, *aov);
+    }
+    else if (sky && fa.kp.integrator != 0) k_resolve<2><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
+    else if (sky)                          k_resolve<1><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
+    else                                   k_resolve<0><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf);
     return cudaGetLastError();
 }
 
-cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, cudaStream_t s)
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
+                                    cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
-    if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
-    else if (sky)                     k_resolve_adaptive<1><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
-    else                              k_resolve_adaptive<0><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad);
+    if (aov_on(aov)) {
+        if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2, true><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad, *aov);
+        else if (sky)                     k_resolve_adaptive<1, true><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad, *aov);
+        else                              k_resolve_adaptive<0, true><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad, *aov);
+    }
+    else if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
+    else if (sky)                          k_resolve_adaptive<1><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
+    else                                   k_resolve_adaptive<0><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad);
     return cudaGetLastError();
 }
 

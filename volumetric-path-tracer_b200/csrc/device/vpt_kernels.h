@@ -90,7 +90,12 @@ cudaError_t launch_build_cells(const float* d_dense, int dx, int dy, int dz, flo
 // the stripe un-permutation fused into the kernel that produces the values.
 constexpr int kMaxPeers = 8;
 struct PeerFrames { int n = 0; float* accum[kMaxPeers] = {}; unsigned int* display[kMaxPeers] = {}; };
-cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers, cudaStream_t s);
+// Compositing AOVs (vpt_set_aov_buffers): [local pixel] running means of the coverage indicator [depth > 0] and of the sample's volume
+// share, next to accum.  Either may be null.  A kernel argument of the AOV instantiations of k_resolve / k_resolve_adaptive only (not in
+// FrameArgs, so every other kernel keeps its parameter block); aov == null or both pointers null selects the instantiations without them.
+struct AovBuffers { float* alpha = nullptr; float3* volume = nullptr; };
+cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers,
+                           const AovBuffers* aov, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -106,7 +111,8 @@ cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& 
 // adaptive frame: k_generate / k_resolve over the tiles of ad.tiles only (stopped pixels sample nothing and keep their buffers); the resolve
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s);
-cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, cudaStream_t s);
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
+                                    cudaStream_t s);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);

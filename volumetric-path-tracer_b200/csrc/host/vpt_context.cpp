@@ -145,6 +145,13 @@ long long vpt_local_pixels(const vpt_context* c, unsigned width, unsigned height
     return make_geom(c, width, height).n_local;
 }
 
+int vpt_set_aov_buffers(vpt_context* c, float* d_alpha, float* d_volume_f3) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_aov_buffers: null context");
+    c->aov_alpha = d_alpha; c->aov_volume = d_volume_f3;
+    c->aov_active = false;          // both null: off from now on; otherwise the buffers take over at the next call with iteration == 0
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -204,6 +211,7 @@ struct FramePlan {
     bool vol_integ = false, lean = false;
     int trace_ctas = 0, slots = 3, chunk = 1, bn_limit = 0;
     unsigned n_sampled = 0;               // how many of the requested passes sample (the rest only re-tonemap)
+    vpt::AovBuffers aov;                  // the active compositing AOVs (both null: off)
 };
 
 // Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
@@ -219,6 +227,29 @@ cudaError_t timed(vpt_context* c, cudaStream_t stream, int kind, F&& fn) {
     return e;
 }
 } // namespace
+
+static bool byte_ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    if (!a || !b) return false;
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + nb && y < x + na;
+}
+
+// The AOV buffers may not share a byte with a Kernel_params output buffer or with each other (n = local pixels).
+static int check_aov_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    const struct { const char* name; vpt_devptr_t p; size_t bytes; } outs[] = {
+        { "accum_buffer", kp.accum_buffer, 12 * n }, { "depth_buffer", kp.depth_buffer, 4 * n }, { "cost_buffer", kp.cost_buffer, 12 * n },
+        { "raw_buffer", kp.raw_buffer, 16 * n }, { "display_buffer", kp.display_buffer, 4 * n } };
+    for (const auto& o : outs) {
+        const void* p = (const void*)(uintptr_t)o.p;
+        if (byte_ranges_overlap(c->aov_alpha, 4 * n, p, o.bytes))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_aov_buffers: the alpha buffer overlaps Kernel_params.") + o.name);
+        if (byte_ranges_overlap(c->aov_volume, 12 * n, p, o.bytes))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_aov_buffers: the volume buffer overlaps Kernel_params.") + o.name);
+    }
+    if (byte_ranges_overlap(c->aov_alpha, 4 * n, c->aov_volume, 12 * n))
+        return fail(c, VPT_ERR_INVALID, "vpt_set_aov_buffers: the alpha buffer and the volume buffer overlap");
+    return VPT_OK;
+}
 
 // The preamble of a render call of n_passes passes: validation, scene-table refresh, trace-kernel choice, chunk size and scratch buffers.
 static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned n_passes, cudaStream_t stream, FramePlan& plan) {
@@ -377,6 +408,14 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     plan.vol_integ = vol_integ; plan.lean = lean; plan.slots = slots; plan.trace_ctas = c->num_sms * ctas_per_sm;
     plan.chunk = chunk; plan.n_sampled = n_sampled;
     plan.bn_limit = frame_px < 65536ull ? (int)frame_px : 65536;
+
+    // compositing AOVs: registered buffers take over at the first call of a frame (iteration == 0) and are checked on every call
+    if (c->aov_active || (kp.iteration == 0 && (c->aov_alpha || c->aov_volume))) {
+        int rc = check_aov_buffers(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+        c->aov_active = true;
+        plan.aov.alpha = c->aov_alpha; plan.aov.volume = reinterpret_cast<float3*>(c->aov_volume);
+    }
     return VPT_OK;
 }
 
@@ -428,7 +467,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, stream); }));
+        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, &plan.aov, stream); }));
         c->launches += 4;
         done += np;
     }
@@ -438,7 +477,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, vpt::launch_resolve(fa, plan.sky, (int)(n_passes - n_sampled), 0, 1, &peers, stream));
+        VPT_CUDA(c, vpt::launch_resolve(fa, plan.sky, (int)(n_passes - n_sampled), 0, 1, &peers, &plan.aov, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2;
     }
@@ -553,7 +592,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, &plan.aov, stream); }));
             c->launches += 3;
         }
         done += np;
@@ -601,12 +640,6 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
 void vpt_denoise_options_defaults(vpt_denoise_options* opt) {
     if (!opt) return;
     opt->iterations = 5; opt->sigma_luminance = 4.0f; opt->sigma_depth = 0.2f;
-}
-
-static bool byte_ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
-    if (!a || !b) return false;
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + nb && y < x + na;
 }
 
 // Denoiser: prep + one a-trous launch per level on `stream` (csrc/device/vpt_denoise.cu), no synchronisation.  The scratch planes are the

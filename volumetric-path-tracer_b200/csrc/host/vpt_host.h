@@ -80,6 +80,11 @@ struct vpt_context {
     float4*   d_dn_cv = nullptr;                                // 2 * cap_dn_px
     float2*   d_dn_yz = nullptr;                                // 2 * cap_dn_px
     size_t    cap_dn_px = 0;
+    // compositing AOVs (vpt_set_aov_buffers): caller-owned [local pixel] float / float3 buffers, either may be null; registered buffers
+    // become active at the next render call with iteration == 0, so no running mean ever continues from what they held before
+    float*    aov_alpha = nullptr;
+    float*    aov_volume = nullptr;
+    bool      aov_active = false;
 };
 
 

@@ -17,7 +17,8 @@ from .scene import Scene, default_kernel_params
 
 
 class FrameBuffers:
-    """accum/cost (float3), depth (float), raw (float4), display (uint32) for `n_pixels` pixels."""
+    """accum/cost (float3), depth (float), raw (float4), display (uint32) for `n_pixels` pixels; alpha (float) and volume (float3),
+    the compositing AOVs, once Renderer.enable_aovs() has allocated them (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -26,10 +27,13 @@ class FrameBuffers:
         self.depth = torch.zeros(self.n, dtype=torch.float32, device=device)
         self.raw = torch.zeros(self.n, 4, dtype=torch.float32, device=device)
         self.display = torch.zeros(self.n, dtype=torch.int32, device=device)
+        self.alpha = None
+        self.volume = None
 
     def zero_(self):
-        for t in (self.accum, self.cost, self.depth, self.raw, self.display):
-            t.zero_()
+        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume):
+            if t is not None:
+                t.zero_()
 
     def bind(self, kp: N.Kernel_params):
         kp.accum_buffer = self.accum.data_ptr(); kp.cost_buffer = self.cost.data_ptr(); kp.depth_buffer = self.depth.data_ptr()
@@ -137,6 +141,33 @@ class Renderer:
                               ptr(out), ptr(words), C.c_void_p(stream or 0)), self.ctx, "vpt_denoise")
         out = out.view(H, W, 3)
         return (out, words) if display else out
+
+    def enable_aovs(self):
+        """Allocate and register the compositing AOVs (vpt_set_aov_buffers): buffers.alpha (n,) float32, the running mean of the
+        coverage [depth > 0], and buffers.volume (n, 3) float32, the volume's share of accum.  They take over at the next render call with
+        kp.iteration == 0.  Under a constant environment of radiance k, accum = volume + (1 - alpha) * k up to rounding; a new plate P
+        composites as volume + (1 - alpha) * P (DESIGN.md section 8c).  n is the renderer's local pixel count (rank-local rows on a partitioned renderer)."""
+        dev = self.buffers.accum.device
+        self.buffers.alpha = torch.zeros(self.n_local, dtype=torch.float32, device=dev)
+        self.buffers.volume = torch.zeros(self.n_local, 3, dtype=torch.float32, device=dev)
+        check(lib.vpt_set_aov_buffers(self.ctx, C.c_void_p(self.buffers.alpha.data_ptr()), C.c_void_p(self.buffers.volume.data_ptr())),
+              self.ctx, "vpt_set_aov_buffers")
+
+    def disable_aovs(self):
+        """Turn the AOVs off at once; buffers.alpha / buffers.volume keep what they hold."""
+        check(lib.vpt_set_aov_buffers(self.ctx, None, None), self.ctx, "vpt_set_aov_buffers")
+
+    def alpha_image(self):
+        """(H, W) float32 view of buffers.alpha ((local rows, W) on a partitioned renderer)."""
+        if self.buffers.alpha is None:
+            raise N.VptError("Renderer.alpha_image: AOVs are not enabled (Renderer.enable_aovs())")
+        return self.buffers.alpha.view(self.n_local // self.width, self.width)
+
+    def volume_image(self):
+        """(H, W, 3) float32 view of buffers.volume ((local rows, W, 3) on a partitioned renderer)."""
+        if self.buffers.volume is None:
+            raise N.VptError("Renderer.volume_image: AOVs are not enabled (Renderer.enable_aovs())")
+        return self.buffers.volume.view(self.n_local // self.width, self.width, 3)
 
     def reset(self):
         self.kp.iteration = 0
