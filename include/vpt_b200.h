@@ -191,6 +191,32 @@ int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], uns
  *     the two AOV buffers overlapping each other. */
 int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
 
+/* ---- light groups: the beauty split by the light class that added each radiance term ------------------------------------------
+ * With group buffers set, every render call also keeps, per pixel, four running means next to accum -- the radiance the sun, the point
+ * lights, the volume's emission and the environment added -- so a compositor can regrade or swap each class without re-rendering.
+ *
+ *   Definition.  Every radiance term the integrator adds to the path's L, and the environment term at the end of the path, belongs to
+ *     exactly one group.  Direct integrator: sun NEE and the sun-lit sphere bounce -> sun; the point-light estimate -> point; the emission
+ *     walk -> emission; the HDRI / precomputed-sky term -> environment.  Volumetric path integrator: each scatter's light estimate goes to
+ *     the class uniform_sample_one_light chose (sun, point, or environment for both halves of the sky estimate), the emission walk to
+ *     emission, the end-of-path sky to environment.  A miss sample is all environment; a pass that samples nothing (render == 0) gives its
+ *     WHITE to the environment and 0 to the others.  Each group follows accum's rule and arithmetic (iteration == 0 assigns,
+ *     iteration < max_interactions updates x + (s - x) / (iteration + 1)); a sample the NaN / Inf guard replaced leaves every group at its
+ *     own mean.  Groups are taken before the viz_dof tint.  So per sample sun + point + emission + environment = the beauty sample up to
+ *     the rounding of the separate sums, and with the direct integrator each group is bit for bit the accum of a render in which only that
+ *     class is lit (the path's draws do not depend on light intensities there).
+ *   Buffers.  Caller-owned device memory, float3, vpt_local_pixels() entries each (rank-local order on a partitioned context).  Any may be
+ *     NULL; all four NULL turns the groups off at once.  Activation as for the AOVs: registered buffers take over at the next render call
+ *     whose Kernel_params.iteration is 0, calls before that leave them untouched.
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active groups; an adaptive frame's stopped pixels keep theirs.  Every
+ *     other output is bit for bit what the same call gives without groups.  Level (A) has none.  The NCCL and peer-memory exchanges do not
+ *     carry them: on a partitioned context they stay rank-local.
+ *   Cost.  Groups make the lean kernels write wide sample records and the generic kernels keep 48 B more per sample (the chunk shrinks
+ *     under max_scratch_mb accordingly).
+ *   Refused at render time (VPT_ERR_INVALID, naming the buffer): a group buffer that overlaps accum, depth, cost, raw or display, an AOV
+ *     buffer, or another group buffer. */
+int  vpt_set_light_group_buffers(vpt_context* ctx, float* d_sun_f3, float* d_point_f3, float* d_emission_f3, float* d_environment_f3);
+
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
  * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.

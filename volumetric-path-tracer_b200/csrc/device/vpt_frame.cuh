@@ -138,6 +138,21 @@ VPT_DEV float3 hdri_radiance(const cudaTextureObject_t env, const float3 sky_col
               pfma(pmul(pmul(e.z, sky_color.z), beta.z), c, L.z));
 }
 
+// hdri_radiance split after its look-up: the product (env * sky) * beta, which pfma(t, 1 / (4 pi), L) turns into hdri_radiance(.., L, beta)
+// bit for bit.  For callers that need the environment term with two values of L (the light groups: the beauty's L and 0) from one fetch.
+VPT_DEV float3 hdri_product(const cudaTextureObject_t env, const float3 sky_color, const float3 dir, const float3 beta)
+{
+    const float4 e = tex2D<float4>(env,
+        pfma(atan2f(dir.z, dir.x), (float)(0.5 / 3.14159265358979323846), 0.5f),
+        pmul(acosf(fmaxf(fminf(dir.y, 1.0f), -1.0f)), (float)(1.0 / 3.14159265358979323846)));
+    return f3(pmul(pmul(e.x, sky_color.x), beta.x), pmul(pmul(e.y, sky_color.y), beta.y), pmul(pmul(e.z, sky_color.z), beta.z));
+}
+VPT_DEV float3 hdri_finish(const float3 t, const float3 L)
+{
+    const float c = 1.0f / (4.0f * VPT_PI_F);
+    return f3(pfma(t.x, c, L.x), pfma(t.y, c, L.y), pfma(t.z, c, L.z));
+}
+
 #include "vpt_texfilter.cuh"
 #include "vpt_trace.cuh"
 #ifndef VPT_LEVEL_A_MODULE          // the level (A) cubin exports exactly one entry: no wavefront kernels in it

@@ -11,6 +11,8 @@
 //   k_resolve<S>    : per pixel, passes in order: environment term (S = 0 HDRI: with compact records for misses only; 1 / 2 precomputed
 //                     sky: vpt_atmosphere.cuh), NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference kernel)
 //   k_resolve<S, true>, k_resolve_adaptive<S, true> : the same, plus the running means of the compositing AOVs (alpha, volume colour)
+//   k_resolve<S, A, true>, k_resolve_adaptive<S, A, true>, k_trace<I, false, 3, false, true> : light groups -- the generic trace kernels
+//                     also keep each ray's per-class radiance sums, the resolve their running means (sun, point, emission, environment)
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
 //   k_generate_adaptive, k_resolve_adaptive<S>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
@@ -268,11 +270,11 @@ template <int kSky> using SkyArg = typename std::conditional<kSky != 0, vpt_atmo
 
 // One pixel of k_resolve (local pixel lp, local row lr, global row y).  kAdaptive (k_resolve_adaptive): the same running mean, plus the
 // pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.  kAov: also the running means of
-// the compositing AOVs in `aov` (DESIGN.md section 8c).
-template <int kSky, bool kAdaptive, bool kAov>
+// the compositing AOVs in `aov` (DESIGN.md section 8c).  kGroups: also the running means of the light groups in `lg` (section 8d).
+template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false>
 __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                               const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
-                                              const AdaptArgs* ad, const AovBuffers* aov)
+                                              const AdaptArgs* ad, const AovBuffers* aov, const LightGroups* lg = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
@@ -295,6 +297,12 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     if constexpr (kAov) {
         if (have_prev || !sampled) { if (aov->alpha) alphav = aov->alpha[lp]; if (aov->volume) volv = aov->volume[lp]; }
     }
+    // light groups: the running mean of each class, read exactly when accum is (a null output is kept at 0 and never stored)
+    float3 gm[kLightGroups];
+    if constexpr (kGroups) {
+        #pragma unroll
+        for (int k = 0; k < kLightGroups; ++k) gm[k] = ((have_prev || !sampled) && lg->out[k]) ? lg->out[k][lp] : f3(0.f);
+    }
     // compact records (HDRI frames traced by a lean kernel, planeB null): one float4 per sample
     const bool compact = kSky == 0 && !fa.planeB;
     // one pass of the running mean; A (and B, C for a hit sample) are the pass's plane records, loaded by the caller.  Compact records:
@@ -304,6 +312,9 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         float3 value = f3(1.0f);                                // WHITE when nothing is sampled (:2248)
         float depth = .0f;
         tr = .0f;
+        // light-group samples; a pass that samples nothing gives its WHITE to the environment
+        float3 gs[kLightGroups];
+        if constexpr (kGroups) { gs[LG_SUN] = gs[LG_POINT] = gs[LG_EMISSION] = f3(0.f); gs[LG_ENVIRONMENT] = f3(1.0f); }
         if (sampled) {
             const size_t s = (size_t)p * g.n_local + lp;
             const float3 ray_dir = f3(A.x, A.y, A.z);
@@ -317,22 +328,52 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
                 beta = f3(C.x, C.y, C.z); L = f3(B.x, B.y, B.z);
                 depth = B.w; tr = A.w;
             }
+            if constexpr (kGroups) {
+                // (records are wide: the host never hands these instantiations compact ones).  A hit sample's in-path sums: the generic
+                // kernels' group planes, or for a lean kernel its L, which only the sun fed.  A miss is all environment.
+                gs[LG_ENVIRONMENT] = f3(0.f);
+                if (hit) {
+                    if (lg->planes) {
+                        const float* q = lg->planes + s;
+                        const size_t n = lg->stride;
+                        #pragma unroll
+                        for (int k = 0; k < (kSky == 2 ? 4 : 3); ++k) gs[k] = f3(q[(3 * k) * n], q[(3 * k + 1) * n], q[(3 * k + 2) * n]);
+                    } else gs[LG_SUN] = L;
+                }
+            }
             if constexpr (kSky == 0) {
+                if constexpr (kGroups) {                        // hdri_radiance with L and with 0, from one look-up
+                    const float3 t = hdri_product((cudaTextureObject_t)kp.env_tex, ld3(kp.sky_color), ray_dir, beta);
+                    L = hdri_finish(t, L);
+                    gs[LG_ENVIRONMENT] = hdri_finish(t, f3(0.f));
+                } else
                 if (!compact) L = hdri_radiance((cudaTextureObject_t)kp.env_tex, ld3(kp.sky_color), ray_dir, L, beta);
             } else if constexpr (kSky == 1) {
                 // precomputed sky seen from env_pos along the final direction (:1838-1841)
                 const float4 D = fa.planeD[s];
+                if constexpr (kGroups) {
+                    // the same fma as the instantiation without groups, once with L and once with 0 (pinned: the product has two uses)
+                    const float3 P = sample_atmosphere(atmo, kp.azimuth, kp.elevation, f3(D.x, D.y, D.z), ray_dir) * beta * kp.sky_mult;
+                    L = pfma3(P, ld3(kp.sky_color), L);
+                    gs[LG_ENVIRONMENT] = pfma3(P, ld3(kp.sky_color), f3(0.f));
+                } else
                 L += sample_atmosphere(atmo, kp.azimuth, kp.elevation, f3(D.x, D.y, D.z), ray_dir) * beta * kp.sky_mult * ld3(kp.sky_color);
             } else if constexpr (kSky == 2) {
                 const float4 D = fa.planeD[s];                       // env_pos or the last path position (:1750-1752)
+                if constexpr (kGroups) {
+                    // the in-path sky sum first, then the end-of-path sky, in the beauty's order
+                    const float3 sa = sample_atmosphere(atmo, kp.azimuth, kp.elevation, f3(D.x, D.y, D.z), ray_dir);
+                    L = pfma3(beta, sa, L);
+                    gs[LG_ENVIRONMENT] = pfma3(beta, sa, gs[LG_ENVIRONMENT]);
+                } else
                 L += beta * sample_atmosphere(atmo, kp.azimuth, kp.elevation, f3(D.x, D.y, D.z), ray_dir);
             }
             tr = fminf(tr, 1.0f);
             value = L;
         }
         // NaN / Inf guard (:2263-2264)
-        bool guarded = false;                                   // AOVs only, apart from the guard: the other instantiations keep their code
-        if constexpr (kAov) guarded = any_nan(value) || any_inf(value);
+        bool guarded = false;                                   // AOVs / groups only, apart from the guard: the other instantiations keep their code
+        if constexpr (kAov || kGroups) guarded = any_nan(value) || any_inf(value);
         if (any_nan(value) || any_inf(value)) value = accum;
         if (isnan(tr) || isinf(tr)) tr = 1.0f;
 
@@ -362,6 +403,15 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
                 volv = volv + (vs - volv) / (float)(iteration + 1);
             }
         }
+        if constexpr (kGroups) {
+            // taken before the viz_dof tint; a sample the guard replaced leaves every group at its own mean
+            #pragma unroll
+            for (int k = 0; k < kLightGroups; ++k) {
+                const float3 gv = guarded ? gm[k] : gs[k];
+                if (iteration == 0) gm[k] = gv;
+                else if (iteration < kp.max_interactions) gm[k] = gm[k] + (gv - gm[k]) / (float)(iteration + 1);
+            }
+        }
         if constexpr (kAdaptive) {                              // the sample as it entered the mean (after the NaN guard and the tint)
             const float lum = 0.2126f * value.x + 0.7152f * value.y + 0.0722f * value.z;
             wn += 1.0f;
@@ -387,6 +437,10 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     }
     accum_buf[lp] = accum; cost_buf[lp] = costv; depth_buf[lp] = depthv;
     if constexpr (kAov) { if (aov->alpha) aov->alpha[lp] = alphav; if (aov->volume) aov->volume[lp] = volv; }
+    if constexpr (kGroups) {
+        #pragma unroll
+        for (int k = 0; k < kLightGroups; ++k) if (lg->out[k]) lg->out[k][lp] = gm[k];
+    }
     if constexpr (kAdaptive) {
         const float err = wn >= 2.0f ? sqrtf(wm2 / (wn * (wn - 1.0f))) / fmaxf(wmean, kAdaptMeanFloor) : INFINITY;
         ad->stat[lp] = make_float4(wn, wmean, wm2, err);
@@ -413,16 +467,18 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     }
 }
 
-// kAov: the instantiations that also keep the compositing AOVs take the AovBuffers as one more argument (the pack `aov`, empty
-// otherwise), so the kernels without AOVs keep their parameter block.
+// kAov / kGroups: the instantiations that also keep the compositing AOVs / the light groups take the AovBuffers / the LightGroups as
+// more arguments (the pack `ext`, in that order, empty otherwise), so the kernels without them keep their parameter block.
 __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a) { return &a; }
+__device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const LightGroups&) { return &a; }
+__device__ __forceinline__ const LightGroups* lg_of(const AovBuffers&, const LightGroups& l) { return &l; }
 
-template <int kSky, bool kAov = false, class... Aov>
+template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
 __global__ void __launch_bounds__(256)
 k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
-          const Aov... aov)
+          const Ext... ext)
 {
-    static_assert(sizeof...(Aov) == (kAov ? 1 : 0), "k_resolve<kSky, true> takes one AovBuffers, k_resolve<kSky> none");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
     const FrameGeom& g = fa.geom;
     const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
     if (lp >= (uint32_t)g.n_local) return;
@@ -430,8 +486,10 @@ k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const
     const int y = global_row(g, lr);
     if (y >= g.height) return;
     const AovBuffers* ap = nullptr;
-    if constexpr (kAov) ap = aov_of(aov...);
-    resolve_pixel<kSky, false, kAov>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap);
+    const LightGroups* gp = nullptr;
+    if constexpr (kAov) ap = aov_of(ext...);
+    if constexpr (kGroups) gp = lg_of(ext...);
+    resolve_pixel<kSky, false, kAov, kGroups>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp);
 }
 
 // 32x4 pixel tile and the lane's pixel in it, for the per-tile adaptive kernels (a warp covers one row of 32 pixels)
@@ -447,19 +505,21 @@ __device__ __forceinline__ TilePixel tile_pixel(const FrameGeom& g, const int ti
 
 // One block of 128 per active tile: the running mean of the pixels that have not stopped, every pass of the chunk sampled; at the end of the
 // chunk their display / raw words, pass count and relative error (so a pixel keeps those of the last pass it took).  kAov: as k_resolve.
-template <int kSky, bool kAov = false, class... Aov>
+template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
 __global__ void __launch_bounds__(128)
-k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Aov... aov)
+k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Ext... ext)
 {
-    static_assert(sizeof...(Aov) == (kAov ? 1 : 0), "k_resolve_adaptive<kSky, true> takes one AovBuffers, k_resolve_adaptive<kSky> none");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_adaptive<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
     const FrameGeom& g = fa.geom;
     const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
     if (!t.inside) return;
     const uint32_t lp = (uint32_t)t.lr * (uint32_t)g.width + (uint32_t)t.x;
     if (ad.stopped[lp]) return;
     const AovBuffers* ap = nullptr;
-    if constexpr (kAov) ap = aov_of(aov...);
-    resolve_pixel<kSky, true, kAov>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap);
+    const LightGroups* gp = nullptr;
+    if constexpr (kAov) ap = aov_of(ext...);
+    if constexpr (kGroups) gp = lg_of(ext...);
+    resolve_pixel<kSky, true, kAov, kGroups>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap, gp);
 }
 
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
@@ -711,8 +771,13 @@ static cudaError_t launch_trace_t(const FrameArgs& fa, const vpt_atmosphere* atm
     return cudaGetLastError();
 }
 
-cudaError_t launch_trace(const FrameArgs& fa, const vpt_atmosphere* atm, bool lean, int slots, int n_ctas, cudaStream_t s)
+cudaError_t launch_trace(const FrameArgs& fa, const vpt_atmosphere* atm, bool lean, int slots, int n_ctas, const LightGroups* lg, cudaStream_t s)
 {
+    if (lg && lg->planes && !lean) {                                           // light groups: generic kernels, 3 rays per lane
+        if (atm) k_trace<1, false, 3, false, true><<<n_ctas, kTraceThreads, trace_smem_bytes(3), s>>>(fa, *atm, *lg);
+        else     k_trace<0, false, 3, false, true><<<n_ctas, kTraceThreads, trace_smem_bytes(3), s>>>(fa, NoAtmo{}, *lg);
+        return cudaGetLastError();
+    }
     if (atm) return launch_trace_t<1, false, 3>(fa, atm, n_ctas, s);
     if (fa.cell_table) {                                                        // the host only sets it for lean scenes
         k_trace<0, true, 2, true><<<n_ctas, kTraceThreads, trace_smem_bytes(2), s>>>(fa, NoAtmo{});
@@ -745,9 +810,16 @@ cudaError_t exchange_kernels_preload()
         (const void*)k_trace<0, false, 2>, (const void*)k_trace<0, true, 2>, (const void*)k_trace<0, true, 2, true>, (const void*)k_trace_brick,
         (const void*)k_resolve<0>, (const void*)k_resolve<1>, (const void*)k_resolve<2>,
         (const void*)k_resolve_adaptive<0>, (const void*)k_resolve_adaptive<1>, (const void*)k_resolve_adaptive<2>,
-        (const void*)k_resolve<0, true, AovBuffers>, (const void*)k_resolve<1, true, AovBuffers>, (const void*)k_resolve<2, true, AovBuffers>,
-        (const void*)k_resolve_adaptive<0, true, AovBuffers>, (const void*)k_resolve_adaptive<1, true, AovBuffers>,
-        (const void*)k_resolve_adaptive<2, true, AovBuffers>,
+        (const void*)k_resolve<0, true, false, AovBuffers>, (const void*)k_resolve<1, true, false, AovBuffers>, (const void*)k_resolve<2, true, false, AovBuffers>,
+        (const void*)k_resolve_adaptive<0, true, false, AovBuffers>, (const void*)k_resolve_adaptive<1, true, false, AovBuffers>,
+        (const void*)k_resolve_adaptive<2, true, false, AovBuffers>,
+        (const void*)k_trace<0, false, 3, false, true, LightGroups>, (const void*)k_trace<1, false, 3, false, true, LightGroups>,
+        (const void*)k_resolve<0, false, true, LightGroups>, (const void*)k_resolve<1, false, true, LightGroups>, (const void*)k_resolve<2, false, true, LightGroups>,
+        (const void*)k_resolve<0, true, true, AovBuffers, LightGroups>, (const void*)k_resolve<1, true, true, AovBuffers, LightGroups>,
+        (const void*)k_resolve<2, true, true, AovBuffers, LightGroups>,
+        (const void*)k_resolve_adaptive<0, false, true, LightGroups>, (const void*)k_resolve_adaptive<1, false, true, LightGroups>,
+        (const void*)k_resolve_adaptive<2, false, true, LightGroups>, (const void*)k_resolve_adaptive<0, true, true, AovBuffers, LightGroups>,
+        (const void*)k_resolve_adaptive<1, true, true, AovBuffers, LightGroups>, (const void*)k_resolve_adaptive<2, true, true, AovBuffers, LightGroups>,
         (const void*)k_adapt_init, (const void*)k_adapt, (const void*)k_adapt_halo, (const void*)k_adapt_count_publish, (const void*)k_adapt_tally,
         (const void*)k_adapt_publish, (const void*)k_peer_signal, (const void*)k_peer_wait };
     for (const void* f : fns) {
@@ -758,11 +830,25 @@ cudaError_t exchange_kernels_preload()
     return cudaSuccess;
 }
 
-cudaError_t trace_kernels_init(int max_ctas[7])
+template <int kInteg>
+static cudaError_t trace_init_groups(int* max_ctas)
+{
+    const void* f = (const void*)k_trace<kInteg, false, 3, false, true, LightGroups>;
+    cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem_bytes(3));
+    if (e != cudaSuccess) return e;
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(max_ctas, f, kTraceThreads, trace_smem_bytes(3));
+}
+
+cudaError_t trace_kernels_init(int max_ctas[9])
 {
     {
         cudaError_t e0 = cudaFuncSetAttribute(k_trace<0, true, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem_bytes(2));
         if (e0 == cudaSuccess) e0 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[6], k_trace<0, true, 2, true>, kTraceThreads, trace_smem_bytes(2));
+        if (e0 != cudaSuccess) return e0;
+    }
+    {
+        cudaError_t e0 = trace_init_groups<0>(&max_ctas[7]);
+        if (e0 == cudaSuccess) e0 = trace_init_groups<1>(&max_ctas[8]);
         if (e0 != cudaSuccess) return e0;
     }
     cudaError_t e = trace_init_t<0, false, 3>(&max_ctas[0]);
@@ -794,16 +880,39 @@ cudaError_t launch_trace_brick(const FrameArgs& fa, const float* pool, const int
 }
 
 static bool aov_on(const AovBuffers* aov) { return aov && (aov->alpha || aov->volume); }
+static bool lg_on(const LightGroups* lg) { return lg && (lg->out[0] || lg->out[1] || lg->out[2] || lg->out[3]); }
+
+// the light-group instantiations, with or without the AOVs
+template <int kSky>
+static void launch_resolve_groups(const FrameArgs& fa, const SkyArg<kSky>& atmo, int n_passes, int sampled, int write_display, const PeerFrames& pf,
+                                  const AovBuffers* aov, const LightGroups& lg, int blocks, cudaStream_t s)
+{
+    if (aov_on(aov)) k_resolve<kSky, true, true><<<blocks, 256, 0, s>>>(fa, atmo, n_passes, sampled, write_display, pf, *aov, lg);
+    else             k_resolve<kSky, false, true><<<blocks, 256, 0, s>>>(fa, atmo, n_passes, sampled, write_display, pf, lg);
+}
+
+template <int kSky>
+static void launch_resolve_adaptive_groups(const FrameArgs& fa, const SkyArg<kSky>& atmo, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
+                                           const LightGroups& lg, cudaStream_t s)
+{
+    if (aov_on(aov)) k_resolve_adaptive<kSky, true, true><<<ad.n_tiles, 128, 0, s>>>(fa, atmo, n_passes, ad, *aov, lg);
+    else             k_resolve_adaptive<kSky, false, true><<<ad.n_tiles, 128, 0, s>>>(fa, atmo, n_passes, ad, lg);
+}
 
 cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers,
-                           const AovBuffers* aov, cudaStream_t s)
+                           const AovBuffers* aov, const LightGroups* lg, cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
-    if (aov_on(aov)) {
+    if (lg_on(lg)) {
+        if (sky && fa.kp.integrator != 0) launch_resolve_groups<2>(fa, *sky, n_passes, sampled, write_display, pf, aov, *lg, blocks, s);
+        else if (sky)                     launch_resolve_groups<1>(fa, *sky, n_passes, sampled, write_display, pf, aov, *lg, blocks, s);
+        else                              launch_resolve_groups<0>(fa, NoSky{}, n_passes, sampled, write_display, pf, aov, *lg, blocks, s);
+    }
+    else if (aov_on(aov)) {
         if (sky && fa.kp.integrator != 0) k_resolve<2, true><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf, *aov);
         else if (sky)                     k_resolve<1, true><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf, *aov);
         else                              k_resolve<0, true><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf, *aov);
@@ -815,10 +924,15 @@ cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n
 }
 
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
-                                    cudaStream_t s)
+                                    const LightGroups* lg, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
-    if (aov_on(aov)) {
+    if (lg_on(lg)) {
+        if (sky && fa.kp.integrator != 0) launch_resolve_adaptive_groups<2>(fa, *sky, n_passes, ad, aov, *lg, s);
+        else if (sky)                     launch_resolve_adaptive_groups<1>(fa, *sky, n_passes, ad, aov, *lg, s);
+        else                              launch_resolve_adaptive_groups<0>(fa, NoSky{}, n_passes, ad, aov, *lg, s);
+    }
+    else if (aov_on(aov)) {
         if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2, true><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad, *aov);
         else if (sky)                     k_resolve_adaptive<1, true><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad, *aov);
         else                              k_resolve_adaptive<0, true><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad, *aov);

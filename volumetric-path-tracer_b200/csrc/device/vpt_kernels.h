@@ -74,10 +74,12 @@ cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* roo
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
 cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s);
-// atm != null selects the volumetric path integrator variant of the trace kernel
-cudaError_t launch_trace(const FrameArgs& fa, const vpt_atmosphere* atm, bool lean, int slots, int n_ctas, cudaStream_t s);   // slots: rays per lane, 2 or 3; fa.cell_table != null: the lean 2-slot cell-table instantiation
+struct LightGroups;
+// atm != null selects the volumetric path integrator variant of the trace kernel.  lg with planes != null (generic kernels only): the
+// light-group instantiation, at 3 rays per lane whatever `slots` says
+cudaError_t launch_trace(const FrameArgs& fa, const vpt_atmosphere* atm, bool lean, int slots, int n_ctas, const LightGroups* lg, cudaStream_t s);   // slots: rays per lane, 2 or 3; fa.cell_table != null: the lean 2-slot cell-table instantiation
 // per device: dynamic shared memory opt-in of the trace kernels + CTAs per SM of [generic, lean, volumetric path, brick]
-cudaError_t trace_kernels_init(int max_ctas[7]);      // [6]: lean, 2 rays per lane, cell table      // [0..2] generic / lean / volumetric path at 3 rays per lane, [3] k_trace_brick, [4..5] generic / lean at 2 rays per lane
+cudaError_t trace_kernels_init(int max_ctas[9]);      // [6]: lean, 2 rays per lane, cell table; [7] / [8]: generic / volumetric path with light groups      // [0..2] generic / lean / volumetric path at 3 rays per lane, [3] k_trace_brick, [4..5] generic / lean at 2 rays per lane
 // fast mode: lean direct integrator reading the density from a brick pool (vpt_trace_brick.cuh); dims = voxels per axis
 cudaError_t launch_trace_brick(const FrameArgs& fa, const float* pool, const int dims[3], int n_ctas, cudaStream_t s);
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s);
@@ -94,8 +96,15 @@ struct PeerFrames { int n = 0; float* accum[kMaxPeers] = {}; unsigned int* displ
 // share, next to accum.  Either may be null.  A kernel argument of the AOV instantiations of k_resolve / k_resolve_adaptive only (not in
 // FrameArgs, so every other kernel keeps its parameter block); aov == null or both pointers null selects the instantiations without them.
 struct AovBuffers { float* alpha = nullptr; float3* volume = nullptr; };
+// Light groups (vpt_set_light_group_buffers): [local pixel] running means of the radiance each light class added to the sample -- sun,
+// point lights, emission, environment -- next to accum.  Any output may be null.  `planes`: the per-sample group sums of the generic trace
+// kernels, float plane (group * 3 + channel) at planes + plane * stride, indexed by the sample slot pass * n_local + local pixel like the
+// records; null when a lean kernel traced the frame (its path radiance L is the sun group).  A kernel argument of the light-group
+// instantiations of k_trace / k_resolve / k_resolve_adaptive only, as AovBuffers is.
+enum LightGroup : int { LG_SUN = 0, LG_POINT = 1, LG_EMISSION = 2, LG_ENVIRONMENT = 3, kLightGroups = 4 };
+struct LightGroups { float3* out[kLightGroups] = {}; float* planes = nullptr; unsigned long long stride = 0; };
 cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers,
-                           const AovBuffers* aov, cudaStream_t s);
+                           const AovBuffers* aov, const LightGroups* lg, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -112,7 +121,7 @@ cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& 
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
-                                    cudaStream_t s);
+                                    const LightGroups* lg, cudaStream_t s);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);

@@ -70,6 +70,25 @@ struct TraceConsts {
     float3 sun_dir;
 };
 
+// ---- light groups (the kGroups instantiations; DESIGN.md section 8d) -----------------------------------------------------------
+// Every `L +=` site of those instantiations also adds its term to the ray's sum of that light class, kept in the sample scratch at the
+// ray's own sample slot: one ray per slot, so a plain read-modify-write (no atomics, deterministic).  ptxas contracts a single-use product
+// into the following add, and a product used for L AND for the group is no longer single-use, so both updates are pinned to the fma the
+// instantiation without groups compiles to: L + a * b -> fma(a, b, L).
+VPT_DEV const LightGroups* lg_of(const LightGroups& a) { return &a; }
+VPT_DEV float3 pfma3(const float3 a, const float3 b, const float3 c) { return f3(pfma(a.x, b.x, c.x), pfma(a.y, b.y, c.y), pfma(a.z, b.z, c.z)); }
+VPT_DEV size_t group_slot(const PathState& st, const FrameArgs& fa) { return (size_t)st.pass * fa.geom.n_local + ray_local_pixel(fa.geom, st.lp); }
+VPT_DEV void group_fma(const LightGroups* lg, const size_t s, const int group, const float3 a, const float3 b) {
+    float* p = lg->planes + (size_t)(group * 3) * lg->stride + s;
+    const size_t n = lg->stride;
+    p[0] = pfma(a.x, b.x, p[0]); p[n] = pfma(a.y, b.y, p[n]); p[2 * n] = pfma(a.z, b.z, p[2 * n]);
+}
+VPT_DEV void group_add(const LightGroups* lg, const size_t s, const int group, const float3 a) {
+    float* p = lg->planes + (size_t)(group * 3) * lg->stride + s;
+    const size_t n = lg->stride;
+    p[0] = padd(p[0], a.x); p[n] = padd(p[n], a.y); p[2 * n] = padd(p[2 * n], a.z);
+}
+
 // ---- ray record <-> registers ------------------------------------------------------------------------------
 // pool layout: word w of slot j of lane l at pool[w * kPool + j * 32 + l]  (bank == lane: conflict-free)
 template <int kPool>                                             // rays per warp = 32 * rays per lane
@@ -274,8 +293,10 @@ VPT_DEV void begin_ratio_walk(PathState& st, const FrameShared& fs, const TraceC
 VPT_DEV float finish_ratio_walk(const PathState& st) { return clampf(st.trv * st.T_c, .0f, 1.0f); }
 
 // ---- the integrator's control flow between heavy operations -------------------------------------------------
-template <bool kLean>
-VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, const TraceConsts& tc, const SphereRec& sph)
+// kGroups (generic instantiation only): every L += also goes to the ray's light-group sums in lg->planes
+template <bool kLean, bool kGroups = false>
+VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, const TraceConsts& tc, const SphereRec& sph,
+                     const LightGroups* lg = nullptr)
 {
     const SceneTables& sc = fs.sc;
     const vpt_kernel_params& kp = fa.kp;
@@ -346,7 +367,11 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
                 const float cos_theta = dot(st.dir, tc.sun_dir);
                 const float phase_pdf = hg_phase(cos_theta, kp.phase_g1);
                 const float3 Ld = f3(tr) * phase_pdf;
-                st.L += Ld * ld3(kp.sun_color) * kp.sun_mult * st.beta;
+                if constexpr (kGroups) {
+                    const float3 t = Ld * ld3(kp.sun_color) * kp.sun_mult;
+                    st.L = pfma3(t, st.beta, st.L);
+                    group_fma(lg, group_slot(st, fa), LG_SUN, t, st.beta);
+                } else st.L += Ld * ld3(kp.sun_color) * kp.sun_mult * st.beta;
                 if (!kLean && fa.lights.num_lights > 0) { st.aux = f3(.0f); st.light_budget = 10; st.phase = PH_POINT_NEXT; }
                 else st.phase = PH_EMISSION;
             } else if (!kLean && st.tr_kind == TR_POINT) {                    // reference point_light::Le, light.h:104-121
@@ -363,7 +388,11 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
                 st.light_budget--;
                 st.phase = PH_POINT_NEXT;
             } else {                                                // sphere branch tail (:1831-1833)
-                st.L += ld3(kp.sun_color) * kp.sun_mult * f3(tr) * fmaxf(dot(tc.sun_dir, st.aux), .0f) * st.beta;
+                if constexpr (kGroups) {
+                    const float3 t = ld3(kp.sun_color) * kp.sun_mult * f3(tr) * fmaxf(dot(tc.sun_dir, st.aux), .0f);
+                    st.L = pfma3(t, st.beta, st.L);
+                    group_fma(lg, group_slot(st, fa), LG_SUN, t, st.beta);
+                } else st.L += ld3(kp.sun_color) * kp.sun_mult * f3(tr) * fmaxf(dot(tc.sun_dir, st.aux), .0f) * st.beta;
                 if (fa.planeD) fa.planeD[(size_t)st.pass * fa.geom.n_local + ray_local_pixel(fa.geom, st.lp)] = make_float4(st.pos.x, st.pos.y, st.pos.z, 0.f);   // env_pos = ray_pos
                 st.sphere_bounced = true;
                 st.rd++; st.have_closest = false;
@@ -373,7 +402,11 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
         }
         case PH_POINT_NEXT: {                                       // reference estimate_point_light (:1445-1475)
             if (kLean) { st.phase = PH_EMISSION; break; }
-            if (st.light_budget < 0) { st.L += st.aux * st.beta; st.phase = PH_EMISSION; break; }
+            if (st.light_budget < 0) {
+                if constexpr (kGroups) { st.L = pfma3(st.aux, st.beta, st.L); group_fma(lg, group_slot(st, fa), LG_POINT, st.aux, st.beta); }
+                else st.L += st.aux * st.beta;
+                st.phase = PH_EMISSION; break;
+            }
             const vpt_point_light* lp = reinterpret_cast<const vpt_point_light*>(fa.lights.light_ptr);
             st.light_index = int(floorf(st.rng.next() * fa.lights.num_lights));
             st.tr_kind = TR_POINT; st.wpos = st.pos; st.wdir = normalize(ld3(lp[st.light_index].pos) - st.pos);
@@ -390,6 +423,7 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
             break;
         case PH_AFTER_EMIT:
             st.L += st.aux;
+            if constexpr (kGroups) group_add(lg, group_slot(st, fa), LG_EMISSION, st.aux);
             st.phase = PH_AFTER_VOLUME;
             break;
         case PH_AFTER_VOLUME: {                                     // the ray moved since the last test
@@ -468,10 +502,16 @@ VPT_DEV void write_sample(const PathState& st, const FrameArgs& fa)
 // caller's AtmosphereParameters in the kernel (sky radiance decides whether a transmittance walk is run at all)
 struct NoAtmo { int pad[4]; };
 
-template <int kInteg, bool kLean, int kSlots, bool kCells = false>
+// kGroups (generic kernels): the light-group instantiation, which takes the LightGroups as one more argument (the pack `lgs`, empty
+// otherwise), so the kernels without groups keep their parameter block
+template <int kInteg, bool kLean, int kSlots, bool kCells = false, bool kGroups = false, class... Lg>
 __global__ void __launch_bounds__(kTraceThreads, trace_min_ctas(kSlots))
-k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atmosphere, NoAtmo>::type atm)
+k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atmosphere, NoAtmo>::type atm, const Lg... lgs)
 {
+    static_assert(sizeof...(Lg) == (kGroups ? 1 : 0), "k_trace<..., true> takes one LightGroups, the other instantiations none");
+    static_assert(!kGroups || !kLean, "lean kernels keep their light groups in the wide records (L is the sun group)");
+    // (the LightGroups are reached through lg_of(lgs...) where they are used: a pointer variable in every instantiation, even unused,
+    // moved two stack stores of k_trace<1, false, 3>)
     __shared__ FrameShared fs;
     extern __shared__ float pool_smem[];                         // kTraceWarps x kRayWords x kPool words (opt-in dynamic shared memory)
     load_frame_shared(fs, fa.scene);
@@ -532,6 +572,11 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
                     st.have_closest = false; st.sphere_free = true;
                     st.phase = kInteg ? (int)VP_AFTER_DELTA : (int)PH_AFTER_DELTA; st.op = OP_STEP;
                 }
+                if constexpr (kGroups) {                          // the sample slot's group sums start at 0 (integrator 0 keeps no environment sum)
+                    const size_t s = group_slot(st, fa);
+                    #pragma unroll
+                    for (int k = 0; k < (kInteg ? 12 : 9); ++k) lg_of(lgs...)->planes[(size_t)k * lg_of(lgs...)->stride + s] = 0.0f;
+                }
                 store_ray(pv, j, st);
                 if (j == 0) tag0 = st.op; else if (j == 1) tag1 = st.op; else tag2 = st.op;
                 lane_rays++;
@@ -560,7 +605,9 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
                     st.have_closest = true; st.op = OP_GLUE;
                 }
                 if (st.op == OP_GLUE) {
-                    if constexpr (kInteg != 0) advance_vol(st, fs, fa, atm, tc, sph);
+                    if constexpr (kInteg != 0 && kGroups) advance_vol<true>(st, fs, fa, atm, tc, sph, lg_of(lgs...));
+                    else if constexpr (kInteg != 0) advance_vol(st, fs, fa, atm, tc, sph);
+                    else if constexpr (kGroups) advance<kLean, true>(st, fs, fa, tc, sph, lg_of(lgs...));
                     else advance<kLean>(st, fs, fa, tc, sph);
                 }
                 if (st.op == OP_TRBEGIN) begin_ratio_walk(st, fs, tc, sph);

@@ -112,7 +112,11 @@ VPT_DEV float3 vol_env_radiance(const FrameArgs& fa, const vpt_atmosphere& atm, 
     return fa.kp.environment_type == 0 ? sky_radiance_noinline(atm, fa.kp.azimuth, fa.kp.elevation, pos, wi) : env_tex_radiance(fa.kp, wi);
 }
 
-VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& fa, const vpt_atmosphere& atm, const TraceConsts& tc, const SphereRec& sph)
+// kGroups: every L += also goes to the ray's light-group sums in lg->planes.  The class of a light estimate is the last transmittance
+// walk's tr_kind: uniform_sample_one_light leaves aux at 0 when it ran no walk, and then the group gains an exact zero.
+template <bool kGroups = false>
+VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& fa, const vpt_atmosphere& atm, const TraceConsts& tc, const SphereRec& sph,
+                         const LightGroups* lg = nullptr)
 {
     const SceneTables& sc = fs.sc;
     const vpt_kernel_params& kp = fa.kp;
@@ -248,7 +252,12 @@ VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& 
             break;
         }
         case VP_LIGHT_DONE:                                         // L += beta * (3 * estimate) [+ emission], then resample the direction
-            st.L += st.beta * (st.aux * 3.0f);
+            if constexpr (kGroups) {
+                const float3 t = st.aux * 3.0f;
+                st.L = pfma3(st.beta, t, st.L);
+                const int group = st.tr_kind == VTR_SUN ? LG_SUN : st.tr_kind == VTR_POINT ? LG_POINT : LG_ENVIRONMENT;
+                group_fma(lg, group_slot(st, fa), group, st.beta, t);
+            } else st.L += st.beta * (st.aux * 3.0f);
             if (kp.emission_scale != 0) {
                 st.wpos = st.pos; st.wdir = st.dir; st.t = 0.0f; st.aux = f3(.0f);
                 st.mode = W_EMIT; st.op = OP_STEP; st.phase = VP_AFTER_EMIT;
@@ -259,6 +268,7 @@ VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& 
             break;
         case VP_AFTER_EMIT:
             st.L += st.aux;
+            if constexpr (kGroups) group_add(lg, group_slot(st, fa), LG_EMISSION, st.aux);
             hg_sample(st.dir, st.rng, kp.phase_g1);
             st.rd++; st.phase = VP_ITER;
             break;

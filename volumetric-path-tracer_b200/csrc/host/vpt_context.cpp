@@ -79,7 +79,7 @@ static void free_context(vpt_context* c) {
     for (auto& e : c->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     cudaFree(c->d_queue_id); cudaFree(c->d_queue_org); cudaFree(c->d_bn_table);
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
-    cudaFree(c->d_plane_tr);
+    cudaFree(c->d_plane_tr); cudaFree(c->d_lg_planes);
     cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
     cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz);
     delete c;
@@ -152,6 +152,13 @@ int vpt_set_aov_buffers(vpt_context* c, float* d_alpha, float* d_volume_f3) {
     return VPT_OK;
 }
 
+int vpt_set_light_group_buffers(vpt_context* c, float* d_sun_f3, float* d_point_f3, float* d_emission_f3, float* d_environment_f3) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_light_group_buffers: null context");
+    c->lg_out[0] = d_sun_f3; c->lg_out[1] = d_point_f3; c->lg_out[2] = d_emission_f3; c->lg_out[3] = d_environment_f3;
+    c->lg_active = false;           // all null: off from now on; otherwise the buffers take over at the next call with iteration == 0
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -174,8 +181,9 @@ int vpt_get_stats(vpt_context* c, unsigned long long* launches, unsigned* last_q
 }
 
 // Scratch of one round: the ray queue and plane A per sample, then either planes B, C (and D) per sample (wide records) or the tr plane
-// per pixel (compact records).  A change of record layout reallocates, so the scratch never holds another layout's planes.
-static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixels, bool wide, bool planeD) {
+// per pixel (compact records).  A change of record layout reallocates, so the scratch never holds another layout's planes.  Light groups
+// traced by a generic kernel also need their 12 float planes per sample, which are kept once grown.
+static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixels, bool wide, bool planeD, bool groups) {
     if (n_samples > c->cap_samples || wide != c->cap_wide || planeD != c->cap_planeD) {
         cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
         cudaFree(c->d_queue_id); cudaFree(c->d_queue_org);
@@ -191,6 +199,11 @@ static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixel
         }
         if (planeD) VPT_CUDA(c, cudaMalloc(&c->d_planeD, n_samples * sizeof(float4)));
         c->cap_samples = n_samples; c->cap_wide = wide; c->cap_planeD = planeD;
+    }
+    if (groups && n_samples > c->cap_lg_samples) {
+        cudaFree(c->d_lg_planes); c->d_lg_planes = nullptr; c->cap_lg_samples = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_lg_planes, n_samples * 12 * sizeof(float)));
+        c->cap_lg_samples = n_samples;
     }
     if (!wide && n_pixels > c->cap_tr) {
         cudaFree(c->d_plane_tr); c->d_plane_tr = nullptr; c->cap_tr = 0;
@@ -212,6 +225,7 @@ struct FramePlan {
     int trace_ctas = 0, slots = 3, chunk = 1, bn_limit = 0;
     unsigned n_sampled = 0;               // how many of the requested passes sample (the rest only re-tonemap)
     vpt::AovBuffers aov;                  // the active compositing AOVs (both null: off)
+    vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
 };
 
 // Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
@@ -248,6 +262,25 @@ static int check_aov_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t
     }
     if (byte_ranges_overlap(c->aov_alpha, 4 * n, c->aov_volume, 12 * n))
         return fail(c, VPT_ERR_INVALID, "vpt_set_aov_buffers: the alpha buffer and the volume buffer overlap");
+    return VPT_OK;
+}
+
+// The light-group buffers may not share a byte with a Kernel_params output buffer, an AOV buffer or each other (n = local pixels).
+static int check_light_group_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    static const char* const names[4] = { "sun", "point", "emission", "environment" };
+    const struct { const char* name; const void* p; size_t bytes; } others[] = {
+        { "Kernel_params.accum_buffer", (const void*)(uintptr_t)kp.accum_buffer, 12 * n }, { "Kernel_params.depth_buffer", (const void*)(uintptr_t)kp.depth_buffer, 4 * n },
+        { "Kernel_params.cost_buffer", (const void*)(uintptr_t)kp.cost_buffer, 12 * n }, { "Kernel_params.raw_buffer", (const void*)(uintptr_t)kp.raw_buffer, 16 * n },
+        { "Kernel_params.display_buffer", (const void*)(uintptr_t)kp.display_buffer, 4 * n },
+        { "the alpha AOV buffer", c->aov_alpha, 4 * n }, { "the volume AOV buffer", c->aov_volume, 12 * n } };
+    for (int k = 0; k < 4; ++k) {
+        for (const auto& o : others)
+            if (byte_ranges_overlap(c->lg_out[k], 12 * n, o.p, o.bytes))
+                return fail(c, VPT_ERR_INVALID, std::string("vpt_set_light_group_buffers: the ") + names[k] + " buffer overlaps " + o.name);
+        for (int j = 0; j < k; ++j)
+            if (byte_ranges_overlap(c->lg_out[k], 12 * n, c->lg_out[j], 12 * n))
+                return fail(c, VPT_ERR_INVALID, std::string("vpt_set_light_group_buffers: the ") + names[j] + " buffer and the " + names[k] + " buffer overlap");
+    }
     return VPT_OK;
 }
 
@@ -359,18 +392,27 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     // max_scratch_bytes.  Compact records: an HDRI frame traced by a lean kernel, which then finishes each ray's environment term
     // itself.  A frame that ends on the precomputed sky needs wide records and env_pos (plane D: k_resolve<1/2> evaluate the sky from
     // them), and so does the generic kernel (the texture look-up in its service round cost it more than k_resolve<0> saved).
+    // light groups, decided before the record layout: registered buffers take over at the first call of a frame (iteration == 0) and are
+    // checked on every call.  They force wide records (a lean kernel's L is then the sun group, in plane B); a generic kernel keeps its
+    // group sums in 12 more float planes per sample
+    const bool groups = c->lg_active || (kp.iteration == 0 && (c->lg_out[0] || c->lg_out[1] || c->lg_out[2] || c->lg_out[3]));
+    if (groups) {
+        int rc = check_light_group_buffers(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+    }
+    const bool group_planes = groups && !lean;
     const bool planeD = sky_env;
-    const bool wide = sky_env || !lean;
+    const bool wide = sky_env || !lean || groups;
     int chunk = c->passes_per_chunk;
     if (c->chunk_auto) chunk = (size_t)fa.geom.n_local <= ((size_t)1 << 20) ? 64 : 32;
     {
-        const size_t per_sample = wide ? 88 + (planeD ? 16 : 0) : 56;
+        const size_t per_sample = (wide ? 88 + (planeD ? 16 : 0) : 56) + (group_planes ? 48 : 0);
         const size_t fit = c->max_scratch_bytes / (per_sample * (size_t)(fa.geom.n_local > 0 ? fa.geom.n_local : 1));
         if ((size_t)chunk > fit) chunk = fit < 1 ? 1 : (int)fit;
     }
     if (n_sampled) {
         const size_t per_chunk = (size_t)fa.geom.n_local * (size_t)(n_sampled < (unsigned)chunk ? n_sampled : (unsigned)chunk);
-        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD);
+        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD, group_planes);
         if (rc != VPT_OK) return rc;
     }
     if (c->cap_chunk < chunk) {
@@ -399,7 +441,9 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     }
     // lanes an operation must gather before it pre-empts stepping, chosen per kernel (26 helps only the lean kernel at 3 rays per lane)
     fa.sched_min_lanes = c->sched_min_lanes > 0 ? c->sched_min_lanes : ((lean && slots == 3 && !vol_integ && !c->brick_pool && !c->cell_table) ? 26 : 20);
-    int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm : c->max_ctas[c->brick_pool ? 3 : c->cell_table ? 6 : vol_integ ? 2 : (slots == 2 ? (lean ? 5 : 4) : (lean ? 1 : 0))];
+    if (group_planes) slots = 3;         // the light-group instantiations of the generic kernels run 3 rays per lane
+    int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm
+                    : c->max_ctas[group_planes ? (vol_integ ? 8 : 7) : c->brick_pool ? 3 : c->cell_table ? 6 : vol_integ ? 2 : (slots == 2 ? (lean ? 5 : 4) : (lean ? 1 : 0))];
     if (ctas_per_sm < 1) ctas_per_sm = 1;
 
     fa.counters = c->count_stats ? c->d_stats : nullptr;
@@ -416,6 +460,11 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         c->aov_active = true;
         plan.aov.alpha = c->aov_alpha; plan.aov.volume = reinterpret_cast<float3*>(c->aov_volume);
     }
+    if (groups) {
+        c->lg_active = true;
+        for (int k = 0; k < 4; ++k) plan.lg.out[k] = reinterpret_cast<float3*>(c->lg_out[k]);
+        if (group_planes) { plan.lg.planes = c->d_lg_planes; plan.lg.stride = (unsigned long long)c->cap_lg_samples; }
+    }
     return VPT_OK;
 }
 
@@ -424,7 +473,7 @@ static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, unsign
     vpt::FrameArgs fa = plan.fa;
     fa.n_passes = (int)np;
     if (c->brick_pool) return vpt::launch_trace_brick(fa, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
-    return vpt::launch_trace(fa, plan.vol_integ ? &plan.atmo : nullptr, plan.lean, plan.slots, plan.trace_ctas, stream);
+    return vpt::launch_trace(fa, plan.vol_integ ? &plan.atmo : nullptr, plan.lean, plan.slots, plan.trace_ctas, &plan.lg, stream);
 }
 
 extern "C" {
@@ -467,7 +516,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, &plan.aov, stream); }));
+        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, &plan.aov, &plan.lg, stream); }));
         c->launches += 4;
         done += np;
     }
@@ -477,7 +526,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, vpt::launch_resolve(fa, plan.sky, (int)(n_passes - n_sampled), 0, 1, &peers, &plan.aov, stream));
+        VPT_CUDA(c, vpt::launch_resolve(fa, plan.sky, (int)(n_passes - n_sampled), 0, 1, &peers, &plan.aov, &plan.lg, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2;
     }
@@ -592,7 +641,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, &plan.aov, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, &plan.aov, &plan.lg, stream); }));
             c->launches += 3;
         }
         done += np;

@@ -16,9 +16,14 @@ from ._native import lib, check
 from .scene import Scene, default_kernel_params
 
 
+# the light groups of vpt_set_light_group_buffers, in its argument order
+LIGHT_GROUPS = ("sun", "point", "emission", "environment")
+
+
 class FrameBuffers:
     """accum/cost (float3), depth (float), raw (float4), display (uint32) for `n_pixels` pixels; alpha (float) and volume (float3),
-    the compositing AOVs, once Renderer.enable_aovs() has allocated them (None until then)."""
+    the compositing AOVs, once Renderer.enable_aovs() has allocated them (None until then); `groups`, the light groups (name -> float3
+    tensor, LIGHT_GROUPS order), once Renderer.enable_light_groups() has allocated them (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -29,9 +34,11 @@ class FrameBuffers:
         self.display = torch.zeros(self.n, dtype=torch.int32, device=device)
         self.alpha = None
         self.volume = None
+        self.groups = None
 
     def zero_(self):
-        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume):
+        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume,
+                  *(self.groups.values() if self.groups else ())):
             if t is not None:
                 t.zero_()
 
@@ -168,6 +175,28 @@ class Renderer:
         if self.buffers.volume is None:
             raise N.VptError("Renderer.volume_image: AOVs are not enabled (Renderer.enable_aovs())")
         return self.buffers.volume.view(self.n_local // self.width, self.width, 3)
+
+    def enable_light_groups(self):
+        """Allocate and register the light groups (vpt_set_light_group_buffers): buffers.groups[name] (n, 3) float32 for every name of
+        LIGHT_GROUPS -- the running means of the radiance the sun, the point lights, the volume's emission and the environment added to
+        each sample.  They take over at the next render call with kp.iteration == 0, and sum to accum up to the rounding of the separate
+        sums (DESIGN.md section 8d).  n is the renderer's local pixel count (rank-local rows on a partitioned renderer)."""
+        dev = self.buffers.accum.device
+        self.buffers.groups = {name: torch.zeros(self.n_local, 3, dtype=torch.float32, device=dev) for name in LIGHT_GROUPS}
+        ptrs = [C.c_void_p(self.buffers.groups[name].data_ptr()) for name in LIGHT_GROUPS]
+        check(lib.vpt_set_light_group_buffers(self.ctx, *ptrs), self.ctx, "vpt_set_light_group_buffers")
+
+    def disable_light_groups(self):
+        """Turn the light groups off at once; buffers.groups keeps what it holds."""
+        check(lib.vpt_set_light_group_buffers(self.ctx, None, None, None, None), self.ctx, "vpt_set_light_group_buffers")
+
+    def light_group_image(self, name):
+        """(H, W, 3) float32 view of light group `name` (one of LIGHT_GROUPS; (local rows, W, 3) on a partitioned renderer)."""
+        if self.buffers.groups is None:
+            raise N.VptError("Renderer.light_group_image: light groups are not enabled (Renderer.enable_light_groups())")
+        if name not in self.buffers.groups:
+            raise N.VptError(f"Renderer.light_group_image: unknown light group {name!r} (one of {', '.join(LIGHT_GROUPS)})")
+        return self.buffers.groups[name].view(self.n_local // self.width, self.width, 3)
 
     def reset(self):
         self.kp.iteration = 0
