@@ -7,6 +7,10 @@ Protocol: the UNMODIFIED reference kernel, launched exactly as main.cpp:1823-182
 most 256 high, the one shape at which the kernel's blue-noise read / update is race-free (every thread touches only its own
 entry, SURVEY 8(c)(i)); octree built by the reference builder; environment = the deterministic procedural map
 `synthetic_env(512, 256)` so that the fixtures need no 13 MB HDRI.
+
+mixed_direct renders scene S1 of tests/mixed_scenes.py (the dragon and three synthetic volumes: a heat grid at its own resolution,
+a colour grid, different majorants) with emission, point lights and the sphere.  `make_golden.py OUT_DIR NAME ...` writes only the
+named fixtures.
 """
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -20,9 +24,17 @@ CASES = {
     "dragon_single": dict(W=256, H=128, passes=2, kp=dict(ray_depth=2, volume_depth=1), lights=None),
     "dragon_multi":  dict(W=256, H=128, passes=2, kp=dict(ray_depth=3, volume_depth=3, phase_g1=0.6, density_mult=2.0, tr_depth=1.5),
                           lights=[((9.0, 6.0, 2.0), (1.0, 0.8, 0.6), 40.0), ((-2.0, 3.0, 8.0), (0.5, 0.7, 1.0), 25.0)]),
+    "mixed_direct":  dict(W=256, H=128, passes=2, kp=dict(ray_depth=3, volume_depth=2, emission_scale=1.0, emission_pivot=1.0),
+                          lights=[((9.0, 6.0, 2.0), (1.0, 0.8, 0.6), 40.0), ((-2.0, 3.0, 8.0), (0.5, 0.7, 1.0), 25.0)], scene="S1"),   # = mixed_scenes.LIGHTS
 }
 
 def build(case):
+    if case.get("scene") == "S1":
+        import mixed_scenes
+        scene = mixed_scenes.build_s1(mixed_scenes.Volumes())              # its own point lights and sphere
+        kp = V.default_kernel_params(); kp.environment_type = 1; kp.max_interactions = 1000
+        for k, v in case["kp"].items(): setattr(kp, k, v)
+        return scene, kp
     vol = V.Volume.load_vdb(V.find_asset("dragon.vdb"))
     scene = V.Scene([vol.instance()], env=synthetic_env(512, 256), lights=case["lights"])
     kp = V.default_kernel_params(); kp.environment_type = 1; kp.max_interactions = 1000
@@ -30,10 +42,11 @@ def build(case):
     return scene, kp
 
 def main():
-    if len(sys.argv) != 2: raise SystemExit("usage: make_golden.py OUT_DIR")
+    if len(sys.argv) < 2: raise SystemExit("usage: make_golden.py OUT_DIR [NAME ...]")
     out = sys.argv[1]; os.makedirs(out, exist_ok=True)
     orc = RefOracle()
-    for name, case in CASES.items():
+    for name in sys.argv[2:] or CASES:
+        case = CASES[name]
         scene, kp = build(case)
         r = V.Renderer(scene, case["W"], case["H"], kp=kp)
         r.params.p_oct.value = orc.build_octree(scene.h_volumes, len(scene.instances))      # reference-built octree
@@ -47,7 +60,7 @@ def main():
                             display=r.buffers.display.cpu().numpy().reshape(case["H"], case["W"]),
                             blue_noise=scene.d_blue_noise.cpu().numpy(),
                             camera=np.frombuffer(bytes(r.cam), dtype=np.uint8),
-                            meta=json.dumps(dict(case=name, W=case["W"], H=case["H"], passes=case["passes"], kp=case["kp"], lights=case["lights"],
+                            meta=json.dumps(dict(case=name, W=case["W"], H=case["H"], passes=case["passes"], kp=case["kp"], lights=case["lights"], scene=case.get("scene"),
                                                  generator="UNMODIFIED reference volume_rt_kernel (sm_90a rebuild, H100), its own launch protocol, race-free frame shape")))
         print("wrote", name, "mean", float(r.buffers.accum.mean()))
 
