@@ -6,15 +6,16 @@
 //   k_generate      : one block per 32x4 pixel tile, all passes of the chunk: Philox stream, jitter, thin-lens ray,
 //                     root/sphere test, draw-free prefix of the first tracking walk; misses write a 16-byte sample
 //                     record, the rest are pushed into a warp-compacted ray queue (one atomic per warp)
-//   k_trace<I, L>   : persistent; every lane owns three rays parked in shared memory (vpt_trace.cuh); I = integrator
-//                     (0 direct, 1 volumetric path: vpt_trace_vol.cuh), L = lean instantiation for the common scene
-//   k_resolve<S>    : per pixel, passes in order: environment term (S = 0 HDRI: with compact records for misses only; 1 / 2 precomputed
-//                     sky: vpt_atmosphere.cuh), NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference kernel)
-//   k_resolve<S, true>, k_resolve_adaptive<S, true> : the same, plus the running means of the compositing AOVs (alpha, volume colour)
-//   k_resolve<S, A, true>, k_resolve_adaptive<S, A, true>, k_trace<I, false, 3, false, true> : light groups -- the generic trace kernels
-//                     also keep each ray's per-class radiance sums, the resolve their running means (sun, point, emission, environment)
+//   k_trace<I, L, R, C, G> : persistent; every lane owns R rays parked in shared memory (vpt_trace.cuh); I = integrator (0 direct,
+//                     1 volumetric path: vpt_trace_vol.cuh), L = lean instantiation for the common scene, C = cell table, G = light groups
+//                     (the generic kernels also keep each ray's per-class radiance sums); k_trace_brick in brick mode.  The nine
+//                     instantiations the host picks from (TraceKernel) are listed once, in trace_kernel below.
+//   k_resolve<S, A, G> : per pixel, passes in order: environment term (S = 0 HDRI: with compact records for misses only; 1 / 2 precomputed
+//                     sky: vpt_atmosphere.cuh), NaN guard, running mean, ACES tonemap, display/raw/depth/cost writes (the tail of the reference
+//                     kernel); A: plus the running means of the compositing AOVs (alpha, volume colour), G: of the light groups (sun, point,
+//                     emission, environment).  Its twelve instantiations, and those of k_resolve_adaptive, are listed in resolve_kernels below.
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
-//   k_generate_adaptive, k_resolve_adaptive<S>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
+//   k_generate_adaptive, k_resolve_adaptive<S, A, G>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
 //   k_adapt_halo, k_adapt_count_publish, k_adapt_tally, k_adapt_publish : the same frame sharded over the peer-memory exchange -- stripe-edge
 //                     errors, the agreement on when to stop, and the final full-frame stores
@@ -761,186 +762,136 @@ cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const Ad
 
 static size_t trace_smem_bytes(int slots) { return (size_t)kTraceWarps * kRayWords * 32 * slots * sizeof(float); }
 
-// atm != null selects the volumetric path integrator variant (Kernel_params.integrator != 0); lean selects the instantiation
-// without multi-volume lists, emission walk and point lights (the caller guarantees none of them is in play); slots = rays per lane
-template <int kInteg, bool kLean, int kSlots>
-static cudaError_t launch_trace_t(const FrameArgs& fa, const vpt_atmosphere* atm, int n_ctas, cudaStream_t s)
+static BrickArgs brick_args(const float* pool, const int dims[3])
 {
-    if constexpr (kInteg != 0) k_trace<kInteg, kLean, kSlots><<<n_ctas, kTraceThreads, trace_smem_bytes(kSlots), s>>>(fa, *atm);
-    else                       k_trace<kInteg, kLean, kSlots><<<n_ctas, kTraceThreads, trace_smem_bytes(kSlots), s>>>(fa, NoAtmo{});
-    return cudaGetLastError();
+    BrickArgs ba;
+    ba.pool = pool; ba.dimx = dims[0]; ba.dimy = dims[1]; ba.dimz = dims[2];
+    ba.nbx = (dims[0] + 3) / 4; ba.nby = (dims[1] + 3) / 4; ba.nbz = (dims[2] + 3) / 4;
+    return ba;
 }
 
-cudaError_t launch_trace(const FrameArgs& fa, const vpt_atmosphere* atm, bool lean, int slots, int n_ctas, const LightGroups* lg, cudaStream_t s)
+// The trace kernels: f(kernel, block size, dynamic shared memory, the arguments after FrameArgs) for TraceKernel k.  Launch, shared
+// memory opt-in, occupancy and preload all go through this list and resolve_kernels below.  (A unary + forms the pointer of an
+// instantiation with a pack argument: inside a template, g++ cannot deduce the lambda's parameter from that template-id.)
+template <class F>
+static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const BrickArgs& ba, F&& f)
 {
-    if (lg && lg->planes && !lean) {                                           // light groups: generic kernels, 3 rays per lane
-        if (atm) k_trace<1, false, 3, false, true><<<n_ctas, kTraceThreads, trace_smem_bytes(3), s>>>(fa, *atm, *lg);
-        else     k_trace<0, false, 3, false, true><<<n_ctas, kTraceThreads, trace_smem_bytes(3), s>>>(fa, NoAtmo{}, *lg);
-        return cudaGetLastError();
+    switch (k) {
+    case TK_GENERIC_3:        return f(k_trace<0, false, 3>, kTraceThreads, trace_smem_bytes(3), NoAtmo{});
+    case TK_LEAN_3:           return f(k_trace<0, true, 3>, kTraceThreads, trace_smem_bytes(3), NoAtmo{});
+    case TK_VOL_3:            return f(k_trace<1, false, 3>, kTraceThreads, trace_smem_bytes(3), atm);
+    case TK_BRICK:            return f(k_trace_brick, kBrickThreads, (size_t)kBrickThreads * kBrickBytes, ba);
+    case TK_GENERIC_2:        return f(k_trace<0, false, 2>, kTraceThreads, trace_smem_bytes(2), NoAtmo{});
+    case TK_LEAN_2:           return f(k_trace<0, true, 2>, kTraceThreads, trace_smem_bytes(2), NoAtmo{});
+    case TK_LEAN_2_CELLS:     return f(k_trace<0, true, 2, true>, kTraceThreads, trace_smem_bytes(2), NoAtmo{});
+    case TK_GENERIC_3_GROUPS: return f(+k_trace<0, false, 3, false, true, LightGroups>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, lg);
+    case TK_VOL_3_GROUPS:     return f(+k_trace<1, false, 3, false, true, LightGroups>, kTraceThreads, trace_smem_bytes(3), atm, lg);
+    default:                  return cudaErrorInvalidValue;
     }
-    if (atm) return launch_trace_t<1, false, 3>(fa, atm, n_ctas, s);
-    if (fa.cell_table) {                                                        // the host only sets it for lean scenes
-        k_trace<0, true, 2, true><<<n_ctas, kTraceThreads, trace_smem_bytes(2), s>>>(fa, NoAtmo{});
-        return cudaGetLastError();
-    }
-    if (slots == 2) return lean ? launch_trace_t<0, true, 2>(fa, nullptr, n_ctas, s) : launch_trace_t<0, false, 2>(fa, nullptr, n_ctas, s);
-    return lean ? launch_trace_t<0, true, 3>(fa, nullptr, n_ctas, s) : launch_trace_t<0, false, 3>(fa, nullptr, n_ctas, s);
 }
 
-// Once per context (= per device): opt the instantiations into their dynamic shared memory and record how many CTAs of each fit
+// The resolve kernels: f(k_resolve<S, A, G>, k_resolve_adaptive<S, A, G>, the sky argument, the trailing AovBuffers / LightGroups) for
+// key {S, A, G}, case S * 4 + A * 2 + G.
+template <class F>
+static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, F&& f)
+{
+    const NoSky hdri{};
+    switch (r.sky * 4 + r.aov * 2 + r.groups) {
+    case 0:  return f(k_resolve<0>, k_resolve_adaptive<0>, hdri);
+    case 1:  return f(+k_resolve<0, false, true, LightGroups>, +k_resolve_adaptive<0, false, true, LightGroups>, hdri, lg);
+    case 2:  return f(+k_resolve<0, true, false, AovBuffers>, +k_resolve_adaptive<0, true, false, AovBuffers>, hdri, aov);
+    case 3:  return f(+k_resolve<0, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<0, true, true, AovBuffers, LightGroups>, hdri, aov, lg);
+    case 4:  return f(k_resolve<1>, k_resolve_adaptive<1>, atm);
+    case 5:  return f(+k_resolve<1, false, true, LightGroups>, +k_resolve_adaptive<1, false, true, LightGroups>, atm, lg);
+    case 6:  return f(+k_resolve<1, true, false, AovBuffers>, +k_resolve_adaptive<1, true, false, AovBuffers>, atm, aov);
+    case 7:  return f(+k_resolve<1, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<1, true, true, AovBuffers, LightGroups>, atm, aov, lg);
+    case 8:  return f(k_resolve<2>, k_resolve_adaptive<2>, atm);
+    case 9:  return f(+k_resolve<2, false, true, LightGroups>, +k_resolve_adaptive<2, false, true, LightGroups>, atm, lg);
+    case 10: return f(+k_resolve<2, true, false, AovBuffers>, +k_resolve_adaptive<2, true, false, AovBuffers>, atm, aov);
+    case 11: return f(+k_resolve<2, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<2, true, true, AovBuffers, LightGroups>, atm, aov, lg);
+    default: return cudaErrorInvalidValue;
+    }
+}
+
+cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const float* brick_pool,
+                         const int brick_dims[3], int n_ctas, cudaStream_t s)
+{
+    return trace_kernel(k, atm, lg, brick_args(brick_pool, brick_dims), [&](auto kernel, int threads, size_t smem, const auto&... args) {
+        kernel<<<n_ctas, threads, smem, s>>>(fa, args...);
+        return cudaGetLastError();
+    });
+}
+
+// Once per context (= per device): opt the trace kernels into their dynamic shared memory and record how many CTAs of each fit
 // on an SM.  The attribute is a per-device property of the function, so this must not be a process-wide static.
-template <int kInteg, bool kLean, int kSlots>
-static cudaError_t trace_init_t(int* max_ctas)
+cudaError_t trace_kernels_init(int max_ctas[kTraceKernels])
 {
-    cudaError_t e = cudaFuncSetAttribute(k_trace<kInteg, kLean, kSlots>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem_bytes(kSlots));
-    if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(max_ctas, k_trace<kInteg, kLean, kSlots>, kTraceThreads, trace_smem_bytes(kSlots));
+    for (int k = 0; k < kTraceKernels; ++k) {
+        const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, [&](auto kernel, int threads, size_t smem, const auto&...) {
+            const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            return r != cudaSuccess ? r : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[k], kernel, threads, smem);
+        });
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
-
-static size_t brick_smem_bytes() { return (size_t)kBrickThreads * kBrickBytes; }
 
 // Under lazy module loading (the CUDA 12 default) the first launch of a kernel loads it, and loading may wait for the device's running
 // kernels.  With a peer exchange, a rank's k_peer_wait spins until the other ranks' kernels have run, so a first launch on one rank
 // can wait behind that spin until the wait gives up.  The exchange therefore loads every kernel it may issue up front.
 cudaError_t exchange_kernels_preload()
 {
-    const void* fns[] = {
-        (const void*)k_bn_prepare, (const void*)k_bn_advance, (const void*)k_generate, (const void*)k_generate_adaptive,
-        (const void*)k_trace<0, false, 3>, (const void*)k_trace<0, true, 3>, (const void*)k_trace<1, false, 3>,
-        (const void*)k_trace<0, false, 2>, (const void*)k_trace<0, true, 2>, (const void*)k_trace<0, true, 2, true>, (const void*)k_trace_brick,
-        (const void*)k_resolve<0>, (const void*)k_resolve<1>, (const void*)k_resolve<2>,
-        (const void*)k_resolve_adaptive<0>, (const void*)k_resolve_adaptive<1>, (const void*)k_resolve_adaptive<2>,
-        (const void*)k_resolve<0, true, false, AovBuffers>, (const void*)k_resolve<1, true, false, AovBuffers>, (const void*)k_resolve<2, true, false, AovBuffers>,
-        (const void*)k_resolve_adaptive<0, true, false, AovBuffers>, (const void*)k_resolve_adaptive<1, true, false, AovBuffers>,
-        (const void*)k_resolve_adaptive<2, true, false, AovBuffers>,
-        (const void*)k_trace<0, false, 3, false, true, LightGroups>, (const void*)k_trace<1, false, 3, false, true, LightGroups>,
-        (const void*)k_resolve<0, false, true, LightGroups>, (const void*)k_resolve<1, false, true, LightGroups>, (const void*)k_resolve<2, false, true, LightGroups>,
-        (const void*)k_resolve<0, true, true, AovBuffers, LightGroups>, (const void*)k_resolve<1, true, true, AovBuffers, LightGroups>,
-        (const void*)k_resolve<2, true, true, AovBuffers, LightGroups>,
-        (const void*)k_resolve_adaptive<0, false, true, LightGroups>, (const void*)k_resolve_adaptive<1, false, true, LightGroups>,
-        (const void*)k_resolve_adaptive<2, false, true, LightGroups>, (const void*)k_resolve_adaptive<0, true, true, AovBuffers, LightGroups>,
-        (const void*)k_resolve_adaptive<1, true, true, AovBuffers, LightGroups>, (const void*)k_resolve_adaptive<2, true, true, AovBuffers, LightGroups>,
-        (const void*)k_adapt_init, (const void*)k_adapt, (const void*)k_adapt_halo, (const void*)k_adapt_count_publish, (const void*)k_adapt_tally,
-        (const void*)k_adapt_publish, (const void*)k_peer_signal, (const void*)k_peer_wait };
-    for (const void* f : fns) {
-        cudaFuncAttributes a;
-        const cudaError_t e = cudaFuncGetAttributes(&a, f);
+    auto load = [](auto... kernels) {
+        for (const void* f : {(const void*)kernels...}) {
+            cudaFuncAttributes a;
+            const cudaError_t e = cudaFuncGetAttributes(&a, f);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    };
+    for (int k = 0; k < kTraceKernels; ++k) {
+        const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, [&](auto kernel, int, size_t, const auto&...) { return load(kernel); });
         if (e != cudaSuccess) return e;
     }
-    return cudaSuccess;
-}
-
-template <int kInteg>
-static cudaError_t trace_init_groups(int* max_ctas)
-{
-    const void* f = (const void*)k_trace<kInteg, false, 3, false, true, LightGroups>;
-    cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem_bytes(3));
-    if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(max_ctas, f, kTraceThreads, trace_smem_bytes(3));
-}
-
-cudaError_t trace_kernels_init(int max_ctas[9])
-{
-    {
-        cudaError_t e0 = cudaFuncSetAttribute(k_trace<0, true, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem_bytes(2));
-        if (e0 == cudaSuccess) e0 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[6], k_trace<0, true, 2, true>, kTraceThreads, trace_smem_bytes(2));
-        if (e0 != cudaSuccess) return e0;
-    }
-    {
-        cudaError_t e0 = trace_init_groups<0>(&max_ctas[7]);
-        if (e0 == cudaSuccess) e0 = trace_init_groups<1>(&max_ctas[8]);
-        if (e0 != cudaSuccess) return e0;
-    }
-    cudaError_t e = trace_init_t<0, false, 3>(&max_ctas[0]);
-    if (e == cudaSuccess) e = trace_init_t<0, true, 3>(&max_ctas[1]);
-    if (e == cudaSuccess) e = trace_init_t<1, false, 3>(&max_ctas[2]);
-    if (e == cudaSuccess) e = trace_init_t<0, false, 2>(&max_ctas[4]);
-    if (e == cudaSuccess) e = trace_init_t<0, true, 2>(&max_ctas[5]);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_trace_brick, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)brick_smem_bytes());
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[3], k_trace_brick, kBrickThreads, brick_smem_bytes());
-    return e;
+    for (int sky = 0; sky < 3; ++sky)
+        for (bool aov : {false, true})
+            for (bool groups : {false, true}) {
+                const cudaError_t e = resolve_kernels(ResolveKey{sky, aov, groups}, {}, {}, {},
+                                                      [&](auto fixed, auto adaptive, const auto&...) { return load(fixed, adaptive); });
+                if (e != cudaSuccess) return e;
+            }
+    return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
+                k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
 {
-    BrickArgs ba;
-    ba.pool = pool; ba.dimx = dims[0]; ba.dimy = dims[1]; ba.dimz = dims[2];
-    ba.nbx = (dims[0] + 3) / 4; ba.nby = (dims[1] + 3) / 4; ba.nbz = (dims[2] + 3) / 4;
-    k_sampler_compare<<<592, 256, 0, s>>>((cudaTextureObject_t)tex, ba, n, seed, d_out12);
+    k_sampler_compare<<<592, 256, 0, s>>>((cudaTextureObject_t)tex, brick_args(pool, dims), n, seed, d_out12);
     return cudaGetLastError();
 }
 
-cudaError_t launch_trace_brick(const FrameArgs& fa, const float* pool, const int dims[3], int n_ctas, cudaStream_t s)
-{
-    BrickArgs ba;
-    ba.pool = pool; ba.dimx = dims[0]; ba.dimy = dims[1]; ba.dimz = dims[2];
-    ba.nbx = (dims[0] + 3) / 4; ba.nby = (dims[1] + 3) / 4; ba.nbz = (dims[2] + 3) / 4;
-    k_trace_brick<<<n_ctas, kBrickThreads, brick_smem_bytes(), s>>>(fa, ba);
-    return cudaGetLastError();
-}
-
-static bool aov_on(const AovBuffers* aov) { return aov && (aov->alpha || aov->volume); }
-static bool lg_on(const LightGroups* lg) { return lg && (lg->out[0] || lg->out[1] || lg->out[2] || lg->out[3]); }
-
-// the light-group instantiations, with or without the AOVs
-template <int kSky>
-static void launch_resolve_groups(const FrameArgs& fa, const SkyArg<kSky>& atmo, int n_passes, int sampled, int write_display, const PeerFrames& pf,
-                                  const AovBuffers* aov, const LightGroups& lg, int blocks, cudaStream_t s)
-{
-    if (aov_on(aov)) k_resolve<kSky, true, true><<<blocks, 256, 0, s>>>(fa, atmo, n_passes, sampled, write_display, pf, *aov, lg);
-    else             k_resolve<kSky, false, true><<<blocks, 256, 0, s>>>(fa, atmo, n_passes, sampled, write_display, pf, lg);
-}
-
-template <int kSky>
-static void launch_resolve_adaptive_groups(const FrameArgs& fa, const SkyArg<kSky>& atmo, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
-                                           const LightGroups& lg, cudaStream_t s)
-{
-    if (aov_on(aov)) k_resolve_adaptive<kSky, true, true><<<ad.n_tiles, 128, 0, s>>>(fa, atmo, n_passes, ad, *aov, lg);
-    else             k_resolve_adaptive<kSky, false, true><<<ad.n_tiles, 128, 0, s>>>(fa, atmo, n_passes, ad, lg);
-}
-
-cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers,
-                           const AovBuffers* aov, const LightGroups* lg, cudaStream_t s)
+cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
-    if (lg_on(lg)) {
-        if (sky && fa.kp.integrator != 0) launch_resolve_groups<2>(fa, *sky, n_passes, sampled, write_display, pf, aov, *lg, blocks, s);
-        else if (sky)                     launch_resolve_groups<1>(fa, *sky, n_passes, sampled, write_display, pf, aov, *lg, blocks, s);
-        else                              launch_resolve_groups<0>(fa, NoSky{}, n_passes, sampled, write_display, pf, aov, *lg, blocks, s);
-    }
-    else if (aov_on(aov)) {
-        if (sky && fa.kp.integrator != 0) k_resolve<2, true><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf, *aov);
-        else if (sky)                     k_resolve<1, true><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf, *aov);
-        else                              k_resolve<0, true><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf, *aov);
-    }
-    else if (sky && fa.kp.integrator != 0) k_resolve<2><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
-    else if (sky)                          k_resolve<1><<<blocks, threads, 0, s>>>(fa, *sky, n_passes, sampled, write_display, pf);
-    else                                   k_resolve<0><<<blocks, threads, 0, s>>>(fa, NoSky{}, n_passes, sampled, write_display, pf);
-    return cudaGetLastError();
+    return resolve_kernels(key, atm, aov, lg, [&](auto kernel, auto, const auto& sky, const auto&... ext) {
+        kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, ext...);
+        return cudaGetLastError();
+    });
 }
 
-cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
-                                    const LightGroups* lg, cudaStream_t s)
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
+                                    const AovBuffers& aov, const LightGroups& lg, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
-    if (lg_on(lg)) {
-        if (sky && fa.kp.integrator != 0) launch_resolve_adaptive_groups<2>(fa, *sky, n_passes, ad, aov, *lg, s);
-        else if (sky)                     launch_resolve_adaptive_groups<1>(fa, *sky, n_passes, ad, aov, *lg, s);
-        else                              launch_resolve_adaptive_groups<0>(fa, NoSky{}, n_passes, ad, aov, *lg, s);
-    }
-    else if (aov_on(aov)) {
-        if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2, true><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad, *aov);
-        else if (sky)                     k_resolve_adaptive<1, true><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad, *aov);
-        else                              k_resolve_adaptive<0, true><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad, *aov);
-    }
-    else if (sky && fa.kp.integrator != 0) k_resolve_adaptive<2><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
-    else if (sky)                          k_resolve_adaptive<1><<<ad.n_tiles, 128, 0, s>>>(fa, *sky, n_passes, ad);
-    else                                   k_resolve_adaptive<0><<<ad.n_tiles, 128, 0, s>>>(fa, NoSky{}, n_passes, ad);
-    return cudaGetLastError();
+    return resolve_kernels(key, atm, aov, lg, [&](auto, auto kernel, const auto& sky, const auto&... ext) {
+        kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, ext...);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s)

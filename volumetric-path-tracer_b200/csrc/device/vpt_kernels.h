@@ -75,18 +75,33 @@ cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* roo
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
 cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s);
 struct LightGroups;
-// atm != null selects the volumetric path integrator variant of the trace kernel.  lg with planes != null (generic kernels only): the
-// light-group instantiation, at 3 rays per lane whatever `slots` says
-cudaError_t launch_trace(const FrameArgs& fa, const vpt_atmosphere* atm, bool lean, int slots, int n_ctas, const LightGroups* lg, cudaStream_t s);   // slots: rays per lane, 2 or 3; fa.cell_table != null: the lean 2-slot cell-table instantiation
-// per device: dynamic shared memory opt-in of the trace kernels + CTAs per SM of [generic, lean, volumetric path, brick]
-cudaError_t trace_kernels_init(int max_ctas[9]);      // [6]: lean, 2 rays per lane, cell table; [7] / [8]: generic / volumetric path with light groups      // [0..2] generic / lean / volumetric path at 3 rays per lane, [3] k_trace_brick, [4..5] generic / lean at 2 rays per lane
-// fast mode: lean direct integrator reading the density from a brick pool (vpt_trace_brick.cuh); dims = voxels per axis
-cudaError_t launch_trace_brick(const FrameArgs& fa, const float* pool, const int dims[3], int n_ctas, cudaStream_t s);
+// The trace kernels, with their instantiations in trace_kernel (vpt_kernels.cu): generic / lean / volumetric path at 3 rays per lane,
+// k_trace_brick, generic / lean at 2, lean at 2 on the cell table, generic / volumetric path keeping the light-group planes.
+enum TraceKernel : int { TK_GENERIC_3, TK_LEAN_3, TK_VOL_3, TK_BRICK, TK_GENERIC_2, TK_LEAN_2, TK_LEAN_2_CELLS, TK_GENERIC_3_GROUPS,
+                         TK_VOL_3_GROUPS, kTraceKernels };
+// The trace kernel of a frame.  brick / cells: volume 0 is read from a brick pool / a cell table (lean scenes only); vol_integ: the volumetric
+// path integrator; group_planes: a generic kernel keeps the light-group planes; slots: rays per lane, 2 or 3 (the group kernels run 3).
+inline TraceKernel pick_trace_kernel(bool brick, bool cells, bool vol_integ, bool lean, bool group_planes, int slots)
+{
+    if (group_planes) return vol_integ ? TK_VOL_3_GROUPS : TK_GENERIC_3_GROUPS;
+    if (brick) return TK_BRICK;
+    if (cells) return TK_LEAN_2_CELLS;
+    if (vol_integ) return TK_VOL_3;
+    if (slots == 2) return lean ? TK_LEAN_2 : TK_GENERIC_2;
+    return lean ? TK_LEAN_3 : TK_GENERIC_3;
+}
+// default of option "sched_min_lanes": lanes an operation must gather before it pre-empts stepping (26 helps only the lean kernel at 3)
+inline int trace_sched_min_lanes(TraceKernel k) { return k == TK_LEAN_3 ? 26 : 20; }
+// per device: dynamic shared memory opt-in of every trace kernel, and how many CTAs of each fit on an SM
+cudaError_t trace_kernels_init(int max_ctas[kTraceKernels]);
+// kernel k on n_ctas persistent CTAs.  atm: the caller's AtmosphereParameters (volumetric path kernels); lg: the light groups (group
+// kernels); brick_pool / brick_dims: the brick pool of volume 0 and its voxels per axis (k_trace_brick)
+cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const float* brick_pool,
+                         const int brick_dims[3], int n_ctas, cudaStream_t s);
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s);
 cudaError_t launch_fill_perlin(float* d_buffer, int dx, int dy, int dz, float scale, int seed, cudaStream_t s);
 cudaError_t launch_build_bricks(const float* d_dense, int dx, int dy, int dz, float* d_bricks, cudaStream_t s);
 cudaError_t launch_build_cells(const float* d_dense, int dx, int dy, int dz, float4* d_cells, cudaStream_t s);
-// sky != null selects the environment_type == 0 variant (host copy of the caller's AtmosphereParameters)
 // Peer-memory exchange (multi-GPU, csrc/host/vpt_comm.cpp): the call's LAST resolve kernel stores every finished pixel straight into the
 // full-frame buffer of every rank (its own included) at the pixel's global position, over NVLink peer mappings -- the all-gather and
 // the stripe un-permutation fused into the kernel that produces the values.
@@ -103,8 +118,11 @@ struct AovBuffers { float* alpha = nullptr; float3* volume = nullptr; };
 // instantiations of k_trace / k_resolve / k_resolve_adaptive only, as AovBuffers is.
 enum LightGroup : int { LG_SUN = 0, LG_POINT = 1, LG_EMISSION = 2, LG_ENVIRONMENT = 3, kLightGroups = 4 };
 struct LightGroups { float3* out[kLightGroups] = {}; float* planes = nullptr; unsigned long long stride = 0; };
-cudaError_t launch_resolve(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, int sampled, int write_display, const PeerFrames* peers,
-                           const AovBuffers* aov, const LightGroups* lg, cudaStream_t s);
+// Which k_resolve / k_resolve_adaptive a frame runs (instantiations: resolve_kernels in vpt_kernels.cu).  sky: 0 HDRI, 1 the precomputed
+// sky, 2 the volumetric path integrator (ends on that sky; atm: the caller's AtmosphereParameters); with the AOVs; with the light groups.
+struct ResolveKey { int sky = 0; bool aov = false, groups = false; };
+cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -120,8 +138,8 @@ cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& 
 // adaptive frame: k_generate / k_resolve over the tiles of ad.tiles only (stopped pixels sample nothing and keep their buffers); the resolve
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s);
-cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const vpt_atmosphere* sky, int n_passes, const AdaptArgs& ad, const AovBuffers* aov,
-                                    const LightGroups* lg, cudaStream_t s);
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
+                                    const AovBuffers& aov, const LightGroups& lg, cudaStream_t s);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);

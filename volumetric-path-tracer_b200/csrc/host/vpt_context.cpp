@@ -220,9 +220,9 @@ namespace {
 struct FramePlan {
     vpt::FrameArgs fa;
     vpt_atmosphere atmo;                  // the caller's AtmosphereParameters
-    const vpt_atmosphere* sky = nullptr;  // &atmo when the frame ends on the precomputed sky (environment_type == 0 or integrator != 0)
-    bool vol_integ = false, lean = false;
-    int trace_ctas = 0, slots = 3, chunk = 1, bn_limit = 0;
+    vpt::TraceKernel trace = vpt::TK_GENERIC_3;
+    vpt::ResolveKey resolve;
+    int trace_ctas = 0, chunk = 1, bn_limit = 0;
     unsigned n_sampled = 0;               // how many of the requested passes sample (the rest only re-tonemap)
     vpt::AovBuffers aov;                  // the active compositing AOVs (both null: off)
     vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
@@ -311,7 +311,6 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         return fail(c, VPT_ERR_INVALID, "integrator != 0 with environment_type == 0 needs the env sampling tables (env_*_tex, env_sample_tex_res) in Kernel_params");
     if (vol_integ && samples && kp.environment_type != 0 && !kp.env_tex)
         return fail(c, VPT_ERR_INVALID, "environment_type != 0 needs Kernel_params.env_tex");
-    plan.sky = sky_env ? &atmo : nullptr;
     if (!d_volumes || !d_sphere || !d_root) return fail(c, VPT_ERR_INVALID, "volumes / sphere / octree device pointer is null");
     if (!kp.accum_buffer || !kp.depth_buffer || !kp.cost_buffer || !kp.display_buffer || !kp.raw_buffer || !kp.blue_noise_buffer)
         return fail(c, VPT_ERR_INVALID, "Kernel_params output buffer pointer is null");
@@ -421,7 +420,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         c->cap_chunk = chunk;
     }
     fa.queue_dir = c->d_queue; fa.queue_id = c->d_queue_id; fa.queue_aux = c->d_queue_org; fa.thin_lens = (fa.cam.lens_radius != 0.0f) ? 1 : 0;
-    fa.bn_table = c->d_bn_table; fa.debug_flags = c->debug_flags;     // fa.sched_min_lanes: set below, once the trace kernel is chosen
+    fa.bn_table = c->d_bn_table; fa.debug_flags = c->debug_flags;
     fa.queue_count = c->d_counters; fa.queue_head = c->d_counters + 1;
     fa.planeA = c->d_planeA;
     fa.planeB = wide ? c->d_planeB : nullptr; fa.planeC = wide ? c->d_planeC : nullptr; fa.planeD = planeD ? c->d_planeD : nullptr;
@@ -439,17 +438,15 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
             if (vpt::scene_registry_find(d_root, &ent) && (ent.max_grid_bytes > 2ull * c->l2_bytes || ent.n >= 64)) slots = 2;
         }
     }
-    // lanes an operation must gather before it pre-empts stepping, chosen per kernel (26 helps only the lean kernel at 3 rays per lane)
-    fa.sched_min_lanes = c->sched_min_lanes > 0 ? c->sched_min_lanes : ((lean && slots == 3 && !vol_integ && !c->brick_pool && !c->cell_table) ? 26 : 20);
-    if (group_planes) slots = 3;         // the light-group instantiations of the generic kernels run 3 rays per lane
-    int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm
-                    : c->max_ctas[group_planes ? (vol_integ ? 8 : 7) : c->brick_pool ? 3 : c->cell_table ? 6 : vol_integ ? 2 : (slots == 2 ? (lean ? 5 : 4) : (lean ? 1 : 0))];
+    const vpt::TraceKernel trace = vpt::pick_trace_kernel(c->brick_pool != nullptr, c->cell_table != nullptr, vol_integ, lean, group_planes, slots);
+    fa.sched_min_lanes = c->sched_min_lanes > 0 ? c->sched_min_lanes : vpt::trace_sched_min_lanes(trace);
+    int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm : c->max_ctas[trace];
     if (ctas_per_sm < 1) ctas_per_sm = 1;
 
     fa.counters = c->count_stats ? c->d_stats : nullptr;
     fa.cell_table = c->cell_table; fa.cell_nx = c->cell_dims[0]; fa.cell_ny = c->cell_dims[1]; fa.cell_nz = c->cell_dims[2];
     const unsigned long long frame_px = (unsigned long long)kp.resolution.x * kp.resolution.y;
-    plan.vol_integ = vol_integ; plan.lean = lean; plan.slots = slots; plan.trace_ctas = c->num_sms * ctas_per_sm;
+    plan.trace = trace; plan.trace_ctas = c->num_sms * ctas_per_sm;
     plan.chunk = chunk; plan.n_sampled = n_sampled;
     plan.bn_limit = frame_px < 65536ull ? (int)frame_px : 65536;
 
@@ -465,15 +462,17 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         for (int k = 0; k < 4; ++k) plan.lg.out[k] = reinterpret_cast<float3*>(c->lg_out[k]);
         if (group_planes) { plan.lg.planes = c->d_lg_planes; plan.lg.stride = (unsigned long long)c->cap_lg_samples; }
     }
+    plan.resolve.sky = sky_env ? (vol_integ ? 2 : 1) : 0;
+    plan.resolve.aov = plan.aov.alpha || plan.aov.volume;
+    plan.resolve.groups = plan.lg.out[0] || plan.lg.out[1] || plan.lg.out[2] || plan.lg.out[3];
     return VPT_OK;
 }
 
-// k_trace (or k_trace_brick in brick mode) over whatever k_generate queued for a chunk of np passes
+// the frame's trace kernel over whatever k_generate queued for a chunk of np passes
 static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, unsigned np, cudaStream_t stream) {
     vpt::FrameArgs fa = plan.fa;
     fa.n_passes = (int)np;
-    if (c->brick_pool) return vpt::launch_trace_brick(fa, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
-    return vpt::launch_trace(fa, plan.vol_integ ? &plan.atmo : nullptr, plan.lean, plan.slots, plan.trace_ctas, &plan.lg, stream);
+    return vpt::launch_trace(fa, plan.trace, plan.atmo, plan.lg, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
 }
 
 extern "C" {
@@ -516,7 +515,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.sky, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, &plan.aov, &plan.lg, stream); }));
+        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, stream); }));
         c->launches += 4;
         done += np;
     }
@@ -526,7 +525,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, vpt::launch_resolve(fa, plan.sky, (int)(n_passes - n_sampled), 0, 1, &peers, &plan.aov, &plan.lg, stream));
+        VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2;
     }
@@ -641,7 +640,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.sky, (int)np, ad, &plan.aov, &plan.lg, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, stream); }));
             c->launches += 3;
         }
         done += np;

@@ -24,7 +24,7 @@ struct vpt_context {
     bool   scene_single_volume = false;
     size_t cap_vrec = 0;              // VolumeRec capacity (grows with the instance count)
     int*   h_pinned = nullptr;        // eight pinned words: the read-back a foreign octree needs, the tile counts of an adaptive test
-    int    max_ctas[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // trace kernel occupancy: [0] generic, [1] lean, [2] volumetric path, [3] brick mode, [4] generic / [5] lean at 2 rays per lane, [6] lean + cell table, [7] generic / [8] volumetric path with light groups
+    int    max_ctas[vpt::kTraceKernels] = {};   // trace kernel occupancy (CTAs per SM), by vpt::TraceKernel
     size_t l2_fetch_default = 0; int l2_sector_fetch = 0;     // option "l2_sector_fetch" (cell mode)
     const float4* cell_table = nullptr; int cell_dims[3] = {0, 0, 0};   // vpt_set_cell_volume
     int    trace_slots = 0;              // option "trace_slots": rays per lane of k_trace, 0 = by grid size (2 when the grid is larger than twice the L2)
