@@ -174,7 +174,7 @@ int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], uns
  *       alpha   sample: c ? 1 : 0.
  *       volume  sample (float3): the sample exactly as it enters accum (after the NaN / Inf guard and the viz_dof tint) if c, +0 otherwise
  *               (a select, not a product).  When the guard replaced the sample, the volume sample is the volume AOV's own mean so far,
- *               as the guard uses accum's.
+ *               as the guard uses accum's (at iteration 0: the buffer's previous content, as for accum).  Alpha is not guarded.
  *     Both follow accum's rule and arithmetic: iteration == 0 assigns, iteration < max_interactions updates x + (s - x) / (iteration + 1),
  *     later passes change nothing.  So per sample, beauty = volume + the transmitted background, and alpha estimates 1 - transmittance
  *     along the camera ray under the reference's tracker; over a new plate P the frame is  volume + (1 - alpha) * P.
@@ -202,7 +202,7 @@ int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
  *     emission, the end-of-path sky to environment.  A miss sample is all environment; a pass that samples nothing (render == 0) gives its
  *     WHITE to the environment and 0 to the others.  Each group follows accum's rule and arithmetic (iteration == 0 assigns,
  *     iteration < max_interactions updates x + (s - x) / (iteration + 1)); a sample the NaN / Inf guard replaced leaves every group at its
- *     own mean.  Groups are taken before the viz_dof tint.  So per sample sun + point + emission + environment = the beauty sample up to
+ *     own mean (at iteration 0: the buffer's previous content, as accum takes accum_buffer's).  Groups are taken before the viz_dof tint.  So per sample sun + point + emission + environment = the beauty sample up to
  *     the rounding of the separate sums, and with the direct integrator each group is bit for bit the accum of a render in which only that
  *     class is lit (the path's draws do not depend on light intensities there).
  *   Buffers.  Caller-owned device memory, float3, vpt_local_pixels() entries each (rank-local order on a partitioned context).  Any may be

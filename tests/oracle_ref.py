@@ -3,7 +3,7 @@ blue-noise update, compiled from the reference tree by oracle/Makefile into orac
 
 Where oracle/_ref is not built, the oracle REPLAYS the outputs stored under tests/golden/oracle/ for the same test and call,
 after checking that a hash of the inputs matches.  To store them: run the tests with the oracle built and VPT_ORACLE_RECORD=<dir>,
-then `python tests/oracle_ref.py <dir>`.  What has no stored output (or did not fit in 1 MB) skips without the oracle.
+then `python tests/oracle_ref.py <dir> [first pack number]`.  What has no stored output (or did not fit in 1 MB) skips without the oracle.
 
 Only tests/, __graft_entry__.smoke() and bench.py's reference arm may import this module.
 """
@@ -135,8 +135,9 @@ class _NoLibrary:
         pytest.skip(f"oracle/_ref not built: {name} has no stored output")
 
 
-def pack(record_dir, out_dir=GOLDEN_DIR, limit=990_000):
-    """Pack the per-array files of a recording run (<key>.<name>.npz) into as few files below 1 MB as the array sizes allow."""
+def pack(record_dir, out_dir=GOLDEN_DIR, limit=990_000, first=0):
+    """Pack the per-array files of a recording run (<key>.<name>.npz) into as few files below 1 MB as the array sizes allow, numbered
+    from pack<first>: a run that recorded only some tests packs them after the existing packs."""
     files = sorted(os.listdir(record_dir))
     os.makedirs(out_dir, exist_ok=True)
     groups, cur, size = [], [], 0
@@ -148,7 +149,7 @@ def pack(record_dir, out_dir=GOLDEN_DIR, limit=990_000):
     if cur: groups.append(cur)
     for i, g in enumerate(groups):
         arrays = {f[:-len(".npz")]: np.load(os.path.join(record_dir, f))["a"] for f in g}
-        path = os.path.join(out_dir, f"pack{i:02d}.npz")
+        path = os.path.join(out_dir, f"pack{first + i:02d}.npz")
         np.savez_compressed(path, **arrays)
         assert os.path.getsize(path) <= MAX_FILE_BYTES, path
 
@@ -354,21 +355,27 @@ class RefOracle:
         rc = self.lib.vptref_bn_advance(C.cast(C.byref(kp), C.c_void_p), 1 if sync else 0, min(int(kp.resolution.x) * int(kp.resolution.y), 65536))
         if rc: raise RuntimeError(f"vptref_bn_advance -> {rc}")
 
-    def render(self, renderer, n_passes, race_free=True):
+    def render(self, renderer, n_passes, race_free=True, full=False):
         """Run n reference passes on `renderer`'s parameter block and buffers (race-free protocol: the
         'nobn' build + the reference's own blue-noise statements as a separate launch, SURVEY 8(c)).
         Replaying: accum, depth, display, the transmittance channel of raw and the blue-noise entries the passes changed
-        come from the stored output; the colour channels of raw, which no test compares with the oracle's, are left at zero."""
+        come from the stored output; the colour channels of raw, which no test compares with the oracle's, are left at zero.
+        full=True (for calls that start from non-zero buffers): the starting contents of accum, depth and cost are part of the
+        inputs' hash, and cost and all four channels of raw are stored and replayed too."""
         key = _key("render")
+        b = renderer.buffers
+        start = (b.accum.cpu().numpy().tobytes(), b.depth.cpu().numpy().tobytes(), b.cost.cpu().numpy().tobytes()) if full else ()
         digest = _digest(bytes(renderer.cam), _kp_scalars(renderer.kp), renderer.width, renderer.height, int(n_passes), bool(race_free),
-                         _volumes_digest(renderer.scene.h_volumes, len(renderer.scene.instances)))
+                         _volumes_digest(renderer.scene.h_volumes, len(renderer.scene.instances)), *start)
         bn = renderer.scene.d_blue_noise
         if self.replay:
             z = _load(key, digest)
-            b = renderer.buffers
             b.accum.copy_(torch.from_numpy(z["accum"])); b.depth.copy_(torch.from_numpy(z["depth"]))
             b.display.copy_(torch.from_numpy(z["display"]))
-            b.raw.zero_(); b.raw[:, 3].copy_(torch.from_numpy(z["raw_w"]))
+            if full:
+                b.cost.copy_(torch.from_numpy(z["cost"])); b.raw.copy_(torch.from_numpy(z["raw"]))
+            else:
+                b.raw.zero_(); b.raw[:, 3].copy_(torch.from_numpy(z["raw_w"]))
             flat = bn.view(bn.shape[0], -1)
             flat[torch.from_numpy(z["bn_index"]).long().to(bn.device)] = torch.from_numpy(z["bn_value"]).to(bn.device)
             renderer.kp.iteration += int(n_passes)
@@ -384,14 +391,15 @@ class RefOracle:
             renderer.kp.iteration += 1
         torch.cuda.synchronize()
         if RECORD_DIR:
-            b = renderer.buffers
             flat, flat0 = bn.view(bn.shape[0], -1), bn0.view(bn0.shape[0], -1)
             changed = torch.nonzero((flat != flat0).any(dim=1)).flatten()
-            _store(key, dict(digest=np.array(digest), accum=b.accum.cpu().numpy(), depth=b.depth.cpu().numpy(), display=b.display.cpu().numpy(),
-                             raw_w=b.raw[:, 3].contiguous().cpu().numpy(), bn_index=changed.cpu().numpy().astype(np.int32),
-                             bn_value=flat[changed].cpu().numpy()))
+            out = dict(digest=np.array(digest), accum=b.accum.cpu().numpy(), depth=b.depth.cpu().numpy(), display=b.display.cpu().numpy(),
+                       bn_index=changed.cpu().numpy().astype(np.int32), bn_value=flat[changed].cpu().numpy())
+            if full: out.update(cost=b.cost.cpu().numpy(), raw=b.raw.cpu().numpy())
+            else: out.update(raw_w=b.raw[:, 3].contiguous().cpu().numpy())
+            _store(key, out)
 
 
 if __name__ == "__main__":
     import sys
-    pack(sys.argv[1])
+    pack(sys.argv[1], first=int(sys.argv[2]) if len(sys.argv) > 2 else 0)

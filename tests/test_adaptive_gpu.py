@@ -53,6 +53,7 @@ CASES = {
     "lights_sphere": (256, 160, 32, 8, 8, 0.08),
     "instanced":     (256, 144, 32, 8, 8, 0.12),
     "brick":         (320, 200, 32, 8, 8, 0.2),
+    "nan_prefilled": (256, 160, 32, 8, 8, 0.1),
 }
 
 
@@ -85,6 +86,15 @@ def make_case(name, dragon, perlin):
         scene = V.Scene(_instances(dragon), env=env)
         cam = scene.frame_camera(W, H)
         return scene, (lambda: V.Renderer(scene, W, H, kp=make_kp(ray_depth=2), cam=cam)), []
+    if name == "nan_prefilled":                                  # NaN / +Inf environment stripes, a frame started on prefilled buffers
+        from test_resolve_tail_gpu import prefill, striped_env
+        scene = V.Scene([dragon.instance()], env=striped_env())
+        cam = scene.frame_camera(W, H)
+        def mk():
+            r = V.Renderer(scene, W, H, kp=make_kp(ray_depth=4), cam=cam)
+            r.prefill = lambda: prefill(r.buffers, 31)
+            return r
+        return scene, mk, []
     if name == "brick":                                          # brick mode on the procedural grid
         scene = V.Scene([perlin.instance()], env=env, keep=[perlin])
         cam = scene.frame_camera(W, H)
@@ -96,8 +106,14 @@ def make_case(name, dragon, perlin):
     raise KeyError(name)
 
 
-def adaptive_frame(scene, r, max_passes, min_passes, interval, thr, error_map=False):
+def restart(scene, r):
+    """A new frame: iteration 0, the initial blue noise, and zeroed buffers or the case's prefilled ones."""
     scene.reset_blue_noise(); r.kp.iteration = 0; r.buffers.zero_()
+    if hasattr(r, "prefill"): r.prefill()
+
+
+def adaptive_frame(scene, r, max_passes, min_passes, interval, thr, error_map=False):
+    restart(scene, r)
     out = r.render_adaptive(max_passes, threshold=thr, min_passes=min_passes, check_interval=interval, error_map=error_map)
     torch.cuda.synchronize()
     return out
@@ -111,7 +127,7 @@ def assert_matches_fixed_frames(scene, r, f, counts, run):
     classes = [int(c) for c in torch.unique(flat).tolist()]
     assert run == max(classes)
     for c in classes:
-        f.reset(); f.render(c); torch.cuda.synchronize()
+        restart(scene, f); f.render(c); torch.cuda.synchronize()
         m = flat == c
         for k in BUFFERS:
             assert torch.equal(bufs[k][m], getattr(f.buffers, k)[m]), f"{k} differs on the {int(m.sum())} pixels of {c} passes"

@@ -364,3 +364,42 @@ def test_guarded_samples_leave_every_group_at_its_mean(dragon):
     assert int(dark.sum()) > 0, "no pixel sees only the NaN region"
     for g in GROUPS:
         assert bool((on[g][dark] == 0).all()), g
+
+
+def test_guarded_samples_leave_every_group_at_its_mean_from_prefilled_buffers(dragon):
+    """(9) as above, from prefilled buffers whose groups sum to accum exactly: a sample the guard replaces at iteration 0 takes every
+    buffer's previous content (accum, each group, the volume AOV), so pixels that only ever see the NaN / +Inf region keep the prefill of
+    all of them bit for bit, and the groups still sum to the beauty."""
+    from test_resolve_tail_gpu import prefill, striped_env
+    scene = V.Scene([dragon.instance()], env=striped_env())
+    cam = scene.frame_camera(240, 160)
+    mk = lambda: V.Renderer(scene, 240, 160, kp=make_kp(ray_depth=4), cam=cam)
+    rng = np.random.RandomState(37)
+    n = 240 * 160
+    parts = {g: torch.from_numpy(rng.randint(0, 1024, (n, 3)).astype(np.float32) / 1024).cuda() for g in GROUPS}
+    volume0 = torch.from_numpy(rng.randint(0, 1024, (n, 3)).astype(np.float32) / 1024).cuda()
+
+    def fill(r):
+        prefill(r.buffers, 37)
+        r.buffers.accum.copy_(sum(parts[g] for g in GROUPS))            # sums of multiples of 1/1024 below 4: exact
+        if r.buffers.groups is not None:
+            for g in GROUPS: r.buffers.groups[g].copy_(parts[g])
+        if r.buffers.volume is not None: r.buffers.volume.copy_(volume0)
+
+    def run(r):
+        scene.reset_blue_noise(); r.kp.iteration = 0; fill(r)
+        r.render(PASSES); torch.cuda.synchronize()
+        return r
+    off = run(mk())
+    r = mk(); r.enable_aovs(); r.enable_light_groups()
+    on = run(r)
+    assert bitwise(on.buffers.accum, off.buffers.accum)
+    out = {"accum": on.buffers.accum, **on.buffers.groups}
+    for g in GROUPS:
+        assert bool(torch.isfinite(out[g]).all()), g
+    assert_sum_is_the_beauty(out, "NaN / +Inf environment from prefilled buffers")
+    kept = (on.buffers.accum == sum(parts[g] for g in GROUPS)).all(dim=1)
+    assert int(kept.sum()) > 0, "no pixel sees only the non-finite region"
+    for g in GROUPS:
+        assert bitwise(out[g][kept], parts[g][kept]), g
+    assert bitwise(on.buffers.volume[kept], volume0[kept])

@@ -372,10 +372,21 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             tr = fminf(tr, 1.0f);
             value = L;
         }
-        // NaN / Inf guard (:2263-2264)
+        // NaN / Inf guard (:2263-2264): the sample becomes accum_buffer[idx].  At iteration 0 (the call's first pass) that is the buffer's
+        // previous content, which was not loaded; the AOVs and groups take their own buffers' previous content likewise.
         bool guarded = false;                                   // AOVs / groups only, apart from the guard: the other instantiations keep their code
         if constexpr (kAov || kGroups) guarded = any_nan(value) || any_inf(value);
-        if (any_nan(value) || any_inf(value)) value = accum;
+        if (any_nan(value) || any_inf(value)) {
+            if (iteration == 0) {
+                accum = accum_buf[lp];
+                if constexpr (kAov) { if (aov->volume) volv = aov->volume[lp]; }
+                if constexpr (kGroups) {
+                    #pragma unroll
+                    for (int k = 0; k < kLightGroups; ++k) if (lg->out[k]) gm[k] = lg->out[k][lp];
+                }
+            }
+            value = accum;
+        }
         if (isnan(tr) || isinf(tr)) tr = 1.0f;
 
         float aof = 1 / cam.lens_radius;

@@ -61,7 +61,7 @@ VPT_DEV void resolve_pixel(const FrameArgs& fa, const vpt_atmosphere& atmo, uint
         tr = fminf(tr, 1.0f);
         value = L;
     }
-    if (any_nan(value) || any_inf(value)) value = accum;
+    if (any_nan(value) || any_inf(value)) value = accum_buf[idx];          // at iteration 0 the previous content, which was not loaded
     if (isnan(tr) || isinf(tr)) tr = 1.0f;
 
     float aof = 1 / cam.lens_radius;
