@@ -15,6 +15,13 @@ constexpr uint32_t kMissSentinel = 0xffffffffu;   // planeA.w bit pattern markin
 
 __device__ __forceinline__ const vpt_octnode* oct_ptr(vpt_devptr_t p) { return reinterpret_cast<const vpt_octnode*>(p); }
 
+// one pass's advance of a blue-noise entry (reference :2320-2325): += golden ratio, mod 1, on all three channels
+VPT_DEV void bn_step(float3& v)
+{
+    v.x += (1.0f + sqrtf(5.0f)) / 2.0f; v.y += (1.0f + sqrtf(5.0f)) / 2.0f; v.z += (1.0f + sqrtf(5.0f)) / 2.0f;
+    v.x = fmodf(v.x, 1.0f); v.y = fmodf(v.y, 1.0f); v.z = fmodf(v.z, 1.0f);
+}
+
 // per-volume world->index affine, evaluated with the reference's own adjugate formula order
 __device__ VolumeRec make_volume_rec(const vpt_gpu_vdb& g)
 {
@@ -110,10 +117,9 @@ VPT_DEV uint32_t ray_local_pixel(const FrameGeom& g, uint32_t w) {
     return (w >> 16) * (uint32_t)g.width + (w & 0xffffu);
 }
 
-// radical inverse of int(xi*100) in `BASE` (reference vanDerCorput, gpu_vdb/camera.h:49-62)
+// radical inverse of n in `BASE` (reference vanDerCorput, gpu_vdb/camera.h:49-62)
 template <int BASE>
-VPT_DEV float van_der_corput(Rng& rng) {
-    int n = int(rng.next() * 100);
+VPT_DEV float radical_inverse(int n) {
     float rand_int = 0, denom = 1, invBase = 1.f / BASE;
     while (n) {
         denom *= BASE;
@@ -123,23 +129,12 @@ VPT_DEV float van_der_corput(Rng& rng) {
     return rand_int;
 }
 
-// Radiance of a finished sample under the HDRI environment (reference :1838-1850): L + env(dir) * sky_color * beta / (4 pi).  A lean
-// k_trace finishes its rays with it, k_resolve<0> its misses (L = 0, beta = 1) and the hits of wide records.  nvcc contracts this
-// expression per call site, so the order is pinned to the one the end-of-path site compiles to: u = fma(atan2, 1/(2 pi), 0.5),
-// v = acos * 1/pi, L + ((env * sky) * beta) / (4 pi) as one fma.  Every caller then gives the same bits.
-VPT_DEV float3 hdri_radiance(const cudaTextureObject_t env, const float3 sky_color, const float3 dir, const float3 L, const float3 beta)
-{
-    const float4 e = tex2D<float4>(env,
-        pfma(atan2f(dir.z, dir.x), (float)(0.5 / 3.14159265358979323846), 0.5f),
-        pmul(acosf(fmaxf(fminf(dir.y, 1.0f), -1.0f)), (float)(1.0 / 3.14159265358979323846)));
-    const float c = 1.0f / (4.0f * VPT_PI_F);                   // isotropic() returns the folded constant
-    return f3(pfma(pmul(pmul(e.x, sky_color.x), beta.x), c, L.x),
-              pfma(pmul(pmul(e.y, sky_color.y), beta.y), c, L.y),
-              pfma(pmul(pmul(e.z, sky_color.z), beta.z), c, L.z));
-}
+// the lens sampler only ever asks for the radical inverse of int(xi * 100)
+template <int BASE>
+VPT_DEV float van_der_corput(Rng& rng) { return radical_inverse<BASE>(int(rng.next() * 100)); }
 
-// hdri_radiance split after its look-up: the product (env * sky) * beta, which pfma(t, 1 / (4 pi), L) turns into hdri_radiance(.., L, beta)
-// bit for bit.  For callers that need the environment term with two values of L (the light groups: the beauty's L and 0) from one fetch.
+// The HDRI environment term (reference :1838-1850), in two halves so that the light groups can add it to two values of L (the beauty's
+// L and 0) from one fetch: hdri_product = (env(dir) * sky_color) * beta, hdri_finish = L + product / (4 pi) as one fma.
 VPT_DEV float3 hdri_product(const cudaTextureObject_t env, const float3 sky_color, const float3 dir, const float3 beta)
 {
     const float4 e = tex2D<float4>(env,
@@ -149,8 +144,17 @@ VPT_DEV float3 hdri_product(const cudaTextureObject_t env, const float3 sky_colo
 }
 VPT_DEV float3 hdri_finish(const float3 t, const float3 L)
 {
-    const float c = 1.0f / (4.0f * VPT_PI_F);
+    const float c = 1.0f / (4.0f * VPT_PI_F);                   // isotropic() returns the folded constant
     return f3(pfma(t.x, c, L.x), pfma(t.y, c, L.y), pfma(t.z, c, L.z));
+}
+
+// Radiance of a finished sample under the HDRI environment: L + env(dir) * sky_color * beta / (4 pi).  A lean k_trace finishes its rays
+// with it, k_resolve<0> its misses (L = 0, beta = 1) and the hits of wide records.  nvcc contracts this expression per call site, so the
+// order is pinned to the one the end-of-path site compiles to: u = fma(atan2, 1/(2 pi), 0.5), v = acos * 1/pi, L + ((env * sky) * beta) /
+// (4 pi) as one fma.  Every caller then gives the same bits.
+VPT_DEV float3 hdri_radiance(const cudaTextureObject_t env, const float3 sky_color, const float3 dir, const float3 L, const float3 beta)
+{
+    return hdri_finish(hdri_product(env, sky_color, dir, beta), L);
 }
 
 #include "vpt_texfilter.cuh"

@@ -108,7 +108,8 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
 {
     __shared__ FrameShared fs;
     __shared__ float vdc2[101], vdc3[101];                     // radical inverses of 0..100 in bases 2 and 3
-    // the lens sampler only ever asks for vanDerCorput(int(xi * 100)): tabulate it with the reference's own loop
+    // the lens sampler only ever asks for vanDerCorput(int(xi * 100)): tabulate it with the reference's own loop -- radical_inverse
+    // (vpt_frame.cuh) written out, because calling it here moves the machine code of k_generate_adaptive
     if (threadIdx.x < 101) {
         { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 2; while (n) { denom *= 2; r = padd(r, __fdividef((float)(n % 2), denom)); n *= inv; } vdc2[threadIdx.x] = r; }
         { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 3; while (n) { denom *= 3; r = padd(r, __fdividef((float)(n % 3), denom)); n *= inv; } vdc3[threadIdx.x] = r; }
@@ -685,8 +686,7 @@ __global__ void k_bn_prepare(float3* bn, float2* table, int np, int limit, unsig
     }
     for (int i = 0; i < np; ++i) {
         table[(size_t)i * 65536 + idx] = make_float2(val.x, val.y);
-        val.x += (1.0f + sqrtf(5.0f)) / 2.0f; val.y += (1.0f + sqrtf(5.0f)) / 2.0f; val.z += (1.0f + sqrtf(5.0f)) / 2.0f;
-        val.x = fmodf(val.x, 1.0f); val.y = fmodf(val.y, 1.0f); val.z = fmodf(val.z, 1.0f);
+        bn_step(val);
     }
     bn[idx] = val;
 }
@@ -696,10 +696,7 @@ __global__ void k_bn_advance(float3* bn, int n, int limit)
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= 256 * 256 || idx >= limit) return;
     float3 val = bn[idx];
-    for (int i = 0; i < n; ++i) {
-        val.x += (1.0f + sqrtf(5.0f)) / 2.0f; val.y += (1.0f + sqrtf(5.0f)) / 2.0f; val.z += (1.0f + sqrtf(5.0f)) / 2.0f;
-        val.x = fmodf(val.x, 1.0f); val.y = fmodf(val.y, 1.0f); val.z = fmodf(val.z, 1.0f);
-    }
+    for (int i = 0; i < n; ++i) bn_step(val);
     bn[idx] = val;
 }
 

@@ -116,11 +116,7 @@ volume_rt_kernel(const vpt_camera cam, const vpt_light_list lights, const vpt_gp
         fa.counters = nullptr; fa.cell_table = nullptr; fa.cell_nx = fa.cell_ny = fa.cell_nz = 0;
         sh.fs.vol0 = make_volume_rec(gpu_vdb[0]);
         sh.sph = load_sphere(&sphere);
-        sh.tc.inv_max = 1.0f / sc.max_extinction;
-        sh.tc.inv_mult = 1.0f / kp.density_mult;
-        sh.tc.sigma_c = sc.min_extinction;
-        sh.tc.sigma_r_inv = 1.0f / (sc.max_extinction - sh.tc.sigma_c);
-        sh.tc.sun_dir = sun_direction(kp.azimuth, kp.elevation);
+        sh.tc = make_trace_consts(sc, kp);
     }
     // internal nodes (root, 8, 64) from the pointer-linked tree, as k_prepare_scene flattens them
     for (int j = tid; j < kOctInternalNodes; j += nthreads) {
@@ -198,11 +194,7 @@ volume_rt_kernel(const vpt_camera cam, const vpt_light_list lights, const vpt_gp
                             psub(psub(pfma(cam.vertical.y, v, pfma(cam.horizontal.y, u, cam.lower_left_corner.y)), cam.origin.y), offset.y),
                             psub(psub(pfma(cam.vertical.z, v, pfma(cam.horizontal.z, u, cam.lower_left_corner.z)), cam.origin.z), offset.z));
         st.dir = normalize(b);
-        st.pos = st.org;
-        st.beta = f3(1.0f); st.L = f3(.0f); st.alpha = .0f; st.depth = .0f;
-        st.wpos = st.pos; st.wdir = st.dir; st.aux = f3(0.f); st.t = 0.f; st.distance = 0.f; st.trv = 1.f; st.T_c = 1.f;
-        st.mi = false; st.first_walk = true; st.sphere_bounced = false; st.rd = 1; st.vd = 1; st.light_budget = 0; st.light_index = 0;
-        st.mode = W_DELTA; st.exit_reason = EX_NONE; st.tr_kind = TR_SUN; st.sphere_free = false;
+        reset_path(st);
         st.obj_c = closest_object(sc, sph, st.pos, st.dir, st.tmin_c);
         st.have_closest = true;
         hit = st.obj_c != 0;
@@ -260,8 +252,7 @@ volume_rt_kernel(const vpt_camera cam, const vpt_light_list lights, const vpt_gp
         for (int i = tid; i < 256 * 256; i += nthreads) {
             if ((unsigned)i >= (unsigned)(W * H)) continue;            // the reference updates entry idx only for pixels that exist (idx < 65536 threads)
             float3 val = bn[i];
-            val.x += (1.0f + sqrtf(5.0f)) / 2.0f; val.y += (1.0f + sqrtf(5.0f)) / 2.0f; val.z += (1.0f + sqrtf(5.0f)) / 2.0f;
-            val.x = fmodf(val.x, 1.0f); val.y = fmodf(val.y, 1.0f); val.z = fmodf(val.z, 1.0f);
+            bn_step(val);
             bn[i] = val;
         }
         if (tid == 0) g_done_ctas = 0;

@@ -70,6 +70,27 @@ struct TraceConsts {
     float3 sun_dir;
 };
 
+VPT_DEV TraceConsts make_trace_consts(const SceneTables& sc, const vpt_kernel_params& kp)
+{
+    TraceConsts tc;
+    tc.inv_max = 1.0f / sc.max_extinction;
+    tc.inv_mult = 1.0f / kp.density_mult;
+    tc.sigma_c = sc.min_extinction;
+    tc.sigma_r_inv = 1.0f / (sc.max_extinction - tc.sigma_c);
+    tc.sun_dir = sun_direction(kp.azimuth, kp.elevation);
+    return tc;
+}
+
+// The state of a path that has not started yet: throughput 1, no radiance, first bounce, first walk (camera ray in st.org / st.dir)
+VPT_DEV void reset_path(PathState& st)
+{
+    st.pos = st.org;
+    st.beta = f3(1.0f); st.L = f3(.0f); st.alpha = .0f; st.depth = .0f;
+    st.wpos = st.pos; st.wdir = st.dir; st.aux = f3(0.f); st.t = 0.f; st.distance = 0.f; st.trv = 1.f; st.T_c = 1.f;
+    st.mi = false; st.first_walk = true; st.sphere_bounced = false; st.rd = 1; st.vd = 1; st.light_budget = 0; st.light_index = 0;
+    st.mode = W_DELTA; st.exit_reason = EX_NONE; st.tr_kind = TR_SUN; st.sphere_free = false;
+}
+
 // ---- light groups (the kGroups instantiations; DESIGN.md section 8d) -----------------------------------------------------------
 // Every `L +=` site of those instantiations also adds its term to the ray's sum of that light class, kept in the sample scratch at the
 // ray's own sample slot: one ray per slot, so a plain read-modify-write (no atomics, deterministic).  ptxas contracts a single-use product
@@ -119,6 +140,12 @@ VPT_DEV void store_ray(const PV& pv, int s, const PathState& st)
     pv.u(33, s) = st.qslot;
 }
 
+// the camera-ray origin of queue record `slot`: its own under a thin lens, the camera's for a pinhole
+VPT_DEV float3 ray_origin(const FrameArgs& fa, uint32_t slot)
+{
+    return fa.thin_lens ? f3(__ldg(fa.queue_aux + slot).x, __ldg(fa.queue_aux + slot).y, __ldg(fa.queue_aux + slot).z) : ld3(fa.cam.origin);
+}
+
 VPT_DEV void ray_rng_init(PathState& st, const FrameArgs& fa, uint32_t k)
 {
     uint32_t idx = st.lp;                                    // the ray's pixel word (vpt_frame.cuh): the pixel index itself for one rank
@@ -142,7 +169,7 @@ VPT_DEV void load_ray(const PV& pv, int s, PathState& st, const FrameArgs& fa)
     st.rd = b & 0xffff; st.vd = b >> 16;
     st.light_budget = (int)(int8_t)(c & 0xff); st.light_index = c >> 8;
     st.qslot = pv.u(33, s);
-    st.org = fa.thin_lens ? f3(__ldg(fa.queue_aux + st.qslot).x, __ldg(fa.queue_aux + st.qslot).y, __ldg(fa.queue_aux + st.qslot).z) : ld3(fa.cam.origin);
+    st.org = ray_origin(fa, st.qslot);
     ray_rng_init(st, fa, k);
 }
 
@@ -471,6 +498,30 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
 
 #include "vpt_trace_vol.cuh"
 
+// A path from queue record `slot` (k_generate): camera ray, pixel, pass, the draw count of the lens sampler in rng.k (the caller seeds the
+// stream), and k_generate's closest-object test.  A prestepped record is a delta walker at the walk start k_generate found.
+template <int kInteg>
+VPT_DEV void start_path(PathState& st, const FrameArgs& fa, uint32_t slot)
+{
+    const float4 r0 = __ldg(fa.queue_dir + slot);
+    const uint2 id = __ldg(fa.queue_id + slot);
+    st.dir = f3(r0.x, r0.y, r0.z);
+    st.qslot = slot;
+    st.org = ray_origin(fa, slot);
+    st.lp = id.x; st.pass = id.y & 63u;
+    st.rng.k = (id.y >> 6) & 1023u;
+    reset_path(st);
+    st.tmin_c = r0.w; st.obj_c = (int)((id.y >> 16) & 3u); st.have_closest = true;       // k_generate already ran the first test
+    st.phase = kInteg ? (int)VP_START : (int)PH_BOUNCE_TOP; st.op = OP_GLUE;
+    if ((id.y >> 18) & 1u) {
+        // k_generate already hopped over the empty nodes in front of this ray: it is a delta walker at `wpos`
+        const float4 ws = __ldg(fa.queue_aux + slot);
+        st.wpos = f3(ws.x, ws.y, ws.z); st.pos = st.wpos;
+        st.have_closest = false; st.sphere_free = true;
+        st.phase = kInteg ? (int)VP_AFTER_DELTA : (int)PH_AFTER_DELTA; st.op = OP_STEP;
+    }
+}
+
 // kLean: the instantiation may write compact records (the host allocates them for the lean kernels only, see frame_setup)
 template <int kInteg, bool kLean>
 VPT_DEV void write_sample(const PathState& st, const FrameArgs& fa)
@@ -516,16 +567,10 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     extern __shared__ float pool_smem[];                         // kTraceWarps x kRayWords x kPool words (opt-in dynamic shared memory)
     load_frame_shared(fs, fa.scene);
     const SceneTables& sc = fs.sc;
-    const vpt_kernel_params& kp = fa.kp;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned lt_mask = (1u << lane) - 1u;
 
-    TraceConsts tc;
-    tc.inv_max = 1.0f / sc.max_extinction;
-    tc.inv_mult = 1.0f / kp.density_mult;
-    tc.sigma_c = sc.min_extinction;
-    tc.sigma_r_inv = 1.0f / (sc.max_extinction - tc.sigma_c);
-    tc.sun_dir = sun_direction(kp.azimuth, kp.elevation);
+    const TraceConsts tc = make_trace_consts(sc, fa.kp);
     const SphereRec sph = load_sphere(fa.sphere);
 
     constexpr int kPool = 32 * kSlots;
@@ -551,27 +596,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
             const unsigned slot = base + __popc(idle_lanes & lt_mask);
             if (has_idle && slot < q_count) {
                 const int j = (tag0 == OP_IDLE) ? 0 : (tag1 == OP_IDLE) ? 1 : 2;
-                const float4 r0 = __ldg(fa.queue_dir + slot);
-                const uint2 id = __ldg(fa.queue_id + slot);
-                st.dir = f3(r0.x, r0.y, r0.z);
-                st.qslot = slot;
-                st.org = fa.thin_lens ? f3(__ldg(fa.queue_aux + slot).x, __ldg(fa.queue_aux + slot).y, __ldg(fa.queue_aux + slot).z) : ld3(fa.cam.origin);
-                st.lp = id.x; st.pass = id.y & 63u;
-                st.rng.k = (id.y >> 6) & 1023u;
-                st.pos = st.org;
-                st.beta = f3(1.0f); st.L = f3(.0f); st.alpha = .0f; st.depth = .0f;
-                st.wpos = st.pos; st.wdir = st.dir; st.aux = f3(0.f); st.t = 0.f; st.distance = 0.f; st.trv = 1.f; st.T_c = 1.f;
-                st.mi = false; st.first_walk = true; st.sphere_bounced = false; st.rd = 1; st.vd = 1; st.light_budget = 0; st.light_index = 0;
-                st.mode = W_DELTA; st.exit_reason = EX_NONE; st.tr_kind = TR_SUN;
-                st.tmin_c = r0.w; st.obj_c = (int)((id.y >> 16) & 3u); st.have_closest = true;       // k_generate already ran the first test
-                st.phase = kInteg ? (int)VP_START : (int)PH_BOUNCE_TOP; st.sphere_free = false; st.op = OP_GLUE;
-                if ((id.y >> 18) & 1u) {
-                    // k_generate already hopped over the empty nodes in front of this ray: it is a delta walker at `wpos`
-                    const float4 ws = __ldg(fa.queue_aux + slot);
-                    st.wpos = f3(ws.x, ws.y, ws.z); st.pos = st.wpos;
-                    st.have_closest = false; st.sphere_free = true;
-                    st.phase = kInteg ? (int)VP_AFTER_DELTA : (int)PH_AFTER_DELTA; st.op = OP_STEP;
-                }
+                start_path<kInteg>(st, fa, slot);
                 if constexpr (kGroups) {                          // the sample slot's group sums start at 0 (integrator 0 keeps no environment sum)
                     const size_t s = group_slot(st, fa);
                     #pragma unroll

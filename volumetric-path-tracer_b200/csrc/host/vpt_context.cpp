@@ -731,7 +731,8 @@ int vpt_denoise(vpt_context* c, unsigned width, unsigned height, const float* d_
 }
 
 // Statistics accumulated since the last call (needs option "count_stats"): out[0..4] = volume lookups, lane-steps,
-// warp step iterations, lane transitions, warp transition rounds.  Synchronises the device.
+// warp step iterations, lane transitions, warp transition rounds; out[5] = rays taken from the queue; out[6] = bricks
+// fetched (k_trace_brick only).  Synchronises the device.
 int vpt_get_counters(vpt_context* c, unsigned long long out[8], int reset) {
     if (!c || !out) return VPT_ERR_INVALID;
     VPT_CUDA(c, cudaDeviceSynchronize());
