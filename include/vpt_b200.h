@@ -53,6 +53,9 @@ int  vpt_abi_sizes(size_t* out, int n);
  * the scene has 64 or more instances, else 3; 2 or 3 to force it),
  * "l2_sector_fetch" (0|1: while a cell table is set, ask the L2 for 32-byte DRAM fetches -- a device-wide hint, see vpt_set_cell_volume),
  * "ctas_per_sm" (0 = occupancy maximum), "generic_kernel" (1: never pick the lean instantiation), "debug_flags" (development),
+ * "miss_cull" (1, the default: a pinhole HDRI frame first marks the pixels whose every jitter misses the volume's root box and the sphere,
+ * and writes and reads no sample records for them -- the miss samples are rebuilt from the camera and the jitter, the frame is bit for
+ * bit the same; 0: off),
  * "count_stats" / "profile" (0|1, see vpt_get_counters / vpt_get_kernel_times). */
 int  vpt_set_option(vpt_context* ctx, const char* key, int value);
 
@@ -271,7 +274,8 @@ int  vpt_get_stats(vpt_context* ctx, unsigned long long* kernel_launches_total, 
 /* Instrumentation.  Option "count_stats" = 1 makes the trace kernel accumulate out[0] volume lookups,
  * out[1] lane-steps, out[2] warp step-loop iterations, out[3] rays serviced, out[4] warp service rounds, out[5] rays
  * fetched from the queue, out[6] bricks staged by TMA (brick mode) (SIMT efficiency of the step loop = out[1] / (32 * out[2])).  Option "profile" = 1 brackets every kernel with
- * CUDA events: ms/n[0..3] = generate, trace, resolve, blue-noise advance (in adaptive frames the convergence tests count as resolve).
+ * CUDA events: ms/n[0..3] = generate, trace, resolve, blue-noise advance (in adaptive frames the convergence tests count as resolve;
+ * the per-call miss cull of option "miss_cull" counts as generate).
  * Both calls synchronise the device. */
 int  vpt_get_counters(vpt_context* ctx, unsigned long long out[8], int reset);
 int  vpt_get_kernel_times(vpt_context* ctx, float ms[4], int n[4]);

@@ -96,6 +96,33 @@ VPT_DEV SphereRec load_sphere(const vpt_sphere* s) {
 
 VPT_DEV float3 ld3(const vpt_f3& v) { return f3(v.x, v.y, v.z); }
 
+// b0 = lower_left_corner + u * horizontal + v * vertical - origin of pixel (x, y) at jitter (jx, jy) (reference camera::get_ray,
+// camera.h:131-136, with the lens offset left out): the pinhole ray's direction before normalize, and the thin-lens ray's before the
+// offset.  The operation order is pinned: k_generate, k_miss_cull and k_resolve (which rebuilds the miss samples of culled pixels) must
+// get the same bits.  Every operation is monotone in the jitter, so over the closed jitter square each component lies between its values
+// at the four corner jitters (k_miss_cull).
+VPT_DEV float3 camera_b0(const vpt_camera& cam, const vpt_u2 res, const int x, const int y, const float jx, const float jy)
+{
+    const float u = __fdividef(padd((float)x, jx), (float)res.x);
+    const float v = __fdividef(padd((float)y, jy), (float)res.y);
+    return f3(psub(pfma(cam.vertical.x, v, pfma(cam.horizontal.x, u, cam.lower_left_corner.x)), cam.origin.x),
+              psub(pfma(cam.vertical.y, v, pfma(cam.horizontal.y, u, cam.lower_left_corner.y)), cam.origin.y),
+              psub(pfma(cam.vertical.z, v, pfma(cam.horizontal.z, u, cam.lower_left_corner.z)), cam.origin.z));
+}
+
+// the pinhole camera: what k_generate and k_miss_cull test before taking the pinhole branch (an origin component of exactly 0 could meet a
+// signed zero of the lens offset, so those cameras take the literal order)
+VPT_DEV bool pinhole_camera(const vpt_camera& cam)
+{
+    return (cam.lens_radius == 0.0f) && cam.origin.x != 0.0f && cam.origin.y != 0.0f && cam.origin.z != 0.0f;
+}
+
+// the pinhole ray of pixel (x, y) at jitter (jx, jy), as k_generate builds it
+VPT_DEV float3 pinhole_dir(const vpt_camera& cam, const vpt_u2 res, const int x, const int y, const float jx, const float jy)
+{
+    return normalize(camera_b0(cam, res, x, y, jx, jy));
+}
+
 // global row of a local row under the interleaved-stripe partition (identity for one rank)
 VPT_DEV int global_row(const FrameGeom& g, int lr) {
     const int s = (g.stripe_h & (g.stripe_h - 1)) == 0 ? (lr >> (__ffs(g.stripe_h) - 1)) : lr / g.stripe_h;   // power-of-two stripes: no division

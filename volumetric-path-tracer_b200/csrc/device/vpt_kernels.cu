@@ -3,9 +3,10 @@
 //
 //   k_prepare_scene : GPU_VDB[] + OCTNode tree (the reference launch parameters) -> flat scene tables
 //   k_bn_prepare    : per-chunk blue-noise jitter table + golden-ratio advance of the 256x256 buffer (race-free, quirk Q6)
+//   k_miss_cull     : once per render call of a pinhole frame: the pixels whose every jitter misses the root box and the sphere
 //   k_generate      : one block per 32x4 pixel tile, all passes of the chunk: Philox stream, jitter, thin-lens ray,
 //                     root/sphere test, draw-free prefix of the first tracking walk; misses write a 16-byte sample
-//                     record, the rest are pushed into a warp-compacted ray queue (one atomic per warp)
+//                     record, the rest are pushed into a warp-compacted ray queue (one atomic per warp); culled pixels sample nothing
 //   k_trace<I, L, R, C, G> : persistent; every lane owns R rays parked in shared memory (vpt_trace.cuh); I = integrator (0 direct,
 //                     1 volumetric path: vpt_trace_vol.cuh), L = lean instantiation for the common scene, C = cell table, G = light groups
 //                     (the generic kernels also keep each ray's per-class radiance sums); k_trace_brick in brick mode.  The nine
@@ -106,6 +107,27 @@ __global__ void k_prepare_scene(const vpt_gpu_vdb* __restrict__ vols, const vpt_
 template <bool kAdaptive>
 __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad)
 {
+    const FrameGeom& g = fa.geom;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int tiles_x = (g.width + 31) / 32, n_tiles = kAdaptive ? ad->n_tiles : tiles_x * ((g.local_rows + 3) / 4);
+    // pixels culled by k_miss_cull (every jitter misses the box and the sphere) sample nothing here: k_resolve rebuilds their miss samples.
+    // A block none of whose pixels samples leaves before staging anything; the vote is block-wide, so all its threads leave together.
+    if (fa.miss_mask) {
+        bool idle = true;
+        for (int ti = blockIdx.x * fa.tiles_per_block; ti < min(n_tiles, (int)(blockIdx.x + 1) * fa.tiles_per_block); ++ti) {
+            const int tile = kAdaptive ? (int)__ldg(ad->tiles + ti) : ti;
+            const int tile_y = tile / tiles_x;
+            const int x = (tile - tile_y * tiles_x) * 32 + warp * 8 + (lane & 7), lr = tile_y * 4 + (lane >> 3);
+            if (x < g.width && lr < g.local_rows && global_row(g, lr) < g.height) {
+                const size_t lp = (size_t)lr * g.width + x;
+                bool stopped = false;
+                if constexpr (kAdaptive) stopped = ad->stopped[lp];
+                if (!stopped && !fa.miss_mask[lp]) idle = false;
+            }
+        }
+        if (__syncthreads_and(idle)) return;
+    }
+
     __shared__ FrameShared fs;
     __shared__ float vdc2[101], vdc3[101];                     // radical inverses of 0..100 in bases 2 and 3
     // the lens sampler only ever asks for vanDerCorput(int(xi * 100)): tabulate it with the reference's own loop -- radical_inverse
@@ -116,14 +138,11 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
     }
     load_frame_shared(fs, fa.scene);
     const SceneTables& sc = fs.sc;
-    const FrameGeom& g = fa.geom;
 
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const SphereRec sph = load_sphere(fa.sphere);
     // one block = a run of 32x4 pixel tiles x a run of passes: enough (tile, pass) pairs per block to amortise the octree / table staging
     // above -- many passes of one tile when passes are fused, several tiles when the caller renders pass by pass; a small local frame
     // (multi-GPU shard, low resolution) splits the chunk's passes over blockIdx.z instead: see launch_generate
-    const int tiles_x = (g.width + 31) / 32, n_tiles = kAdaptive ? ad->n_tiles : tiles_x * ((g.local_rows + 3) / 4);
     for (int ti = blockIdx.x * fa.tiles_per_block; ti < min(n_tiles, (int)(blockIdx.x + 1) * fa.tiles_per_block); ++ti) {
     const int tile = kAdaptive ? (int)__ldg(ad->tiles + ti) : ti;
     const int tile_y = tile / tiles_x, tile_x = tile - tile_y * tiles_x;
@@ -132,6 +151,7 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
     const int y = global_row(g, lr);
     bool valid = (x < g.width) && (lr < g.local_rows) && (y < g.height);
     if constexpr (kAdaptive) { if (valid && ad->stopped[(size_t)lr * g.width + x]) valid = false; }
+    if (valid && fa.miss_mask && fa.miss_mask[(size_t)lr * g.width + x]) valid = false;
 
     const int pass_begin = blockIdx.z * fa.passes_per_block;
     const int pass_end = min(fa.n_passes, pass_begin + fa.passes_per_block);
@@ -155,10 +175,6 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         const uint32_t idx = (uint32_t)y * (uint32_t)g.width + (uint32_t)x;
         Rng rng; rng.init(idx, kp.iteration + (uint32_t)pass, 0u);
 
-        const float bnx = bnv.x, bny = bnv.y;
-        const float u = __fdividef(padd((float)x, bnx), (float)kp.resolution.x);
-        const float v = __fdividef(padd((float)y, bny), (float)kp.resolution.y);
-
         // thin-lens ray (reference camera::get_ray, camera.h:131-136).  The lens sample is drawn by a rejection loop on the pixel's
         // Philox stream BEFORE the ray exists -- but with a pinhole (lens_radius == 0) the sample is multiplied by zero: the ray
         // does not depend on it and the only thing the path needs from the loop is HOW MANY draws it consumed.  So the pinhole ray is
@@ -166,12 +182,10 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         // generator (70 % of the samples of the headline frame are misses and never touch it).  Bit-exactness: offset = u*0*p.x +
         // v*0*p.y is +-0; x + (+-0) == x and x - (+-0) == x for every x != 0, so lanes where a zero could meet a signed zero
         // (an origin or direction component that is exactly 0) take the literal order instead.
-        const bool pinhole = (cam.lens_radius == 0.0f) && cam.origin.x != 0.0f && cam.origin.y != 0.0f && cam.origin.z != 0.0f;
+        const bool pinhole = pinhole_camera(cam);
         bool lens_pending = false;
         {
-            const float3 b0 = f3(psub(pfma(cam.vertical.x, v, pfma(cam.horizontal.x, u, cam.lower_left_corner.x)), cam.origin.x),
-                                 psub(pfma(cam.vertical.y, v, pfma(cam.horizontal.y, u, cam.lower_left_corner.y)), cam.origin.y),
-                                 psub(pfma(cam.vertical.z, v, pfma(cam.horizontal.z, u, cam.lower_left_corner.z)), cam.origin.z));
+            const float3 b0 = camera_b0(cam, kp.resolution, x, y, bnv.x, bnv.y);
             if (pinhole && b0.x != 0.0f && b0.y != 0.0f && b0.z != 0.0f) {
                 org = ld3(cam.origin);
                 dir = normalize(b0);
@@ -258,6 +272,133 @@ k_generate(const FrameArgs fa) { generate_body<false>(fa, nullptr); }
 __global__ void __launch_bounds__(128)
 k_generate_adaptive(const FrameArgs fa, const AdaptArgs ad) { generate_body<true>(fa, &ad); }
 
+// =====================================================================================================
+// k_miss_cull
+// =====================================================================================================
+// One thread per strip of kCullStrip pixels of a local row, once per render call.  The strip's pixels are culled (mask 1) only when
+//   (a) the camera is a pinhole (pinhole_camera);
+//   (b) every component of b0 keeps one strict sign over the strip's closed jitter range (x + jx from x0 to x1, y + jy from y to y + 1),
+//       away from 0 by kCullSignMargin of the largest: each operation of camera_b0 is monotone in x + jx and in y + jy, so every b0 of
+//       the strip lies in the box D spanned by its values at the four corners, computed here by the same helper (the same bits).
+//       k_generate then takes the pinhole branch for every sample;
+//   (c) a plane through the camera origin has every root-box corner on one side and every d of D at least kCullSlack |d| inside the other
+//       (candidates: the coordinate planes and the planes through two box corners, which include the facets of the cone over the box);
+//   (d) the sphere, grown as in line_misses_sphere (r'^2 = 1.02 r^2 + 2e-3 |c - o|^2 + 1e-6), is further than kCullSlack from a circular
+//       cone holding D.
+// Then every ray of the pixel passes the box and the sphere at an angle of at least kCullSlack (1e-3 rad, about 8000 float ulps: far
+// beyond the rounding of normalize and of the float slab and quadratic tests), so k_generate finds obj == 0 and stores direction +
+// kMissSentinel -- what k_resolve rebuilds.  (c) and (d) are evaluated in double.  A pixel near a silhouette that is not culled only
+// costs time.
+constexpr double kCullSlack = 1e-3, kCullSignMargin = 1e-3, kCullPlaneTol = 1e-9;
+constexpr int kCullPlanes = 6 + 2 * 28;
+constexpr int kCullStrip = 4;                   // pixels of one row tested together (one box D for the strip)
+
+__device__ __forceinline__ double3 box_corner(const double pmin[3], const double pmax[3], const int i, const double3 o)
+{
+    return make_double3(((i & 1) ? pmax[0] : pmin[0]) - o.x, ((i & 2) ? pmax[1] : pmin[1]) - o.y, ((i & 4) ? pmax[2] : pmin[2]) - o.z);
+}
+__device__ __forceinline__ double dot_d(const double3 a, const double3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ double len_d(const double3 a) { return sqrt(dot_d(a, a)); }
+
+__global__ void __launch_bounds__(256)
+k_miss_cull(const FrameArgs fa, uint8_t* __restrict__ mask)
+{
+    __shared__ double3 planes[kCullPlanes];
+    __shared__ int n_planes;
+    const vpt_camera& cam = fa.cam;
+    const FrameGeom& g = fa.geom;
+    const double3 o = make_double3(cam.origin.x, cam.origin.y, cam.origin.z);
+    double pmin[3], pmax[3];
+    bool ok = pinhole_camera(cam);
+    for (int a = 0; a < 3; ++a) {
+        pmin[a] = fa.scene->root_pmin[a]; pmax[a] = fa.scene->root_pmax[a];
+        ok = ok && isfinite(pmin[a]) && isfinite(pmax[a]) && pmin[a] <= pmax[a];       // an empty or broken root box culls nothing
+    }
+    if (threadIdx.x == 0) n_planes = 0;
+    __syncthreads();
+    if (ok && threadIdx.x < kCullPlanes) {
+        const int t = threadIdx.x;
+        double3 n = make_double3(0.0, 0.0, 0.0);
+        if (t < 6) {
+            const double s = (t & 1) ? -1.0 : 1.0;
+            if (t >> 1 == 0) n.x = s; else if (t >> 1 == 1) n.y = s; else n.z = s;
+        } else {
+            int i = 0, k = (t - 6) >> 1;                          // pair k of the 28 pairs i < j of box corners
+            while (k >= 7 - i) { k -= 7 - i; ++i; }
+            const double3 a = box_corner(pmin, pmax, i, o), b = box_corner(pmin, pmax, i + 1 + k, o);
+            const double s = ((t - 6) & 1) ? -1.0 : 1.0;
+            n = make_double3(s * (a.y * b.z - a.z * b.y), s * (a.z * b.x - a.x * b.z), s * (a.x * b.y - a.y * b.x));
+        }
+        const double ln = len_d(n);
+        bool keep = ln > 0.0;
+        if (keep) {
+            n = make_double3(n.x / ln, n.y / ln, n.z / ln);
+            for (int i = 0; i < 8; ++i) { const double3 c = box_corner(pmin, pmax, i, o); keep = keep && dot_d(n, c) >= -kCullPlaneTol * len_d(c); }
+        }
+        if (keep) planes[atomicAdd(&n_planes, 1)] = n;
+    }
+    __syncthreads();
+
+    // one thread per strip of kCullStrip pixels of one row: x0 .. x1 - 1
+    const int strips_x = (g.width + kCullStrip - 1) / kCullStrip;
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (uint32_t)(g.local_rows * strips_x)) return;
+    const int lr = (int)(t / (uint32_t)strips_x), x0 = (int)(t - (uint32_t)lr * (uint32_t)strips_x) * kCullStrip;
+    const int x1 = min(x0 + kCullStrip, g.width);
+    const int y = global_row(g, lr);
+    bool culled = false;
+    const SphereRec sph = load_sphere(fa.sphere);
+    const double3 sa = make_double3(sph.center.x - o.x, sph.center.y - o.y, sph.center.z - o.z);
+    const double L2 = dot_d(sa, sa), r2 = 1.02 * (double)sph.radius * (double)sph.radius + 2e-3 * L2 + 1e-6;
+    if (ok && y < g.height && L2 > r2) {                         // (the comparison is false for a NaN sphere)
+        // (b): D from the corners of the strip's jitter range: x0 + 0 .. (x1 - 1) + 1 = x1 + 0 (both exact), y + 0 .. y + 1
+        double lo[3], hi[3], big = 0.0;
+        for (int k = 0; k < 4; ++k) {
+            const float3 b = camera_b0(cam, fa.kp.resolution, (k & 1) ? x1 : x0, y, 0.0f, (k & 2) ? 1.0f : 0.0f);
+            const double c[3] = {b.x, b.y, b.z};
+            for (int a = 0; a < 3; ++a) {
+                lo[a] = k ? fmin(lo[a], c[a]) : c[a]; hi[a] = k ? fmax(hi[a], c[a]) : c[a];
+                big = fmax(big, fabs(c[a]));
+            }
+        }
+        bool signs = true;
+        for (int a = 0; a < 3; ++a) signs = signs && (lo[a] > kCullSignMargin * big || hi[a] < -kCullSignMargin * big);
+        if (signs) {
+            const double3 mid = make_double3((lo[0] + hi[0]) / 2, (lo[1] + hi[1]) / 2, (lo[2] + hi[2]) / 2);
+            const double3 half = make_double3((hi[0] - lo[0]) / 2, (hi[1] - lo[1]) / 2, (hi[2] - lo[2]) / 2);
+            // |d| and the angle to a fixed axis are convex / quasi-convex on D: their largest values are at its corners
+            const double ml = len_d(mid);
+            const double3 f = make_double3(mid.x / ml, mid.y / ml, mid.z / ml);
+            double dmax = 0.0, cos_theta = 1.0;                  // theta: the half-angle of the cone around f that holds D
+            for (int i = 0; i < 8; ++i) {
+                const double3 d = make_double3((i & 1) ? hi[0] : lo[0], (i & 2) ? hi[1] : lo[1], (i & 4) ? hi[2] : lo[2]);
+                const double dl = len_d(d);
+                dmax = fmax(dmax, dl);
+                cos_theta = fmin(cos_theta, dot_d(f, d) / dl);
+            }
+            // (c)
+            bool box_miss = false;
+            for (int k = 0; k < n_planes && !box_miss; ++k) {
+                const double3 n = planes[k];
+                box_miss = dot_d(mid, n) + half.x * fabs(n.x) + half.y * fabs(n.y) + half.z * fabs(n.z) + kCullSlack * dmax < 0.0;
+            }
+            // (d): the angle beta between f and the sphere's centre exceeds gamma = theta + alpha + kCullSlack (alpha: the grown sphere's
+            // angular radius), compared through cosines -- gamma stays below pi (theta < pi / 2 for D inside one octant, alpha < pi / 2)
+            // unless sin(gamma) comes out negative, and then nothing is culled
+            if (box_miss) {
+                const double st = sqrt(fmax(0.0, 1.0 - cos_theta * cos_theta));
+                const double sa_ = sqrt(r2 / L2), ca = sqrt(1.0 - r2 / L2);
+                const double c1 = cos_theta * ca - st * sa_, s1 = st * ca + cos_theta * sa_;
+                const double cs = 0.9999995000000417, ss = 9.999998333333417e-4;      // cos, sin of kCullSlack
+                const double cg = c1 * cs - s1 * ss, sg = s1 * cs + c1 * ss;
+                culled = sg > 0.0 && dot_d(f, sa) / sqrt(L2) < cg;
+            }
+        }
+    }
+    uint8_t* m = mask + (size_t)lr * g.width;
+    for (int x = x0; x < x1; ++x) m[x] = culled ? 1 : 0;
+}
+
 
 // =====================================================================================================
 // k_resolve
@@ -307,6 +448,12 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
     }
     // compact records (HDRI frames traced by a lean kernel, planeB null): one float4 per sample
     const bool compact = kSky == 0 && !fa.planeB;
+    // a pixel culled by k_miss_cull has no records: every sample is the pinhole miss k_generate would have stored, direction rebuilt from
+    // the chunk's jitter table, origin = the camera's
+    const int px = (int)(lp - (uint32_t)lr * (uint32_t)g.width);
+    // (HDRI frames only: the host hands the sky variants no mask -- their sky model is not written in pinned arithmetic, and with a second
+    // source of env_pos in this function nvcc compiled it otherwise in some instantiations, which moved bits between them)
+    const bool culled = kSky == 0 && sampled && fa.miss_mask && fa.miss_mask[lp];
     // one pass of the running mean; A (and B, C for a hit sample) are the pass's plane records, loaded by the caller.  Compact records:
     // B.x carries tr of a hit sample of the chunk's last pass when the display / raw words are written, C is unused.
     auto one_pass = [&](const int p, const float4 A, const float4 B, const float4 C) {
@@ -434,7 +581,14 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         }
     };
     const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    {
+    if (culled) {
+        // two loops, so the one over the records keeps the code (and register budget) it had without the cull
+        for (int p = 0; p < n_passes; ++p) {
+            const float2 j = __ldg(fa.bn_table + (size_t)p * 65536 + (y % 256) * 256 + px % 256);
+            const float3 d = pinhole_dir(cam, kp.resolution, px, y, j.x, j.y);
+            one_pass(p, make_float4(d.x, d.y, d.z, __uint_as_float(kMissSentinel)), zero4, zero4);
+        }
+    } else {
         for (int p = 0; p < n_passes; ++p) {
             float4 A = zero4, B = zero4, C = zero4;
             if (sampled) {
@@ -759,6 +913,14 @@ cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s)
     return cudaGetLastError();
 }
 
+cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, cudaStream_t s)
+{
+    if (fa.geom.n_local <= 0) return cudaSuccess;
+    const long long strips = (long long)fa.geom.local_rows * ((fa.geom.width + kCullStrip - 1) / kCullStrip);
+    k_miss_cull<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
@@ -868,7 +1030,7 @@ cudaError_t exchange_kernels_preload()
                                                       [&](auto fixed, auto adaptive, const auto&...) { return load(fixed, adaptive); });
                 if (e != cudaSuccess) return e;
             }
-    return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
+    return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait);
 }
 

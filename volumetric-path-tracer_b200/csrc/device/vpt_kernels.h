@@ -53,6 +53,9 @@ struct FrameArgs {
     int       cell_nx, cell_ny, cell_nz;
     int       tiles_per_block;     // k_generate: consecutive 32x4 tiles handled by one block (blockIdx.x selects the run)
     float*    plane_tr;            // compact records: [local pixel] tr of the hit samples of pass n_passes - 1 (k_resolve writes it to raw.w)
+    // [local pixel] 1 = k_miss_cull proved that every jitter of the pixel misses the root box and the sphere: k_generate samples nothing
+    // there and k_resolve<0> rebuilds the pinhole miss samples.  Null = nothing culled (option "miss_cull" 0, thin lens, sky frames).
+    const uint8_t* miss_mask;
 };
 
 // Adaptive sampling (vpt_render_adaptive): pixels are grouped in the 32x4 tiles k_generate works on; a chunk only visits the tiles that
@@ -74,6 +77,9 @@ cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* roo
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
 cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s);
+// once per render call, before the first chunk: mask[local pixel] = 1 where every jitter misses the root box and the sphere (pinhole
+// cameras only; a thin lens or a root box that is empty or not finite culls nothing)
+cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, cudaStream_t s);
 struct LightGroups;
 // The trace kernels, with their instantiations in trace_kernel (vpt_kernels.cu): generic / lean / volumetric path at 3 rays per lane,
 // k_trace_brick, generic / lean at 2, lean at 2 on the cell table, generic / volumetric path keeping the light-group planes.

@@ -79,7 +79,7 @@ static void free_context(vpt_context* c) {
     for (auto& e : c->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     cudaFree(c->d_queue_id); cudaFree(c->d_queue_org); cudaFree(c->d_bn_table);
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
-    cudaFree(c->d_plane_tr); cudaFree(c->d_lg_planes);
+    cudaFree(c->d_plane_tr); cudaFree(c->d_lg_planes); cudaFree(c->d_miss_mask);
     cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
     cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz);
     delete c;
@@ -130,6 +130,7 @@ int vpt_set_option(vpt_context* c, const char* key, int value) {
     else if (k == "generic_kernel") { c->force_generic = value ? 1 : 0; }
     else if (k == "count_stats") { c->count_stats = value ? 1 : 0; }
     else if (k == "profile") { c->profile = value ? 1 : 0; }
+    else if (k == "miss_cull") { c->miss_cull = value ? 1 : 0; }
     else return fail(c, VPT_ERR_INVALID, "unknown option " + k);
     return VPT_OK;
 }
@@ -425,6 +426,17 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     fa.planeA = c->d_planeA;
     fa.planeB = wide ? c->d_planeB : nullptr; fa.planeC = wide ? c->d_planeC : nullptr; fa.planeD = planeD ? c->d_planeD : nullptr;
     fa.plane_tr = wide ? nullptr : c->d_plane_tr;
+    // pixels no jitter can take to the root box or the sphere (pinhole HDRI frames that sample): k_miss_cull marks them once per call, and
+    // k_generate / k_resolve skip their sample records.  Frames that end on the precomputed sky keep every record (see resolve_pixel).
+    fa.miss_mask = nullptr;
+    if (c->miss_cull && n_sampled && !sky_env && fa.cam.lens_radius == 0.0f && fa.geom.n_local > 0) {
+        if ((size_t)fa.geom.n_local > c->cap_miss_mask) {
+            cudaFree(c->d_miss_mask); c->d_miss_mask = nullptr; c->cap_miss_mask = 0;
+            VPT_CUDA(c, cudaMalloc(&c->d_miss_mask, (size_t)fa.geom.n_local));
+            c->cap_miss_mask = (size_t)fa.geom.n_local;
+        }
+        fa.miss_mask = c->d_miss_mask;
+    }
 
     // rays per lane: 3 by default; 2 (one more CTA per SM) when a look-up is a chain of cache misses -- a density grid that cannot live
     // in L2 (every look-up a DRAM round trip) or long per-leaf instance lists (dependent loads): warps in flight then matter more than
@@ -504,6 +516,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         return fail(c, VPT_ERR_INVALID, "the peer exchange block was exported for another frame size (vpt_comm_p2p_export)");
     { int rc = vpt::comm_p2p_begin(c, stream); if (rc != VPT_OK) return rc; }      // multi-GPU peer exchange: this rank's frame may be overwritten from here on
     const uint32_t it0 = kp.iteration;
+    if (fa.miss_mask) {
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
+        c->launches++;
+    }
     unsigned done = 0;
     while (done < n_sampled) {
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
@@ -624,6 +640,10 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         vpt::comm_p2p_adapt_views(c, &peers, &own);
         { int rc = vpt::comm_p2p_begin(c, stream); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, vpt::launch_adapt_tally(nullptr, 0, own.error_word, d_next_count, 4, stream));
+        c->launches++;
+    }
+    if (fa.miss_mask) {
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
         c->launches++;
     }
     const void* bn = (const void*)(uintptr_t)kp0.blue_noise_buffer;

@@ -47,6 +47,9 @@ struct vpt_context {
     int debug_flags = 0;
     float4 *d_queue = nullptr, *d_planeA = nullptr, *d_planeB = nullptr, *d_planeC = nullptr, *d_planeD = nullptr;
     unsigned* d_counters = nullptr;   // [0] queue_count, [1] queue_head
+    int      miss_cull = 1;           // option "miss_cull": k_miss_cull marks the pixels no jitter can take to the volume or the sphere
+    uint8_t* d_miss_mask = nullptr;   // [local pixel] its mask, rebuilt by every render call of a pinhole frame
+    size_t   cap_miss_mask = 0;
     // stats
     unsigned long long launches = 0;
     int count_stats = 0;              // option "count_stats": accumulate trace counters
