@@ -220,6 +220,28 @@ int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
  *     buffer, or another group buffer. */
 int  vpt_set_light_group_buffers(vpt_context* ctx, float* d_sun_f3, float* d_point_f3, float* d_emission_f3, float* d_environment_f3);
 
+/* ---- render region: sample and write only a rectangle of the frame ------------------------------------------------------------
+ * A viewer that tunes the density, the phase or a light on part of a volume re-renders only that part.  The region R is the half-open
+ * rectangle [x0, x1) x [y0, y1) in pixels of the full frame, also on a partitioned context; (0, 0, 0, 0) clears it.
+ *
+ *   Activation.  A region set or cleared here takes effect at the next render call whose Kernel_params.iteration is 0; calls before that
+ *     keep the old one (the rule of the AOVs and light groups).  A viewer that moves the region resets the iteration, as on every scene
+ *     edit, so no pixel ever continues a running mean from another frame.
+ *   vpt_render_pass(es).  Every pixel of R gets bit for bit what the same call gives without a region: accum, depth, cost, raw, display,
+ *     the active AOVs and light groups -- also in the passes that sample nothing (render == 0, iteration >= max_interactions).  Outside R
+ *     nothing is written, in the caller's buffers or in the peer-exchange frame.  The blue-noise buffer is advanced exactly as without a
+ *     region (its limit still comes from the full resolution).  A partitioned context renders R's rows among its stripes; the peer exchange
+ *     stores only R's pixels into every rank's frame, which inside R is then the single-context region frame bit for bit.  The NCCL
+ *     exchange gathers the rank-local buffers as they are, so outside R the gathered frame holds whatever those buffers held.
+ *   vpt_render_adaptive (one context).  Only R's pixels take passes; the 3x3 neighbourhood is clipped at R's edge, so the rule is the one
+ *     above applied to R as if R were the frame.  d_pass_count and d_rel_error outside R are left untouched.  R = the whole frame gives the
+ *     frame without a region.  A sharded adaptive frame with a region set is refused (VPT_ERR_UNSUPPORTED).
+ *   Refused at render time (VPT_ERR_INVALID, naming the bound): x0 >= x1, y0 >= y1, x1 > resolution.x, y1 > resolution.y.  R need not be
+ *     aligned to anything; 1 x 1 is legal.
+ *   Cost.  The sample scratch keeps its full-frame size, and every chunk still prepares the whole blue-noise jitter table and starts the
+ *     persistent trace grid, so a small region has a floor of a few tens of microseconds per chunk.  Level (A) has no regions. */
+int  vpt_set_render_region(vpt_context* ctx, unsigned x0, unsigned y0, unsigned x1, unsigned y1);
+
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
  * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.

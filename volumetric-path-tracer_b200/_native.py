@@ -160,7 +160,7 @@ EXPORTED_SYMBOLS = [
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
     "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
     "vpt_denoise_options_defaults", "vpt_denoise",
-    "vpt_set_aov_buffers", "vpt_set_light_group_buffers",
+    "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region",
 ]
 
 # ---- prototypes ------------------------------------------------------------------------------------
@@ -188,6 +188,7 @@ lib.vpt_render_adaptive.argtypes = [_vp, C.POINTER(_vp), C.c_uint, C.POINTER(ada
 lib.vpt_render_adaptive.restype = C.c_int
 lib.vpt_set_aov_buffers.argtypes = [_vp, _vp, _vp]; lib.vpt_set_aov_buffers.restype = C.c_int
 lib.vpt_set_light_group_buffers.argtypes = [_vp, _vp, _vp, _vp, _vp]; lib.vpt_set_light_group_buffers.restype = C.c_int
+lib.vpt_set_render_region.argtypes = [_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint]; lib.vpt_set_render_region.restype = C.c_int
 
 
 class denoise_options(C.Structure):

@@ -20,6 +20,8 @@
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
 //   k_adapt_halo, k_adapt_count_publish, k_adapt_tally, k_adapt_publish : the same frame sharded over the peer-memory exchange -- stripe-edge
 //                     errors, the agreement on when to stop, and the final full-frame stores
+//   k_generate_region, k_miss_cull_region, k_resolve_region<S, A, G>, k_adapt_init_region, k_adapt_region : render regions
+//                     (vpt_set_render_region) -- the same per-pixel work over the pixels of one rectangle of the frame
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -104,21 +106,32 @@ __global__ void k_prepare_scene(const vpt_gpu_vdb* __restrict__ vols, const vpt_
 // =====================================================================================================
 // kAdaptive: the grid runs over the active tiles of `ad` instead of all tiles, and a lane whose pixel has stopped samples nothing (no
 // plane record, no ray).  Two kernels (k_generate, k_generate_adaptive) so the fixed-count one is the very same machine code as before.
-template <bool kAdaptive>
-__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad)
+// kRegion (k_generate_region): the grid runs over the tile rectangle of `rg`, and a lane whose pixel lies outside R samples nothing.
+template <bool kAdaptive, bool kRegion = false>
+__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad, const RenderRegion* rg = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int tiles_x = (g.width + 31) / 32, n_tiles = kAdaptive ? ad->n_tiles : tiles_x * ((g.local_rows + 3) / 4);
+    const int tiles_x = (g.width + 31) / 32;
+    const int n_tiles = kAdaptive ? ad->n_tiles : kRegion ? (rg->tx1 - rg->tx0) * (rg->ty1 - rg->ty0) : tiles_x * ((g.local_rows + 3) / 4);
+    // the tile of list entry ti: the active-tile list, R's tile rectangle row by row, or every tile
+    auto tile_of = [&](const int ti) {
+        if constexpr (kAdaptive) return (int)__ldg(ad->tiles + ti);
+        else if constexpr (kRegion) { const int w = rg->tx1 - rg->tx0, r = ti / w; return (rg->ty0 + r) * tiles_x + rg->tx0 + (ti - r * w); }
+        else return ti;
+    };
+    // a pixel of R (local row lr, column x)
+    auto in_region = [&](const int x, const int lr) { return !kRegion || (x >= rg->x0 && x < rg->x1 && lr >= rg->lr0 && lr < rg->lr1); };
     // pixels culled by k_miss_cull (every jitter misses the box and the sphere) sample nothing here: k_resolve rebuilds their miss samples.
     // A block none of whose pixels samples leaves before staging anything; the vote is block-wide, so all its threads leave together.
+    // (Every tile of R's rectangle holds a pixel of R, so without the cull a region block always has work.)
     if (fa.miss_mask) {
         bool idle = true;
         for (int ti = blockIdx.x * fa.tiles_per_block; ti < min(n_tiles, (int)(blockIdx.x + 1) * fa.tiles_per_block); ++ti) {
-            const int tile = kAdaptive ? (int)__ldg(ad->tiles + ti) : ti;
+            const int tile = tile_of(ti);
             const int tile_y = tile / tiles_x;
             const int x = (tile - tile_y * tiles_x) * 32 + warp * 8 + (lane & 7), lr = tile_y * 4 + (lane >> 3);
-            if (x < g.width && lr < g.local_rows && global_row(g, lr) < g.height) {
+            if (x < g.width && lr < g.local_rows && global_row(g, lr) < g.height && in_region(x, lr)) {
                 const size_t lp = (size_t)lr * g.width + x;
                 bool stopped = false;
                 if constexpr (kAdaptive) stopped = ad->stopped[lp];
@@ -144,13 +157,14 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
     // above -- many passes of one tile when passes are fused, several tiles when the caller renders pass by pass; a small local frame
     // (multi-GPU shard, low resolution) splits the chunk's passes over blockIdx.z instead: see launch_generate
     for (int ti = blockIdx.x * fa.tiles_per_block; ti < min(n_tiles, (int)(blockIdx.x + 1) * fa.tiles_per_block); ++ti) {
-    const int tile = kAdaptive ? (int)__ldg(ad->tiles + ti) : ti;
+    const int tile = tile_of(ti);
     const int tile_y = tile / tiles_x, tile_x = tile - tile_y * tiles_x;
     const int x = tile_x * 32 + warp * 8 + (lane & 7);
     const int lr = tile_y * 4 + (lane >> 3);
     const int y = global_row(g, lr);
     bool valid = (x < g.width) && (lr < g.local_rows) && (y < g.height);
     if constexpr (kAdaptive) { if (valid && ad->stopped[(size_t)lr * g.width + x]) valid = false; }
+    if constexpr (kRegion) { if (!in_region(x, lr)) valid = false; }
     if (valid && fa.miss_mask && fa.miss_mask[(size_t)lr * g.width + x]) valid = false;
 
     const int pass_begin = blockIdx.z * fa.passes_per_block;
@@ -272,6 +286,9 @@ k_generate(const FrameArgs fa) { generate_body<false>(fa, nullptr); }
 __global__ void __launch_bounds__(128)
 k_generate_adaptive(const FrameArgs fa, const AdaptArgs ad) { generate_body<true>(fa, &ad); }
 
+__global__ void __launch_bounds__(128)
+k_generate_region(const FrameArgs fa, const RenderRegion rg) { generate_body<false, true>(fa, nullptr, &rg); }
+
 // =====================================================================================================
 // k_miss_cull
 // =====================================================================================================
@@ -300,8 +317,9 @@ __device__ __forceinline__ double3 box_corner(const double pmin[3], const double
 __device__ __forceinline__ double dot_d(const double3 a, const double3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 __device__ __forceinline__ double len_d(const double3 a) { return sqrt(dot_d(a, a)); }
 
-__global__ void __launch_bounds__(256)
-k_miss_cull(const FrameArgs fa, uint8_t* __restrict__ mask)
+// kRegion (k_miss_cull_region): only the strips that hold a pixel of R -- the same strips, on the same kCullStrip grid, as a full frame
+template <bool kRegion>
+__device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __restrict__ mask, const RenderRegion* rg)
 {
     __shared__ double3 planes[kCullPlanes];
     __shared__ int n_planes;
@@ -340,10 +358,19 @@ k_miss_cull(const FrameArgs fa, uint8_t* __restrict__ mask)
     __syncthreads();
 
     // one thread per strip of kCullStrip pixels of one row: x0 .. x1 - 1
-    const int strips_x = (g.width + kCullStrip - 1) / kCullStrip;
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= (uint32_t)(g.local_rows * strips_x)) return;
-    const int lr = (int)(t / (uint32_t)strips_x), x0 = (int)(t - (uint32_t)lr * (uint32_t)strips_x) * kCullStrip;
+    int lr, x0;
+    if constexpr (kRegion) {
+        const int sx0 = rg->x0 / kCullStrip, strips_x = (rg->x1 + kCullStrip - 1) / kCullStrip - sx0;
+        const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+        if (t >= (uint32_t)((rg->lr1 - rg->lr0) * strips_x)) return;
+        const int r = (int)(t / (uint32_t)strips_x);
+        lr = rg->lr0 + r; x0 = (sx0 + (int)(t - (uint32_t)r * (uint32_t)strips_x)) * kCullStrip;
+    } else {
+        const int strips_x = (g.width + kCullStrip - 1) / kCullStrip;
+        const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+        if (t >= (uint32_t)(g.local_rows * strips_x)) return;
+        lr = (int)(t / (uint32_t)strips_x); x0 = (int)(t - (uint32_t)lr * (uint32_t)strips_x) * kCullStrip;
+    }
     const int x1 = min(x0 + kCullStrip, g.width);
     const int y = global_row(g, lr);
     bool culled = false;
@@ -398,6 +425,12 @@ k_miss_cull(const FrameArgs fa, uint8_t* __restrict__ mask)
     uint8_t* m = mask + (size_t)lr * g.width;
     for (int x = x0; x < x1; ++x) m[x] = culled ? 1 : 0;
 }
+
+__global__ void __launch_bounds__(256)
+k_miss_cull(const FrameArgs fa, uint8_t* __restrict__ mask) { miss_cull_body<false>(fa, mask, nullptr); }
+
+__global__ void __launch_bounds__(256)
+k_miss_cull_region(const FrameArgs fa, uint8_t* __restrict__ mask, const RenderRegion rg) { miss_cull_body<true>(fa, mask, &rg); }
 
 
 // =====================================================================================================
@@ -659,6 +692,28 @@ k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const
     resolve_pixel<kSky, false, kAov, kGroups>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp);
 }
 
+// k_resolve over R only: one thread per pixel of R on this rank, region row by region row (rg.lr0 .. rg.lr1 - 1, columns rg.x0 .. rg.x1 - 1),
+// so a warp reads and writes consecutive pixels of one row as k_resolve does.  Every pixel it visits is a pixel of R.
+template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve_region(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+                 const RenderRegion rg, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_region<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    const FrameGeom& g = fa.geom;
+    const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= w * (uint32_t)(rg.lr1 - rg.lr0)) return;
+    const uint32_t r = i / w;
+    const int lr = rg.lr0 + (int)r;
+    const uint32_t lp = (uint32_t)lr * (uint32_t)g.width + (uint32_t)rg.x0 + (i - r * w);
+    const AovBuffers* ap = nullptr;
+    const LightGroups* gp = nullptr;
+    if constexpr (kAov) ap = aov_of(ext...);
+    if constexpr (kGroups) gp = lg_of(ext...);
+    resolve_pixel<kSky, false, kAov, kGroups>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, global_row(g, lr), nullptr, ap, gp);
+}
+
 // 32x4 pixel tile and the lane's pixel in it, for the per-tile adaptive kernels (a warp covers one row of 32 pixels)
 struct TilePixel { int x, lr; bool inside; };
 __device__ __forceinline__ TilePixel tile_pixel(const FrameGeom& g, const int tile)
@@ -694,11 +749,14 @@ k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_pass
 // rank owns is read from ad.stat, a row of another rank from `halo` (the local exchange block's full-frame err plane, which k_adapt_halo of
 // every rank filled before the barrier ahead of this launch).  One rank owns every row: the neighbour set is the local one.  A tile with a
 // pixel still active is appended to the next list (one atomic per tile).
-__global__ void __launch_bounds__(128)
-k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo)
+// kRegion (k_adapt_region): the neighbourhood is clipped at R's edge instead, so the rule is the one above applied to R as if R were the frame.
+template <bool kRegion>
+__device__ __forceinline__ void adapt_body(const FrameGeom& g, const AdaptArgs& ad, const float* __restrict__ halo, const RenderRegion* rg)
 {
     const int tile = (int)__ldg(ad.tiles + blockIdx.x);
     const TilePixel t = tile_pixel(g, tile);
+    const int ylo = kRegion ? rg->y0 : 0, yhi = kRegion ? rg->y1 : g.height;
+    const int xlo = kRegion ? rg->x0 : 0, xhi = kRegion ? rg->x1 : g.width;
     bool active = false;
     if (t.inside) {
         const size_t lp = (size_t)t.lr * g.width + t.x;
@@ -707,7 +765,7 @@ k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo)
             const int y = g.n_ranks > 1 ? global_row(g, t.lr) : t.lr;
             for (int dy = -1; dy <= 1; ++dy) {
                 const int gy = y + dy;
-                if (gy < 0 || gy >= g.height) continue;
+                if (gy < ylo || gy >= yhi) continue;
                 int r = gy; bool own = true;                           // r: local row of gy when this rank owns it
                 if (g.n_ranks > 1) {
                     const int s = gy / g.stripe_h;
@@ -716,7 +774,7 @@ k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo)
                 }
                 for (int dx = -1; dx <= 1; ++dx) {
                     const int c = t.x + dx;
-                    if (c < 0 || c >= g.width) continue;
+                    if (c < xlo || c >= xhi) continue;
                     worst = fmaxf(worst, own ? ad.stat[(size_t)r * g.width + c].w : halo[(size_t)gy * g.width + c]);
                 }
             }
@@ -727,11 +785,31 @@ k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo)
     if (__syncthreads_or(active) && threadIdx.x == 0) ad.next_tiles[atomicAdd(ad.next_count, 1u)] = (unsigned)tile;
 }
 
+__global__ void __launch_bounds__(128)
+k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo) { adapt_body<false>(g, ad, halo, nullptr); }
+
+__global__ void __launch_bounds__(128)
+k_adapt_region(const FrameGeom g, const AdaptArgs ad, const RenderRegion rg) { adapt_body<true>(g, ad, nullptr, &rg); }
+
 __global__ void k_adapt_init(uint8_t* stopped, unsigned* tiles, int n_local, int n_tiles)
 {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(n_local, n_tiles); i += gridDim.x * blockDim.x) {
         if (i < n_local) stopped[i] = 0;
         if (i < n_tiles) tiles[i] = (unsigned)i;
+    }
+}
+
+// start of an adaptive region frame: the tile list is R's tile rectangle, and every local pixel outside R is stopped -- it never samples
+// and never writes, so its buffers, pass count and error keep what they held
+__global__ void k_adapt_init_region(const FrameGeom g, uint8_t* stopped, unsigned* tiles, const RenderRegion rg)
+{
+    const int tiles_x = (g.width + 31) / 32, w = rg.tx1 - rg.tx0, n_tiles = w * (rg.ty1 - rg.ty0);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < max(g.n_local, n_tiles); i += gridDim.x * blockDim.x) {
+        if (i < g.n_local) {
+            const int lr = i / g.width, x = i - lr * g.width;
+            stopped[i] = (x >= rg.x0 && x < rg.x1 && lr >= rg.lr0 && lr < rg.lr1) ? 0 : 1;
+        }
+        if (i < n_tiles) { const int r = i / w; tiles[i] = (unsigned)((rg.ty0 + r) * tiles_x + rg.tx0 + (i - r * w)); }
     }
 }
 
@@ -921,6 +999,24 @@ cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, cudaStream_t s)
     return cudaGetLastError();
 }
 
+cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, cudaStream_t s)
+{
+    const long long tiles = region_tiles(rg);
+    if (tiles <= 0) return cudaSuccess;
+    FrameArgs a = fa;
+    const dim3 grid = generate_grid(a, tiles, n_passes);
+    k_generate_region<<<grid, 128, 0, s>>>(a, rg);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, cudaStream_t s)
+{
+    if (rg.lr1 <= rg.lr0) return cudaSuccess;
+    const long long strips = (long long)(rg.lr1 - rg.lr0) * ((rg.x1 + kCullStrip - 1) / kCullStrip - rg.x0 / kCullStrip);
+    k_miss_cull_region<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
@@ -960,25 +1056,25 @@ static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const 
     }
 }
 
-// The resolve kernels: f(k_resolve<S, A, G>, k_resolve_adaptive<S, A, G>, the sky argument, the trailing AovBuffers / LightGroups) for
-// key {S, A, G}, case S * 4 + A * 2 + G.
+// The resolve kernels: f(k_resolve<S, A, G>, k_resolve_adaptive<S, A, G>, k_resolve_region<S, A, G>, the sky argument, the trailing
+// AovBuffers / LightGroups) for key {S, A, G}, case S * 4 + A * 2 + G.
 template <class F>
 static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, F&& f)
 {
     const NoSky hdri{};
     switch (r.sky * 4 + r.aov * 2 + r.groups) {
-    case 0:  return f(k_resolve<0>, k_resolve_adaptive<0>, hdri);
-    case 1:  return f(+k_resolve<0, false, true, LightGroups>, +k_resolve_adaptive<0, false, true, LightGroups>, hdri, lg);
-    case 2:  return f(+k_resolve<0, true, false, AovBuffers>, +k_resolve_adaptive<0, true, false, AovBuffers>, hdri, aov);
-    case 3:  return f(+k_resolve<0, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<0, true, true, AovBuffers, LightGroups>, hdri, aov, lg);
-    case 4:  return f(k_resolve<1>, k_resolve_adaptive<1>, atm);
-    case 5:  return f(+k_resolve<1, false, true, LightGroups>, +k_resolve_adaptive<1, false, true, LightGroups>, atm, lg);
-    case 6:  return f(+k_resolve<1, true, false, AovBuffers>, +k_resolve_adaptive<1, true, false, AovBuffers>, atm, aov);
-    case 7:  return f(+k_resolve<1, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<1, true, true, AovBuffers, LightGroups>, atm, aov, lg);
-    case 8:  return f(k_resolve<2>, k_resolve_adaptive<2>, atm);
-    case 9:  return f(+k_resolve<2, false, true, LightGroups>, +k_resolve_adaptive<2, false, true, LightGroups>, atm, lg);
-    case 10: return f(+k_resolve<2, true, false, AovBuffers>, +k_resolve_adaptive<2, true, false, AovBuffers>, atm, aov);
-    case 11: return f(+k_resolve<2, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<2, true, true, AovBuffers, LightGroups>, atm, aov, lg);
+    case 0:  return f(k_resolve<0>, k_resolve_adaptive<0>, k_resolve_region<0>, hdri);
+    case 1:  return f(+k_resolve<0, false, true, LightGroups>, +k_resolve_adaptive<0, false, true, LightGroups>, +k_resolve_region<0, false, true, LightGroups>, hdri, lg);
+    case 2:  return f(+k_resolve<0, true, false, AovBuffers>, +k_resolve_adaptive<0, true, false, AovBuffers>, +k_resolve_region<0, true, false, AovBuffers>, hdri, aov);
+    case 3:  return f(+k_resolve<0, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<0, true, true, AovBuffers, LightGroups>, +k_resolve_region<0, true, true, AovBuffers, LightGroups>, hdri, aov, lg);
+    case 4:  return f(k_resolve<1>, k_resolve_adaptive<1>, k_resolve_region<1>, atm);
+    case 5:  return f(+k_resolve<1, false, true, LightGroups>, +k_resolve_adaptive<1, false, true, LightGroups>, +k_resolve_region<1, false, true, LightGroups>, atm, lg);
+    case 6:  return f(+k_resolve<1, true, false, AovBuffers>, +k_resolve_adaptive<1, true, false, AovBuffers>, +k_resolve_region<1, true, false, AovBuffers>, atm, aov);
+    case 7:  return f(+k_resolve<1, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<1, true, true, AovBuffers, LightGroups>, +k_resolve_region<1, true, true, AovBuffers, LightGroups>, atm, aov, lg);
+    case 8:  return f(k_resolve<2>, k_resolve_adaptive<2>, k_resolve_region<2>, atm);
+    case 9:  return f(+k_resolve<2, false, true, LightGroups>, +k_resolve_adaptive<2, false, true, LightGroups>, +k_resolve_region<2, false, true, LightGroups>, atm, lg);
+    case 10: return f(+k_resolve<2, true, false, AovBuffers>, +k_resolve_adaptive<2, true, false, AovBuffers>, +k_resolve_region<2, true, false, AovBuffers>, atm, aov);
+    case 11: return f(+k_resolve<2, true, true, AovBuffers, LightGroups>, +k_resolve_adaptive<2, true, true, AovBuffers, LightGroups>, +k_resolve_region<2, true, true, AovBuffers, LightGroups>, atm, aov, lg);
     default: return cudaErrorInvalidValue;
     }
 }
@@ -1027,11 +1123,12 @@ cudaError_t exchange_kernels_preload()
         for (bool aov : {false, true})
             for (bool groups : {false, true}) {
                 const cudaError_t e = resolve_kernels(ResolveKey{sky, aov, groups}, {}, {}, {},
-                                                      [&](auto fixed, auto adaptive, const auto&...) { return load(fixed, adaptive); });
+                                                      [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
                 if (e != cudaSuccess) return e;
             }
     return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
-                k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait);
+                k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
+                k_adapt_init_region, k_adapt_region);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1048,8 +1145,21 @@ cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
-    return resolve_kernels(key, atm, aov, lg, [&](auto kernel, auto, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
         kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, ext...);
+        return cudaGetLastError();
+    });
+}
+
+cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, cudaStream_t s)
+{
+    const long long n = region_pixels(rg);
+    if (n <= 0) return cudaSuccess;
+    const int threads = 256;
+    const PeerFrames pf = peers ? *peers : PeerFrames{};
+    return resolve_kernels(key, atm, aov, lg, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+        kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, ext...);
         return cudaGetLastError();
     });
 }
@@ -1058,7 +1168,7 @@ cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, 
                                     const AovBuffers& aov, const LightGroups& lg, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
-    return resolve_kernels(key, atm, aov, lg, [&](auto, auto kernel, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
         kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, ext...);
         return cudaGetLastError();
     });
@@ -1102,6 +1212,19 @@ cudaError_t launch_adapt_publish(const FrameGeom& g, const vpt_kernel_params& kp
 cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, int n_tiles, cudaStream_t s)
 {
     k_adapt_init<<<1184, 256, 0, s>>>(stopped, tiles, g.n_local, n_tiles);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s)
+{
+    k_adapt_init_region<<<1184, 256, 0, s>>>(g, stopped, tiles, rg);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s)
+{
+    if (ad.n_tiles <= 0) return cudaSuccess;
+    k_adapt_region<<<ad.n_tiles, 128, 0, s>>>(g, ad, rg);
     return cudaGetLastError();
 }
 

@@ -73,6 +73,35 @@ struct AdaptArgs {
     float     threshold;
 };
 
+// Render region (vpt_set_render_region): a call samples and writes only the global pixels [x0, x1) x [y0, y1).  global_row increases with
+// the local row, so R and this rank's stripes meet in the local rows [lr0, lr1) (lr0 == lr1: none), and the 32x4 tiles of the local frame
+// that hold a pixel of R are the rectangle [tx0, tx1) x [ty0, ty1) -- every tile of it holds at least one.  A kernel argument of the region
+// kernels only (k_generate_region, k_miss_cull_region, k_resolve_region, k_adapt_init_region, k_adapt_region), as AovBuffers is.
+struct RenderRegion {
+    int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
+    int lr0 = 0, lr1 = 0;
+    int tx0 = 0, ty0 = 0, tx1 = 0, ty1 = 0;
+};
+// the number of local rows whose global row is below y (0 <= y <= height): the first local row at or past global row y
+inline int region_local_row(const FrameGeom& g, int y)
+{
+    const int s = y / g.stripe_h, own = s % g.n_ranks;                 // the stripe of row y and the rank that owns it
+    const int lr = own == g.rank ? (s / g.n_ranks) * g.stripe_h + (y - s * g.stripe_h)
+                                 : ((s + (g.rank - own + g.n_ranks) % g.n_ranks) / g.n_ranks) * g.stripe_h;   // next stripe of this rank
+    return lr < g.local_rows ? lr : g.local_rows;
+}
+// R's local rows and tile rectangle on this rank; the caller has checked x0 < x1 <= width and y0 < y1 <= height
+inline RenderRegion region_geometry(const FrameGeom& g, int x0, int y0, int x1, int y1)
+{
+    RenderRegion r;
+    r.x0 = x0; r.y0 = y0; r.x1 = x1; r.y1 = y1;
+    r.lr0 = region_local_row(g, y0); r.lr1 = region_local_row(g, y1);
+    if (r.lr0 < r.lr1) { r.tx0 = x0 / 32; r.tx1 = (x1 + 31) / 32; r.ty0 = r.lr0 / 4; r.ty1 = (r.lr1 + 3) / 4; }
+    return r;
+}
+inline long long region_tiles(const RenderRegion& r) { return (long long)(r.tx1 - r.tx0) * (r.ty1 - r.ty0); }
+inline long long region_pixels(const RenderRegion& r) { return (long long)(r.x1 - r.x0) * (r.lr1 - r.lr0); }
+
 cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* root, SceneTables* out, OctInternal* internal,
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
@@ -151,6 +180,16 @@ cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, 
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);
 // start of an adaptive frame: no pixel stopped, tile list = every tile
 cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, int n_tiles, cudaStream_t s);
+// Region frames (RenderRegion above): the same kernels over R only.  k_generate_region samples the pixels of R in R's tiles;
+// k_miss_cull_region tests the strips that hold a pixel of R; k_resolve_region resolves R's pixels (the peer stores as launch_resolve).
+// Adaptive, one rank: the tile list starts as R's tiles with every pixel outside R stopped, and k_adapt_region clips the 3x3 neighbourhood
+// at R's edge.
+cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, cudaStream_t s);
+cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, cudaStream_t s);
+cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, cudaStream_t s);
+cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s);
+cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s);
 
 // Sharded adaptive frame over the peer-memory exchange: every rank's block as mapped here, full-frame planes [H][W] at global pixels.
 struct AdaptPeers {

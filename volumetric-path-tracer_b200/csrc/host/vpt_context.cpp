@@ -160,6 +160,12 @@ int vpt_set_light_group_buffers(vpt_context* c, float* d_sun_f3, float* d_point_
     return VPT_OK;
 }
 
+int vpt_set_render_region(vpt_context* c, unsigned x0, unsigned y0, unsigned x1, unsigned y1) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_render_region: null context");
+    c->region_req[0] = x0; c->region_req[1] = y0; c->region_req[2] = x1; c->region_req[3] = y1;   // checked and taken at the next iteration-0 call
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -227,6 +233,8 @@ struct FramePlan {
     unsigned n_sampled = 0;               // how many of the requested passes sample (the rest only re-tonemap)
     vpt::AovBuffers aov;                  // the active compositing AOVs (both null: off)
     vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
+    bool region = false;                  // a render region is active: the region kernels over rg
+    vpt::RenderRegion rg;
 };
 
 // Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
@@ -316,6 +324,17 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     if (!kp.accum_buffer || !kp.depth_buffer || !kp.cost_buffer || !kp.display_buffer || !kp.raw_buffer || !kp.blue_noise_buffer)
         return fail(c, VPT_ERR_INVALID, "Kernel_params output buffer pointer is null");
     if (kp.resolution.x == 0 || kp.resolution.y == 0) return fail(c, VPT_ERR_INVALID, "resolution is zero");
+    // render region: the one set last takes over at a call with iteration == 0, checked against this call's resolution first
+    const unsigned* reg = kp.iteration == 0 ? c->region_req : c->region_cur;
+    const bool region = (reg[0] | reg[1] | reg[2] | reg[3]) != 0;
+    if (region) {
+        const std::string r = "render region (" + std::to_string(reg[0]) + ", " + std::to_string(reg[1]) + ", " + std::to_string(reg[2]) + ", " +
+                              std::to_string(reg[3]) + "): ";
+        if (reg[0] >= reg[2]) return fail(c, VPT_ERR_INVALID, r + "x0 must be < x1");
+        if (reg[1] >= reg[3]) return fail(c, VPT_ERR_INVALID, r + "y0 must be < y1");
+        if (reg[2] > kp.resolution.x) return fail(c, VPT_ERR_INVALID, r + "x1 exceeds Kernel_params.resolution.x = " + std::to_string(kp.resolution.x));
+        if (reg[3] > kp.resolution.y) return fail(c, VPT_ERR_INVALID, r + "y1 exceeds Kernel_params.resolution.y = " + std::to_string(kp.resolution.y));
+    }
 
     // ---- scene tables ---------------------------------------------------------------------------------------
     // Octrees built by vpt_octree_build are registered with their flat tables and instance count: nothing is read
@@ -477,6 +496,9 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     plan.resolve.sky = sky_env ? (vol_integ ? 2 : 1) : 0;
     plan.resolve.aov = plan.aov.alpha || plan.aov.volume;
     plan.resolve.groups = plan.lg.out[0] || plan.lg.out[1] || plan.lg.out[2] || plan.lg.out[3];
+    if (kp.iteration == 0) memcpy(c->region_cur, c->region_req, sizeof(c->region_cur));
+    plan.region = region;
+    if (region) plan.rg = vpt::region_geometry(fa.geom, (int)reg[0], (int)reg[1], (int)reg[2], (int)reg[3]);
     return VPT_OK;
 }
 
@@ -516,8 +538,12 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         return fail(c, VPT_ERR_INVALID, "the peer exchange block was exported for another frame size (vpt_comm_p2p_export)");
     { int rc = vpt::comm_p2p_begin(c, stream); if (rc != VPT_OK) return rc; }      // multi-GPU peer exchange: this rank's frame may be overwritten from here on
     const uint32_t it0 = kp.iteration;
+    // a render region runs the region kernels over R's tiles / pixels; the scratch layout, the trace kernel and the blue noise are the same
+    const bool region = plan.region;
+    const vpt::RenderRegion& rg = plan.rg;
     if (fa.miss_mask) {
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, rg, stream)
+                                                            : vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
         c->launches++;
     }
     unsigned done = 0;
@@ -525,13 +551,15 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
         fa.kp.iteration = it0 + done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate(fa, (int)np, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, stream) : vpt::launch_generate(fa, (int)np, stream); }));
         VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, stream); }));
+        VPT_CUDA(c, timed(c, stream, 2, [&] {
+            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, rg, stream)
+                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, stream); }));
         c->launches += 4;
         done += np;
     }
@@ -541,7 +569,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, stream));
+        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, rg, stream));
+        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2;
     }
@@ -582,6 +611,9 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         return fail(c, VPT_ERR_UNSUPPORTED, "vpt_render_adaptive: a partitioned context is supported only with an active peer-memory exchange "
                                             "(vpt_comm_p2p_export + import); vpt_set_partition alone, a suspended exchange and NCCL are not");
     const bool sharded = c->p2p_on;
+    if (sharded && (c->region_req[0] | c->region_req[1] | c->region_req[2] | c->region_req[3]))
+        return fail(c, VPT_ERR_UNSUPPORTED, "vpt_render_adaptive: a render region is not supported on a sharded adaptive frame (the convergence "
+                                            "test and the final publish cover the whole frame); clear it with vpt_set_render_region(ctx, 0, 0, 0, 0)");
     vpt_kernel_params kp0;
     memcpy(&kp0, params[VPT_ARG_KERNEL_PARAMS], sizeof(vpt_kernel_params));
     if (sharded && ((int)kp0.resolution.x != c->p2p_w || (int)kp0.resolution.y != c->p2p_h))
@@ -621,7 +653,10 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
     ad.next_tiles = lists[1]; ad.next_count = d_next_count; ad.threshold = o.threshold;
 
     c->adaptive_accum = kp0.accum_buffer;        // from here on the buffers hold an adaptive frame
-    VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt_init(g, c->d_adapt_stopped, lists[0], n_tiles, stream); }));
+    // a render region: the frame starts on R's tiles, with every pixel outside R stopped
+    if (plan.region) ad.n_tiles = (int)vpt::region_tiles(plan.rg);
+    VPT_CUDA(c, timed(c, stream, 2, [&] { return plan.region ? vpt::launch_adapt_init_region(g, c->d_adapt_stopped, lists[0], plan.rg, stream)
+                                                             : vpt::launch_adapt_init(g, c->d_adapt_stopped, lists[0], n_tiles, stream); }));
     c->launches++;
 
     // Sharded frame (peer-memory exchange): at every test the stripe-edge errors travel through the err planes of the blocks (halo), and
@@ -643,12 +678,13 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         c->launches++;
     }
     if (fa.miss_mask) {
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return plan.region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, plan.rg, stream)
+                                                                 : vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
         c->launches++;
     }
     const void* bn = (const void*)(uintptr_t)kp0.blue_noise_buffer;
     unsigned done = 0, next_test = o.min_passes;
-    unsigned active_anywhere = (unsigned)n_tiles;      // sharded: tiles still active on any rank (a rank may have none left of its own)
+    unsigned active_anywhere = (unsigned)ad.n_tiles;      // sharded: tiles still active on any rank (a rank may have none left of its own)
     int cur = 0;
     while (done < n_total && active_anywhere > 0) {
         // a chunk never crosses a test point
@@ -671,7 +707,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
                 VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt_halo(g, ad, peers, stream); }));
                 { int rc = vpt::comm_p2p_adapt_barrier(c, stream); if (rc != VPT_OK) return rc; }         // halo barrier
             }
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_adapt(g, ad, own.halo, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return plan.region ? vpt::launch_adapt_region(g, ad, plan.rg, stream) : vpt::launch_adapt(g, ad, own.halo, stream); }));
             c->launches++;
             if (sharded) {
                 VPT_CUDA(c, vpt::launch_adapt_count_publish(peers, c->rank, d_next_count, own.error_word, d_next_count, stream));

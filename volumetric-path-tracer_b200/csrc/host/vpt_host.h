@@ -95,6 +95,10 @@ struct vpt_context {
     bool      lg_active = false;
     float*    d_lg_planes = nullptr;
     size_t    cap_lg_samples = 0;
+    // render region (vpt_set_render_region): global pixels [x0, x1) x [y0, y1), all 0 = the whole frame.  region_req is what the caller
+    // set last; it becomes region_cur at the next render call with iteration == 0, so a running mean never continues under another region
+    unsigned  region_req[4] = {0, 0, 0, 0};
+    unsigned  region_cur[4] = {0, 0, 0, 0};
 };
 
 

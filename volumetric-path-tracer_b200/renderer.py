@@ -198,6 +198,17 @@ class Renderer:
             raise N.VptError(f"Renderer.light_group_image: unknown light group {name!r} (one of {', '.join(LIGHT_GROUPS)})")
         return self.buffers.groups[name].view(self.n_local // self.width, self.width, 3)
 
+    def set_region(self, x0, y0, x1, y1):
+        """Render only the full-frame pixels [x0, x1) x [y0, y1) (vpt_set_render_region) from the next call with kp.iteration == 0 on:
+        inside it every buffer gets what a full-frame render gives there, bit for bit; outside it nothing is written, so the display keeps
+        the last full frame there.  Set kp.iteration = 0 when the region moves (reset() also zeroes the buffers).  A bad rectangle is
+        refused by that next render call."""
+        check(lib.vpt_set_render_region(self.ctx, int(x0), int(y0), int(x1), int(y1)), self.ctx, "vpt_set_render_region")
+
+    def clear_region(self):
+        """Render the whole frame again from the next call with kp.iteration == 0 on."""
+        check(lib.vpt_set_render_region(self.ctx, 0, 0, 0, 0), self.ctx, "vpt_set_render_region")
+
     def reset(self):
         self.kp.iteration = 0
         self.buffers.zero_()
@@ -369,6 +380,14 @@ class DistributedRenderer:
         if not error_map:
             return out[0], counts
         return out[0], counts, torch.as_tensor(_DeviceView(pe.value, (H, W), "<f4"), device=dev)
+
+    def set_region(self, x0, y0, x1, y1):
+        """Renderer.set_region on this rank; every rank sets the same region.  The peer-memory exchange then stores only the region's
+        pixels into full_accum(); the NCCL exchange gathers each rank's buffers whole, so outside the region they hold what they held."""
+        self.r.set_region(x0, y0, x1, y1)
+
+    def clear_region(self):
+        self.r.clear_region()
 
     def set_gather(self, enabled: bool):
         """Switch the per-call exchange off (rank-local work only: profiling runs that not every rank takes part in) or back on."""
