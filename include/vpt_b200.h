@@ -242,6 +242,32 @@ int  vpt_set_light_group_buffers(vpt_context* ctx, float* d_sun_f3, float* d_poi
  *     persistent trace grid, so a small region has a floor of a few tens of microseconds per chunk.  Level (A) has no regions. */
 int  vpt_set_render_region(vpt_context* ctx, unsigned x0, unsigned y0, unsigned x1, unsigned y1);
 
+/* ---- camera projection: perspective (the reference camera) or an equirectangular panorama -------------------------------------
+ * A cloudscape baked into an environment map, a dome or a VR frame is a latitude-longitude panorama.  VPT_PROJECTION_EQUIRECT takes
+ * the orientation of the caller's camera (vpt_camera_look_at): forward -w, right u, up v.  Pixel (x, y) at jitter (jx, jy) has
+ * s = (x + jx) / W, t = (y + jy) / H, phi = (s - 1/2) hfov, theta = (t - 1/2) vfov, and its ray is (origin, normalize(b0)) with
+ * b0 = cos theta (sin phi u - cos phi w) + sin theta v.  Row 0 is at the bottom, as with the reference's `vertical`; phi grows to the
+ * right.  hfov_deg = 360, vfov_deg = 180 is the full sphere.
+ *
+ *   Activation.  A projection set here takes effect at the next render call whose Kernel_params.iteration is 0; calls before that keep
+ *     the old one (the rule of the AOVs, light groups and regions).  VPT_PROJECTION_PERSPECTIVE (the default) brings the reference camera
+ *     back; its fields of view are ignored.
+ *   Samples.  A sample draws exactly what a pinhole sample draws (the lens rejection loop and the shutter-time draw), from the pixel's own
+ *     Philox stream; from the ray on it is the reference kernel's path, to the parity a perspective frame has.  Everything else works as
+ *     with a perspective camera: adaptive frames, render regions, AOVs, light groups, brick mode, both integrators, partitioned contexts
+ *     and both exchanges.  The miss cull
+ *     (option "miss_cull") skips the pixels of an HDRI panorama that cannot reach the volume or the sphere, with the same result bit for bit.
+ *   Refused when set (VPT_ERR_INVALID): an unknown kind; for VPT_PROJECTION_EQUIRECT an hfov_deg outside (0, 360] or a vfov_deg outside
+ *     (0, 180] (NaN included).  Refused at render time (VPT_ERR_UNSUPPORTED): an equirectangular frame with camera.lens_radius != 0.
+ *   Level (A) has no projections. */
+#define VPT_PROJECTION_PERSPECTIVE 0
+#define VPT_PROJECTION_EQUIRECT    1
+int  vpt_set_projection(vpt_context* ctx, int kind, double hfov_deg, double vfov_deg);
+/* Diagnostic: writes, for every local pixel, float4 (b0, 0) -- the ray direction before normalize that the next render call's first pass
+ * gives that pixel: pano_b0 of the projection that call takes, or the reference camera's llc + s horizontal + t vertical - origin, at the
+ * jitter the blue-noise buffer holds now.  Reads params (camera, Kernel_params, blue noise); writes d_out_f4 only, on the default stream. */
+int  vpt_debug_camera_rays(vpt_context* ctx, void* const params[VPT_NUM_ARGS], float* d_out_f4);
+
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
  * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.

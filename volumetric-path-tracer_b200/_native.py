@@ -160,7 +160,7 @@ EXPORTED_SYMBOLS = [
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
     "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
     "vpt_denoise_options_defaults", "vpt_denoise",
-    "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region",
+    "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
 ]
 
 # ---- prototypes ------------------------------------------------------------------------------------
@@ -189,6 +189,9 @@ lib.vpt_render_adaptive.restype = C.c_int
 lib.vpt_set_aov_buffers.argtypes = [_vp, _vp, _vp]; lib.vpt_set_aov_buffers.restype = C.c_int
 lib.vpt_set_light_group_buffers.argtypes = [_vp, _vp, _vp, _vp, _vp]; lib.vpt_set_light_group_buffers.restype = C.c_int
 lib.vpt_set_render_region.argtypes = [_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint]; lib.vpt_set_render_region.restype = C.c_int
+VPT_PROJECTION_PERSPECTIVE, VPT_PROJECTION_EQUIRECT = 0, 1          # vpt_set_projection kinds
+lib.vpt_set_projection.argtypes = [_vp, C.c_int, C.c_double, C.c_double]; lib.vpt_set_projection.restype = C.c_int
+lib.vpt_debug_camera_rays.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_camera_rays.restype = C.c_int
 
 
 class denoise_options(C.Structure):

@@ -110,6 +110,29 @@ VPT_DEV float3 camera_b0(const vpt_camera& cam, const vpt_u2 res, const int x, c
               psub(pfma(cam.vertical.z, v, pfma(cam.horizontal.z, u, cam.lower_left_corner.z)), cam.origin.z));
 }
 
+// The equirectangular projection's angles of pixel (x, y) at jitter (jx, jy): phi = (s - 1/2) hfov, theta = (t - 1/2) vfov with
+// s = (x + jx) / W, t = (y + jy) / H.  Every operation is monotone in x + jx (phi) and y + jy (theta), so over a closed jitter range
+// each angle lies between its values at the range's ends (k_miss_cull_equirect); |phi| <= hfov / 2 <= pi keeps __sinf / __cosf in
+// their accurate range.
+VPT_DEV float2 pano_angles(const Projection& pj, const vpt_u2 res, const int x, const int y, const float jx, const float jy)
+{
+    const float s = __fdividef(padd((float)x, jx), (float)res.x);
+    const float t = __fdividef(padd((float)y, jy), (float)res.y);
+    return make_float2(pmul(psub(s, 0.5f), pj.hfov), pmul(psub(t, 0.5f), pj.vfov));
+}
+
+// b0 = cos theta (sin phi u - cos phi w) + sin theta v of the equirectangular projection (forward -w, right u, up v of the caller's
+// camera; row 0 at the bottom, as the reference's `vertical`): the ray's direction before normalize, from the camera origin.  The
+// operation order is pinned: k_generate_equirect, k_miss_cull_equirect, k_resolve_equirect (which rebuilds the miss samples of culled
+// pixels) and vpt_debug_camera_rays must get the same bits.
+VPT_DEV float3 pano_b0(const vpt_camera& cam, const Projection& pj, const vpt_u2 res, const int x, const int y, const float jx, const float jy)
+{
+    const float2 a = pano_angles(pj, res, x, y, jx, jy);
+    const float sp = __sinf(a.x), cp = __cosf(a.x), st = __sinf(a.y), ct = __cosf(a.y);
+    const float hx = pfma(sp, cam.u.x, -pmul(cp, cam.w.x)), hy = pfma(sp, cam.u.y, -pmul(cp, cam.w.y)), hz = pfma(sp, cam.u.z, -pmul(cp, cam.w.z));
+    return f3(pfma(st, cam.v.x, pmul(ct, hx)), pfma(st, cam.v.y, pmul(ct, hy)), pfma(st, cam.v.z, pmul(ct, hz)));
+}
+
 // the pinhole camera: what k_generate and k_miss_cull test before taking the pinhole branch (an origin component of exactly 0 could meet a
 // signed zero of the lens offset, so those cameras take the literal order)
 VPT_DEV bool pinhole_camera(const vpt_camera& cam)

@@ -22,6 +22,9 @@
 //                     errors, the agreement on when to stop, and the final full-frame stores
 //   k_generate_region, k_miss_cull_region, k_resolve_region<S, A, G>, k_adapt_init_region, k_adapt_region : render regions
 //                     (vpt_set_render_region) -- the same per-pixel work over the pixels of one rectangle of the frame
+//   k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect, k_miss_cull_equirect, k_miss_cull_region_equirect,
+//   k_resolve_equirect<A, G>, k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G> : the equirectangular projection
+//                     (vpt_set_projection) -- the same kernels with the camera ray of pano_b0; k_camera_rays: vpt_debug_camera_rays
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -107,8 +110,10 @@ __global__ void k_prepare_scene(const vpt_gpu_vdb* __restrict__ vols, const vpt_
 // kAdaptive: the grid runs over the active tiles of `ad` instead of all tiles, and a lane whose pixel has stopped samples nothing (no
 // plane record, no ray).  Two kernels (k_generate, k_generate_adaptive) so the fixed-count one is the very same machine code as before.
 // kRegion (k_generate_region): the grid runs over the tile rectangle of `rg`, and a lane whose pixel lies outside R samples nothing.
-template <bool kAdaptive, bool kRegion = false>
-__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad, const RenderRegion* rg = nullptr)
+// kPano (k_generate_equirect, ...): the ray is (camera origin, normalize(pano_b0)) under the projection `pj` (lens_radius is 0, the host
+// refuses anything else), and takes the pinhole branch below: its lens draws are counted after the box / octree prefix, as a pinhole's.
+template <bool kAdaptive, bool kRegion = false, bool kPano = false>
+__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad, const RenderRegion* rg = nullptr, const Projection* pj = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -196,9 +201,14 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         // generator (70 % of the samples of the headline frame are misses and never touch it).  Bit-exactness: offset = u*0*p.x +
         // v*0*p.y is +-0; x + (+-0) == x and x - (+-0) == x for every x != 0, so lanes where a zero could meet a signed zero
         // (an origin or direction component that is exactly 0) take the literal order instead.
-        const bool pinhole = pinhole_camera(cam);
         bool lens_pending = false;
-        {
+        if constexpr (kPano) {
+            // no lens offset is ever added, so no signed zero can meet the origin or b0: every sample takes the pinhole order
+            org = ld3(cam.origin);
+            dir = normalize(pano_b0(cam, *pj, kp.resolution, x, y, bnv.x, bnv.y));
+            lens_pending = true;
+        } else {
+            const bool pinhole = pinhole_camera(cam);
             const float3 b0 = camera_b0(cam, kp.resolution, x, y, bnv.x, bnv.y);
             if (pinhole && b0.x != 0.0f && b0.y != 0.0f && b0.z != 0.0f) {
                 org = ld3(cam.origin);
@@ -289,6 +299,15 @@ k_generate_adaptive(const FrameArgs fa, const AdaptArgs ad) { generate_body<true
 __global__ void __launch_bounds__(128)
 k_generate_region(const FrameArgs fa, const RenderRegion rg) { generate_body<false, true>(fa, nullptr, &rg); }
 
+__global__ void __launch_bounds__(128)
+k_generate_equirect(const FrameArgs fa, const Projection pj) { generate_body<false, false, true>(fa, nullptr, nullptr, &pj); }
+
+__global__ void __launch_bounds__(128)
+k_generate_adaptive_equirect(const FrameArgs fa, const AdaptArgs ad, const Projection pj) { generate_body<true, false, true>(fa, &ad, nullptr, &pj); }
+
+__global__ void __launch_bounds__(128)
+k_generate_region_equirect(const FrameArgs fa, const RenderRegion rg, const Projection pj) { generate_body<false, true, true>(fa, nullptr, &rg, &pj); }
+
 // =====================================================================================================
 // k_miss_cull
 // =====================================================================================================
@@ -317,9 +336,49 @@ __device__ __forceinline__ double3 box_corner(const double pmin[3], const double
 __device__ __forceinline__ double dot_d(const double3 a, const double3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 __device__ __forceinline__ double len_d(const double3 a) { return sqrt(dot_d(a, a)); }
 
-// kRegion (k_miss_cull_region): only the strips that hold a pixel of R -- the same strips, on the same kCullStrip grid, as a full frame
-template <bool kRegion>
-__device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __restrict__ mask, const RenderRegion* rg)
+// The equirectangular strip x0 .. x1 - 1 of global row y (tests (a) - (d) of miss_cull_body, kPano).  The float angles of its samples lie in
+// [phi(x0 + 0), phi(x1 + 0)] x [theta(y + 0), theta(y + 1)] (pano_angles is monotone), computed here by the same helper (the same bits).  In
+// the orthonormal frame (u, v, -w) a direction of that range is within |theta - theta_c| of (phi_c, theta) along a meridian, and that one
+// within cos(theta) |phi - phi_c| of (phi_c, theta_c) along a parallel: the cone around f = d(phi_c, theta_c) of half-angle
+// alpha = dtheta / 2 + max cos(theta) dphi / 2 holds them all, at the poles and at the seam too.  The stored basis is orthonormal only up
+// to float rounding: with every entry of M^T M - I (M = [u v w]) at most e, M's condition number k has k^2 <= (1 + 3e) / (1 - 3e), and M
+// moves no angle by more than 2 asin((k - 1) / (k + 1)), which alpha takes in.  The float rounding of __sinf / __cosf, pano_b0 and normalize
+// (about 1e-6 rad) is far below kCullSlack.
+__device__ __forceinline__ bool pano_strip_culled(const vpt_camera& cam, const Projection& pj, const vpt_u2 res, const int x0, const int x1,
+                                                  const int y, const double3* planes, const int n_planes, const double3 sa, const double L2,
+                                                  const double r2)
+{
+    const double3 U = make_double3(cam.u.x, cam.u.y, cam.u.z), V = make_double3(cam.v.x, cam.v.y, cam.v.z), Wd = make_double3(cam.w.x, cam.w.y, cam.w.z);
+    const double e = fmax(fmax(fmax(fabs(dot_d(U, U) - 1.0), fabs(dot_d(V, V) - 1.0)), fmax(fabs(dot_d(Wd, Wd) - 1.0), fabs(dot_d(U, V)))),
+                          fmax(fabs(dot_d(U, Wd)), fabs(dot_d(V, Wd))));
+    if (!(e < 1e-4)) return false;                                // (also a NaN basis)
+    const double k = sqrt((1.0 + 3.0 * e) / (1.0 - 3.0 * e));
+    const float2 lo = pano_angles(pj, res, x0, y, 0.0f, 0.0f), hi = pano_angles(pj, res, x1, y, 0.0f, 1.0f);
+    const double p0 = lo.x, p1 = hi.x, t0 = lo.y, t1 = hi.y;
+    const double pc = (p0 + p1) / 2, tc = (t0 + t1) / 2;
+    const double cmax = (t0 <= 0.0 && t1 >= 0.0) ? 1.0 : fmax(cos(t0), cos(t1));
+    const double alpha = (t1 - t0) / 2 + cmax * (p1 - p0) / 2 + 2.0 * asin((k - 1.0) / (k + 1.0));
+    if (!(alpha + kCullSlack < 1.5707963267948966)) return false;
+    const double ct = cos(tc), st = sin(tc), sp = sin(pc), cp = cos(pc);
+    double3 f = make_double3(ct * (sp * U.x - cp * Wd.x) + st * V.x, ct * (sp * U.y - cp * Wd.y) + st * V.y, ct * (sp * U.z - cp * Wd.z) + st * V.z);
+    const double fl = len_d(f);
+    f = make_double3(f.x / fl, f.y / fl, f.z / fl);
+    // (c)
+    const double lim = -sin(alpha + kCullSlack);
+    bool box_miss = false;
+    for (int i = 0; i < n_planes && !box_miss; ++i) box_miss = dot_d(f, planes[i]) < lim;
+    if (!box_miss) return false;
+    // (d): the angle between f and the sphere's centre exceeds alpha + asin(r' / L) + kCullSlack (below pi: alpha < pi / 2)
+    return dot_d(f, sa) / sqrt(L2) < cos(alpha + asin(sqrt(r2 / L2)) + kCullSlack);
+}
+
+// kRegion (k_miss_cull_region): only the strips that hold a pixel of R -- the same strips, on the same kCullStrip grid, as a full frame.
+// kPano (k_miss_cull_equirect, k_miss_cull_region_equirect): the equirectangular projection `pj`, whose rays all start at the camera
+// origin.  (a) and (b) become: the camera has no lens, and the strip's directions lie in a cone of half-angle alpha < pi / 2 - kCullSlack
+// around the direction f of the centre of its (phi, theta) range (see below).  (c) holds when f . n < -sin(alpha + kCullSlack) for a
+// candidate plane n: every direction of the cone is then more than kCullSlack past the plane.  (d) is the test above with that cone.
+template <bool kRegion, bool kPano = false>
+__device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __restrict__ mask, const RenderRegion* rg, const Projection* pj = nullptr)
 {
     __shared__ double3 planes[kCullPlanes];
     __shared__ int n_planes;
@@ -327,7 +386,9 @@ __device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __r
     const FrameGeom& g = fa.geom;
     const double3 o = make_double3(cam.origin.x, cam.origin.y, cam.origin.z);
     double pmin[3], pmax[3];
-    bool ok = pinhole_camera(cam);
+    bool ok;
+    if constexpr (kPano) ok = cam.lens_radius == 0.0f;
+    else ok = pinhole_camera(cam);
     for (int a = 0; a < 3; ++a) {
         pmin[a] = fa.scene->root_pmin[a]; pmax[a] = fa.scene->root_pmax[a];
         ok = ok && isfinite(pmin[a]) && isfinite(pmax[a]) && pmin[a] <= pmax[a];       // an empty or broken root box culls nothing
@@ -377,6 +438,9 @@ __device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __r
     const SphereRec sph = load_sphere(fa.sphere);
     const double3 sa = make_double3(sph.center.x - o.x, sph.center.y - o.y, sph.center.z - o.z);
     const double L2 = dot_d(sa, sa), r2 = 1.02 * (double)sph.radius * (double)sph.radius + 2e-3 * L2 + 1e-6;
+    if constexpr (kPano) {
+        if (ok && y < g.height && L2 > r2) culled = pano_strip_culled(cam, *pj, fa.kp.resolution, x0, x1, y, planes, n_planes, sa, L2, r2);
+    } else
     if (ok && y < g.height && L2 > r2) {                         // (the comparison is false for a NaN sphere)
         // (b): D from the corners of the strip's jitter range: x0 + 0 .. (x1 - 1) + 1 = x1 + 0 (both exact), y + 0 .. y + 1
         double lo[3], hi[3], big = 0.0;
@@ -432,6 +496,15 @@ k_miss_cull(const FrameArgs fa, uint8_t* __restrict__ mask) { miss_cull_body<fal
 __global__ void __launch_bounds__(256)
 k_miss_cull_region(const FrameArgs fa, uint8_t* __restrict__ mask, const RenderRegion rg) { miss_cull_body<true>(fa, mask, &rg); }
 
+__global__ void __launch_bounds__(256)
+k_miss_cull_equirect(const FrameArgs fa, uint8_t* __restrict__ mask, const Projection pj) { miss_cull_body<false, true>(fa, mask, nullptr, &pj); }
+
+__global__ void __launch_bounds__(256)
+k_miss_cull_region_equirect(const FrameArgs fa, uint8_t* __restrict__ mask, const RenderRegion rg, const Projection pj)
+{
+    miss_cull_body<true, true>(fa, mask, &rg, &pj);
+}
+
 
 // =====================================================================================================
 // k_resolve
@@ -447,10 +520,12 @@ template <int kSky> using SkyArg = typename std::conditional<kSky != 0, vpt_atmo
 // One pixel of k_resolve (local pixel lp, local row lr, global row y).  kAdaptive (k_resolve_adaptive): the same running mean, plus the
 // pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.  kAov: also the running means of
 // the compositing AOVs in `aov` (DESIGN.md section 8c).  kGroups: also the running means of the light groups in `lg` (section 8d).
-template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false>
+// kPano (k_resolve_equirect, ...; HDRI frames): a culled pixel's miss samples are the equirectangular rays of the projection `pj`.
+template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false>
 __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                               const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
-                                              const AdaptArgs* ad, const AovBuffers* aov, const LightGroups* lg = nullptr)
+                                              const AdaptArgs* ad, const AovBuffers* aov, const LightGroups* lg = nullptr,
+                                              const Projection* pj = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
@@ -618,7 +693,9 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         // two loops, so the one over the records keeps the code (and register budget) it had without the cull
         for (int p = 0; p < n_passes; ++p) {
             const float2 j = __ldg(fa.bn_table + (size_t)p * 65536 + (y % 256) * 256 + px % 256);
-            const float3 d = pinhole_dir(cam, kp.resolution, px, y, j.x, j.y);
+            float3 d;
+            if constexpr (kPano) d = normalize(pano_b0(cam, *pj, kp.resolution, px, y, j.x, j.y));
+            else d = pinhole_dir(cam, kp.resolution, px, y, j.x, j.y);
             one_pass(p, make_float4(d.x, d.y, d.z, __uint_as_float(kMissSentinel)), zero4, zero4);
         }
     } else {
@@ -673,12 +750,11 @@ __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a) { retur
 __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const LightGroups&) { return &a; }
 __device__ __forceinline__ const LightGroups* lg_of(const AovBuffers&, const LightGroups& l) { return &l; }
 
-template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
-__global__ void __launch_bounds__(256)
-k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
-          const Ext... ext)
+// The thread's pixel and its resolve_pixel, shared by k_resolve and k_resolve_equirect (kPano: the projection `pj`)
+template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
+__device__ __forceinline__ void resolve_body(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
+                                             const int write_display, const PeerFrames& peers, const Projection* pj, const Ext&... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
     const FrameGeom& g = fa.geom;
     const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
     if (lp >= (uint32_t)g.n_local) return;
@@ -689,17 +765,26 @@ k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const
     const LightGroups* gp = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp);
+    resolve_pixel<kSky, false, kAov, kGroups, kPano>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp, pj);
+}
+
+template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+          const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    resolve_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, sampled, write_display, peers, nullptr, ext...);
 }
 
 // k_resolve over R only: one thread per pixel of R on this rank, region row by region row (rg.lr0 .. rg.lr1 - 1, columns rg.x0 .. rg.x1 - 1),
-// so a warp reads and writes consecutive pixels of one row as k_resolve does.  Every pixel it visits is a pixel of R.
-template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
-__global__ void __launch_bounds__(256)
-k_resolve_region(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
-                 const RenderRegion rg, const Ext... ext)
+// so a warp reads and writes consecutive pixels of one row as k_resolve does.  Every pixel it visits is a pixel of R.  Shared by
+// k_resolve_region and k_resolve_region_equirect.
+template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
+__device__ __forceinline__ void resolve_region_body(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
+                                                    const int write_display, const PeerFrames& peers, const RenderRegion& rg, const Projection* pj,
+                                                    const Ext&... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_region<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
     const FrameGeom& g = fa.geom;
     const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -711,7 +796,36 @@ k_resolve_region(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes
     const LightGroups* gp = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, global_row(g, lr), nullptr, ap, gp);
+    resolve_pixel<kSky, false, kAov, kGroups, kPano>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, global_row(g, lr), nullptr, ap, gp, pj);
+}
+
+template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve_region(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+                 const RenderRegion rg, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_region<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    resolve_region_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, sampled, write_display, peers, rg, nullptr, ext...);
+}
+
+// The equirectangular frames of the HDRI environment (sky 0): k_resolve, k_resolve_region and k_resolve_adaptive with the projection `pj` as
+// one more argument, for the culled pixels' miss samples.  (Frames that end on the precomputed sky cull nothing and run k_resolve<1/2>.)
+template <bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+                   const Projection pj, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    resolve_body<0, kAov, kGroups, true>(fa, atmo, n_passes, sampled, write_display, peers, &pj, ext...);
+}
+
+template <bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve_region_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+                          const RenderRegion rg, const Projection pj, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_region_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    resolve_region_body<0, kAov, kGroups, true>(fa, atmo, n_passes, sampled, write_display, peers, rg, &pj, ext...);
 }
 
 // 32x4 pixel tile and the lane's pixel in it, for the per-tile adaptive kernels (a warp covers one row of 32 pixels)
@@ -727,11 +841,10 @@ __device__ __forceinline__ TilePixel tile_pixel(const FrameGeom& g, const int ti
 
 // One block of 128 per active tile: the running mean of the pixels that have not stopped, every pass of the chunk sampled; at the end of the
 // chunk their display / raw words, pass count and relative error (so a pixel keeps those of the last pass it took).  kAov: as k_resolve.
-template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
-__global__ void __launch_bounds__(128)
-k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Ext... ext)
+template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
+__device__ __forceinline__ void resolve_adaptive_body(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const AdaptArgs& ad,
+                                                      const Projection* pj, const Ext&... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_adaptive<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
     const FrameGeom& g = fa.geom;
     const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
     if (!t.inside) return;
@@ -741,7 +854,23 @@ k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_pass
     const LightGroups* gp = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
-    resolve_pixel<kSky, true, kAov, kGroups>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap, gp);
+    resolve_pixel<kSky, true, kAov, kGroups, kPano>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap, gp, pj);
+}
+
+template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(128)
+k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_adaptive<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    resolve_adaptive_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, ad, nullptr, ext...);
+}
+
+template <bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(128)
+k_resolve_adaptive_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const AdaptArgs ad, const Projection pj, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_adaptive_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    resolve_adaptive_body<0, kAov, kGroups, true>(fa, atmo, n_passes, ad, &pj, ext...);
 }
 
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
@@ -950,6 +1079,20 @@ __global__ void k_unpermute(const uint8_t* __restrict__ gathered, uint8_t* __res
     }
 }
 
+// vpt_debug_camera_rays: every local pixel's b0 at the jitter of the next render call's first pass (k_bn_prepare's table row 0 is the
+// blue-noise buffer as it is now), by the projection's own helper
+__global__ void k_camera_rays(const vpt_camera cam, const vpt_u2 res, const FrameGeom g, const Projection pj, const float3* __restrict__ bn, float4* out)
+{
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= (uint32_t)g.n_local) return;
+    const int lr = lp / g.width, x = lp - lr * g.width;
+    const int y = global_row(g, lr);
+    if (y >= g.height) { out[lp] = make_float4(0.f, 0.f, 0.f, 0.f); return; }
+    const float3 j = bn[(y % 256) * 256 + x % 256];
+    const float3 b = pj.kind == kProjEquirect ? pano_b0(cam, pj, res, x, y, j.x, j.y) : camera_b0(cam, res, x, y, j.x, j.y);
+    out[lp] = make_float4(b.x, b.y, b.z, 0.f);
+}
+
 // =====================================================================================================
 // host-callable launchers
 // =====================================================================================================
@@ -982,47 +1125,52 @@ static dim3 generate_grid(FrameArgs& a, long long tiles, int n_passes)
     return dim3((unsigned)((tiles + tpb - 1) / tpb), 1, (unsigned)((n_passes + ppb - 1) / ppb));
 }
 
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s)
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, cudaStream_t s)
 {
     FrameArgs a = fa;
     const long long tiles = (long long)((fa.geom.width + 31) / 32) * ((fa.geom.local_rows + 3) / 4);
     const dim3 grid = generate_grid(a, tiles, n_passes);
-    k_generate<<<grid, 128, 0, s>>>(a);
+    if (equirect(pj)) k_generate_equirect<<<grid, 128, 0, s>>>(a, pj);
+    else k_generate<<<grid, 128, 0, s>>>(a);
     return cudaGetLastError();
 }
 
-cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, cudaStream_t s)
+cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s)
 {
     if (fa.geom.n_local <= 0) return cudaSuccess;
     const long long strips = (long long)fa.geom.local_rows * ((fa.geom.width + kCullStrip - 1) / kCullStrip);
-    k_miss_cull<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask);
+    if (equirect(pj)) k_miss_cull_equirect<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, pj);
+    else k_miss_cull<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask);
     return cudaGetLastError();
 }
 
-cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, cudaStream_t s)
+cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, cudaStream_t s)
 {
     const long long tiles = region_tiles(rg);
     if (tiles <= 0) return cudaSuccess;
     FrameArgs a = fa;
     const dim3 grid = generate_grid(a, tiles, n_passes);
-    k_generate_region<<<grid, 128, 0, s>>>(a, rg);
+    if (equirect(pj)) k_generate_region_equirect<<<grid, 128, 0, s>>>(a, rg, pj);
+    else k_generate_region<<<grid, 128, 0, s>>>(a, rg);
     return cudaGetLastError();
 }
 
-cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, cudaStream_t s)
+cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s)
 {
     if (rg.lr1 <= rg.lr0) return cudaSuccess;
     const long long strips = (long long)(rg.lr1 - rg.lr0) * ((rg.x1 + kCullStrip - 1) / kCullStrip - rg.x0 / kCullStrip);
-    k_miss_cull_region<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg);
+    if (equirect(pj)) k_miss_cull_region_equirect<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg, pj);
+    else k_miss_cull_region<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg);
     return cudaGetLastError();
 }
 
-cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s)
+cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
     FrameArgs a = fa;
     const dim3 grid = generate_grid(a, ad.n_tiles, n_passes);
-    k_generate_adaptive<<<grid, 128, 0, s>>>(a, ad);
+    if (equirect(pj)) k_generate_adaptive_equirect<<<grid, 128, 0, s>>>(a, ad, pj);
+    else k_generate_adaptive<<<grid, 128, 0, s>>>(a, ad);
     return cudaGetLastError();
 }
 
@@ -1079,6 +1227,22 @@ static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& at
     }
 }
 
+// The equirectangular resolve kernels of the HDRI frames, in the form of resolve_kernels: f(k_resolve_equirect<A, G>,
+// k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G>, the sky argument, the trailing AovBuffers / LightGroups), case A * 2 + G.
+template <class F>
+static cudaError_t resolve_kernels_equirect(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, F&& f)
+{
+    const NoSky hdri{};
+    if (r.sky != 0) return cudaErrorInvalidValue;
+    switch (r.aov * 2 + r.groups) {
+    case 0:  return f(k_resolve_equirect<false, false>, k_resolve_adaptive_equirect<false, false>, k_resolve_region_equirect<false, false>, hdri);
+    case 1:  return f(+k_resolve_equirect<false, true, LightGroups>, +k_resolve_adaptive_equirect<false, true, LightGroups>, +k_resolve_region_equirect<false, true, LightGroups>, hdri, lg);
+    case 2:  return f(+k_resolve_equirect<true, false, AovBuffers>, +k_resolve_adaptive_equirect<true, false, AovBuffers>, +k_resolve_region_equirect<true, false, AovBuffers>, hdri, aov);
+    case 3:  return f(+k_resolve_equirect<true, true, AovBuffers, LightGroups>, +k_resolve_adaptive_equirect<true, true, AovBuffers, LightGroups>, +k_resolve_region_equirect<true, true, AovBuffers, LightGroups>, hdri, aov, lg);
+    default: return cudaErrorInvalidValue;
+    }
+}
+
 cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const float* brick_pool,
                          const int brick_dims[3], int n_ctas, cudaStream_t s)
 {
@@ -1125,10 +1289,15 @@ cudaError_t exchange_kernels_preload()
                 const cudaError_t e = resolve_kernels(ResolveKey{sky, aov, groups}, {}, {}, {},
                                                       [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
                 if (e != cudaSuccess) return e;
+                if (sky != 0) continue;
+                const cudaError_t ep = resolve_kernels_equirect(ResolveKey{sky, aov, groups}, {}, {},
+                                                                [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
+                if (ep != cudaSuccess) return ep;
             }
     return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
-                k_adapt_init_region, k_adapt_region);
+                k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
+                k_miss_cull_equirect, k_miss_cull_region_equirect);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1138,11 +1307,16 @@ cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, co
 }
 
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, cudaStream_t s)
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
+    if (equirect(pj) && key.sky == 0)
+        return resolve_kernels_equirect(key, aov, lg, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+            kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, pj, ext...);
+            return cudaGetLastError();
+        });
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
     return resolve_kernels(key, atm, aov, lg, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
@@ -1152,12 +1326,18 @@ cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt
 }
 
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, cudaStream_t s)
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, const Projection& pj,
+                                  cudaStream_t s)
 {
     const long long n = region_pixels(rg);
     if (n <= 0) return cudaSuccess;
     const int threads = 256;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
+    if (equirect(pj) && key.sky == 0)
+        return resolve_kernels_equirect(key, aov, lg, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+            kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, pj, ext...);
+            return cudaGetLastError();
+        });
     return resolve_kernels(key, atm, aov, lg, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
         kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, ext...);
         return cudaGetLastError();
@@ -1165,9 +1345,14 @@ cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, co
 }
 
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, cudaStream_t s)
+                                    const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
+    if (equirect(pj) && key.sky == 0)
+        return resolve_kernels_equirect(key, aov, lg, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+            kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, pj, ext...);
+            return cudaGetLastError();
+        });
     return resolve_kernels(key, atm, aov, lg, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
         kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, ext...);
         return cudaGetLastError();
@@ -1250,6 +1435,14 @@ cudaError_t launch_bn_prepare(void* bn, float2* table, int np, int limit, unsign
 cudaError_t launch_bn_advance(void* bn, int n, int limit, cudaStream_t s)
 {
     k_bn_advance<<<256, 256, 0, s>>>(reinterpret_cast<float3*>(bn), n, limit);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_camera_rays(const vpt_camera& cam, const vpt_u2 res, const FrameGeom& g, const Projection& pj, const void* bn, float4* out,
+                               cudaStream_t s)
+{
+    if (g.n_local <= 0) return cudaSuccess;
+    k_camera_rays<<<(g.n_local + 255) / 256, 256, 0, s>>>(cam, res, g, pj, reinterpret_cast<const float3*>(bn), out);
     return cudaGetLastError();
 }
 

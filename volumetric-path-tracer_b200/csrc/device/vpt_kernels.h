@@ -54,7 +54,8 @@ struct FrameArgs {
     int       tiles_per_block;     // k_generate: consecutive 32x4 tiles handled by one block (blockIdx.x selects the run)
     float*    plane_tr;            // compact records: [local pixel] tr of the hit samples of pass n_passes - 1 (k_resolve writes it to raw.w)
     // [local pixel] 1 = k_miss_cull proved that every jitter of the pixel misses the root box and the sphere: k_generate samples nothing
-    // there and k_resolve<0> rebuilds the pinhole miss samples.  Null = nothing culled (option "miss_cull" 0, thin lens, sky frames).
+    // there and k_resolve<0> (k_resolve_equirect) rebuilds the pinhole (equirectangular) miss samples.  Null = nothing culled (option
+    // "miss_cull" 0, thin lens, sky frames).
     const uint8_t* miss_mask;
 };
 
@@ -102,13 +103,22 @@ inline RenderRegion region_geometry(const FrameGeom& g, int x0, int y0, int x1, 
 inline long long region_tiles(const RenderRegion& r) { return (long long)(r.tx1 - r.tx0) * (r.ty1 - r.ty0); }
 inline long long region_pixels(const RenderRegion& r) { return (long long)(r.x1 - r.x0) * (r.lr1 - r.lr0); }
 
+// Camera projection (vpt_set_projection).  kind: kProjPerspective (the reference camera) or kProjEquirect, whose ray through pixel (x, y)
+// at jitter (jx, jy) has the direction pano_b0 (vpt_frame.cuh); hfov / vfov in radians.  A kernel argument of the equirectangular kernels
+// only (k_generate_equirect, k_miss_cull_equirect, k_resolve_equirect, ...: the launchers below pick them for kProjEquirect), as
+// RenderRegion is, so every other kernel keeps its parameter block.
+constexpr int kProjPerspective = 0, kProjEquirect = 1;          // VPT_PROJECTION_PERSPECTIVE, VPT_PROJECTION_EQUIRECT of vpt_b200.h
+struct Projection { int kind = kProjPerspective; float hfov = 0.f, vfov = 0.f; };
+inline bool equirect(const Projection& p) { return p.kind == kProjEquirect; }
+
 cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* root, SceneTables* out, OctInternal* internal,
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, cudaStream_t s);
+// pj: the frame's projection -- the launchers below run the equirectangular kernels when equirect(pj)
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, cudaStream_t s);
 // once per render call, before the first chunk: mask[local pixel] = 1 where every jitter misses the root box and the sphere (pinhole
-// cameras only; a thin lens or a root box that is empty or not finite culls nothing)
-cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, cudaStream_t s);
+// and equirectangular cameras; a thin lens or a root box that is empty or not finite culls nothing)
+cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s);
 struct LightGroups;
 // The trace kernels, with their instantiations in trace_kernel (vpt_kernels.cu): generic / lean / volumetric path at 3 rays per lane,
 // k_trace_brick, generic / lean at 2, lean at 2 on the cell table, generic / volumetric path keeping the light-group planes.
@@ -157,7 +167,7 @@ struct LightGroups { float3* out[kLightGroups] = {}; float* planes = nullptr; un
 // sky, 2 the volumetric path integrator (ends on that sky; atm: the caller's AtmosphereParameters); with the AOVs; with the light groups.
 struct ResolveKey { int sky = 0; bool aov = false, groups = false; };
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, cudaStream_t s);
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -170,11 +180,15 @@ constexpr int kPeerFlagsAdapt = 3;                    // flag array of the two b
 cudaError_t launch_bn_prepare(void* bn, float2* table, int np, int limit, unsigned* queue_counters, cudaStream_t s);   // also zeroes queue_counters[0..1]
 cudaError_t launch_bn_advance(void* bn, int n, int limit, cudaStream_t s);
 cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& g, int elem_bytes, cudaStream_t s);
+// vpt_debug_camera_rays: out[local pixel] = (b0, 0), the ray direction before normalize of the next render call's first pass: pano_b0 or
+// camera_b0 at the jitter the blue-noise buffer `bn` holds now (read only)
+cudaError_t launch_camera_rays(const vpt_camera& cam, const vpt_u2 res, const FrameGeom& g, const Projection& pj, const void* bn, float4* out,
+                               cudaStream_t s);
 // adaptive frame: k_generate / k_resolve over the tiles of ad.tiles only (stopped pixels sample nothing and keep their buffers); the resolve
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
-cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, cudaStream_t s);
+cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, cudaStream_t s);
+                                    const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);
@@ -184,10 +198,11 @@ cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* ti
 // k_miss_cull_region tests the strips that hold a pixel of R; k_resolve_region resolves R's pixels (the peer stores as launch_resolve).
 // Adaptive, one rank: the tile list starts as R's tiles with every pixel outside R stopped, and k_adapt_region clips the 3x3 neighbourhood
 // at R's edge.
-cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, cudaStream_t s);
-cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, cudaStream_t s);
+cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
+cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, cudaStream_t s);
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, const Projection& pj,
+                                  cudaStream_t s);
 cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s);
 cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s);
 

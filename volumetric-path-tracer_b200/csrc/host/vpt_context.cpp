@@ -166,6 +166,24 @@ int vpt_set_render_region(vpt_context* c, unsigned x0, unsigned y0, unsigned x1,
     return VPT_OK;
 }
 
+static_assert(vpt::kProjPerspective == VPT_PROJECTION_PERSPECTIVE && vpt::kProjEquirect == VPT_PROJECTION_EQUIRECT, "projection kinds");
+
+int vpt_set_projection(vpt_context* c, int kind, double hfov_deg, double vfov_deg) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_projection: null context");
+    vpt::Projection p;
+    if (kind == VPT_PROJECTION_EQUIRECT) {
+        if (!(hfov_deg > 0.0 && hfov_deg <= 360.0)) return fail(c, VPT_ERR_INVALID, "vpt_set_projection: hfov_deg must be in (0, 360], got " + std::to_string(hfov_deg));
+        if (!(vfov_deg > 0.0 && vfov_deg <= 180.0)) return fail(c, VPT_ERR_INVALID, "vpt_set_projection: vfov_deg must be in (0, 180], got " + std::to_string(vfov_deg));
+        p.kind = kind;
+        p.hfov = (float)(hfov_deg * (3.14159265358979323846 / 180.0));
+        p.vfov = (float)(vfov_deg * (3.14159265358979323846 / 180.0));
+    } else if (kind != VPT_PROJECTION_PERSPECTIVE) {
+        return fail(c, VPT_ERR_INVALID, "vpt_set_projection: unknown projection kind " + std::to_string(kind));
+    }
+    c->proj_req = p;                // taken at the next iteration-0 call
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -235,6 +253,7 @@ struct FramePlan {
     vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
     bool region = false;                  // a render region is active: the region kernels over rg
     vpt::RenderRegion rg;
+    vpt::Projection proj;                 // the frame's projection: the equirectangular kernels when equirect(proj)
 };
 
 // Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
@@ -335,6 +354,10 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         if (reg[2] > kp.resolution.x) return fail(c, VPT_ERR_INVALID, r + "x1 exceeds Kernel_params.resolution.x = " + std::to_string(kp.resolution.x));
         if (reg[3] > kp.resolution.y) return fail(c, VPT_ERR_INVALID, r + "y1 exceeds Kernel_params.resolution.y = " + std::to_string(kp.resolution.y));
     }
+    // projection: the one set last takes over at a call with iteration == 0
+    const vpt::Projection& proj = kp.iteration == 0 ? c->proj_req : c->proj_cur;
+    if (vpt::equirect(proj) && fa.cam.lens_radius != 0.0f)
+        return fail(c, VPT_ERR_UNSUPPORTED, "the equirectangular projection has no lens: camera.lens_radius must be 0 (got " + std::to_string(fa.cam.lens_radius) + ")");
 
     // ---- scene tables ---------------------------------------------------------------------------------------
     // Octrees built by vpt_octree_build are registered with their flat tables and instance count: nothing is read
@@ -445,7 +468,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     fa.planeA = c->d_planeA;
     fa.planeB = wide ? c->d_planeB : nullptr; fa.planeC = wide ? c->d_planeC : nullptr; fa.planeD = planeD ? c->d_planeD : nullptr;
     fa.plane_tr = wide ? nullptr : c->d_plane_tr;
-    // pixels no jitter can take to the root box or the sphere (pinhole HDRI frames that sample): k_miss_cull marks them once per call, and
+    // pixels no jitter can take to the root box or the sphere (pinhole and equirectangular HDRI frames that sample): k_miss_cull marks them once per call, and
     // k_generate / k_resolve skip their sample records.  Frames that end on the precomputed sky keep every record (see resolve_pixel).
     fa.miss_mask = nullptr;
     if (c->miss_cull && n_sampled && !sky_env && fa.cam.lens_radius == 0.0f && fa.geom.n_local > 0) {
@@ -496,7 +519,8 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     plan.resolve.sky = sky_env ? (vol_integ ? 2 : 1) : 0;
     plan.resolve.aov = plan.aov.alpha || plan.aov.volume;
     plan.resolve.groups = plan.lg.out[0] || plan.lg.out[1] || plan.lg.out[2] || plan.lg.out[3];
-    if (kp.iteration == 0) memcpy(c->region_cur, c->region_req, sizeof(c->region_cur));
+    plan.proj = proj;
+    if (kp.iteration == 0) { memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req; }
     plan.region = region;
     if (region) plan.rg = vpt::region_geometry(fa.geom, (int)reg[0], (int)reg[1], (int)reg[2], (int)reg[3]);
     return VPT_OK;
@@ -542,8 +566,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
     const bool region = plan.region;
     const vpt::RenderRegion& rg = plan.rg;
     if (fa.miss_mask) {
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, rg, stream)
-                                                            : vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, rg, plan.proj, stream)
+                                                            : vpt::launch_miss_cull(fa, c->d_miss_mask, plan.proj, stream); }));
         c->launches++;
     }
     unsigned done = 0;
@@ -551,15 +575,18 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
         fa.kp.iteration = it0 + done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, stream) : vpt::launch_generate(fa, (int)np, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, plan.proj, stream)
+                                                            : vpt::launch_generate(fa, (int)np, plan.proj, stream); }));
         VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
-            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, rg, stream)
-                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, stream); }));
+            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, rg,
+                                                       plan.proj, stream)
+                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg,
+                                                plan.proj, stream); }));
         c->launches += 4;
         done += np;
     }
@@ -569,8 +596,9 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, rg, stream));
-        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, stream));
+        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, rg,
+                                                           plan.proj, stream));
+        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.proj, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2;
     }
@@ -678,8 +706,8 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         c->launches++;
     }
     if (fa.miss_mask) {
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return plan.region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, plan.rg, stream)
-                                                                 : vpt::launch_miss_cull(fa, c->d_miss_mask, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return plan.region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, plan.rg, plan.proj, stream)
+                                                                 : vpt::launch_miss_cull(fa, c->d_miss_mask, plan.proj, stream); }));
         c->launches++;
     }
     const void* bn = (const void*)(uintptr_t)kp0.blue_noise_buffer;
@@ -694,9 +722,9 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)bn, c->d_bn_table, (int)np, plan.bn_limit, c->d_counters, stream); }));
         c->launches++;
         if (ad.n_tiles > 0) {
-            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, stream); }));
+            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.proj, stream); }));
             c->launches += 3;
         }
         done += np;
@@ -814,6 +842,23 @@ int vpt_get_kernel_times(vpt_context* c, float ms[4], int n[4]) {
 
 int vpt_render_pass(vpt_context* c, void* const params[VPT_NUM_ARGS], void* stream) {
     return vpt_render_passes(c, params, 1, stream);
+}
+
+// b0 of every local pixel at the next render call's first pass: the projection that call takes (proj_req at iteration 0, else proj_cur)
+// at the jitter the blue-noise buffer holds now, on the default stream.  Reads the camera, Kernel_params and the blue noise; writes d_out_f4 only.
+int vpt_debug_camera_rays(vpt_context* c, void* const params[VPT_NUM_ARGS], float* d_out_f4) {
+    if (!c || !params || !d_out_f4 || !params[VPT_ARG_CAMERA] || !params[VPT_ARG_KERNEL_PARAMS])
+        return fail(c, VPT_ERR_INVALID, "vpt_debug_camera_rays: null argument");
+    vpt_camera cam; vpt_kernel_params kp;
+    memcpy(&cam, params[VPT_ARG_CAMERA], sizeof(cam));
+    memcpy(&kp, params[VPT_ARG_KERNEL_PARAMS], sizeof(kp));
+    if (!kp.blue_noise_buffer) return fail(c, VPT_ERR_INVALID, "vpt_debug_camera_rays: Kernel_params.blue_noise_buffer is null");
+    if (kp.resolution.x == 0 || kp.resolution.y == 0) return fail(c, VPT_ERR_INVALID, "vpt_debug_camera_rays: resolution is zero");
+    const vpt::Projection& pj = kp.iteration == 0 ? c->proj_req : c->proj_cur;
+    VPT_CUDA(c, vpt::launch_camera_rays(cam, kp.resolution, make_geom(c, kp.resolution.x, kp.resolution.y), pj, (const void*)(uintptr_t)kp.blue_noise_buffer,
+                                        reinterpret_cast<float4*>(d_out_f4), 0));
+    c->launches++;
+    return VPT_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------

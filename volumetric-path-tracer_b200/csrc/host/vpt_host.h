@@ -99,6 +99,9 @@ struct vpt_context {
     // set last; it becomes region_cur at the next render call with iteration == 0, so a running mean never continues under another region
     unsigned  region_req[4] = {0, 0, 0, 0};
     unsigned  region_cur[4] = {0, 0, 0, 0};
+    // camera projection (vpt_set_projection), checked when set: proj_req is what the caller set last; it becomes proj_cur at the next render
+    // call with iteration == 0, so a running mean never continues under another projection
+    vpt::Projection proj_req, proj_cur;
 };
 
 

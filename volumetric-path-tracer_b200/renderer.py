@@ -209,6 +209,23 @@ class Renderer:
         """Render the whole frame again from the next call with kp.iteration == 0 on."""
         check(lib.vpt_set_render_region(self.ctx, 0, 0, 0, 0), self.ctx, "vpt_set_render_region")
 
+    def set_projection(self, kind, hfov=360.0, vfov=180.0):
+        """Camera projection (vpt_set_projection) from the next call with kp.iteration == 0 on: "perspective", the reference camera (the
+        default), or "equirect", a latitude-longitude panorama of hfov x vfov degrees (hfov in (0, 360], vfov in (0, 180]) around the
+        camera's origin, oriented by its u, v, w (forward -w).  A bad kind or field of view raises VptError here; an equirectangular frame
+        with a lens (cam.lens_radius != 0) is refused by the render call."""
+        kinds = {"perspective": N.VPT_PROJECTION_PERSPECTIVE, "equirect": N.VPT_PROJECTION_EQUIRECT}
+        if kind not in kinds:
+            raise N.VptError(f"Renderer.set_projection: unknown projection {kind!r} (one of {', '.join(kinds)})")
+        check(lib.vpt_set_projection(self.ctx, kinds[kind], float(hfov), float(vfov)), self.ctx, "vpt_set_projection")
+
+    def camera_rays(self):
+        """(n_local, 4) float32: per local pixel (b0, 0), the ray direction before normalize that the next render call's first pass takes
+        (vpt_debug_camera_rays).  Writes nothing else and leaves the blue noise as it is."""
+        out = torch.empty(self.n_local, 4, dtype=torch.float32, device=self.buffers.accum.device)
+        check(lib.vpt_debug_camera_rays(self.ctx, self.params.array, C.c_void_p(out.data_ptr())), self.ctx, "vpt_debug_camera_rays")
+        return out
+
     def reset(self):
         self.kp.iteration = 0
         self.buffers.zero_()
@@ -388,6 +405,10 @@ class DistributedRenderer:
 
     def clear_region(self):
         self.r.clear_region()
+
+    def set_projection(self, kind, hfov=360.0, vfov=180.0):
+        """Renderer.set_projection on this rank; every rank sets the same projection."""
+        self.r.set_projection(kind, hfov=hfov, vfov=vfov)
 
     def set_gather(self, enabled: bool):
         """Switch the per-call exchange off (rank-local work only: profiling runs that not every rank takes part in) or back on."""
