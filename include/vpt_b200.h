@@ -112,6 +112,34 @@ int  vpt_comm_p2p_adaptive_frame(vpt_context* ctx, vpt_devptr_t* d_full_pass_cou
 int  vpt_comm_p2p_enable(vpt_context* ctx, int on);
 int  vpt_comm_p2p_status(vpt_context* ctx, unsigned long long* abandoned_waits);
 
+/* Exchange layers: depth, the compositing AOVs and the light groups full-frame on every rank, next to the accumulators.
+ *   Export.  vpt_comm_p2p_export_layers is vpt_comm_p2p_export with `layers`, a mask of the VPT_LAYER_* bits below; each bit adds one
+ *     full-frame [H][W] plane to the block (float for depth and alpha, float3 for the others: 68 B per pixel for all seven), each on a
+ *     256-byte boundary after the parts vpt_comm_p2p_export allocates.  vpt_comm_p2p_export is this call with layers = 0: same block, same
+ *     behaviour.  Unknown bits are refused (VPT_ERR_INVALID).  vpt_comm_p2p_block_bytes gives the size of the block for a frame (pure host
+ *     code).  Every rank exports the same frame size, display flag and layers: the block header records them, and vpt_comm_p2p_import /
+ *     _import_local refuse a peer whose block differs (VPT_ERR_INVALID, naming the rank) and map nothing.
+ *   Calls.  Once the exchange is active, every vpt_render_pass(es) and sharded vpt_render_adaptive call ends, before the final flag exchange,
+ *     with a copy of this rank's depth_buffer and of its active AOV and light-group buffers (vpt_set_aov_buffers,
+ *     vpt_set_light_group_buffers) into every rank's planes at the global pixels, so after the call vpt_comm_p2p_layer's planes hold the
+ *     single-context frame's buffers bit for bit on every rank, like the accumulators.  Padding rows are not stored; with a render region
+ *     only R's pixels are.  A layer that is exported but not active on the context (a NULL buffer, or AOVs / groups not yet activated by an
+ *     iteration-0 call) keeps its plane as it is.  Every rank activates the same AOVs and groups, like every other option of a sharded call.
+ *     Nothing is copied while the exchange is suspended (vpt_comm_p2p_enable(ctx, 0)) or on one rank (n_ranks == 1: the context's own
+ *     buffers are the full frame).  The NCCL exchange does not carry layers: there they stay rank-local.
+ *   vpt_comm_p2p_layer returns the full-frame plane of ONE layer bit; a layer the block was exported without is refused (VPT_ERR_INVALID). */
+#define VPT_LAYER_DEPTH        0x01u   /* float: depth_buffer */
+#define VPT_LAYER_ALPHA        0x02u   /* float: the alpha AOV */
+#define VPT_LAYER_VOLUME       0x04u   /* float3: the volume AOV */
+#define VPT_LAYER_SUN          0x08u   /* float3: light group sun */
+#define VPT_LAYER_POINT        0x10u   /* float3: light group point */
+#define VPT_LAYER_EMISSION     0x20u   /* float3: light group emission */
+#define VPT_LAYER_ENVIRONMENT  0x40u   /* float3: light group environment */
+int  vpt_comm_p2p_export_layers(vpt_context* ctx, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
+                                unsigned layers, unsigned char handle_out[VPT_P2P_HANDLE_BYTES]);
+int  vpt_comm_p2p_layer(vpt_context* ctx, unsigned layer, vpt_devptr_t* d_full);
+int  vpt_comm_p2p_block_bytes(unsigned width, unsigned height, int with_display, unsigned layers, size_t* out);
+
 /* ---- the hot path --------------------------------------------------------------------------------
  * vpt_render_pass   replaces ONE launch of the reference `volume_rt_kernel` (render_kernel.cu:2216):
  *                   same inputs, same buffer updates (accum/depth/cost running means, display, raw,
@@ -189,7 +217,8 @@ int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], uns
  *     that enables AOVs mid-frame never continues a mean from garbage (vpt_render_adaptive always starts at 0).
  *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active AOVs.  An adaptive frame's stopped pixels keep theirs, and every
  *     pixel's AOVs are bit for bit what a fixed-count frame of its own pass count leaves there.  Level (A) (volume_rt_kernel) has none.
- *     The NCCL and peer-memory exchanges do not carry AOVs: on a partitioned context they stay rank-local.
+ *     On a partitioned context the buffers are rank-local; the peer-memory exchange carries them full-frame to every rank when the block is
+ *     exported with VPT_LAYER_ALPHA / VPT_LAYER_VOLUME (vpt_comm_p2p_export_layers).  The NCCL exchange does not carry them.
  *   Refused at render time (VPT_ERR_INVALID, naming the buffer): an AOV buffer that overlaps accum, depth, cost, raw or display, and
  *     the two AOV buffers overlapping each other. */
 int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
@@ -212,8 +241,9 @@ int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
  *     NULL; all four NULL turns the groups off at once.  Activation as for the AOVs: registered buffers take over at the next render call
  *     whose Kernel_params.iteration is 0, calls before that leave them untouched.
  *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active groups; an adaptive frame's stopped pixels keep theirs.  Every
- *     other output is bit for bit what the same call gives without groups.  Level (A) has none.  The NCCL and peer-memory exchanges do not
- *     carry them: on a partitioned context they stay rank-local.
+ *     other output is bit for bit what the same call gives without groups.  Level (A) has none.  On a partitioned context the buffers are
+ *     rank-local; the peer-memory exchange carries them full-frame to every rank when the block is exported with VPT_LAYER_SUN, _POINT,
+ *     _EMISSION, _ENVIRONMENT (vpt_comm_p2p_export_layers).  The NCCL exchange does not carry them.
  *   Cost.  Groups make the lean kernels write wide sample records and the generic kernels keep 48 B more per sample (the chunk shrinks
  *     under max_scratch_mb accordingly).
  *   Refused at render time (VPT_ERR_INVALID, naming the buffer): a group buffer that overlaps accum, depth, cost, raw or display, an AOV

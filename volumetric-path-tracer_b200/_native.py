@@ -161,7 +161,11 @@ EXPORTED_SYMBOLS = [
     "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
     "vpt_denoise_options_defaults", "vpt_denoise",
     "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
+    "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
 ]
+
+# exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
+LAYER_BITS = {"depth": 0x01, "alpha": 0x02, "volume": 0x04, "sun": 0x08, "point": 0x10, "emission": 0x20, "environment": 0x40}
 
 # ---- prototypes ------------------------------------------------------------------------------------
 _vp = C.c_void_p
@@ -231,6 +235,10 @@ lib.vpt_comm_p2p_frame.argtypes = [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uin
 lib.vpt_comm_p2p_adaptive_frame.argtypes = [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_adaptive_frame.restype = C.c_int
 lib.vpt_comm_p2p_enable.argtypes = [_vp, C.c_int]; lib.vpt_comm_p2p_enable.restype = C.c_int
 lib.vpt_comm_p2p_status.argtypes = [_vp, C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_status.restype = C.c_int
+lib.vpt_comm_p2p_export_layers.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_int, C.c_uint, C.POINTER(C.c_ubyte)]
+lib.vpt_comm_p2p_export_layers.restype = C.c_int
+lib.vpt_comm_p2p_layer.argtypes = [_vp, C.c_uint, C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_layer.restype = C.c_int
+lib.vpt_comm_p2p_block_bytes.argtypes = [C.c_uint, C.c_uint, C.c_int, C.c_uint, C.POINTER(C.c_size_t)]; lib.vpt_comm_p2p_block_bytes.restype = C.c_int
 
 
 lib.vpt_texture_create_3d_from_device.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.POINTER(_vp)]

@@ -20,6 +20,7 @@
 //                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
 //   k_adapt_halo, k_adapt_count_publish, k_adapt_tally, k_adapt_publish : the same frame sharded over the peer-memory exchange -- stripe-edge
 //                     errors, the agreement on when to stop, and the final full-frame stores
+//   k_layers_publish : depth, the compositing AOVs and the light groups into every rank's full-frame planes (vpt_comm_p2p_export_layers)
 //   k_generate_region, k_miss_cull_region, k_resolve_region<S, A, G>, k_adapt_init_region, k_adapt_region : render regions
 //                     (vpt_set_render_region) -- the same per-pixel work over the pixels of one rectangle of the frame
 //   k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect, k_miss_cull_equirect, k_miss_cull_region_equirect,
@@ -1004,6 +1005,36 @@ k_adapt_publish(const FrameGeom g, const float3* __restrict__ accum, const unsig
     }
 }
 
+// Exchange layers, one thread per pixel of the rectangle rg (the whole local frame, or R's pixels on this rank), row by row as
+// k_resolve_region: depth and the active compositing layers at the pixel's global position in every rank's planes, as k_adapt_publish
+// does for accum.  A copy behind the resolve, so no resolve kernel's parameter block grows.
+__global__ void __launch_bounds__(256)
+k_layers_publish(const FrameGeom g, const RenderRegion rg, const LayerSources src, const LayerPlanes dst)
+{
+    const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= w * (uint32_t)(rg.lr1 - rg.lr0)) return;
+    const uint32_t r = i / w;
+    const int lr = rg.lr0 + (int)r, x = rg.x0 + (int)(i - r * w);
+    const int y = global_row(g, lr);
+    if (y >= g.height) return;                                    // padding row
+    const size_t lp = (size_t)lr * g.width + x, gp = (size_t)y * g.width + x;
+    #pragma unroll
+    for (int l = 0; l < kExchangeLayers; ++l) {
+        if (!src.src[l] || !dst.plane[l][0]) continue;             // not active here / not exported (then on no rank: import checks the masks)
+        if (l < XL_VOLUME) {
+            const float v = src.src[l][lp];
+            #pragma unroll
+            for (int p = 0; p < kMaxPeers; ++p) if (p < dst.n) dst.plane[l][p][gp] = v;
+        } else {
+            const float* s = src.src[l] + 3 * lp;
+            const float a = s[0], b = s[1], c = s[2];
+            #pragma unroll
+            for (int p = 0; p < kMaxPeers; ++p) if (p < dst.n) { float* q = dst.plane[l][p] + 3 * gp; q[0] = a; q[1] = b; q[2] = c; }
+        }
+    }
+}
+
 __global__ void k_peer_signal(PeerFlagPtrs fl, int n, int rank, int which, unsigned long long epoch)
 {
     const int p = threadIdx.x;
@@ -1297,7 +1328,7 @@ cudaError_t exchange_kernels_preload()
     return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
-                k_miss_cull_equirect, k_miss_cull_region_equirect);
+                k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1391,6 +1422,17 @@ cudaError_t launch_adapt_publish(const FrameGeom& g, const vpt_kernel_params& kp
     if (g.n_local <= 0) return cudaSuccess;
     k_adapt_publish<<<(g.n_local + 255) / 256, 256, 0, s>>>(g, reinterpret_cast<const float3*>(kp.accum_buffer),
                                                             reinterpret_cast<const unsigned*>(kp.display_buffer), ad.pass_count, ad.rel_error, ad.stat, pp);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_layers_publish(const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, const LayerPlanes& dst, cudaStream_t s)
+{
+    RenderRegion all;                                             // the whole local frame
+    all.x1 = g.width; all.lr1 = g.local_rows;
+    const RenderRegion& r = rg ? *rg : all;
+    const long long n = region_pixels(r);
+    if (n <= 0 || dst.n <= 0) return cudaSuccess;
+    k_layers_publish<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(g, r, src, dst);
     return cudaGetLastError();
 }
 

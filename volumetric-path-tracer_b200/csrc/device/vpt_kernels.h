@@ -174,8 +174,18 @@ cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], 
 cudaError_t launch_peer_wait(unsigned long long* local_flags, int n, int which, unsigned long long epoch, cudaStream_t s);
 // loads every kernel a render call may issue (lazy module loading): no first launch may have to wait behind a peer's spinning flag wait
 cudaError_t exchange_kernels_preload();
-constexpr int kPeerFlagStride = 16;                   // u64 slots per flag array; layout of a block header: ready[16] done[16] error[1] (+15 unused) adapt[16]
+constexpr int kPeerFlagStride = 16;                   // u64 slots per flag array; layout of a block header: ready[16] done[16] error[1] layout[1] (+14 unused) adapt[16]
 constexpr int kPeerFlagsAdapt = 3;                    // flag array of the two barriers of every convergence test of a sharded adaptive frame
+// Exchange layers (vpt_comm_p2p_export_layers): full-frame planes [H][W] of depth and the compositing layers in every rank's block, in the
+// order of the VPT_LAYER_* bits (bit l = 1 << l).  Depth and alpha are float, the others float3.
+enum ExchangeLayer : int { XL_DEPTH = 0, XL_ALPHA = 1, XL_VOLUME = 2, XL_SUN = 3, XL_POINT = 4, XL_EMISSION = 5, XL_ENVIRONMENT = 6, kExchangeLayers = 7 };
+// src: this rank's [local pixel] buffer of each layer, null where the layer is not active on the context.  plane: every rank's full-frame
+// plane of each layer as mapped here, null where the block was exported without it.  A kernel argument of k_layers_publish only.
+struct LayerSources { const float* src[kExchangeLayers] = {}; };
+struct LayerPlanes { int n = 0; float* plane[kExchangeLayers][kMaxPeers] = {}; };
+// after the call's last resolve (or k_adapt_publish): every active, exported layer of every local pixel at its global position in every rank's
+// planes; rg: the frame's render region (null: the whole frame).  Padding rows and pixels outside R are not written.
+cudaError_t launch_layers_publish(const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, const LayerPlanes& dst, cudaStream_t s);
 // limit = min(W*H, 65536) entries are advanced (the reference updates entry y*W + x from pixel (x, y))
 cudaError_t launch_bn_prepare(void* bn, float2* table, int np, int limit, unsigned* queue_counters, cudaStream_t s);   // also zeroes queue_counters[0..1]
 cudaError_t launch_bn_advance(void* bn, int n, int limit, cudaStream_t s);

@@ -16,6 +16,7 @@
 #include "vpt_host.h"
 
 #include <dlfcn.h>
+#include <cstdio>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -106,15 +107,63 @@ int comm_gather_frame(vpt_context* c, const FrameGeom& g, const void* d_local_ac
 // ---- peer-memory exchange ---------------------------------------------------------------------------------------------------------
 // Block layout: header (u64 flag arrays: ready[16] done[16] error[1], adapt[16] at kPeerFlagsAdapt) | float3 accum [H][W] | u32 display
 // [H][W] (exported with display only) | u32 pass counts [H][W] | f32 relative errors [H][W] | u32 active-tile count per rank [16].
-// The last three serve vpt_render_adaptive; each part starts on a 256-byte boundary.
+// The last three serve vpt_render_adaptive.  Then, in VPT_LAYER_* bit order, one [H][W] plane of each exported layer (f32 depth and alpha,
+// float3 the others).  Each part starts on a 256-byte boundary.
 static constexpr size_t kP2pHeader = 512;
 static size_t p2p_round(size_t b) { return (b + 255) & ~(size_t)255; }
-static size_t p2p_accum_bytes(const vpt_context* c) { return p2p_round((size_t)c->p2p_w * c->p2p_h * 12); }
-static size_t p2p_plane_bytes(const vpt_context* c) { return p2p_round((size_t)c->p2p_w * c->p2p_h * 4); }
+static size_t p2p_accum_bytes(size_t px) { return p2p_round(px * 12); }
+static size_t p2p_plane_bytes(size_t px) { return p2p_round(px * 4); }
+static size_t p2p_tiles_offset(size_t px, bool display) { return kP2pHeader + p2p_accum_bytes(px) + (display ? p2p_plane_bytes(px) : 0) + 2 * p2p_plane_bytes(px); }
+// the block of a w x h frame; layer_off[l] (may be null) = byte offset of layer l's plane, 0 for a layer not in `layers`
+static size_t p2p_block_layout(size_t w, size_t h, bool display, unsigned layers, size_t layer_off[kExchangeLayers])
+{
+    const size_t px = w * h;
+    size_t end = p2p_tiles_offset(px, display) + sizeof(unsigned) * kPeerFlagStride;
+    if (layers) end = p2p_round(end);
+    for (int l = 0; l < kExchangeLayers; ++l) {
+        const bool on = (layers >> l) & 1u;
+        if (layer_off) layer_off[l] = on ? end : 0;
+        if (on) end += p2p_round(px * (l < XL_VOLUME ? 4 : 12));
+    }
+    return end;
+}
+static size_t p2p_accum_bytes(const vpt_context* c) { return p2p_accum_bytes((size_t)c->p2p_w * c->p2p_h); }
+static size_t p2p_plane_bytes(const vpt_context* c) { return p2p_plane_bytes((size_t)c->p2p_w * c->p2p_h); }
 static size_t p2p_count_offset(const vpt_context* c) { return kP2pHeader + p2p_accum_bytes(c) + (c->p2p_display ? p2p_plane_bytes(c) : 0); }
 static size_t p2p_err_offset(const vpt_context* c) { return p2p_count_offset(c) + p2p_plane_bytes(c); }
-static size_t p2p_tiles_offset(const vpt_context* c) { return p2p_err_offset(c) + p2p_plane_bytes(c); }
+static size_t p2p_tiles_offset(const vpt_context* c) { return p2p_tiles_offset((size_t)c->p2p_w * c->p2p_h, c->p2p_display); }
 static unsigned long long* p2p_flags(void* block) { return reinterpret_cast<unsigned long long*>(block); }
+static constexpr unsigned kLayerMask = (1u << kExchangeLayers) - 1;
+// Header slot after the error word: what the block was exported for -- width (bits 0-27), height (28-55), display (56), layers (57-63).
+// Every rank's must equal every other's: a rank exported with more planes would store past the end of its peers' blocks.  28 bits hold
+// any size a partitioned frame can have (at most 65535 per side).
+static constexpr int kP2pLayoutSlot = 2 * kPeerFlagStride + 1;
+static unsigned long long p2p_layout_word(const vpt_context* c)
+{
+    return ((unsigned long long)c->p2p_w & 0xfffffffull) | (((unsigned long long)c->p2p_h & 0xfffffffull) << 28) |
+           ((unsigned long long)(c->p2p_display ? 1 : 0) << 56) | ((unsigned long long)c->p2p_layers << 57);
+}
+static std::string hex2(unsigned v) { char b[16]; snprintf(b, sizeof b, "0x%02x", v); return b; }
+static std::string p2p_layout_text(unsigned long long w)
+{
+    return std::to_string(w & 0xfffffffull) + " x " + std::to_string((w >> 28) & 0xfffffffull) + ", display " + std::to_string((w >> 56) & 1ull) +
+           ", layers " + hex2((unsigned)(w >> 57));
+}
+// every mapped peer block must carry this rank's layout word
+static int p2p_check_layouts(vpt_context* c, const char* fn)
+{
+    const unsigned long long mine = p2p_layout_word(c);
+    for (int p = 0; p < c->p2p_n; ++p) {
+        if (p == c->rank) continue;
+        unsigned long long w = 0;
+        VPT_CU(c, cudaMemcpy(&w, p2p_flags(c->p2p_peer[p]) + kP2pLayoutSlot, sizeof(w), cudaMemcpyDefault));
+        if (w != mine)
+            return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block for " + p2p_layout_text(w) +
+                                                ", this rank (" + std::to_string(c->rank) + ") for " + p2p_layout_text(mine) +
+                                                "; every rank must export the same frame size, display and layers");
+    }
+    return VPT_OK;
+}
 
 int comm_p2p_begin(vpt_context* c, cudaStream_t stream) {
     if (!c->p2p_on) return VPT_OK;
@@ -147,6 +196,19 @@ int comm_p2p_end(vpt_context* c, cudaStream_t stream) {
     VPT_CU(c, launch_peer_signal(fl, c->p2p_n, c->rank, 1, c->p2p_epoch, stream));     // my stripes are in every frame ...
     VPT_CU(c, launch_peer_wait(p2p_flags(c->p2p_block), c->p2p_n, 1, c->p2p_epoch, stream));   // ... and everybody's are in mine
     c->launches += 2;
+    return VPT_OK;
+}
+
+int comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream) {
+    if (!c->p2p_on || c->p2p_n < 2 || !c->p2p_layers) return VPT_OK;
+    size_t off[kExchangeLayers];
+    p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, off);
+    LayerPlanes dst;
+    dst.n = c->p2p_n;
+    for (int l = 0; l < kExchangeLayers; ++l)
+        for (int p = 0; off[l] && p < c->p2p_n; ++p) dst.plane[l][p] = reinterpret_cast<float*>(reinterpret_cast<char*>(c->p2p_peer[p]) + off[l]);
+    VPT_CU(c, launch_layers_publish(g, rg, src, dst, stream));
+    c->launches++;
     return VPT_OK;
 }
 
@@ -183,22 +245,54 @@ extern "C" {
 
 int vpt_comm_p2p_export(vpt_context* c, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
                         unsigned char handle_out[VPT_P2P_HANDLE_BYTES]) {
+    return vpt_comm_p2p_export_layers(c, rank, n_ranks, stripe_rows, width, height, with_display, 0u, handle_out);
+}
+
+int vpt_comm_p2p_export_layers(vpt_context* c, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
+                               unsigned layers, unsigned char handle_out[VPT_P2P_HANDLE_BYTES]) {
     if (!c || !handle_out || n_ranks < 1 || n_ranks > vpt::kMaxPeers || rank < 0 || rank >= n_ranks || stripe_rows < 1 || !width || !height)
         return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export: bad arguments (at most 8 ranks: one NVSwitch domain)");
+    if (layers & ~vpt::kLayerMask)
+        return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export_layers: unknown layer bits " + vpt::hex2(layers & ~vpt::kLayerMask));
     if (c->p2p_block) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export: already exported");
     static_assert(sizeof(cudaIpcMemHandle_t) == VPT_P2P_HANDLE_BYTES, "IPC handle size");
+    static_assert(VPT_LAYER_DEPTH == 1u << vpt::XL_DEPTH && VPT_LAYER_ALPHA == 1u << vpt::XL_ALPHA && VPT_LAYER_VOLUME == 1u << vpt::XL_VOLUME &&
+                  VPT_LAYER_SUN == 1u << vpt::XL_SUN && VPT_LAYER_POINT == 1u << vpt::XL_POINT && VPT_LAYER_EMISSION == 1u << vpt::XL_EMISSION &&
+                  VPT_LAYER_ENVIRONMENT == 1u << vpt::XL_ENVIRONMENT, "layer bits");
     VPT_CU(c, cudaSetDevice(c->device));
     int rc = vpt_set_partition(c, rank, n_ranks, stripe_rows);
     if (rc != VPT_OK) return rc;
     VPT_CU(c, vpt::exchange_kernels_preload());
-    c->p2p_w = (int)width; c->p2p_h = (int)height; c->p2p_display = with_display != 0; c->p2p_n = n_ranks;
-    c->p2p_bytes = vpt::p2p_tiles_offset(c) + sizeof(unsigned) * vpt::kPeerFlagStride;
+    c->p2p_w = (int)width; c->p2p_h = (int)height; c->p2p_display = with_display != 0; c->p2p_n = n_ranks; c->p2p_layers = layers;
+    c->p2p_bytes = vpt::p2p_block_layout(width, height, c->p2p_display, layers, nullptr);
     VPT_CU(c, cudaMalloc(&c->p2p_block, c->p2p_bytes));
     VPT_CU(c, cudaMemset(c->p2p_block, 0, c->p2p_bytes));
+    const unsigned long long word = vpt::p2p_layout_word(c);
+    VPT_CU(c, cudaMemcpy(vpt::p2p_flags(c->p2p_block) + vpt::kP2pLayoutSlot, &word, sizeof(word), cudaMemcpyHostToDevice));
     VPT_CU(c, cudaDeviceSynchronize());
     cudaIpcMemHandle_t h;
     VPT_CU(c, cudaIpcGetMemHandle(&h, c->p2p_block));
     memcpy(handle_out, &h, sizeof(h));
+    return VPT_OK;
+}
+
+int vpt_comm_p2p_block_bytes(unsigned width, unsigned height, int with_display, unsigned layers, size_t* out) {
+    if (!out || !width || !height) return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes: bad arguments");
+    if (layers & ~vpt::kLayerMask) return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes: unknown layer bits");
+    *out = vpt::p2p_block_layout(width, height, with_display != 0, layers, nullptr);
+    return VPT_OK;
+}
+
+int vpt_comm_p2p_layer(vpt_context* c, unsigned layer, vpt_devptr_t* d_full) {
+    if (!c || !d_full || !c->p2p_block) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: no exchange block");
+    int l = 0;
+    while (l < vpt::kExchangeLayers && layer != 1u << l) ++l;
+    if (l == vpt::kExchangeLayers) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: " + std::to_string(layer) + " is not one VPT_LAYER_* bit");
+    if (!(c->p2p_layers & layer))
+        return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: the block was exported without layer " + std::to_string(layer) + " (vpt_comm_p2p_export_layers)");
+    size_t off[vpt::kExchangeLayers];
+    vpt::p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, off);
+    *d_full = (vpt_devptr_t)(reinterpret_cast<char*>(c->p2p_block) + off[l]);
     return VPT_OK;
 }
 
@@ -209,6 +303,10 @@ int vpt_comm_p2p_import(vpt_context* c, const unsigned char* handles) {
         cudaIpcMemHandle_t h; memcpy(&h, handles + (size_t)p * VPT_P2P_HANDLE_BYTES, sizeof(h));
         VPT_CU(c, cudaIpcOpenMemHandle(&c->p2p_peer[p], h, cudaIpcMemLazyEnablePeerAccess));
     }
+    if (int rc = vpt::p2p_check_layouts(c, "vpt_comm_p2p_import"); rc != VPT_OK) {
+        for (int p = 0; p < c->p2p_n; ++p) { if (p != c->rank && c->p2p_peer[p]) cudaIpcCloseMemHandle(c->p2p_peer[p]); c->p2p_peer[p] = nullptr; }
+        return rc;
+    }
     c->p2p_on = true; c->p2p_epoch = 0; c->p2p_adapt_epoch = 0;
     return VPT_OK;
 }
@@ -218,6 +316,10 @@ int vpt_comm_p2p_import_local(vpt_context* c, const vpt_devptr_t* blocks) {
     for (int p = 0; p < c->p2p_n; ++p) {
         if (p != c->rank && !blocks[p]) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_import_local: null block");
         c->p2p_peer[p] = p == c->rank ? c->p2p_block : reinterpret_cast<void*>(blocks[p]);
+    }
+    if (int rc = vpt::p2p_check_layouts(c, "vpt_comm_p2p_import_local"); rc != VPT_OK) {
+        for (auto& q : c->p2p_peer) q = nullptr;
+        return rc;
     }
     c->p2p_local = true; c->p2p_on = true; c->p2p_epoch = 0; c->p2p_adapt_epoch = 0;
     return VPT_OK;
@@ -321,7 +423,7 @@ int vpt_comm_destroy(vpt_context* c) {
     if (c->p2p_block) {
         cudaDeviceSynchronize();
         if (!c->p2p_local) for (int p = 0; p < c->p2p_n; ++p) if (p != c->rank && c->p2p_peer[p]) cudaIpcCloseMemHandle(c->p2p_peer[p]);
-        cudaFree(c->p2p_block); c->p2p_block = nullptr; c->p2p_on = false; c->p2p_n = 0;
+        cudaFree(c->p2p_block); c->p2p_block = nullptr; c->p2p_on = false; c->p2p_n = 0; c->p2p_layers = 0;
         for (auto& q : c->p2p_peer) q = nullptr;
     }
     return VPT_OK;

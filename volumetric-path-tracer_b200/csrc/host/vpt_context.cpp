@@ -526,6 +526,16 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     return VPT_OK;
 }
 
+// the rank-local sources of the exchange layers: depth and the frame's active AOVs and light groups (null: not active)
+static vpt::LayerSources layer_sources(const FramePlan& plan) {
+    vpt::LayerSources s;
+    s.src[vpt::XL_DEPTH] = reinterpret_cast<const float*>(plan.fa.kp.depth_buffer);
+    s.src[vpt::XL_ALPHA] = plan.aov.alpha;
+    s.src[vpt::XL_VOLUME] = reinterpret_cast<const float*>(plan.aov.volume);
+    for (int k = 0; k < vpt::kLightGroups; ++k) s.src[vpt::XL_SUN + k] = reinterpret_cast<const float*>(plan.lg.out[k]);
+    return s;
+}
+
 // the frame's trace kernel over whatever k_generate queued for a chunk of np passes
 static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, unsigned np, cudaStream_t stream) {
     vpt::FrameArgs fa = plan.fa;
@@ -603,7 +613,9 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         c->launches += 2;
     }
     // multi-GPU: the one exchange of the path.  Peer-memory mode: the last resolve above already stored every pixel into every rank's
-    // frame; publish and wait for the peers.  NCCL mode: all-gather of the rank-local frame into the caller's full-frame buffers.
+    // frame, the exported layers follow; publish and wait for the peers.  NCCL mode: all-gather of the rank-local frame into the caller's
+    // full-frame buffers.
+    { int rc = vpt::comm_p2p_layers(c, fa.geom, region ? &rg : nullptr, layer_sources(plan), stream); if (rc != VPT_OK) return rc; }
     { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     if (c->nccl_comm && (c->d_full_accum || c->d_full_display)) {
         int rc = vpt::comm_gather_frame(c, fa.geom, (const void*)kp.accum_buffer, (const void*)kp.display_buffer, stream);
@@ -763,6 +775,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         { int rc = await_peers(); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, vpt::launch_adapt_publish(g, fa.kp, ad, peers, stream));
         c->launches++;
+        { int rc = vpt::comm_p2p_layers(c, g, nullptr, layer_sources(plan), stream); if (rc != VPT_OK) return rc; }
         { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }
     if (passes_run) *passes_run = done;

@@ -69,6 +69,7 @@ struct vpt_context {
     void*  p2p_peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [rank] -> that rank's block as mapped here (own: p2p_block)
     int    p2p_n = 0; bool p2p_on = false, p2p_display = false, p2p_local = false; unsigned long long p2p_epoch = 0;
     unsigned long long p2p_adapt_epoch = 0;                     // barriers of the convergence tests of sharded adaptive frames (flag array kPeerFlagsAdapt)
+    unsigned p2p_layers = 0;                                    // VPT_LAYER_* mask the block was exported with (vpt_comm_p2p_export_layers)
     int    gather_async = 0;                                    // option "gather_async": gather on the side stream (see vpt_comm_wait)
     bool   gather_pending = false;
     size_t max_scratch_bytes = (size_t)12 << 30;                // cap of the per-chunk ray queue + sample planes
@@ -144,6 +145,9 @@ FrameGeom make_frame_geom(const vpt_context* c, unsigned w, unsigned h);
 int  comm_p2p_begin(vpt_context* c, cudaStream_t stream);                                        // call start: tell the peers this rank's frame may be overwritten
 int  comm_p2p_peers(vpt_context* c, cudaStream_t stream, PeerFrames* out);                       // before the call's last resolve: wait for the peers, hand out their frames
 int  comm_p2p_end(vpt_context* c, cudaStream_t stream);                                          // after it: publish, and wait until every peer has published
+// right before comm_p2p_end: the exported layers that src holds into every rank's planes (k_layers_publish); nothing when the exchange is
+// suspended, on one rank or without layers.  rg: the frame's render region, null for the whole frame
+int  comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream);
 // sharded adaptive frames: every rank's planes as mapped here, and the local block's halo (err plane), count slots and error word
 struct P2pAdaptLocal { const float* halo = nullptr; const unsigned* tiles = nullptr; const unsigned long long* error_word = nullptr; };
 void comm_p2p_adapt_views(vpt_context* c, AdaptPeers* out, P2pAdaptLocal* local);

@@ -293,6 +293,21 @@ def _frame_tensor(t, numel, name, device):
     return t
 
 
+def _layer_names(layers):
+    """The exchange layers asked for, checked against N.LAYER_BITS, in bit order without repeats."""
+    unknown = [n for n in layers if n not in N.LAYER_BITS]
+    if unknown:
+        raise N.VptError(f"DistributedRenderer: unknown layer(s) {', '.join(map(repr, unknown))} (one of {', '.join(N.LAYER_BITS)})")
+    return tuple(n for n in N.LAYER_BITS if n in layers)
+
+
+def _layer_mask(names):
+    m = 0
+    for n in names:
+        m |= N.LAYER_BITS[n]
+    return m
+
+
 class _DeviceView:
     """Zero-copy torch view of library-owned device memory (__cuda_array_interface__)."""
     def __init__(self, ptr, shape, typestr):
@@ -308,16 +323,23 @@ class DistributedRenderer:
         straight into every rank's full frame over peer mappings -- gather and stripe un-permutation fused into the producer;
       * "nccl": one ncclAllGather of the rank-local accumulators + an un-permutation kernel behind the last kernel of the call.
     Pixels are independent and every Philox stream is keyed by the GLOBAL pixel index, so the gathered frame is bit-identical to a
-    single-GPU render whatever the partition (SURVEY 8(e))."""
+    single-GPU render whatever the partition (SURVEY 8(e)).
 
-    def __init__(self, scene: Scene, width, height, cam=None, kp=None, stripe_rows=16, options=None, gather_display=False, exchange="p2p"):
+    layers: names of N.LAYER_BITS -- "depth", "alpha", "volume" and the LIGHT_GROUPS -- that the peer-memory exchange also carries full-frame
+    to every rank (vpt_comm_p2p_export_layers): full_depth(), full_alpha(), full_volume(), full_light_group(name).  The AOVs and groups must
+    be enabled on every rank (enable_aovs(), enable_light_groups()) and take over at the next call with kp.iteration == 0."""
+
+    def __init__(self, scene: Scene, width, height, cam=None, kp=None, stripe_rows=16, options=None, gather_display=False, exchange="p2p",
+                 layers=()):
         import torch.distributed as dist
         self.dist = dist
         self.rank, self.world = dist.get_rank(), dist.get_world_size()
         if self.world > 8 and exchange == "p2p": exchange = "nccl"
         self.exchange = exchange if self.world > 1 else "none"
+        self.layers = _layer_names(layers)
         self.r = Renderer(scene, width, height, cam=cam, kp=kp, rank=self.rank, n_ranks=self.world,
                           stripe_rows=stripe_rows, options=options)
+        self.last_adaptive = False; self._err1 = None
         n_px = self.r.height * self.r.width
         self.full = None; self.full_display = None
         self.collective_note = "none (1 rank)"
@@ -327,8 +349,9 @@ class DistributedRenderer:
             ok, err = 1, ""
             raw = (C.c_ubyte * 64)()
             try:
-                check(lib.vpt_comm_p2p_export(self.r.ctx, self.rank, self.world, stripe_rows, self.r.width, self.r.height, 1 if gather_display else 0, raw),
-                      self.r.ctx, "vpt_comm_p2p_export")
+                check(lib.vpt_comm_p2p_export_layers(self.r.ctx, self.rank, self.world, stripe_rows, self.r.width, self.r.height,
+                                                     1 if gather_display else 0, _layer_mask(self.layers), raw),
+                      self.r.ctx, "vpt_comm_p2p_export_layers")
             except N.VptError as e:
                 ok, err = 0, str(e)
             mine = torch.tensor(list(raw), dtype=torch.uint8, device=scene.device)
@@ -346,10 +369,7 @@ class DistributedRenderer:
                 if ok: lib.vpt_comm_p2p_enable(self.r.ctx, 0)
                 self.exchange = "nccl"; self.p2p_error = err or "another rank could not set up the peer mappings"
         if self.world > 1 and self.exchange == "p2p":
-            pa, pd = C.c_uint64(0), C.c_uint64(0)
-            check(lib.vpt_comm_p2p_frame(self.r.ctx, C.byref(pa), C.byref(pd)), self.r.ctx, "vpt_comm_p2p_frame")
-            self.full = torch.as_tensor(_DeviceView(pa.value, (n_px, 3), "<f4"), device=scene.device)
-            if gather_display: self.full_display = torch.as_tensor(_DeviceView(pd.value, (n_px,), "<i4"), device=scene.device)
+            self._map_frame(gather_display)
             self.collective_note = ("peer-memory exchange: the last resolve kernel stores each pixel into every rank's frame over NVLink peer mappings "
                                     "(all-gather + un-permutation fused into the producer), two flag exchanges per call; no NCCL on the data path")
         else:
@@ -369,8 +389,33 @@ class DistributedRenderer:
             self.collective_note = (f"1 ncclAllGather (NCCL {v.value}) of the float3 accumulators per step, issued by libvpt_b200.so behind the last "
                                     "resolve kernel, + stripe un-permutation kernel")
 
+    @classmethod
+    def over_exchange(cls, renderer: Renderer, layers=(), gather_display=False):
+        """A DistributedRenderer over a partitioned `renderer` whose peer-memory exchange is already active (vpt_comm_p2p_export_layers with
+        the mask of `layers`, then vpt_comm_p2p_import or _import_local): what __init__ leaves after its torch.distributed bootstrap.  For one
+        process that drives several shards (one Renderer per GPU, or several on one GPU), each shard's calls on its own thread."""
+        self = cls.__new__(cls)
+        self.dist = None
+        self.rank, self.world, self.r = renderer.rank, renderer.n_ranks, renderer
+        self.exchange = "p2p" if self.world > 1 else "none"
+        self.layers = _layer_names(layers)
+        self.last_adaptive = False; self._err1 = None
+        self.full = None; self.full_display = None
+        self.collective_note = "peer-memory exchange set up by the caller"
+        self._map_frame(gather_display)
+        return self
+
+    def _map_frame(self, gather_display):
+        """Zero-copy views of this rank's exchange block: the full-frame accumulators (and display words)."""
+        n_px, dev = self.r.height * self.r.width, self.r.buffers.accum.device
+        pa, pd = C.c_uint64(0), C.c_uint64(0)
+        check(lib.vpt_comm_p2p_frame(self.r.ctx, C.byref(pa), C.byref(pd)), self.r.ctx, "vpt_comm_p2p_frame")
+        self.full = torch.as_tensor(_DeviceView(pa.value, (n_px, 3), "<f4"), device=dev)
+        if gather_display: self.full_display = torch.as_tensor(_DeviceView(pd.value, (n_px,), "<i4"), device=dev)
+
     def render(self, n_passes, stream=None):
         self.r.render(n_passes, stream=stream)                               # the exchange is part of the call
+        self.last_adaptive = False
         if self.world == 1:
             self.full.copy_(self.r.buffers.accum)
             if self.full_display is not None: self.full_display.copy_(self.r.buffers.display)
@@ -384,12 +429,14 @@ class DistributedRenderer:
             raise N.VptError("DistributedRenderer.render_adaptive: adaptive frames need the peer-memory exchange (exchange='p2p'); "
                              "the NCCL exchange does not support them")
         out = self.r.render_adaptive(max_passes, threshold=threshold, min_passes=min_passes, check_interval=check_interval,
-                                     error_map=error_map, stream=stream)
+                                     error_map=error_map or self.world == 1, stream=stream)      # one rank: denoise() keeps the error map
+        self.last_adaptive = True
         H, W = self.r.height, self.r.width
         if self.world == 1:
             self.full.copy_(self.r.buffers.accum)
             if self.full_display is not None: self.full_display.copy_(self.r.buffers.display)
-            return out
+            self._err1 = out[2]
+            return out if error_map else out[:2]
         pc, pe = C.c_uint64(0), C.c_uint64(0)
         check(lib.vpt_comm_p2p_adaptive_frame(self.r.ctx, C.byref(pc), C.byref(pe)), self.r.ctx, "vpt_comm_p2p_adaptive_frame")
         dev = self.full.device
@@ -397,6 +444,69 @@ class DistributedRenderer:
         if not error_map:
             return out[0], counts
         return out[0], counts, torch.as_tensor(_DeviceView(pe.value, (H, W), "<f4"), device=dev)
+
+    def enable_aovs(self):
+        """Renderer.enable_aovs on this rank; every rank enables them.  With layers "alpha" / "volume" the exchange carries them."""
+        self.r.enable_aovs()
+
+    def enable_light_groups(self):
+        """Renderer.enable_light_groups on this rank; every rank enables them.  With LIGHT_GROUPS names in `layers` the exchange carries them."""
+        self.r.enable_light_groups()
+
+    def _layer(self, name, caller):
+        """(H*W, k) full frame of layer `name`: a view of this rank's exchange block, or on one rank a copy of the renderer's buffer."""
+        if name not in self.layers:
+            raise N.VptError(f"DistributedRenderer.{caller}: layer {name!r} was not requested (DistributedRenderer(..., layers=...) has "
+                             f"{', '.join(self.layers) or 'none'})")
+        n_px = self.r.height * self.r.width
+        k = 1 if name in ("depth", "alpha") else 3
+        if self.world == 1:
+            b = self.r.buffers
+            src = b.depth if name == "depth" else getattr(b, name) if name in ("alpha", "volume") else (b.groups or {}).get(name)
+            if src is None:
+                what = "AOVs are" if name in ("alpha", "volume") else "light groups are"
+                raise N.VptError(f"DistributedRenderer.{caller}: {what} not enabled (enable_aovs() / enable_light_groups())")
+            return src.reshape(n_px, k).clone()
+        if self.exchange != "p2p":
+            raise N.VptError(f"DistributedRenderer.{caller}: the {self.exchange} exchange does not carry layers, they stay rank-local; the "
+                             f"peer-memory exchange could not be set up ({getattr(self, 'p2p_error', 'exchange=' + repr(self.exchange))})")
+        p = C.c_uint64(0)
+        check(lib.vpt_comm_p2p_layer(self.r.ctx, N.LAYER_BITS[name], C.byref(p)), self.r.ctx, "vpt_comm_p2p_layer")
+        return torch.as_tensor(_DeviceView(p.value, (n_px, k), "<f4"), device=self.full.device)
+
+    def full_depth(self):
+        """(H, W) float32 depth of the whole frame: a view of this rank's exchange block that the next call overwrites (a copy on one rank)."""
+        return self._layer("depth", "full_depth").view(self.r.height, self.r.width)
+
+    def full_alpha(self):
+        """(H, W) float32 alpha AOV of the whole frame (see full_depth)."""
+        return self._layer("alpha", "full_alpha").view(self.r.height, self.r.width)
+
+    def full_volume(self):
+        """(H, W, 3) float32 volume AOV of the whole frame (see full_depth)."""
+        return self._layer("volume", "full_volume").view(self.r.height, self.r.width, 3)
+
+    def full_light_group(self, name):
+        """(H, W, 3) float32 light group `name` (one of LIGHT_GROUPS) of the whole frame (see full_depth)."""
+        if name not in LIGHT_GROUPS:
+            raise N.VptError(f"DistributedRenderer.full_light_group: unknown light group {name!r} (one of {', '.join(LIGHT_GROUPS)})")
+        return self._layer(name, "full_light_group").view(self.r.height, self.r.width, 3)
+
+    def denoise(self, depth=True, out=None, display=False, iterations=5, sigma_luminance=4.0, sigma_depth=0.2, stream=None):
+        """Renderer.denoise of this rank's full frame: full_accum() guided by full_depth() (depth=False: no depth term) and, after an
+        adaptive frame, by its error map.  Returns what Renderer.denoise returns; equal bit for bit to Renderer.denoise of the same frame
+        rendered on one context."""
+        depth = self.full_depth() if depth else None
+        rel_error = None
+        if self.last_adaptive:
+            if self.world == 1:
+                rel_error = self._err1
+            else:
+                pe = C.c_uint64(0)
+                check(lib.vpt_comm_p2p_adaptive_frame(self.r.ctx, None, C.byref(pe)), self.r.ctx, "vpt_comm_p2p_adaptive_frame")
+                rel_error = torch.as_tensor(_DeviceView(pe.value, (self.r.height, self.r.width), "<f4"), device=self.full.device)
+        return self.r.denoise(color=self.full_accum(), depth=depth if depth is not None else False, rel_error=rel_error, out=out,
+                              display=display, iterations=iterations, sigma_luminance=sigma_luminance, sigma_depth=sigma_depth, stream=stream)
 
     def set_region(self, x0, y0, x1, y1):
         """Renderer.set_region on this rank; every rank sets the same region.  The peer-memory exchange then stores only the region's
