@@ -250,6 +250,40 @@ int  vpt_set_aov_buffers(vpt_context* ctx, float* d_alpha, float* d_volume_f3);
  *     buffer, or another group buffer. */
 int  vpt_set_light_group_buffers(vpt_context* ctx, float* d_sun_f3, float* d_point_f3, float* d_emission_f3, float* d_environment_f3);
 
+/* ---- deep slices: the compositing AOVs binned by the camera ray's collision depth ------------------------------------------------
+ * alpha and volume flatten the whole camera ray, so an element at distance z can only go in front of the volume or behind it.  With a
+ * slice buffer set, every render call also keeps the two AOVs split into K depth intervals, so an element can be put INSIDE the cloud
+ * (deep compositing: a holdout at z keeps the slices in front of it).
+ *
+ *   Slices.  K = n_slices intervals given by the host bounds z_0 < z_1 < ... < z_K (copied at the call), in the units of depth_buffer:
+ *     distance along the camera ray from its origin (the lens sample for a thin lens, the camera origin for a panorama).  A pass sample
+ *     of depth d (the one depth_buffer averages) falls in slice k when d > 0, z_k <= d, and d < z_{k+1} or z_{k+1} = +inf.  So a NaN, a
+ *     miss and a depth outside [z_0, z_K) fall in no slice, and at most one slice takes a sample.
+ *   Per slice, per pixel one float4: (r, g, b) the premultiplied colour, w the coverage.
+ *       coverage sample: 1 if the sample falls in slice k, else 0 (not guarded).
+ *       colour   sample: the sample exactly as it enters accum (after the NaN / Inf guard and the viz_dof tint, as for the volume AOV) if it
+ *                falls in slice k, +0 otherwise (a select, not a product).  When the guard replaced the sample, every slice's colour sample
+ *                is that slice's own mean so far (at iteration 0: the buffer's previous content).
+ *     Both follow accum's rule and arithmetic: iteration == 0 assigns, iteration < max_interactions updates x + (s - x) / (iteration + 1),
+ *     later passes change nothing.  So K = 1 with bounds {0, +inf} is (volume, alpha) bit for bit; slice k of any K is bit for bit the one
+ *     slice of a K = 1 frame with bounds {z_k, z_{k+1}}; with z_0 = 0 and z_K = +inf the slices sum to the AOVs up to the rounding of the
+ *     separate means.  A pass that samples nothing (render == 0, the kernel tail) gives coverage 0 and colour +0.
+ *   Buffer.  Caller-owned device memory of K * vpt_local_pixels() float4, slice-major [K][local pixel] (rank-local order on a partitioned
+ *     context), 16-byte aligned (cudaMalloc's memory is).  A NULL buffer turns the slices off at once (n_slices and h_bounds are then ignored).  Buffer, K and bounds take over at the
+ *     next render call whose Kernel_params.iteration is 0; calls before that leave the buffer untouched.
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active slices.  An adaptive frame's stopped pixels keep theirs, and every
+ *     pixel's slices are bit for bit what a fixed-count frame of its own pass count leaves there.  A render region writes no slice outside
+ *     it.  Every other output is bit for bit what the same call gives without slices.  Level (A) has none.  On a partitioned context the
+ *     slices are rank-local; neither exchange carries them.
+ *   Cost.  A second resolve kernel per chunk: it reads the chunk's sample records again, reads and writes each slice once per pixel
+ *     (K * 32 B) plus once per sample that lands in a slice, and updates every slice once per pass (DESIGN.md section 8h).
+ *   Refused when set (VPT_ERR_INVALID), with a non-NULL buffer: a buffer not 16-byte aligned, n_slices outside 1..VPT_DEEP_MAX_SLICES,
+ *     NULL h_bounds, a NaN or negative bound, bounds not strictly increasing, +inf anywhere but z_K.  A refused call changes nothing.
+ *   Refused at render time (VPT_ERR_INVALID, naming the buffer): a slice buffer that overlaps accum, depth, cost, raw or display, an AOV
+ *     buffer or a light-group buffer. */
+#define VPT_DEEP_MAX_SLICES 32
+int  vpt_set_deep_buffers(vpt_context* ctx, float* d_slices_f4, unsigned n_slices, const float* h_bounds /* n_slices + 1 */);
+
 /* ---- render region: sample and write only a rectangle of the frame ------------------------------------------------------------
  * A viewer that tunes the density, the phase or a light on part of a volume re-renders only that part.  The region R is the half-open
  * rectangle [x0, x1) x [y0, y1) in pixels of the full frame, also on a partitioned context; (0, 0, 0, 0) clears it.

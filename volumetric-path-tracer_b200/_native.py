@@ -162,6 +162,7 @@ EXPORTED_SYMBOLS = [
     "vpt_denoise_options_defaults", "vpt_denoise",
     "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
     "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
+    "vpt_set_deep_buffers",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -192,6 +193,8 @@ lib.vpt_render_adaptive.argtypes = [_vp, C.POINTER(_vp), C.c_uint, C.POINTER(ada
 lib.vpt_render_adaptive.restype = C.c_int
 lib.vpt_set_aov_buffers.argtypes = [_vp, _vp, _vp]; lib.vpt_set_aov_buffers.restype = C.c_int
 lib.vpt_set_light_group_buffers.argtypes = [_vp, _vp, _vp, _vp, _vp]; lib.vpt_set_light_group_buffers.restype = C.c_int
+VPT_DEEP_MAX_SLICES = 32                                            # vpt_set_deep_buffers: most slices
+lib.vpt_set_deep_buffers.argtypes = [_vp, _vp, C.c_uint, C.POINTER(C.c_float)]; lib.vpt_set_deep_buffers.restype = C.c_int
 lib.vpt_set_render_region.argtypes = [_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint]; lib.vpt_set_render_region.restype = C.c_int
 VPT_PROJECTION_PERSPECTIVE, VPT_PROJECTION_EQUIRECT = 0, 1          # vpt_set_projection kinds
 lib.vpt_set_projection.argtypes = [_vp, C.c_int, C.c_double, C.c_double]; lib.vpt_set_projection.restype = C.c_int

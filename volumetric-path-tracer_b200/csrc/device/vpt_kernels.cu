@@ -518,15 +518,93 @@ struct PeerFlagPtrs { unsigned long long* p[kMaxPeers]; };
 
 template <int kSky> using SkyArg = typename std::conditional<kSky != 0, vpt_atmosphere, NoSky>::type;
 
+// The deep slice of a sample of depth d: the k with z[k] <= d < z[k + 1] (or z[n] = +inf), -1 when d is not > 0 (a miss, NaN) or lies
+// outside [z[0], z[n]).  Binary search over the bounds in the parameter block.
+__device__ __forceinline__ int deep_slice(const DeepSlices& dp, const float d)
+{
+    if (!(d > 0.0f) || !(d >= dp.z[0])) return -1;
+    int lo = 0, hi = dp.n + 1;                                  // z[lo] <= d < z[hi] (z[n + 1] standing for +inf)
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (dp.z[mid] <= d) lo = mid; else hi = mid;
+    }
+    if (lo < dp.n) return lo;
+    return isinf(dp.z[dp.n]) ? dp.n - 1 : -1;                   // d >= z[n]: only d = +inf under an open last slice
+}
+// One pass of a deep slice's running means {colour, coverage} with colour sample s and coverage sample c: accum's rule and arithmetic,
+// written as the AOVs' (iteration 0 assigns, iteration < max_interactions updates x + (s - x) / (iteration + 1), later passes keep x)
+__device__ __forceinline__ float4 deep_step(const float4 x, const float3 s, const float c, const uint32_t iteration, const uint32_t max_interactions)
+{
+    if (iteration == 0) return make_float4(s.x, s.y, s.z, c);
+    if (iteration < max_interactions) {
+        float3 v = f3(x.x, x.y, x.z);
+        float w = x.w;
+        v = v + (s - v) / (float)(iteration + 1);
+        w = w + (c - w) / (float)(iteration + 1);
+        return make_float4(v.x, v.y, v.z, w);
+    }
+    return x;
+}
+
+// The deep slices of one pixel during a chunk (resolve_pixel, kDeep).  K running means do not fit in registers, so each stays in its buffer
+// and is updated lazily.  A pass that puts no sample in slice k updates it by x + (0 - x) / (iteration + 1), which needs nothing but x,
+// so those updates wait until a sample lands in the slice (or the guard replaces a sample: then every slice takes a pass) and the end of
+// the chunk, where every slice catches up.  done[k] = the passes of the chunk applied to slice k so far (a chunk that samples has at most
+// 64 passes; one that samples nothing lands no sample, so done[] stays 0 there).
+// The deep instantiations of resolve_pixel keep only the slices and store nothing else; launch_resolve runs the frame's own resolve kernel
+// after them.  (Computing the slices inside that kernel moved accum and raw by an ulp in some frames: nvcc contracts the unpinned sky and
+// tonemap arithmetic differently once the slice code is in the kernel, inlined or behind a call.)
+struct DeepPixel { uint32_t lp, n_local, it0, max_interactions; };
+
+// slice k's means after the chunk's passes before `upto`, none of which since done[k] put a sample in it (at iteration 0 the zero sample
+// is assigned, so the buffer is not read)
+__device__ __forceinline__ float4 deep_catch_up(const DeepSlices& dp, const uint8_t* done, const DeepPixel& px, const int k, const int upto)
+{
+    int q = done[k];
+    float4 x;
+    if (q < upto && px.it0 + (uint32_t)q == 0) { x = make_float4(0.f, 0.f, 0.f, 0.f); ++q; }
+    else x = dp.out[(size_t)k * px.n_local + px.lp];
+    for (; q < upto && px.it0 + (uint32_t)q < px.max_interactions; ++q) x = deep_step(x, f3(0.f), 0.0f, px.it0 + (uint32_t)q, px.max_interactions);
+    return x;
+}
+
+// pass p of the chunk with the sample `value` (as it entered accum) of depth `depth`: its slice takes (value, 1) as the volume AOV takes
+// it; a sample the guard replaced gives every slice its own mean as colour (at iteration 0: the buffer's previous content) and its slice
+// the coverage 1 (coverage is not guarded)
+__device__ __forceinline__ void deep_pass(const DeepSlices& dp, uint8_t* done, const DeepPixel px, const int p, const float3 value, const float depth,
+                                          const bool guarded)
+{
+    const uint32_t iteration = px.it0 + (uint32_t)p;
+    const int b = deep_slice(dp, depth);
+    if (guarded) {
+        for (int k = 0; k < dp.n; ++k) {
+            const float4 x = deep_catch_up(dp, done, px, k, p);
+            dp.out[(size_t)k * px.n_local + px.lp] = deep_step(x, f3(x.x, x.y, x.z), k == b ? 1.0f : 0.0f, iteration, px.max_interactions);
+            done[k] = (uint8_t)(p + 1);
+        }
+    } else if (b >= 0) {
+        dp.out[(size_t)b * px.n_local + px.lp] = deep_step(deep_catch_up(dp, done, px, b, p), value, 1.0f, iteration, px.max_interactions);
+        done[b] = (uint8_t)(p + 1);
+    }
+}
+
+// the end of a chunk of n_passes passes: every slice catches up
+__device__ __forceinline__ void deep_end(const DeepSlices& dp, const uint8_t* done, const DeepPixel px, const int n_passes)
+{
+    for (int k = 0; k < dp.n; ++k)
+        if (done[k] < n_passes) dp.out[(size_t)k * px.n_local + px.lp] = deep_catch_up(dp, done, px, k, n_passes);
+}
+
 // One pixel of k_resolve (local pixel lp, local row lr, global row y).  kAdaptive (k_resolve_adaptive): the same running mean, plus the
 // pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.  kAov: also the running means of
 // the compositing AOVs in `aov` (DESIGN.md section 8c).  kGroups: also the running means of the light groups in `lg` (section 8d).
 // kPano (k_resolve_equirect, ...; HDRI frames): a culled pixel's miss samples are the equirectangular rays of the projection `pj`.
-template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false>
+// kDeep: the deep slices in `dp` (section 8h), updated lazily in their buffer, and no other store (see deep_pass).
+template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false, bool kDeep = false>
 __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                               const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
                                               const AdaptArgs* ad, const AovBuffers* aov, const LightGroups* lg = nullptr,
-                                              const Projection* pj = nullptr)
+                                              const Projection* pj = nullptr, const DeepSlices* dp = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
@@ -555,6 +633,9 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         #pragma unroll
         for (int k = 0; k < kLightGroups; ++k) gm[k] = ((have_prev || !sampled) && lg->out[k]) ? lg->out[k][lp] : f3(0.f);
     }
+    // deep slices: the passes of the chunk applied to each slice so far (deep_pass)
+    uint8_t done[kDeep ? kDeepMaxSlices : 1] = {};
+    const DeepPixel dpx{lp, (uint32_t)g.n_local, kp.iteration, kp.max_interactions};
     // compact records (HDRI frames traced by a lean kernel, planeB null): one float4 per sample
     const bool compact = kSky == 0 && !fa.planeB;
     // a pixel culled by k_miss_cull has no records: every sample is the pinhole miss k_generate would have stored, direction rebuilt from
@@ -632,7 +713,7 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         // NaN / Inf guard (:2263-2264): the sample becomes accum_buffer[idx].  At iteration 0 (the call's first pass) that is the buffer's
         // previous content, which was not loaded; the AOVs and groups take their own buffers' previous content likewise.
         bool guarded = false;                                   // AOVs / groups only, apart from the guard: the other instantiations keep their code
-        if constexpr (kAov || kGroups) guarded = any_nan(value) || any_inf(value);
+        if constexpr (kAov || kGroups || kDeep) guarded = any_nan(value) || any_inf(value);
         if (any_nan(value) || any_inf(value)) {
             if (iteration == 0) {
                 accum = accum_buf[lp];
@@ -681,6 +762,7 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
                 else if (iteration < kp.max_interactions) gm[k] = gm[k] + (gv - gm[k]) / (float)(iteration + 1);
             }
         }
+        if constexpr (kDeep) deep_pass(*dp, done, dpx, p, value, depth, guarded);
         if constexpr (kAdaptive) {                              // the sample as it entered the mean (after the NaN guard and the tint)
             const float lum = 0.2126f * value.x + 0.7152f * value.y + 0.0722f * value.z;
             wn += 1.0f;
@@ -713,6 +795,8 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             one_pass(p, A, B, C);
         }
     }
+    // the deep instantiations keep the slices and store nothing else: the frame's own resolve kernel runs after them (launch_resolve)
+    if constexpr (kDeep) { deep_end(*dp, done, dpx, n_passes); return; }
     accum_buf[lp] = accum; cost_buf[lp] = costv; depth_buf[lp] = depthv;
     if constexpr (kAov) { if (aov->alpha) aov->alpha[lp] = alphav; if (aov->volume) aov->volume[lp] = volv; }
     if constexpr (kGroups) {
@@ -746,10 +830,21 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
 }
 
 // kAov / kGroups: the instantiations that also keep the compositing AOVs / the light groups take the AovBuffers / the LightGroups as
-// more arguments (the pack `ext`, in that order, empty otherwise), so the kernels without them keep their parameter block.
+// more arguments (the pack `ext`, in that order, empty otherwise), so the kernels without them keep their parameter block.  The deep
+// instantiations end the pack with a DeepSlices; it is the pack, not a template flag, that selects them, so every kernel without deep
+// slices keeps its name as well.
 __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a) { return &a; }
 __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const LightGroups&) { return &a; }
 __device__ __forceinline__ const LightGroups* lg_of(const AovBuffers&, const LightGroups& l) { return &l; }
+__device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const DeepSlices&) { return &a; }
+__device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const LightGroups&, const DeepSlices&) { return &a; }
+__device__ __forceinline__ const LightGroups* lg_of(const LightGroups& l, const DeepSlices&) { return &l; }
+__device__ __forceinline__ const LightGroups* lg_of(const AovBuffers&, const LightGroups& l, const DeepSlices&) { return &l; }
+template <class... Ext> constexpr bool has_deep = (std::is_same<Ext, DeepSlices>::value || ... || false);
+__device__ __forceinline__ const DeepSlices* deep_of(const DeepSlices& d) { return &d; }
+__device__ __forceinline__ const DeepSlices* deep_of(const AovBuffers&, const DeepSlices& d) { return &d; }
+__device__ __forceinline__ const DeepSlices* deep_of(const LightGroups&, const DeepSlices& d) { return &d; }
+__device__ __forceinline__ const DeepSlices* deep_of(const AovBuffers&, const LightGroups&, const DeepSlices& d) { return &d; }
 
 // The thread's pixel and its resolve_pixel, shared by k_resolve and k_resolve_equirect (kPano: the projection `pj`)
 template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
@@ -764,9 +859,12 @@ __device__ __forceinline__ void resolve_body(const FrameArgs& fa, const SkyArg<k
     if (y >= g.height) return;
     const AovBuffers* ap = nullptr;
     const LightGroups* gp = nullptr;
+    const DeepSlices* dq = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups, kPano>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp, pj);
+    if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
+    resolve_pixel<kSky, false, kAov, kGroups, kPano, has_deep<Ext...>>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp,
+                                                                       pj, dq);
 }
 
 template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
@@ -774,7 +872,7 @@ __global__ void __launch_bounds__(256)
 k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
           const Ext... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
     resolve_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, sampled, write_display, peers, nullptr, ext...);
 }
 
@@ -795,9 +893,12 @@ __device__ __forceinline__ void resolve_region_body(const FrameArgs& fa, const S
     const uint32_t lp = (uint32_t)lr * (uint32_t)g.width + (uint32_t)rg.x0 + (i - r * w);
     const AovBuffers* ap = nullptr;
     const LightGroups* gp = nullptr;
+    const DeepSlices* dq = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups, kPano>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, global_row(g, lr), nullptr, ap, gp, pj);
+    if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
+    resolve_pixel<kSky, false, kAov, kGroups, kPano, has_deep<Ext...>>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, global_row(g, lr),
+                                                                       nullptr, ap, gp, pj, dq);
 }
 
 template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
@@ -805,7 +906,7 @@ __global__ void __launch_bounds__(256)
 k_resolve_region(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
                  const RenderRegion rg, const Ext... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_region<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_region<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
     resolve_region_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, sampled, write_display, peers, rg, nullptr, ext...);
 }
 
@@ -816,7 +917,7 @@ __global__ void __launch_bounds__(256)
 k_resolve_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
                    const Projection pj, const Ext... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
     resolve_body<0, kAov, kGroups, true>(fa, atmo, n_passes, sampled, write_display, peers, &pj, ext...);
 }
 
@@ -825,7 +926,7 @@ __global__ void __launch_bounds__(256)
 k_resolve_region_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
                           const RenderRegion rg, const Projection pj, const Ext... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_region_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_region_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
     resolve_region_body<0, kAov, kGroups, true>(fa, atmo, n_passes, sampled, write_display, peers, rg, &pj, ext...);
 }
 
@@ -853,16 +954,19 @@ __device__ __forceinline__ void resolve_adaptive_body(const FrameArgs& fa, const
     if (ad.stopped[lp]) return;
     const AovBuffers* ap = nullptr;
     const LightGroups* gp = nullptr;
+    const DeepSlices* dq = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
-    resolve_pixel<kSky, true, kAov, kGroups, kPano>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap, gp, pj);
+    if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
+    resolve_pixel<kSky, true, kAov, kGroups, kPano, has_deep<Ext...>>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap,
+                                                                      gp, pj, dq);
 }
 
 template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
 __global__ void __launch_bounds__(128)
 k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Ext... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_adaptive<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_adaptive<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
     resolve_adaptive_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, ad, nullptr, ext...);
 }
 
@@ -870,7 +974,7 @@ template <bool kAov = false, bool kGroups = false, class... Ext>
 __global__ void __launch_bounds__(128)
 k_resolve_adaptive_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const AdaptArgs ad, const Projection pj, const Ext... ext)
 {
-    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0), "k_resolve_adaptive_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups");
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_adaptive_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
     resolve_adaptive_body<0, kAov, kGroups, true>(fa, atmo, n_passes, ad, &pj, ext...);
 }
 
@@ -1235,12 +1339,35 @@ static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const 
     }
 }
 
+// The three resolve kernels of key {S, A, G} whose pack `e` ends with the DeepSlices, in the form of resolve_kernels below
+template <int S, bool A, bool G, class F, class Sky, class... E>
+static cudaError_t resolve_kernels_deep(F&& f, const Sky& sky, const E&... e)
+{
+    return f(+k_resolve<S, A, G, E...>, +k_resolve_adaptive<S, A, G, E...>, +k_resolve_region<S, A, G, E...>, sky, e...);
+}
+
 // The resolve kernels: f(k_resolve<S, A, G>, k_resolve_adaptive<S, A, G>, k_resolve_region<S, A, G>, the sky argument, the trailing
-// AovBuffers / LightGroups) for key {S, A, G}, case S * 4 + A * 2 + G.
+// AovBuffers / LightGroups / DeepSlices) for key {S, A, G, D}, case S * 4 + A * 2 + G of the table without (D false) or with the deep slices.
 template <class F>
-static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, F&& f)
+static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp,
+                                   F&& f)
 {
     const NoSky hdri{};
+    if (r.deep) switch (r.sky * 4 + r.aov * 2 + r.groups) {
+    case 0:  return resolve_kernels_deep<0, false, false>(f, hdri, dp);
+    case 1:  return resolve_kernels_deep<0, false, true>(f, hdri, lg, dp);
+    case 2:  return resolve_kernels_deep<0, true, false>(f, hdri, aov, dp);
+    case 3:  return resolve_kernels_deep<0, true, true>(f, hdri, aov, lg, dp);
+    case 4:  return resolve_kernels_deep<1, false, false>(f, atm, dp);
+    case 5:  return resolve_kernels_deep<1, false, true>(f, atm, lg, dp);
+    case 6:  return resolve_kernels_deep<1, true, false>(f, atm, aov, dp);
+    case 7:  return resolve_kernels_deep<1, true, true>(f, atm, aov, lg, dp);
+    case 8:  return resolve_kernels_deep<2, false, false>(f, atm, dp);
+    case 9:  return resolve_kernels_deep<2, false, true>(f, atm, lg, dp);
+    case 10: return resolve_kernels_deep<2, true, false>(f, atm, aov, dp);
+    case 11: return resolve_kernels_deep<2, true, true>(f, atm, aov, lg, dp);
+    default: return cudaErrorInvalidValue;
+    }
     switch (r.sky * 4 + r.aov * 2 + r.groups) {
     case 0:  return f(k_resolve<0>, k_resolve_adaptive<0>, k_resolve_region<0>, hdri);
     case 1:  return f(+k_resolve<0, false, true, LightGroups>, +k_resolve_adaptive<0, false, true, LightGroups>, +k_resolve_region<0, false, true, LightGroups>, hdri, lg);
@@ -1258,13 +1385,27 @@ static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& at
     }
 }
 
+template <bool A, bool G, class F, class... E>
+static cudaError_t resolve_kernels_equirect_deep(F&& f, const NoSky& sky, const E&... e)
+{
+    return f(+k_resolve_equirect<A, G, E...>, +k_resolve_adaptive_equirect<A, G, E...>, +k_resolve_region_equirect<A, G, E...>, sky, e...);
+}
+
 // The equirectangular resolve kernels of the HDRI frames, in the form of resolve_kernels: f(k_resolve_equirect<A, G>,
-// k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G>, the sky argument, the trailing AovBuffers / LightGroups), case A * 2 + G.
+// k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G>, the sky argument, the trailing AovBuffers / LightGroups / DeepSlices),
+// case A * 2 + G of the table without or with the deep slices.
 template <class F>
-static cudaError_t resolve_kernels_equirect(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, F&& f)
+static cudaError_t resolve_kernels_equirect(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, F&& f)
 {
     const NoSky hdri{};
     if (r.sky != 0) return cudaErrorInvalidValue;
+    if (r.deep) switch (r.aov * 2 + r.groups) {
+    case 0:  return resolve_kernels_equirect_deep<false, false>(f, hdri, dp);
+    case 1:  return resolve_kernels_equirect_deep<false, true>(f, hdri, lg, dp);
+    case 2:  return resolve_kernels_equirect_deep<true, false>(f, hdri, aov, dp);
+    case 3:  return resolve_kernels_equirect_deep<true, true>(f, hdri, aov, lg, dp);
+    default: return cudaErrorInvalidValue;
+    }
     switch (r.aov * 2 + r.groups) {
     case 0:  return f(k_resolve_equirect<false, false>, k_resolve_adaptive_equirect<false, false>, k_resolve_region_equirect<false, false>, hdri);
     case 1:  return f(+k_resolve_equirect<false, true, LightGroups>, +k_resolve_adaptive_equirect<false, true, LightGroups>, +k_resolve_region_equirect<false, true, LightGroups>, hdri, lg);
@@ -1316,15 +1457,17 @@ cudaError_t exchange_kernels_preload()
     }
     for (int sky = 0; sky < 3; ++sky)
         for (bool aov : {false, true})
-            for (bool groups : {false, true}) {
-                const cudaError_t e = resolve_kernels(ResolveKey{sky, aov, groups}, {}, {}, {},
-                                                      [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
-                if (e != cudaSuccess) return e;
-                if (sky != 0) continue;
-                const cudaError_t ep = resolve_kernels_equirect(ResolveKey{sky, aov, groups}, {}, {},
-                                                                [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
-                if (ep != cudaSuccess) return ep;
-            }
+            for (bool groups : {false, true})
+                for (bool deep : {false, true}) {
+                    const ResolveKey key{sky, aov, groups, deep};
+                    const cudaError_t e = resolve_kernels(key, {}, {}, {}, {},
+                                                          [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
+                    if (e != cudaSuccess) return e;
+                    if (sky != 0) continue;
+                    const cudaError_t ep = resolve_kernels_equirect(key, {}, {}, {},
+                                                                    [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
+                    if (ep != cudaSuccess) return ep;
+                }
     return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
@@ -1337,57 +1480,94 @@ cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, co
     return cudaGetLastError();
 }
 
-cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s)
+static cudaError_t resolve_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
+                                  cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     if (equirect(pj) && key.sky == 0)
-        return resolve_kernels_equirect(key, aov, lg, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+        return resolve_kernels_equirect(key, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
             kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, pj, ext...);
             return cudaGetLastError();
         });
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
-    return resolve_kernels(key, atm, aov, lg, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
         kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, ext...);
         return cudaGetLastError();
     });
 }
 
-cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, const Projection& pj,
-                                  cudaStream_t s)
+static cudaError_t resolve_region_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled,
+                                         int write_display, const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp,
+                                         const RenderRegion& rg, const Projection& pj, cudaStream_t s)
 {
     const long long n = region_pixels(rg);
     if (n <= 0) return cudaSuccess;
     const int threads = 256;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     if (equirect(pj) && key.sky == 0)
-        return resolve_kernels_equirect(key, aov, lg, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+        return resolve_kernels_equirect(key, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
             kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, pj, ext...);
             return cudaGetLastError();
         });
-    return resolve_kernels(key, atm, aov, lg, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
         kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, ext...);
         return cudaGetLastError();
     });
 }
 
-cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s)
+static cudaError_t resolve_adaptive_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
+                                           const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
     if (equirect(pj) && key.sky == 0)
-        return resolve_kernels_equirect(key, aov, lg, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+        return resolve_kernels_equirect(key, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
             kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, pj, ext...);
             return cudaGetLastError();
         });
-    return resolve_kernels(key, atm, aov, lg, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
         kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, ext...);
         return cudaGetLastError();
     });
+}
+
+// With deep slices (key.deep) a resolve is two launches: the deep instantiation, which keeps the slices only and reads accum and the AOVs
+// before they change, then the frame's own kernel, the very one without slices -- so every other output is bit for bit the same.
+static ResolveKey without_deep(const ResolveKey& key) { ResolveKey k = key; k.deep = false; return k; }
+
+cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
+                           cudaStream_t s)
+{
+    if (key.deep) {
+        const cudaError_t e = resolve_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, pj, s);
+        if (e != cudaSuccess) return e;
+    }
+    return resolve_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, pj, s);
+}
+
+cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,
+                                  const Projection& pj, cudaStream_t s)
+{
+    if (key.deep) {
+        const cudaError_t e = resolve_region_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, rg, pj, s);
+        if (e != cudaSuccess) return e;
+    }
+    return resolve_region_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, rg, pj, s);
+}
+
+cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
+                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s)
+{
+    if (key.deep) {
+        const cudaError_t e = resolve_adaptive_launch(fa, key, atm, n_passes, ad, aov, lg, dp, pj, s);
+        if (e != cudaSuccess) return e;
+    }
+    return resolve_adaptive_launch(fa, without_deep(key), atm, n_passes, ad, aov, lg, dp, pj, s);
 }
 
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s)

@@ -163,11 +163,18 @@ struct AovBuffers { float* alpha = nullptr; float3* volume = nullptr; };
 // instantiations of k_trace / k_resolve / k_resolve_adaptive only, as AovBuffers is.
 enum LightGroup : int { LG_SUN = 0, LG_POINT = 1, LG_EMISSION = 2, LG_ENVIRONMENT = 3, kLightGroups = 4 };
 struct LightGroups { float3* out[kLightGroups] = {}; float* planes = nullptr; unsigned long long stride = 0; };
+// Deep slices (vpt_set_deep_buffers): out[k * n_local + local pixel] = slice k's running means {premultiplied colour, coverage} of the
+// samples whose depth d has z[k] <= d < z[k + 1] (z[n] may be +inf), d > 0.  n = 1..kDeepMaxSlices, z strictly increasing.  A kernel
+// argument of the deep instantiations of k_resolve / k_resolve_adaptive / k_resolve_region only (the last of the pack), as AovBuffers is.
+constexpr int kDeepMaxSlices = 32;                    // VPT_DEEP_MAX_SLICES of vpt_b200.h
+struct DeepSlices { float4* out = nullptr; int n = 0; float z[kDeepMaxSlices + 1] = {}; };
 // Which k_resolve / k_resolve_adaptive a frame runs (instantiations: resolve_kernels in vpt_kernels.cu).  sky: 0 HDRI, 1 the precomputed
-// sky, 2 the volumetric path integrator (ends on that sky; atm: the caller's AtmosphereParameters); with the AOVs; with the light groups.
-struct ResolveKey { int sky = 0; bool aov = false, groups = false; };
+// sky, 2 the volumetric path integrator (ends on that sky; atm: the caller's AtmosphereParameters); with the AOVs; with the light groups;
+// with the deep slices.
+struct ResolveKey { int sky = 0; bool aov = false, groups = false, deep = false; };
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s);
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
+                           cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -198,7 +205,7 @@ cudaError_t launch_camera_rays(const vpt_camera& cam, const vpt_u2 res, const Fr
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, const Projection& pj, cudaStream_t s);
+                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);
@@ -211,8 +218,8 @@ cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* ti
 cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
 cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const RenderRegion& rg, const Projection& pj,
-                                  cudaStream_t s);
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,
+                                  const Projection& pj, cudaStream_t s);
 cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s);
 cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s);
 

@@ -160,6 +160,33 @@ int vpt_set_light_group_buffers(vpt_context* c, float* d_sun_f3, float* d_point_
     return VPT_OK;
 }
 
+static_assert(vpt::kDeepMaxSlices == VPT_DEEP_MAX_SLICES, "deep slice limit");
+
+int vpt_set_deep_buffers(vpt_context* c, float* d_slices_f4, unsigned n_slices, const float* h_bounds) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_deep_buffers: null context");
+    vpt::DeepSlices d;
+    if (d_slices_f4) {
+        if (n_slices < 1 || n_slices > VPT_DEEP_MAX_SLICES)
+            return fail(c, VPT_ERR_INVALID, "vpt_set_deep_buffers: n_slices must be in 1.." + std::to_string(VPT_DEEP_MAX_SLICES) + ", got " + std::to_string(n_slices));
+        if ((uintptr_t)d_slices_f4 % 16 != 0)
+            return fail(c, VPT_ERR_INVALID, "vpt_set_deep_buffers: the slice buffer must be 16-byte aligned (the kernels move float4)");
+        if (!h_bounds) return fail(c, VPT_ERR_INVALID, "vpt_set_deep_buffers: null bounds");
+        for (unsigned k = 0; k <= n_slices; ++k) {
+            const float z = h_bounds[k];
+            const std::string at = "vpt_set_deep_buffers: bound " + std::to_string(k) + " (" + std::to_string(z) + ") ";
+            if (std::isnan(z) || z < 0.0f) return fail(c, VPT_ERR_INVALID, at + "must be a number >= 0");
+            if (std::isinf(z) && k < n_slices) return fail(c, VPT_ERR_INVALID, at + "is infinite: only the last bound may be +inf");
+            if (k > 0 && !(z > h_bounds[k - 1])) return fail(c, VPT_ERR_INVALID, at + "must be greater than the bound before it");
+            d.z[k] = z;
+        }
+        d.out = reinterpret_cast<float4*>(d_slices_f4);
+        d.n = (int)n_slices;
+    }
+    c->deep_req = d;
+    c->deep_active = false;         // null: off from now on; otherwise the slices take over at the next call with iteration == 0
+    return VPT_OK;
+}
+
 int vpt_set_render_region(vpt_context* c, unsigned x0, unsigned y0, unsigned x1, unsigned y1) {
     if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_render_region: null context");
     c->region_req[0] = x0; c->region_req[1] = y0; c->region_req[2] = x1; c->region_req[3] = y1;   // checked and taken at the next iteration-0 call
@@ -251,6 +278,7 @@ struct FramePlan {
     unsigned n_sampled = 0;               // how many of the requested passes sample (the rest only re-tonemap)
     vpt::AovBuffers aov;                  // the active compositing AOVs (both null: off)
     vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
+    vpt::DeepSlices deep;                 // the active deep slices (out null: off)
     bool region = false;                  // a render region is active: the region kernels over rg
     vpt::RenderRegion rg;
     vpt::Projection proj;                 // the frame's projection: the equirectangular kernels when equirect(proj)
@@ -309,6 +337,21 @@ static int check_light_group_buffers(vpt_context* c, const vpt_kernel_params& kp
             if (byte_ranges_overlap(c->lg_out[k], 12 * n, c->lg_out[j], 12 * n))
                 return fail(c, VPT_ERR_INVALID, std::string("vpt_set_light_group_buffers: the ") + names[j] + " buffer and the " + names[k] + " buffer overlap");
     }
+    return VPT_OK;
+}
+
+// The slice buffer may not share a byte with a Kernel_params output buffer, an AOV buffer or a light-group buffer (n = local pixels).
+static int check_deep_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    const struct { const char* name; const void* p; size_t bytes; } others[] = {
+        { "Kernel_params.accum_buffer", (const void*)(uintptr_t)kp.accum_buffer, 12 * n }, { "Kernel_params.depth_buffer", (const void*)(uintptr_t)kp.depth_buffer, 4 * n },
+        { "Kernel_params.cost_buffer", (const void*)(uintptr_t)kp.cost_buffer, 12 * n }, { "Kernel_params.raw_buffer", (const void*)(uintptr_t)kp.raw_buffer, 16 * n },
+        { "Kernel_params.display_buffer", (const void*)(uintptr_t)kp.display_buffer, 4 * n },
+        { "the alpha AOV buffer", c->aov_alpha, 4 * n }, { "the volume AOV buffer", c->aov_volume, 12 * n },
+        { "the sun light-group buffer", c->lg_out[0], 12 * n }, { "the point light-group buffer", c->lg_out[1], 12 * n },
+        { "the emission light-group buffer", c->lg_out[2], 12 * n }, { "the environment light-group buffer", c->lg_out[3], 12 * n } };
+    for (const auto& o : others)
+        if (byte_ranges_overlap(c->deep_req.out, 16 * n * (size_t)c->deep_req.n, o.p, o.bytes))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_deep_buffers: the slice buffer overlaps ") + o.name);
     return VPT_OK;
 }
 
@@ -519,6 +562,14 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     plan.resolve.sky = sky_env ? (vol_integ ? 2 : 1) : 0;
     plan.resolve.aov = plan.aov.alpha || plan.aov.volume;
     plan.resolve.groups = plan.lg.out[0] || plan.lg.out[1] || plan.lg.out[2] || plan.lg.out[3];
+    // deep slices: the buffer, its slice count and bounds take over at the first call of a frame (iteration == 0), checked on every call
+    if (c->deep_active || (kp.iteration == 0 && c->deep_req.out)) {
+        int rc = check_deep_buffers(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+        c->deep_active = true;
+        plan.deep = c->deep_req;
+    }
+    plan.resolve.deep = plan.deep.out != nullptr;
     plan.proj = proj;
     if (kp.iteration == 0) { memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req; }
     plan.region = region;
@@ -593,11 +644,11 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
-            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, rg,
+            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, rg,
                                                        plan.proj, stream)
-                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg,
+                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep,
                                                 plan.proj, stream); }));
-        c->launches += 4;
+        c->launches += 4 + (plan.resolve.deep ? 1 : 0);            // with deep slices the resolve is two kernels
         done += np;
     }
     if (n_sampled < n_passes) {
@@ -606,11 +657,11 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, rg,
+        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, rg,
                                                            plan.proj, stream));
-        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.proj, stream));
+        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.proj, stream));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
-        c->launches += 2;
+        c->launches += 2 + (plan.resolve.deep ? 1 : 0);
     }
     // multi-GPU: the one exchange of the path.  Peer-memory mode: the last resolve above already stored every pixel into every rank's
     // frame, the exported layers follow; publish and wait for the peers.  NCCL mode: all-gather of the rank-local frame into the caller's
@@ -736,8 +787,8 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.proj, stream); }));
-            c->launches += 3;
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.proj, stream); }));
+            c->launches += 3 + (plan.resolve.deep ? 1 : 0);
         }
         done += np;
         if (done == next_test && done < n_total) {

@@ -96,6 +96,10 @@ struct vpt_context {
     bool      lg_active = false;
     float*    d_lg_planes = nullptr;
     size_t    cap_lg_samples = 0;
+    // deep slices (vpt_set_deep_buffers): a caller-owned [slice][local pixel] float4 buffer with its slice count and bounds, checked when set
+    // (deep_req.out null: off) and activated like the AOVs
+    vpt::DeepSlices deep_req;
+    bool      deep_active = false;
     // render region (vpt_set_render_region): global pixels [x0, x1) x [y0, y1), all 0 = the whole frame.  region_req is what the caller
     // set last; it becomes region_cur at the next render call with iteration == 0, so a running mean never continues under another region
     unsigned  region_req[4] = {0, 0, 0, 0};

@@ -23,7 +23,8 @@ LIGHT_GROUPS = ("sun", "point", "emission", "environment")
 class FrameBuffers:
     """accum/cost (float3), depth (float), raw (float4), display (uint32) for `n_pixels` pixels; alpha (float) and volume (float3),
     the compositing AOVs, once Renderer.enable_aovs() has allocated them (None until then); `groups`, the light groups (name -> float3
-    tensor, LIGHT_GROUPS order), once Renderer.enable_light_groups() has allocated them (None until then)."""
+    tensor, LIGHT_GROUPS order), once Renderer.enable_light_groups() has allocated them (None until then); `deep`, the deep slices
+    ((K, n, 4) float32), once Renderer.enable_deep() has allocated them (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -35,9 +36,10 @@ class FrameBuffers:
         self.alpha = None
         self.volume = None
         self.groups = None
+        self.deep = None
 
     def zero_(self):
-        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume,
+        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep,
                   *(self.groups.values() if self.groups else ())):
             if t is not None:
                 t.zero_()
@@ -197,6 +199,32 @@ class Renderer:
         if name not in self.buffers.groups:
             raise N.VptError(f"Renderer.light_group_image: unknown light group {name!r} (one of {', '.join(LIGHT_GROUPS)})")
         return self.buffers.groups[name].view(self.n_local // self.width, self.width, 3)
+
+    def enable_deep(self, bounds):
+        """Allocate and register the deep slices (vpt_set_deep_buffers): `bounds` z_0 < z_1 < ... < z_K (K = 1..VPT_DEEP_MAX_SLICES;
+        z_K may be inf) are K depth intervals in the units of the depth buffer.  buffers.deep (K, n, 4) float32 holds per slice and pixel
+        the running means (premultiplied colour, coverage) of the samples whose depth d has z_k <= d < z_{k+1}: the compositing AOVs binned
+        by depth, so an element can be inserted at a depth inside the volume (deep.flatten).  They take over at the next render call with
+        kp.iteration == 0 (DESIGN.md section 8h).  Bad bounds raise VptError and leave the slices as they were.  n is the renderer's
+        local pixel count (rank-local rows on a partitioned renderer)."""
+        z = np.asarray(bounds, dtype=np.float32).reshape(-1)
+        k = len(z) - 1
+        if not 1 <= k <= N.VPT_DEEP_MAX_SLICES:
+            raise N.VptError(f"Renderer.enable_deep: {len(z)} bounds give {k} slices (1..{N.VPT_DEEP_MAX_SLICES})")
+        deep = torch.zeros(k, self.n_local, 4, dtype=torch.float32, device=self.buffers.accum.device)
+        check(lib.vpt_set_deep_buffers(self.ctx, C.c_void_p(deep.data_ptr()), k, z.ctypes.data_as(C.POINTER(C.c_float))),
+              self.ctx, "vpt_set_deep_buffers")
+        self.buffers.deep, self.deep_bounds = deep, tuple(float(v) for v in z)
+
+    def disable_deep(self):
+        """Turn the deep slices off at once; buffers.deep keeps what it holds."""
+        check(lib.vpt_set_deep_buffers(self.ctx, None, 0, None), self.ctx, "vpt_set_deep_buffers")
+
+    def deep_image(self):
+        """(K, H, W, 4) float32 view of buffers.deep ((K, local rows, W, 4) on a partitioned renderer); the bounds are deep_bounds."""
+        if self.buffers.deep is None:
+            raise N.VptError("Renderer.deep_image: deep slices are not enabled (Renderer.enable_deep(bounds))")
+        return self.buffers.deep.view(self.buffers.deep.shape[0], self.n_local // self.width, self.width, 4)
 
     def set_region(self, x0, y0, x1, y1):
         """Render only the full-frame pixels [x0, x1) x [y0, y1) (vpt_set_render_region) from the next call with kp.iteration == 0 on:
