@@ -332,6 +332,34 @@ int  vpt_set_projection(vpt_context* ctx, int kind, double hfov_deg, double vfov
  * jitter the blue-noise buffer holds now.  Reads params (camera, Kernel_params, blue noise); writes d_out_f4 only, on the default stream. */
 int  vpt_debug_camera_rays(vpt_context* ctx, void* const params[VPT_NUM_ARGS], float* d_out_f4);
 
+/* ---- camera motion: motion blur from a camera that moves between two poses over the shutter --------------------------------------
+ * The reference draws a shutter time for every camera ray (camera::get_ray, right after the lens rejection loop) and never reads it.
+ * Here that draw, xi in (0, 1] from the pixel's Philox stream, places the sample's camera between two poses: the Kernel_params camera is
+ * the pose at shutter open, `shutter_close` (typically a second vpt_camera_look_at) the pose at shutter close.  The call copies it; NULL
+ * clears the motion.
+ *
+ *   The sample's camera.  Its origin, lower_left_corner, horizontal, vertical, u and v are, per component, c == o ? o : fma(xi, c - o, o)
+ *     (o the open pose's value, c the close pose's).  A component that does not move keeps the open pose's bits, -0 included, so a pure
+ *     translation keeps the basis and shutter_close == the open camera is the static camera.  xi = 1 reaches the close pose only up to the
+ *     rounding of c - o.  The weight is xi itself: time0 and time1 stay unread, as in the reference.  lens_radius, focus_dist and viz_dof
+ *     are the open camera's; shutter_close's copies, its w, time0 and time1 are not read.  No draw of any path changes, so every sample is
+ *     the reference kernel's path for the ray of the reference camera whose fields are that sample's camera.  Depth (and with it the
+ *     AOVs' and deep slices' collision depth) is measured from the sample's own origin.
+ *   Activation.  Motion set or cleared here takes effect at the next render call whose Kernel_params.iteration is 0; a continued frame
+ *     keeps the pose it started with (the rule of the projection and regions).
+ *   Works with vpt_render_pass(es), vpt_render_adaptive, render regions, AOVs, light groups, deep slices, brick mode, both integrators,
+ *     both environments, partitioned contexts and both exchanges.  A motion frame runs no miss cull (option "miss_cull") and keeps every
+ *     sample record, so it costs more than a static frame even when the poses are equal.
+ *   Refused when set (VPT_ERR_INVALID; the motion is left as it was): a non-finite component in any of the six interpolated fields of
+ *     shutter_close.  Refused at render time (VPT_ERR_UNSUPPORTED): motion with VPT_PROJECTION_EQUIRECT.  Level (A) has no motion. */
+int  vpt_set_camera_motion(vpt_context* ctx, const vpt_camera* shutter_close);
+/* Diagnostic: writes, for every local pixel, 20 floats: the shutter draw xi of the next render call's first pass, then origin,
+ * lower_left_corner, horizontal, vertical, u and v of that sample's camera (19 floats, padded with 0; padding rows of a partitioned
+ * context all 0), the same bits the generator computes.  Reads params (camera, Kernel_params); writes d_out only, on the default stream,
+ * and leaves the blue noise as it is.  VPT_ERR_INVALID when the next call has no camera motion.  vpt_debug_camera_rays refuses such a
+ * call (VPT_ERR_UNSUPPORTED): its rays depend on each sample's draw. */
+int  vpt_debug_motion_cameras(vpt_context* ctx, void* const params[VPT_NUM_ARGS], float* d_out);
+
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
  * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.

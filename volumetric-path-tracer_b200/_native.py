@@ -162,7 +162,7 @@ EXPORTED_SYMBOLS = [
     "vpt_denoise_options_defaults", "vpt_denoise",
     "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
     "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
-    "vpt_set_deep_buffers",
+    "vpt_set_deep_buffers", "vpt_set_camera_motion", "vpt_debug_motion_cameras",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -299,6 +299,8 @@ lib.vpt_bvh_destroy.argtypes = [C.c_uint64, C.c_uint64]; lib.vpt_bvh_destroy.res
 lib.vpt_volume_bounds.argtypes = [C.POINTER(GPU_VDB), C.POINTER(C.c_float)]; lib.vpt_volume_bounds.restype = None
 lib.vpt_camera_look_at.argtypes = [C.POINTER(camera), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_float]
 lib.vpt_camera_look_at.restype = None
+lib.vpt_set_camera_motion.argtypes = [_vp, C.POINTER(camera)]; lib.vpt_set_camera_motion.restype = C.c_int
+lib.vpt_debug_motion_cameras.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_motion_cameras.restype = C.c_int
 lib.vpt_kernel_params_defaults.argtypes = [C.POINTER(Kernel_params)]; lib.vpt_kernel_params_defaults.restype = None
 
 

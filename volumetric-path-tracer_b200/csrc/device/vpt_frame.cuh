@@ -133,6 +133,30 @@ VPT_DEV float3 pano_b0(const vpt_camera& cam, const Projection& pj, const vpt_u2
     return f3(pfma(st, cam.v.x, pmul(ct, hx)), pfma(st, cam.v.y, pmul(ct, hy)), pfma(st, cam.v.z, pmul(ct, hz)));
 }
 
+// The camera of a sample whose shutter draw is xi in (0, 1] under camera motion `mo` (the pose at shutter close; `cam` is the pose at shutter
+// open): every component of origin, lower_left_corner, horizontal, vertical, u and v is c == o ? o : fma(xi, c - o, o), with o the open and c
+// the close pose's value.  A component that does not move keeps the open pose's bits (-0 included), so close == open is the static camera
+// and a pure translation keeps the basis; xi = 1 reaches c only up to the rounding of c - o.  lens_radius, focus_dist and viz_dof stay the
+// open camera's.  The operation order is pinned: k_generate_motion (and its adaptive / region forms) and vpt_debug_motion_cameras must get
+// the same bits.
+VPT_DEV float motion_lerp(const float o, const float c, const float xi) { return c == o ? o : pfma(xi, psub(c, o), o); }
+VPT_DEV vpt_f3 motion_lerp3(const vpt_f3 o, const vpt_f3 c, const float xi)
+{
+    vpt_f3 r; r.x = motion_lerp(o.x, c.x, xi); r.y = motion_lerp(o.y, c.y, xi); r.z = motion_lerp(o.z, c.z, xi);
+    return r;
+}
+VPT_DEV vpt_camera motion_camera(const vpt_camera& cam, const CameraMotion& mo, const float xi)
+{
+    vpt_camera m = cam;
+    m.origin = motion_lerp3(cam.origin, mo.origin, xi);
+    m.lower_left_corner = motion_lerp3(cam.lower_left_corner, mo.lower_left_corner, xi);
+    m.horizontal = motion_lerp3(cam.horizontal, mo.horizontal, xi);
+    m.vertical = motion_lerp3(cam.vertical, mo.vertical, xi);
+    m.u = motion_lerp3(cam.u, mo.u, xi);
+    m.v = motion_lerp3(cam.v, mo.v, xi);
+    return m;
+}
+
 // the pinhole camera: what k_generate and k_miss_cull test before taking the pinhole branch (an origin component of exactly 0 could meet a
 // signed zero of the lens offset, so those cameras take the literal order)
 VPT_DEV bool pinhole_camera(const vpt_camera& cam)

@@ -26,6 +26,8 @@
 //   k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect, k_miss_cull_equirect, k_miss_cull_region_equirect,
 //   k_resolve_equirect<A, G>, k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G> : the equirectangular projection
 //                     (vpt_set_projection) -- the same kernels with the camera ray of pano_b0; k_camera_rays: vpt_debug_camera_rays
+//   k_generate_motion, k_generate_adaptive_motion, k_generate_region_motion : camera motion (vpt_set_camera_motion) -- k_generate with each
+//                     sample's camera placed between two poses by its shutter draw (motion_camera); k_motion_cameras: vpt_debug_motion_cameras
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -113,8 +115,13 @@ __global__ void k_prepare_scene(const vpt_gpu_vdb* __restrict__ vols, const vpt_
 // kRegion (k_generate_region): the grid runs over the tile rectangle of `rg`, and a lane whose pixel lies outside R samples nothing.
 // kPano (k_generate_equirect, ...): the ray is (camera origin, normalize(pano_b0)) under the projection `pj` (lens_radius is 0, the host
 // refuses anything else), and takes the pinhole branch below: its lens draws are counted after the box / octree prefix, as a pinhole's.
-template <bool kAdaptive, bool kRegion = false, bool kPano = false>
-__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad, const RenderRegion* rg = nullptr, const Projection* pj = nullptr)
+// kMotion (k_generate_motion, ...): the camera moves over the shutter (`mo`, the pose at shutter close).  The ray depends on the shutter
+// draw, whose index depends on how many trials the lens loop took, so every sample runs the loop first, takes xi where the static kernels
+// skip the shutter draw, and builds its ray from motion_camera(xi) in the thin-lens order (a pinhole's rd is +-0).  No pre-step: queue_aux
+// carries the per-ray origin (the host sets thin_lens), and the host runs no miss cull.
+template <bool kAdaptive, bool kRegion = false, bool kPano = false, bool kMotion = false>
+__device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad, const RenderRegion* rg = nullptr, const Projection* pj = nullptr,
+                                              const CameraMotion* mo = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -208,6 +215,20 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
             org = ld3(cam.origin);
             dir = normalize(pano_b0(cam, *pj, kp.resolution, x, y, bnv.x, bnv.y));
             lens_pending = true;
+        } else if constexpr (kMotion) {
+            float3 p;
+            do {
+                const float a = vdc2[int(rng.next() * 100)];
+                const float b = vdc3[int(rng.next() * 100)];
+                p = f3(pfma(a, 2.0f, -1.0f), pfma(b, 2.0f, -1.0f), 0.0f);
+            } while (pfma(p.x, p.x, pmul(p.y, p.y)) >= 1.0f);
+            const vpt_camera mc = motion_camera(cam, *mo, rng.next());  // the shutter-time draw places the camera between the poses
+            const float3 rd = f3(pmul(cam.lens_radius, p.x), pmul(cam.lens_radius, p.y), 0.0f);
+            const float3 offset = f3(pfma(mc.u.x, rd.x, pmul(mc.v.x, rd.y)), pfma(mc.u.y, rd.x, pmul(mc.v.y, rd.y)), pfma(mc.u.z, rd.x, pmul(mc.v.z, rd.y)));
+            const float3 b0 = camera_b0(mc, kp.resolution, x, y, bnv.x, bnv.y);
+            org = f3(padd(mc.origin.x, offset.x), padd(mc.origin.y, offset.y), padd(mc.origin.z, offset.z));
+            dir = normalize(f3(psub(b0.x, offset.x), psub(b0.y, offset.y), psub(b0.z, offset.z)));
+            kdraws = rng.k;
         } else {
             const bool pinhole = pinhole_camera(cam);
             const float3 b0 = camera_b0(cam, kp.resolution, x, y, bnv.x, bnv.y);
@@ -241,7 +262,7 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         // leaves the box without ever meeting a populated leaf contributes exactly what a miss does and never enters the
         // queue, the others are queued at the position where stepping really starts.  (Pinhole camera and a ray whose line
         // provably misses the sphere only; everything else takes the generic route.)
-        if (obj == 1 && kp.ray_depth >= 1 && kp.volume_depth >= 1 && cam.lens_radius == 0.0f && sphere_clear) {
+        if (!kMotion && obj == 1 && kp.ray_depth >= 1 && kp.volume_depth >= 1 && cam.lens_radius == 0.0f && sphere_clear) {
             float3 p = madd3(org, dir, padd(t_min, VPT_EPS));
             int leaf = -2;
             if (!aabb_contains(sc.root_pmin, sc.root_pmax, p)) leaf = -1;
@@ -308,6 +329,15 @@ k_generate_adaptive_equirect(const FrameArgs fa, const AdaptArgs ad, const Proje
 
 __global__ void __launch_bounds__(128)
 k_generate_region_equirect(const FrameArgs fa, const RenderRegion rg, const Projection pj) { generate_body<false, true, true>(fa, nullptr, &rg, &pj); }
+
+__global__ void __launch_bounds__(128)
+k_generate_motion(const FrameArgs fa, const CameraMotion mo) { generate_body<false, false, false, true>(fa, nullptr, nullptr, nullptr, &mo); }
+
+__global__ void __launch_bounds__(128)
+k_generate_adaptive_motion(const FrameArgs fa, const AdaptArgs ad, const CameraMotion mo) { generate_body<true, false, false, true>(fa, &ad, nullptr, nullptr, &mo); }
+
+__global__ void __launch_bounds__(128)
+k_generate_region_motion(const FrameArgs fa, const RenderRegion rg, const CameraMotion mo) { generate_body<false, true, false, true>(fa, nullptr, &rg, nullptr, &mo); }
 
 // =====================================================================================================
 // k_miss_cull
@@ -1228,6 +1258,36 @@ __global__ void k_camera_rays(const vpt_camera cam, const vpt_u2 res, const Fram
     out[lp] = make_float4(b.x, b.y, b.z, 0.f);
 }
 
+// vpt_debug_motion_cameras: every local pixel's shutter draw at pass `iteration` -- the lens loop and the draw after it, as k_generate_motion
+// takes them (the same radical-inverse tables) -- and the camera motion_camera makes of it
+__global__ void k_motion_cameras(const vpt_camera cam, const CameraMotion mo, const FrameGeom g, const uint32_t iteration, float* out)
+{
+    __shared__ float vdc2[101], vdc3[101];
+    if (threadIdx.x < 101) {
+        { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 2; while (n) { denom *= 2; r = padd(r, __fdividef((float)(n % 2), denom)); n *= inv; } vdc2[threadIdx.x] = r; }
+        { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 3; while (n) { denom *= 3; r = padd(r, __fdividef((float)(n % 3), denom)); n *= inv; } vdc3[threadIdx.x] = r; }
+    }
+    __syncthreads();
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= (uint32_t)g.n_local) return;
+    const int lr = lp / g.width, x = lp - lr * g.width;
+    const int y = global_row(g, lr);
+    float* o = out + (size_t)lp * 20;
+    if (y >= g.height) { for (int i = 0; i < 20; ++i) o[i] = 0.f; return; }
+    Rng rng; rng.init((uint32_t)y * (uint32_t)g.width + (uint32_t)x, iteration, 0u);
+    float px, py;
+    do {
+        px = pfma(vdc2[int(rng.next() * 100)], 2.0f, -1.0f);
+        py = pfma(vdc3[int(rng.next() * 100)], 2.0f, -1.0f);
+    } while (pfma(px, px, pmul(py, py)) >= 1.0f);
+    const float xi = rng.next();
+    const vpt_camera m = motion_camera(cam, mo, xi);
+    const vpt_f3 f[6] = { m.origin, m.lower_left_corner, m.horizontal, m.vertical, m.u, m.v };
+    o[0] = xi;
+    for (int i = 0; i < 6; ++i) { o[1 + 3 * i] = f[i].x; o[2 + 3 * i] = f[i].y; o[3 + 3 * i] = f[i].z; }
+    o[19] = 0.f;
+}
+
 // =====================================================================================================
 // host-callable launchers
 // =====================================================================================================
@@ -1260,12 +1320,13 @@ static dim3 generate_grid(FrameArgs& a, long long tiles, int n_passes)
     return dim3((unsigned)((tiles + tpb - 1) / tpb), 1, (unsigned)((n_passes + ppb - 1) / ppb));
 }
 
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, cudaStream_t s)
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, cudaStream_t s)
 {
     FrameArgs a = fa;
     const long long tiles = (long long)((fa.geom.width + 31) / 32) * ((fa.geom.local_rows + 3) / 4);
     const dim3 grid = generate_grid(a, tiles, n_passes);
-    if (equirect(pj)) k_generate_equirect<<<grid, 128, 0, s>>>(a, pj);
+    if (mo) k_generate_motion<<<grid, 128, 0, s>>>(a, *mo);
+    else if (equirect(pj)) k_generate_equirect<<<grid, 128, 0, s>>>(a, pj);
     else k_generate<<<grid, 128, 0, s>>>(a);
     return cudaGetLastError();
 }
@@ -1279,13 +1340,15 @@ cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projectio
     return cudaGetLastError();
 }
 
-cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, cudaStream_t s)
+cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, const CameraMotion* mo,
+                                   cudaStream_t s)
 {
     const long long tiles = region_tiles(rg);
     if (tiles <= 0) return cudaSuccess;
     FrameArgs a = fa;
     const dim3 grid = generate_grid(a, tiles, n_passes);
-    if (equirect(pj)) k_generate_region_equirect<<<grid, 128, 0, s>>>(a, rg, pj);
+    if (mo) k_generate_region_motion<<<grid, 128, 0, s>>>(a, rg, *mo);
+    else if (equirect(pj)) k_generate_region_equirect<<<grid, 128, 0, s>>>(a, rg, pj);
     else k_generate_region<<<grid, 128, 0, s>>>(a, rg);
     return cudaGetLastError();
 }
@@ -1299,12 +1362,14 @@ cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const Re
     return cudaGetLastError();
 }
 
-cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, cudaStream_t s)
+cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, const CameraMotion* mo,
+                                     cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
     FrameArgs a = fa;
     const dim3 grid = generate_grid(a, ad.n_tiles, n_passes);
-    if (equirect(pj)) k_generate_adaptive_equirect<<<grid, 128, 0, s>>>(a, ad, pj);
+    if (mo) k_generate_adaptive_motion<<<grid, 128, 0, s>>>(a, ad, *mo);
+    else if (equirect(pj)) k_generate_adaptive_equirect<<<grid, 128, 0, s>>>(a, ad, pj);
     else k_generate_adaptive<<<grid, 128, 0, s>>>(a, ad);
     return cudaGetLastError();
 }
@@ -1471,7 +1536,8 @@ cudaError_t exchange_kernels_preload()
     return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
-                k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish);
+                k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish, k_generate_motion, k_generate_adaptive_motion,
+                k_generate_region_motion);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1665,6 +1731,13 @@ cudaError_t launch_camera_rays(const vpt_camera& cam, const vpt_u2 res, const Fr
 {
     if (g.n_local <= 0) return cudaSuccess;
     k_camera_rays<<<(g.n_local + 255) / 256, 256, 0, s>>>(cam, res, g, pj, reinterpret_cast<const float3*>(bn), out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_motion_cameras(const vpt_camera& cam, const CameraMotion& mo, const FrameGeom& g, uint32_t iteration, float* out, cudaStream_t s)
+{
+    if (g.n_local <= 0) return cudaSuccess;
+    k_motion_cameras<<<(g.n_local + 255) / 256, 256, 0, s>>>(cam, mo, g, iteration, out);
     return cudaGetLastError();
 }
 

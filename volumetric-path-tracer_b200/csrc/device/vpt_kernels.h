@@ -33,8 +33,8 @@ struct FrameArgs {
     // ray queue (hits), SoA: direction + entry distance | (local pixel, pass | draws<<6 | obj<<16) | origin (thin lens only)
     float4*   queue_dir;
     uint2*    queue_id;
-    float4*   queue_aux;           // thin lens: per-ray origin; pre-stepped ray (pinhole only): position where stepping starts
-    int       thin_lens;           // cam.lens_radius != 0
+    float4*   queue_aux;           // per-ray origin (thin lens or camera motion); pre-stepped ray (pinhole only): position where stepping starts
+    int       thin_lens;           // per-ray origin: thin lens or camera motion (cam.lens_radius != 0 or a CameraMotion)
     const float2* bn_table;        // [pass][65536] blue-noise jitter of the chunk
     int       n_passes;            // passes in this chunk (k_generate loops over them; k_trace keeps tr of the last one)
     int       passes_per_block;    // k_generate: passes handled by one block (blockIdx.z selects the run)
@@ -111,11 +111,18 @@ constexpr int kProjPerspective = 0, kProjEquirect = 1;          // VPT_PROJECTIO
 struct Projection { int kind = kProjPerspective; float hfov = 0.f, vfov = 0.f; };
 inline bool equirect(const Projection& p) { return p.kind == kProjEquirect; }
 
+// Camera motion (vpt_set_camera_motion): the camera's pose at shutter close.  A sample with shutter draw xi uses the camera whose six
+// fields below are motion_camera's lerp (vpt_frame.cuh) from the frame camera (the pose at shutter open) towards these.  A kernel argument
+// of the motion kernels only (k_generate_motion, k_generate_adaptive_motion, k_generate_region_motion, k_motion_cameras: the launchers below
+// pick them for a non-null CameraMotion), as Projection is.
+struct CameraMotion { vpt_f3 origin, lower_left_corner, horizontal, vertical, u, v; };
+
 cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* root, SceneTables* out, OctInternal* internal,
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
-// pj: the frame's projection -- the launchers below run the equirectangular kernels when equirect(pj)
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, cudaStream_t s);
+// pj: the frame's projection -- the launchers below run the equirectangular kernels when equirect(pj); mo: the frame's shutter-close pose
+// (null: no motion) -- the generate launchers run the motion kernels when it is set (never together with equirect(pj): the host refuses that)
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, cudaStream_t s);
 // once per render call, before the first chunk: mask[local pixel] = 1 where every jitter misses the root box and the sphere (pinhole
 // and equirectangular cameras; a thin lens or a root box that is empty or not finite culls nothing)
 cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s);
@@ -201,9 +208,13 @@ cudaError_t launch_unpermute(const void* gathered, void* full, const FrameGeom& 
 // camera_b0 at the jitter the blue-noise buffer `bn` holds now (read only)
 cudaError_t launch_camera_rays(const vpt_camera& cam, const vpt_u2 res, const FrameGeom& g, const Projection& pj, const void* bn, float4* out,
                                cudaStream_t s);
+// vpt_debug_motion_cameras: out[local pixel * 20 ..] = xi, then origin, lower_left_corner, horizontal, vertical, u, v of motion_camera at the
+// shutter draw of the pixel's first pass at `iteration` (19 floats, padded with 0; padding rows all 0)
+cudaError_t launch_motion_cameras(const vpt_camera& cam, const CameraMotion& mo, const FrameGeom& g, uint32_t iteration, float* out, cudaStream_t s);
 // adaptive frame: k_generate / k_resolve over the tiles of ad.tiles only (stopped pixels sample nothing and keep their buffers); the resolve
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
-cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, cudaStream_t s);
+cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, const CameraMotion* mo,
+                                     cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
                                     const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
@@ -215,7 +226,8 @@ cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* ti
 // k_miss_cull_region tests the strips that hold a pixel of R; k_resolve_region resolves R's pixels (the peer stores as launch_resolve).
 // Adaptive, one rank: the tile list starts as R's tiles with every pixel outside R stopped, and k_adapt_region clips the 3x3 neighbourhood
 // at R's edge.
-cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
+cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, const CameraMotion* mo,
+                                   cudaStream_t s);
 cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                                   const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,

@@ -211,6 +211,22 @@ int vpt_set_projection(vpt_context* c, int kind, double hfov_deg, double vfov_de
     return VPT_OK;
 }
 
+int vpt_set_camera_motion(vpt_context* c, const vpt_camera* shutter_close) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_camera_motion: null context");
+    if (!shutter_close) { c->motion_req = false; return VPT_OK; }          // taken at the next iteration-0 call
+    const struct { const char* name; vpt_f3 v; } fields[] = {
+        { "origin", shutter_close->origin }, { "lower_left_corner", shutter_close->lower_left_corner }, { "horizontal", shutter_close->horizontal },
+        { "vertical", shutter_close->vertical }, { "u", shutter_close->u }, { "v", shutter_close->v } };
+    for (const auto& f : fields)
+        if (!std::isfinite(f.v.x) || !std::isfinite(f.v.y) || !std::isfinite(f.v.z))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_camera_motion: shutter_close.") + f.name + " is not finite");
+    vpt::CameraMotion m;
+    m.origin = shutter_close->origin; m.lower_left_corner = shutter_close->lower_left_corner; m.horizontal = shutter_close->horizontal;
+    m.vertical = shutter_close->vertical; m.u = shutter_close->u; m.v = shutter_close->v;
+    c->motion_close_req = m; c->motion_req = true;
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -282,6 +298,9 @@ struct FramePlan {
     bool region = false;                  // a render region is active: the region kernels over rg
     vpt::RenderRegion rg;
     vpt::Projection proj;                 // the frame's projection: the equirectangular kernels when equirect(proj)
+    bool motion = false;                  // camera motion: the motion generate kernels with the shutter-close pose mo
+    vpt::CameraMotion mo;
+    const vpt::CameraMotion* motion_arg() const { return motion ? &mo : nullptr; }
 };
 
 // Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
@@ -401,6 +420,10 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     const vpt::Projection& proj = kp.iteration == 0 ? c->proj_req : c->proj_cur;
     if (vpt::equirect(proj) && fa.cam.lens_radius != 0.0f)
         return fail(c, VPT_ERR_UNSUPPORTED, "the equirectangular projection has no lens: camera.lens_radius must be 0 (got " + std::to_string(fa.cam.lens_radius) + ")");
+    // camera motion: the shutter-close pose set last takes over at a call with iteration == 0
+    const bool motion = kp.iteration == 0 ? c->motion_req : c->motion_cur;
+    if (motion && vpt::equirect(proj))
+        return fail(c, VPT_ERR_UNSUPPORTED, "camera motion (vpt_set_camera_motion) is not supported with the equirectangular projection");
 
     // ---- scene tables ---------------------------------------------------------------------------------------
     // Octrees built by vpt_octree_build are registered with their flat tables and instance count: nothing is read
@@ -505,16 +528,17 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         VPT_CUDA(c, cudaMalloc(&c->d_bn_table, sizeof(float2) * 65536 * (size_t)chunk));
         c->cap_chunk = chunk;
     }
-    fa.queue_dir = c->d_queue; fa.queue_id = c->d_queue_id; fa.queue_aux = c->d_queue_org; fa.thin_lens = (fa.cam.lens_radius != 0.0f) ? 1 : 0;
+    fa.queue_dir = c->d_queue; fa.queue_id = c->d_queue_id; fa.queue_aux = c->d_queue_org; fa.thin_lens = (fa.cam.lens_radius != 0.0f || motion) ? 1 : 0;
     fa.bn_table = c->d_bn_table; fa.debug_flags = c->debug_flags;
     fa.queue_count = c->d_counters; fa.queue_head = c->d_counters + 1;
     fa.planeA = c->d_planeA;
     fa.planeB = wide ? c->d_planeB : nullptr; fa.planeC = wide ? c->d_planeC : nullptr; fa.planeD = planeD ? c->d_planeD : nullptr;
     fa.plane_tr = wide ? nullptr : c->d_plane_tr;
     // pixels no jitter can take to the root box or the sphere (pinhole and equirectangular HDRI frames that sample): k_miss_cull marks them once per call, and
-    // k_generate / k_resolve skip their sample records.  Frames that end on the precomputed sky keep every record (see resolve_pixel).
+    // k_generate / k_resolve skip their sample records.  Frames that end on the precomputed sky keep every record (see resolve_pixel), and
+    // so do motion frames: the cull assumes one camera per strip, and k_resolve rebuilds a culled sample without the lens loop.
     fa.miss_mask = nullptr;
-    if (c->miss_cull && n_sampled && !sky_env && fa.cam.lens_radius == 0.0f && fa.geom.n_local > 0) {
+    if (c->miss_cull && n_sampled && !sky_env && fa.cam.lens_radius == 0.0f && !motion && fa.geom.n_local > 0) {
         if ((size_t)fa.geom.n_local > c->cap_miss_mask) {
             cudaFree(c->d_miss_mask); c->d_miss_mask = nullptr; c->cap_miss_mask = 0;
             VPT_CUDA(c, cudaMalloc(&c->d_miss_mask, (size_t)fa.geom.n_local));
@@ -571,7 +595,12 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     }
     plan.resolve.deep = plan.deep.out != nullptr;
     plan.proj = proj;
-    if (kp.iteration == 0) { memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req; }
+    plan.motion = motion;
+    plan.mo = kp.iteration == 0 ? c->motion_close_req : c->motion_close_cur;
+    if (kp.iteration == 0) {
+        memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req;
+        c->motion_cur = c->motion_req; c->motion_close_cur = c->motion_close_req;
+    }
     plan.region = region;
     if (region) plan.rg = vpt::region_geometry(fa.geom, (int)reg[0], (int)reg[1], (int)reg[2], (int)reg[3]);
     return VPT_OK;
@@ -636,8 +665,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
         fa.kp.iteration = it0 + done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, plan.proj, stream)
-                                                            : vpt::launch_generate(fa, (int)np, plan.proj, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, plan.proj, plan.motion_arg(), stream)
+                                                            : vpt::launch_generate(fa, (int)np, plan.proj, plan.motion_arg(), stream); }));
         VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
@@ -785,7 +814,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)bn, c->d_bn_table, (int)np, plan.bn_limit, c->d_counters, stream); }));
         c->launches++;
         if (ad.n_tiles > 0) {
-            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, stream); }));
+            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, plan.motion_arg(), stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.proj, stream); }));
             c->launches += 3 + (plan.resolve.deep ? 1 : 0);
@@ -918,9 +947,29 @@ int vpt_debug_camera_rays(vpt_context* c, void* const params[VPT_NUM_ARGS], floa
     memcpy(&kp, params[VPT_ARG_KERNEL_PARAMS], sizeof(kp));
     if (!kp.blue_noise_buffer) return fail(c, VPT_ERR_INVALID, "vpt_debug_camera_rays: Kernel_params.blue_noise_buffer is null");
     if (kp.resolution.x == 0 || kp.resolution.y == 0) return fail(c, VPT_ERR_INVALID, "vpt_debug_camera_rays: resolution is zero");
+    if (kp.iteration == 0 ? c->motion_req : c->motion_cur)
+        return fail(c, VPT_ERR_UNSUPPORTED, "vpt_debug_camera_rays: the next call is a camera-motion frame, whose rays depend on each sample's "
+                                            "shutter draw; use vpt_debug_motion_cameras");
     const vpt::Projection& pj = kp.iteration == 0 ? c->proj_req : c->proj_cur;
     VPT_CUDA(c, vpt::launch_camera_rays(cam, kp.resolution, make_geom(c, kp.resolution.x, kp.resolution.y), pj, (const void*)(uintptr_t)kp.blue_noise_buffer,
                                         reinterpret_cast<float4*>(d_out_f4), 0));
+    c->launches++;
+    return VPT_OK;
+}
+
+// The camera of every local pixel's first sample of the next render call under camera motion (motion_req at iteration 0, else motion_cur):
+// its shutter draw and motion_camera of it, on the default stream.  Reads the camera and Kernel_params; writes d_out only.
+int vpt_debug_motion_cameras(vpt_context* c, void* const params[VPT_NUM_ARGS], float* d_out) {
+    if (!c || !params || !d_out || !params[VPT_ARG_CAMERA] || !params[VPT_ARG_KERNEL_PARAMS])
+        return fail(c, VPT_ERR_INVALID, "vpt_debug_motion_cameras: null argument");
+    vpt_camera cam; vpt_kernel_params kp;
+    memcpy(&cam, params[VPT_ARG_CAMERA], sizeof(cam));
+    memcpy(&kp, params[VPT_ARG_KERNEL_PARAMS], sizeof(kp));
+    if (kp.resolution.x == 0 || kp.resolution.y == 0) return fail(c, VPT_ERR_INVALID, "vpt_debug_motion_cameras: resolution is zero");
+    const bool motion = kp.iteration == 0 ? c->motion_req : c->motion_cur;
+    if (!motion) return fail(c, VPT_ERR_INVALID, "vpt_debug_motion_cameras: the next call has no camera motion (vpt_set_camera_motion)");
+    VPT_CUDA(c, vpt::launch_motion_cameras(cam, kp.iteration == 0 ? c->motion_close_req : c->motion_close_cur,
+                                           make_geom(c, kp.resolution.x, kp.resolution.y), kp.iteration, d_out, 0));
     c->launches++;
     return VPT_OK;
 }

@@ -254,6 +254,24 @@ class Renderer:
         check(lib.vpt_debug_camera_rays(self.ctx, self.params.array, C.c_void_p(out.data_ptr())), self.ctx, "vpt_debug_camera_rays")
         return out
 
+    def set_camera_motion(self, cam_close: N.camera):
+        """Camera motion blur (vpt_set_camera_motion) from the next call with kp.iteration == 0 on: self.cam is the pose at shutter open,
+        `cam_close` (e.g. a second look_at camera) the pose at shutter close; each sample's shutter draw xi places its camera between them
+        (DESIGN.md section 8i).  The pose is copied.  A non-finite field raises VptError and leaves the motion as it was."""
+        check(lib.vpt_set_camera_motion(self.ctx, C.byref(cam_close)), self.ctx, "vpt_set_camera_motion")
+
+    def clear_camera_motion(self):
+        """Back to the static camera from the next call with kp.iteration == 0 on."""
+        check(lib.vpt_set_camera_motion(self.ctx, None), self.ctx, "vpt_set_camera_motion")
+
+    def motion_cameras(self):
+        """(local_rows, W, 20) float32: per local pixel the shutter draw xi of the next render call's first pass, then the origin,
+        lower_left_corner, horizontal, vertical, u and v of that sample's camera, padded with 0 (vpt_debug_motion_cameras).  Writes nothing
+        else and leaves the blue noise as it is.  Raises VptError when the next call has no camera motion."""
+        out = torch.empty(self.n_local, 20, dtype=torch.float32, device=self.buffers.accum.device)
+        check(lib.vpt_debug_motion_cameras(self.ctx, self.params.array, C.c_void_p(out.data_ptr())), self.ctx, "vpt_debug_motion_cameras")
+        return out.view(self.n_local // self.width, self.width, 20)
+
     def reset(self):
         self.kp.iteration = 0
         self.buffers.zero_()
@@ -547,6 +565,13 @@ class DistributedRenderer:
     def set_projection(self, kind, hfov=360.0, vfov=180.0):
         """Renderer.set_projection on this rank; every rank sets the same projection."""
         self.r.set_projection(kind, hfov=hfov, vfov=vfov)
+
+    def set_camera_motion(self, cam_close):
+        """Renderer.set_camera_motion on this rank; every rank sets the same poses."""
+        self.r.set_camera_motion(cam_close)
+
+    def clear_camera_motion(self):
+        self.r.clear_camera_motion()
 
     def set_gather(self, enabled: bool):
         """Switch the per-call exchange off (rank-local work only: profiling runs that not every rank takes part in) or back on."""
