@@ -56,6 +56,8 @@ int  vpt_abi_sizes(size_t* out, int n);
  * "miss_cull" (1, the default: a pinhole HDRI frame first marks the pixels whose every jitter misses the volume's root box and the sphere,
  * and writes and reads no sample records for them -- the miss samples are rebuilt from the camera and the jitter, the frame is bit for
  * bit the same; 0: off),
+ * "empty_ahead" (1, the default: a walk that reaches an empty octree node from which no populated leaf lies in its direction of travel
+ * ends there instead of hopping to the root box's exit -- bit for bit the same frame; 0: off, every walk hops),
  * "count_stats" / "profile" (0|1, see vpt_get_counters / vpt_get_kernel_times). */
 int  vpt_set_option(vpt_context* ctx, const char* key, int value);
 
@@ -418,6 +420,11 @@ int  vpt_get_stats(vpt_context* ctx, unsigned long long* kernel_launches_total, 
  * the per-call miss cull of option "miss_cull" counts as generate).
  * Both calls synchronise the device. */
 int  vpt_get_counters(vpt_context* ctx, unsigned long long out[8], int reset);
+/* Hop statistics of option "count_stats" (a reset of vpt_get_counters clears them too): out[0..2] = hops over empty octree nodes of
+ * the lean k_trace's delta / ratio / emission walks (the kernels that take the "empty ahead" shortcut; the lean kernel runs no emission
+ * walk, so out[2] stays 0), out[3] = k_trace walks ended by "empty ahead" (option "empty_ahead"), out[4..6] = rays that
+ * entered k_generate's octree pre-step / its hops / those ended at once by "empty ahead"; out[7] = 0.  Synchronises the device. */
+int  vpt_get_hop_counters(vpt_context* ctx, unsigned long long out[8], int reset);
 int  vpt_get_kernel_times(vpt_context* ctx, float ms[4], int n[4]);
 
 /* ---- host-side scene helpers (what the reference does in main.cpp / gpu_vdb.cpp / bvh_builder.cpp) -- */

@@ -163,7 +163,11 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 3; while (n) { denom *= 3; r = padd(r, __fdividef((float)(n % 3), denom)); n *= inv; } vdc3[threadIdx.x] = r; }
     }
     load_frame_shared(fs, fa.scene);
+    __shared__ EmptyAhead ea;
+    __shared__ AheadScratch eas;
+    if constexpr (!kMotion) build_empty_ahead(ea, eas, fs.oct, fa.empty_ahead != 0);   // the pre-step's table (no pre-step under motion)
     const SceneTables& sc = fs.sc;
+    uint32_t n_pre = 0, n_hop = 0, n_ahead = 0;                 // statistics of the pre-step: rays, hops, rays ended by "empty ahead"
 
     const SphereRec sph = load_sphere(fa.sphere);
     // one block = a run of 32x4 pixel tiles x a run of passes: enough (tile, pass) pairs per block to amortise the octree / table staging
@@ -266,7 +270,10 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
             float3 p = madd3(org, dir, padd(t_min, VPT_EPS));
             int leaf = -2;
             if (!aabb_contains(sc.root_pmin, sc.root_pmax, p)) leaf = -1;
-            for (int it = 0; it < 256 && leaf == -2; ++it) leaf = oct_locate_or_skip<true>(fs.oct, sc, p, dir);
+            n_pre++;
+            // -3: no populated leaf ahead, the hops would end outside the box -- the miss record needs only org and dir
+            for (int it = 0; it < 256 && leaf == -2; ++it) { leaf = oct_locate_or_skip<true, true>(fs.oct, sc, p, dir, &ea); n_hop += (leaf == -2); }
+            if (leaf == -3) { n_ahead++; leaf = -1; }
             if (leaf == -1) {                                    // walked out through empty space: sample == miss sample
                 hit = false;
                 if (kp.integrator != 0) dir = normalize(dir);    // vol_integrator renormalises after a box hit (:1747)
@@ -310,6 +317,16 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
     }
     }   // pass loop
     }   // tile loop
+
+    if (fa.counters) {                                           // optional statistics: [12] pre-step rays, [13] hops, [14] ended at once
+        for (int o = 16; o > 0; o >>= 1) {
+            n_pre += __shfl_xor_sync(0xffffffffu, n_pre, o); n_hop += __shfl_xor_sync(0xffffffffu, n_hop, o); n_ahead += __shfl_xor_sync(0xffffffffu, n_ahead, o);
+        }
+        if (lane == 0) {
+            atomicAdd(fa.counters + 12, (unsigned long long)n_pre); atomicAdd(fa.counters + 13, (unsigned long long)n_hop);
+            atomicAdd(fa.counters + 14, (unsigned long long)n_ahead);
+        }
+    }
 }
 
 __global__ void __launch_bounds__(128)

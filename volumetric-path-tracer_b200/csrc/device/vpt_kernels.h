@@ -35,6 +35,10 @@ struct FrameArgs {
     uint2*    queue_id;
     float4*   queue_aux;           // per-ray origin (thin lens or camera motion); pre-stepped ray (pinhole only): position where stepping starts
     int       thin_lens;           // per-ray origin: thin lens or camera motion (cam.lens_radius != 0 or a CameraMotion)
+    // option "empty_ahead": k_generate's pre-step and the lean k_trace end a walk at the first empty node from which no populated leaf lies
+    // ahead (build_empty_ahead, vpt_walk.cuh).  0: the table stays empty and every walk hops to the box exit.  (In the padding after
+    // thin_lens: the struct's size and every other offset stay as they were.)
+    int       empty_ahead;
     const float2* bn_table;        // [pass][65536] blue-noise jitter of the chunk
     int       n_passes;            // passes in this chunk (k_generate loops over them; k_trace keeps tr of the last one)
     int       passes_per_block;    // k_generate: passes handled by one block (blockIdx.z selects the run)
@@ -46,7 +50,9 @@ struct FrameArgs {
     // B = L + depth, C = beta, D = env_pos.  Compact records (HDRI frames traced by a lean kernel; planeB/C/D null): A = the finished radiance
     // + depth, and plane_tr (below) holds tr of the hit samples of the chunk's last pass.  A miss is always A = direction + kMissSentinel.
     float4 *planeA, *planeB, *planeC, *planeD;
-    // optional statistics: [0] volume lookups, [1] lane-steps, [2] warp step iterations, [3] lane transitions, [4] warp transition rounds
+    // optional statistics: [0] volume lookups, [1] lane-steps, [2] warp step iterations, [3] lane transitions, [4] warp transition rounds,
+    // [5] rays, [6] brick fetches, [8..10] k_trace hops of delta / ratio / emission walks, [11] k_trace walks ended by "empty ahead",
+    // [12..14] k_generate pre-step rays / hops / rays ended by "empty ahead" (16 counters)
     unsigned long long* counters;
     // cell table of volume 0 (vpt_cells_create; null = texture path): per texel cell its eight corner values, 32 bytes = ONE sector per look-up
     const float4* cell_table;

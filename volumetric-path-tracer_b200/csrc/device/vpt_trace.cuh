@@ -219,21 +219,45 @@ VPT_DEV float cell_density(const FrameArgs& fa, const VolumeRec& v, float3 p)
 // of that instantiation (smaller hot loop: the kernel is fetch-stall bound)
 // the per-step sphere test of a delta walk is rare (only lines that may hit the sphere): out of line, it keeps the hot loop shorter
 __device__ __noinline__ bool sphere_intersect_cold(const SphereRec& s, float3 ray_pos, float3 ray_dir, float& t_min, float& t_max) { return sphere_intersect(s, ray_pos, ray_dir, t_min, t_max); }
-template <bool kLean, bool kCells = false>
+// hop statistics of k_trace (counters [8..11]): hops of delta / ratio / emission walks, walks ended by "empty ahead"
+struct HopStats { uint32_t delta, ratio, emit, ahead; };
+
+// kAhead (the lean k_trace only; the generic instantiations and the level (A) entry keep it off, DESIGN.md section 8j): end walks at an
+// empty node from which no populated leaf lies ahead (`ea`).
+//   Ratio walks: hops draw nothing and change nothing but wpos, so the walk would end outside the box with the same trv and Philox
+//   position; finish_ratio_walk never reads wpos.
+//   Delta walks whose line provably misses the sphere: such a walk leaves the box with no scatter and no draw, and the path then retires
+//   whatever volume_depth and ray_depth are (quirk Q21, PH_AFTER_DELTA .. PH_AFTER_VOLUME) with its L, beta, dir, depth (0 when the first
+//   walk ends so) and the first walk's doubled alpha; its position is never written.  So the walk finishes the path here: the first-walk
+//   alpha update, then OP_FINISH.
+template <bool kLean, bool kCells = false, bool kAhead = false>
 VPT_DEV void walk_step(PathState& st, const FrameShared& fs, const FrameArgs& fa, const TraceConsts& tc, const SphereRec& sph, uint32_t& nlook,
-                       float* beta = nullptr, int beta_stride = 0)   // kLean: the path's throughput in the parked record (x, y, z one stride apart)
+                       float* beta = nullptr, int beta_stride = 0,   // kLean: the path's throughput in the parked record (x, y, z one stride apart)
+                       const EmptyAhead* ea = nullptr, HopStats* hs = nullptr)
 {
     const SceneTables& sc = fs.sc;
     const vpt_kernel_params& kp = fa.kp;
     // ONE point location per call: an empty node is hopped over (no draw consumed) and the call returns.  A second and a third in-line copy
     // were slower -- the kernel is bound by instruction fetch, every copy of the octree descent in the hot loop costs more than the
     // iterations it saves.
-    int leaf = oct_locate_or_skip(fs.oct, sc, st.wpos, st.wdir);
+    int leaf = oct_locate_or_skip<false, kAhead>(fs.oct, sc, st.wpos, st.wdir, ea, st.mode != W_DELTA || st.sphere_free);
 #if defined(VPT_WALK_HOPS) && VPT_WALK_HOPS >= 2
     if (leaf == -2) leaf = oct_locate_or_skip(fs.oct, sc, st.wpos, st.wdir);
 #endif
-    if (leaf == -2) return;
+    if (leaf == -2) {
+        if (kAhead) { hs->delta += st.mode == W_DELTA; hs->ratio += st.mode == W_RATIO; }   // (a lean kernel runs no emission walk)
+        return;
+    }
     if (leaf == -1) { st.op = OP_GLUE; st.exit_reason = EX_OUTSIDE; return; }
+    if (kAhead && leaf == -3) {
+        hs->ahead++;
+        st.op = OP_GLUE; st.exit_reason = EX_OUTSIDE;
+        if (st.mode == W_DELTA) {
+            if (((st.packed >> 14) & 1u) && st.alpha < 1.0f) st.alpha += st.alpha;   // first walk: the depth pass's replay (depth stays 0)
+            st.op = OP_FINISH;
+        }
+        return;
+    }
 
     if (st.mode == W_DELTA) {
         // distance to the box exit (or to the sphere) from the CURRENT position, every step (:1647-1651)
@@ -565,7 +589,11 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     // moved two stack stores of k_trace<1, false, 3>)
     __shared__ FrameShared fs;
     extern __shared__ float pool_smem[];                         // kTraceWarps x kRayWords x kPool words (opt-in dynamic shared memory)
+    __shared__ EmptyAhead ea;
     load_frame_shared(fs, fa.scene);
+    // the lean kernels end walks at "empty ahead"; the generic ones keep their hot loop as it was (on the fireball, config 3, the extra
+    // code of the shortcut cost more in the fetch-bound loop than its hops saved)
+    if constexpr (kLean) build_empty_ahead(ea, *reinterpret_cast<AheadScratch*>(pool_smem), fs.oct, fa.empty_ahead != 0);   // the ray pool is free until the first refill
     const SceneTables& sc = fs.sc;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned lt_mask = (1u << lane) - 1u;
@@ -581,6 +609,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     const unsigned q_count = *fa.queue_count;
     bool queue_dry = (q_count == 0);
     uint32_t nlook = 0, lane_steps = 0, warp_iters = 0, lane_ops = 0, warp_ops = 0, lane_rays = 0;   // statistics
+    HopStats hs = {0u, 0u, 0u, 0u};
     PathState st;
 
     for (;;) {
@@ -662,7 +691,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
                     break;
                 }
                 if (cur >= 0) {
-                    walk_step<kLean, kCells>(st, fs, fa, tc, sph, nlook, &pv.f(9, cur), kPool); lane_steps++;
+                    walk_step<kLean, kCells, kLean>(st, fs, fa, tc, sph, nlook, &pv.f(9, cur), kPool, &ea, &hs); lane_steps++;
                     if (st.op != OP_STEP) {                        // walk ended: park the ray with its new tag
                         store_walk(pv, cur, st);
                         if (cur == 0) tag0 = st.op; else if (cur == 1) tag1 = st.op; else tag2 = st.op;
@@ -683,6 +712,14 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
         if (lane == 0) {
             atomicAdd(fa.counters + 0, a); atomicAdd(fa.counters + 1, b); atomicAdd(fa.counters + 2, (unsigned long long)warp_iters);
             atomicAdd(fa.counters + 3, c); atomicAdd(fa.counters + 4, (unsigned long long)warp_ops); atomicAdd(fa.counters + 5, d);
+        }
+        if constexpr (kLean) {                                // hop statistics: counted by the kernels that end walks at "empty ahead"
+            uint32_t h[4] = {hs.delta, hs.ratio, hs.emit, hs.ahead};
+            #pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                for (int o = 16; o > 0; o >>= 1) h[k] += __shfl_xor_sync(0xffffffffu, h[k], o);
+                if (lane == 0) atomicAdd(fa.counters + 8 + k, (unsigned long long)h[k]);
+            }
         }
     }
 }

@@ -132,32 +132,146 @@ VPT_DEV float oct_child_exit(const OctInternal& n, int c, float3 o, float3 d) {
     return tmax;
 }
 
+// ---- "nothing populated ahead": the orthant occupancy table (DESIGN.md section 8j) -----------------------------------------------
+// A walk only moves forward: every move is p += d * t with t >= 0, so along each axis no coordinate ever moves against the sign of d.
+// Read the octree as an 8x8x8 grid of cells, the cell coordinate on an axis being the three "upper side" bits of the descent (x: p.x >
+// half.x, y: p.y >= half.y, z: p.z > half.z, levels 1, 2, 3 from the top).  Each bit is monotone in its coordinate, and two points
+// whose descents share a prefix on an axis are compared against the same split plane at the next level -- provided every non-empty
+// node with that prefix splits the axis at the same float, which build_empty_ahead checks.  So the cell coordinate is monotone too:
+// from any point in an empty node N, every later position of the walk lies in a cell of N's block or beyond it in the direction of d
+// (the orthant of N's block for the octant of d).  If no populated leaf lies there, the walk only hops over empty nodes until it
+// leaves the root box.  The table holds that answer for every (node, child) pair below the root and every octant: integer-only and
+// conservative, no float margin.
+constexpr int kAheadEntries = 8 + 64 + 512;       // entry of child c of internal node i: i * 8 + c
+struct EmptyAhead { uint8_t bit[kAheadEntries + 8]; };   // bit o of entry e: no populated leaf in the orthant of e's block for octant o
+struct AheadScratch {
+    unsigned long long occ[8];                    // [z] populated leaves, bit y * 8 + x (cell coordinates)
+    unsigned long long sfx[8][8];                 // [octant][z] cells whose orthant holds a populated leaf
+    int bad;                                      // the split planes do not form one grid: every entry stays "maybe"
+};
+
+// octant of a direction: bit 0 x < 0, bit 1 y < 0, bit 2 z < 0 (a zero component may take either side: it never moves)
+VPT_DEV int dir_octant(float3 d) { return (d.x < 0.0f ? 1 : 0) | (d.y < 0.0f ? 2 : 0) | (d.z < 0.0f ? 4 : 0); }
+VPT_DEV bool empty_ahead(const EmptyAhead& ea, int entry, float3 d) { return (ea.bit[entry] >> dir_octant(d)) & 1u; }
+
+// upper-side bit of child c on axis a (y is reversed in the child order: bit 1 set means y-minus)
+VPT_DEV int child_upper(int c, int a) { return a == 1 ? ((c >> 1) & 1) ^ 1 : (c >> (a == 0 ? 0 : 2)) & 1; }
+
+// Built by the whole CTA from the staged internal nodes (`oct` must be complete; ends with a barrier).  enable == false leaves every
+// entry 0: the walks then hop exactly as without the table.
+VPT_DEV void build_empty_ahead(EmptyAhead& ea, AheadScratch& s, const OctShared& oct, bool enable)
+{
+    const int t = threadIdx.y * blockDim.x + threadIdx.x, nt = blockDim.x * blockDim.y;
+    const uint32_t re = oct.node[0].child_empty;
+    auto node_full = [&](int i) {                  // internal node i (1..72) holds a volume
+        if (i < 9) return !((re >> (i - 1)) & 1u);
+        const int c1 = (i - 9) >> 3, c2 = (i - 9) & 7;
+        return !((re >> c1) & 1u) && !((oct.node[1 + c1].child_empty >> c2) & 1u);
+    };
+    if (t == 0) s.bad = enable ? 0 : 1;
+    __syncthreads();
+    // (1) every non-empty node splits an axis at the same float as the non-empty nodes of its level that share its cell prefix on that
+    //     axis (their children differ only in the other two axes' bits)
+    int bad = 0;
+    for (int i = 1 + t; i < kOctInternalNodes; i += nt) {
+        if (!node_full(i)) continue;
+        const bool l1 = i < 9;
+        const int c1 = l1 ? i - 1 : (i - 9) >> 3, c2 = l1 ? 0 : (i - 9) & 7;
+        for (int a = 0; a < 3; ++a) {
+            const int free_bits = 7 & ~(1 << a);
+            for (int m1 = 0; m1 < 8; ++m1) for (int m2 = 0; m2 < (l1 ? 1 : 8); ++m2) {
+                if ((m1 & ~free_bits) || (m2 & ~free_bits) || (m1 | m2) == 0) continue;
+                const int j = l1 ? 1 + (c1 ^ m1) : 9 + (c1 ^ m1) * 8 + (c2 ^ m2);
+                if (node_full(j) && !(oct.node[j].half[a] == oct.node[i].half[a])) bad = 1;
+            }
+        }
+    }
+    if (bad) s.bad = 1;
+    // (2) populated leaves, one (y, z) row of cells per thread
+    for (int r = t; r < 64; r += nt) {
+        const int iy = r & 7, iz = r >> 3;
+        uint32_t row = 0;
+        for (int ix = 0; ix < 8; ++ix) {
+            auto child = [&](int b) { return ((ix >> b) & 1) | ((((iy >> b) & 1) ^ 1) << 1) | (((iz >> b) & 1) << 2); };
+            const int c1 = child(2), c2 = child(1), c3 = child(0);
+            const bool full = !((re >> c1) & 1u) && !((oct.node[1 + c1].child_empty >> c2) & 1u) &&
+                              !((oct.node[9 + c1 * 8 + c2].child_empty >> c3) & 1u);
+            row |= (uint32_t)full << ix;
+        }
+        reinterpret_cast<uint8_t*>(s.occ)[r] = (uint8_t)row;
+    }
+    __syncthreads();
+    // (3) per octant, the cells from which a populated leaf lies ahead: OR over z in the direction of travel, then suffix-OR sweeps in x
+    //     (within each byte) and y (across bytes)
+    for (int k = t; k < 64; k += nt) {
+        const int o = k >> 3, iz = k & 7;
+        unsigned long long p = 0;
+        for (int z = 0; z < 8; ++z) if ((o & 4) ? z <= iz : z >= iz) p |= s.occ[z];
+        if (o & 1) { p |= (p << 1) & 0xfefefefefefefefeull; p |= (p << 2) & 0xfcfcfcfcfcfcfcfcull; p |= (p << 4) & 0xf0f0f0f0f0f0f0f0ull; }
+        else       { p |= (p >> 1) & 0x7f7f7f7f7f7f7f7full; p |= (p >> 2) & 0x3f3f3f3f3f3f3f3full; p |= (p >> 4) & 0x0f0f0f0f0f0f0f0full; }
+        if (o & 2) { p |= p << 8; p |= p << 16; p |= p << 32; }
+        else       { p |= p >> 8; p |= p >> 16; p |= p >> 32; }
+        s.sfx[o][iz] = p;
+    }
+    __syncthreads();
+    // (4) each entry's block corner that comes first along the octant's direction; its bit answers for the whole block
+    for (int e = t; e < kAheadEntries + 8; e += nt) {
+        uint32_t v = 0;
+        if (e < kAheadEntries && !s.bad) {
+            const int lvl = e < 8 ? 1 : e < 72 ? 2 : 3;
+            const int j = lvl == 1 ? e : lvl == 2 ? e - 8 : e - 72;
+            const int cs[3] = {lvl == 1 ? j : lvl == 2 ? j >> 3 : j >> 6, lvl == 2 ? j & 7 : (j >> 3) & 7, j & 7};
+            const int size = 8 >> lvl;
+            int lo[3];
+            for (int a = 0; a < 3; ++a) {
+                lo[a] = 0;
+                for (int l = 0; l < lvl; ++l) lo[a] += child_upper(cs[l], a) << (2 - l);
+            }
+            for (int o = 0; o < 8; ++o) {
+                const int cx = (o & 1) ? lo[0] + size - 1 : lo[0];
+                const int cy = (o & 2) ? lo[1] + size - 1 : lo[1];
+                const int cz = (o & 4) ? lo[2] + size - 1 : lo[2];
+                if (!((s.sfx[o][cz] >> (cy * 8 + cx)) & 1ull)) v |= 1u << o;
+            }
+        }
+        ea.bit[e] = (uint8_t)v;
+    }
+    __syncthreads();
+}
+
 // Returns leaf index 0..511, or -1 "outside the root box", or -2 "skipped an empty node" (ray_pos advanced).
 // kOneExit: one code site for the empty-child exit instead of one per level -- 64 instructions shorter; faster in k_generate
 // and slightly slower in the trace kernel's stepping loop, so each caller picks its form.  Same arithmetic either way.
-template <bool kOneExit = false>
-VPT_DEV int oct_locate_or_skip(const OctShared& oct, const SceneTables& sc, float3& ray_pos, float3 ray_dir) {
+// kAhead: at an empty node whose entry in `ea` says no populated leaf lies ahead (and `allow`), return -3 "empty ahead" instead of
+// hopping: the hops would only carry ray_pos out of the root box, drawing nothing.  ray_pos is then left where it was.
+template <bool kOneExit = false, bool kAhead = false>
+VPT_DEV int oct_locate_or_skip(const OctShared& oct, const SceneTables& sc, float3& ray_pos, float3 ray_dir,
+                               const EmptyAhead* ea = nullptr, bool allow = true) {
     if (!aabb_contains(sc.root_pmin, sc.root_pmax, ray_pos)) return -1;
     if (kOneExit) {
     // three levels of descent, ONE code site for the empty-child exit (the slab test of the child box is the bulky part)
     const OctInternal* n = &oct.node[0];
     int c = oct_child(*n, ray_pos);
     int leaf = c * 64;
+    int entry = c;
     bool empty = (n->child_empty >> c) & 1u;
     if (!empty) {
         const int c1 = c;
         n = &oct.node[1 + c1];
         c = oct_child(*n, ray_pos);
         leaf += c * 8;
+        if (kAhead) entry = 8 + leaf / 8;
         empty = (n->child_empty >> c) & 1u;
         if (!empty) {
             n = &oct.node[9 + c1 * 8 + c];
             c = oct_child(*n, ray_pos);
             leaf += c;
+            if (kAhead) entry = 72 + leaf;
             empty = (n->child_empty >> c) & 1u;
         }
     }
     if (empty) {
+        if (kAhead && allow && empty_ahead(*ea, entry, ray_dir)) return -3;
         const float t_max = fmaxf(oct_child_exit(*n, c, ray_pos, ray_dir), 0.1f);
         ray_pos = madd3(ray_pos, ray_dir, t_max);
         return -2;
@@ -167,6 +281,7 @@ VPT_DEV int oct_locate_or_skip(const OctShared& oct, const SceneTables& sc, floa
     const OctInternal& r = oct.node[0];
     const int c1 = oct_child(r, ray_pos);
     if ((r.child_empty >> c1) & 1u) {
+        if (kAhead && allow && empty_ahead(*ea, c1, ray_dir)) return -3;
         float t_max = fmaxf(oct_child_exit(r, c1, ray_pos, ray_dir), 0.1f);
         ray_pos = madd3(ray_pos, ray_dir, t_max);
         return -2;
@@ -174,6 +289,7 @@ VPT_DEV int oct_locate_or_skip(const OctShared& oct, const SceneTables& sc, floa
     const OctInternal& n1 = oct.node[1 + c1];
     const int c2 = oct_child(n1, ray_pos);
     if ((n1.child_empty >> c2) & 1u) {
+        if (kAhead && allow && empty_ahead(*ea, 8 + c1 * 8 + c2, ray_dir)) return -3;
         float t_max = fmaxf(oct_child_exit(n1, c2, ray_pos, ray_dir), 0.1f);
         ray_pos = madd3(ray_pos, ray_dir, t_max);
         return -2;
@@ -181,6 +297,7 @@ VPT_DEV int oct_locate_or_skip(const OctShared& oct, const SceneTables& sc, floa
     const OctInternal& n2 = oct.node[9 + c1 * 8 + c2];
     const int c3 = oct_child(n2, ray_pos);
     if ((n2.child_empty >> c3) & 1u) {
+        if (kAhead && allow && empty_ahead(*ea, 72 + c1 * 64 + c2 * 8 + c3, ray_dir)) return -3;
         float t_max = fmaxf(oct_child_exit(n2, c3, ray_pos, ray_dir), 0.1f);
         ray_pos = madd3(ray_pos, ray_dir, t_max);
         return -2;

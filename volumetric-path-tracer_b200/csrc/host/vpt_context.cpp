@@ -104,8 +104,8 @@ int vpt_create(vpt_context** out) {
     c->l2_bytes = (size_t)prop.l2CacheSize;
     VPT_CREATE(cudaMalloc(&c->d_scene, sizeof(vpt::SceneTables)));
     VPT_CREATE(cudaMalloc(&c->d_counters, sizeof(unsigned) * 4));
-    VPT_CREATE(cudaMalloc(&c->d_stats, sizeof(unsigned long long) * 8));
-    VPT_CREATE(cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 8));
+    VPT_CREATE(cudaMalloc(&c->d_stats, sizeof(unsigned long long) * 16));
+    VPT_CREATE(cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 16));
     VPT_CREATE(cudaHostAlloc((void**)&c->h_pinned, sizeof(int) * 8, cudaHostAllocDefault));
     // per-DEVICE kernel attributes (dynamic shared memory opt-in) and the occupancy the persistent grid is sized with
     VPT_CREATE(vpt::trace_kernels_init(c->max_ctas));
@@ -131,6 +131,7 @@ int vpt_set_option(vpt_context* c, const char* key, int value) {
     else if (k == "count_stats") { c->count_stats = value ? 1 : 0; }
     else if (k == "profile") { c->profile = value ? 1 : 0; }
     else if (k == "miss_cull") { c->miss_cull = value ? 1 : 0; }
+    else if (k == "empty_ahead") { c->empty_ahead = value ? 1 : 0; }
     else return fail(c, VPT_ERR_INVALID, "unknown option " + k);
     return VPT_OK;
 }
@@ -565,6 +566,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     if (ctas_per_sm < 1) ctas_per_sm = 1;
 
     fa.counters = c->count_stats ? c->d_stats : nullptr;
+    fa.empty_ahead = c->empty_ahead;
     fa.cell_table = c->cell_table; fa.cell_nx = c->cell_dims[0]; fa.cell_ny = c->cell_dims[1]; fa.cell_nz = c->cell_dims[2];
     const unsigned long long frame_px = (unsigned long long)kp.resolution.x * kp.resolution.y;
     plan.trace = trace; plan.trace_ctas = c->num_sms * ctas_per_sm;
@@ -914,7 +916,18 @@ int vpt_get_counters(vpt_context* c, unsigned long long out[8], int reset) {
     if (!c || !out) return VPT_ERR_INVALID;
     VPT_CUDA(c, cudaDeviceSynchronize());
     VPT_CUDA(c, cudaMemcpy(out, c->d_stats, sizeof(unsigned long long) * 8, cudaMemcpyDeviceToHost));
-    if (reset) VPT_CUDA(c, cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 8));
+    if (reset) VPT_CUDA(c, cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 16));
+    return VPT_OK;
+}
+
+// The hop statistics accumulated since the last reset (option "count_stats"; vpt_get_counters with reset clears them too): out[0..2] =
+// k_trace hops over empty nodes in delta / ratio / emission walks, out[3] = k_trace walks ended by "empty ahead", out[4..6] = k_generate
+// pre-step rays / their hops / pre-step rays ended by "empty ahead"; out[7] = 0.  Synchronises the device.
+int vpt_get_hop_counters(vpt_context* c, unsigned long long out[8], int reset) {
+    if (!c || !out) return VPT_ERR_INVALID;
+    VPT_CUDA(c, cudaDeviceSynchronize());
+    VPT_CUDA(c, cudaMemcpy(out, c->d_stats + 8, sizeof(unsigned long long) * 8, cudaMemcpyDeviceToHost));
+    if (reset) VPT_CUDA(c, cudaMemset(c->d_stats + 8, 0, sizeof(unsigned long long) * 8));
     return VPT_OK;
 }
 

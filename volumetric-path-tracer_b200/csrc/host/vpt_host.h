@@ -53,7 +53,8 @@ struct vpt_context {
     // stats
     unsigned long long launches = 0;
     int count_stats = 0;              // option "count_stats": accumulate trace counters
-    unsigned long long* d_stats = nullptr;   // 8 counters
+    int empty_ahead = 1;              // option "empty_ahead": walks end at the first empty node with no populated leaf ahead (same result)
+    unsigned long long* d_stats = nullptr;   // 16 counters (vpt_kernels.h FrameArgs::counters)
     int profile = 0;                  // option "profile": CUDA-event timing of every kernel (debug / bench breakdown)
     struct Ev { int kind; cudaEvent_t a, b; };
     std::vector<Ev> events;

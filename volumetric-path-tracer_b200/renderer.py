@@ -307,6 +307,14 @@ class Renderer:
         v = list(out)
         return dict(lookups=v[0], lane_steps=v[1], warp_step_iters=v[2], lane_services=v[3], warp_service_rounds=v[4], rays=v[5], brick_fetches=v[6])
 
+    def hop_counters(self, reset=True):
+        """Hop statistics (option "count_stats"); read them before counters(reset=True), which clears them too."""
+        out = (C.c_ulonglong * 8)()
+        check(lib.vpt_get_hop_counters(self.ctx, out, 1 if reset else 0), self.ctx, "vpt_get_hop_counters")
+        v = list(out)
+        return dict(hops_delta=v[0], hops_ratio=v[1], hops_emission=v[2], walks_ended_ahead=v[3],
+                    prestep_rays=v[4], prestep_hops=v[5], prestep_ended_ahead=v[6])
+
     def kernel_times(self):
         ms = (C.c_float * 4)(); n = (C.c_int * 4)()
         check(lib.vpt_get_kernel_times(self.ctx, ms, n), self.ctx, "vpt_get_kernel_times")
