@@ -334,6 +334,51 @@ int  vpt_set_projection(vpt_context* ctx, int kind, double hfov_deg, double vfov
  * jitter the blue-noise buffer holds now.  Reads params (camera, Kernel_params, blue noise); writes d_out_f4 only, on the default stream. */
 int  vpt_debug_camera_rays(vpt_context* ctx, void* const params[VPT_NUM_ARGS], float* d_out_f4);
 
+/* ---- omni-directional stereo (ODS): a stereo panorama for VR players, domes and video platforms -------------------------------------
+ * A mono panorama seen in a headset has no depth.  VPT_PROJECTION_ODS renders each eye's panorama from a point on a circle of radius ipd/2
+ * around the camera origin, so that every ray is tangent to that circle (the ODS construction every VR player expects).  The orientation is
+ * the camera's, as for VPT_PROJECTION_EQUIRECT: forward -w, right u, up v; row 0 at the bottom.
+ *
+ *   The sample's camera.  For pixel (x, y) at jitter (jx, jy): the layout gives the eye e (-1 left, +1 right), the row y_e within the eye and
+ *     the eye's height H_e (H, or H/2 over-under).  (phi, theta) and b0 are the equirectangular projection's at resolution (W, H_e), row y_e.
+ *     The pole merge k is 1 for |theta| <= from, 0 for |theta| >= to and (to - |theta|) / (to - from) in between, so the circle shrinks to the
+ *     centre near the poles (a step when from == to).  With s = (e ipd/2) k and r = cos phi u + sin phi w (the viewer's right at azimuth phi),
+ *     the sample's camera has origin' = fma(s, r, origin), lower_left_corner' = origin' + b0, horizontal = vertical = 0 and the caller's
+ *     u, v, w.  Its ray is the reference's camera::get_ray of that camera, bit for bit (the pinhole rule of the perspective camera), so
+ *     from the ray on every sample is the reference kernel's path for it.  Depth (and with it the AOVs' and deep slices' collision depth)
+ *     is measured from origin'.  The direction is llc' - origin', which is b0 only up to a rounding that grows with |origin| -- as the
+ *     reference's own perspective camera, whose lower_left_corner is stored in absolute coordinates too.
+ *   Layouts.  VPT_ODS_OVER_UNDER (the delivery format of VR players and video platforms): rows [H/2, H) -- the top, since row 0 is the
+ *     bottom -- are the left eye, rows [0, H/2) the right eye; H must be even.  VPT_ODS_LEFT / VPT_ODS_RIGHT: the whole frame is one eye.
+ *   Activation.  As vpt_set_projection: from the next render call whose Kernel_params.iteration is 0; vpt_set_projection(PERSPECTIVE or
+ *     EQUIRECT) switches back.
+ *   Works with vpt_render_pass(es), vpt_render_adaptive, render regions, AOVs, light groups, deep slices, brick and cell mode, both
+ *     integrators, both environments, partitioned contexts and both exchanges (a sharded adaptive frame with a region stays refused).  The
+ *     miss cull (option "miss_cull") skips the pixels of an HDRI frame that no ray from any point of the viewing circle can take to the
+ *     volume or the sphere, with the same result bit for bit.  An ODS frame runs no octree pre-step and keeps a per-ray origin, so it costs
+ *     more than an equirectangular frame of the same size.
+ *   Refused when set (VPT_ERR_INVALID; the projection stays as it was): vpt_set_projection with VPT_PROJECTION_ODS (its options are
+ *     missing); the field-of-view ranges of VPT_PROJECTION_EQUIRECT; a negative or non-finite ipd; an unknown layout; pole-merge angles
+ *     outside 0 <= from <= to <= 90.  Refused at render time (VPT_ERR_UNSUPPORTED): camera.lens_radius != 0; camera motion;
+ *     VPT_ODS_OVER_UNDER with an odd height.  Level (A) has no ODS projection. */
+#define VPT_PROJECTION_ODS 2
+#define VPT_ODS_LEFT       0   /* the whole frame is the left eye */
+#define VPT_ODS_RIGHT      1   /* the whole frame is the right eye */
+#define VPT_ODS_OVER_UNDER 2   /* rows [H/2, H) (the top: row 0 is the bottom) left eye, rows [0, H/2) right eye; H must be even */
+typedef struct vpt_ods_options {
+    float ipd;                  /* interocular distance in scene units; finite, >= 0 (default 0.064) */
+    int   layout;               /* VPT_ODS_* (default VPT_ODS_OVER_UNDER) */
+    float pole_merge_from_deg;  /* the eye separation is full up to this |elevation| ... (default 60) */
+    float pole_merge_to_deg;    /* ... and 0 from this one on, linear in between; 0 <= from <= to <= 90 (default 75) */
+} vpt_ods_options;
+void vpt_ods_options_defaults(vpt_ods_options* opt);
+int  vpt_set_projection_ods(vpt_context* ctx, double hfov_deg, double vfov_deg, const vpt_ods_options* opt);  /* opt NULL = defaults */
+/* Diagnostic: writes, for every local pixel, 8 floats: origin' (3), lower_left_corner' (3), e and k of the camera of that pixel's sample in
+ * the next render call's first pass, at the jitter the blue-noise buffer holds now (padding rows of a partitioned context all 0).  Reads
+ * params (camera, Kernel_params, blue noise); writes d_out only, on the default stream, and leaves the blue noise as it is.  VPT_ERR_INVALID
+ * when the next call has no ODS projection.  vpt_debug_camera_rays on an ODS frame writes llc' - origin' of that camera (camera_b0). */
+int  vpt_debug_ods_cameras(vpt_context* ctx, void* const params[VPT_NUM_ARGS], float* d_out);
+
 /* ---- camera motion: motion blur from a camera that moves between two poses over the shutter --------------------------------------
  * The reference draws a shutter time for every camera ray (camera::get_ray, right after the lens rejection loop) and never reads it.
  * Here that draw, xi in (0, 1] from the pixel's Philox stream, places the sample's camera between two poses: the Kernel_params camera is

@@ -163,6 +163,7 @@ EXPORTED_SYMBOLS = [
     "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
     "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
     "vpt_set_deep_buffers", "vpt_set_camera_motion", "vpt_debug_motion_cameras",
+    "vpt_ods_options_defaults", "vpt_set_projection_ods", "vpt_debug_ods_cameras",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -196,9 +197,19 @@ lib.vpt_set_light_group_buffers.argtypes = [_vp, _vp, _vp, _vp, _vp]; lib.vpt_se
 VPT_DEEP_MAX_SLICES = 32                                            # vpt_set_deep_buffers: most slices
 lib.vpt_set_deep_buffers.argtypes = [_vp, _vp, C.c_uint, C.POINTER(C.c_float)]; lib.vpt_set_deep_buffers.restype = C.c_int
 lib.vpt_set_render_region.argtypes = [_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint]; lib.vpt_set_render_region.restype = C.c_int
-VPT_PROJECTION_PERSPECTIVE, VPT_PROJECTION_EQUIRECT = 0, 1          # vpt_set_projection kinds
+VPT_PROJECTION_PERSPECTIVE, VPT_PROJECTION_EQUIRECT, VPT_PROJECTION_ODS = 0, 1, 2   # vpt_set_projection kinds
 lib.vpt_set_projection.argtypes = [_vp, C.c_int, C.c_double, C.c_double]; lib.vpt_set_projection.restype = C.c_int
 lib.vpt_debug_camera_rays.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_camera_rays.restype = C.c_int
+VPT_ODS_LEFT, VPT_ODS_RIGHT, VPT_ODS_OVER_UNDER = 0, 1, 2          # vpt_ods_options.layout
+
+
+class ods_options(C.Structure):
+    _fields_ = [("ipd", C.c_float), ("layout", C.c_int), ("pole_merge_from_deg", C.c_float), ("pole_merge_to_deg", C.c_float)]
+
+
+lib.vpt_ods_options_defaults.argtypes = [C.POINTER(ods_options)]; lib.vpt_ods_options_defaults.restype = None
+lib.vpt_set_projection_ods.argtypes = [_vp, C.c_double, C.c_double, C.POINTER(ods_options)]; lib.vpt_set_projection_ods.restype = C.c_int
+lib.vpt_debug_ods_cameras.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_ods_cameras.restype = C.c_int
 
 
 class denoise_options(C.Structure):

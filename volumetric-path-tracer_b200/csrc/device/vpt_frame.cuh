@@ -157,6 +157,45 @@ VPT_DEV vpt_camera motion_camera(const vpt_camera& cam, const CameraMotion& mo, 
     return m;
 }
 
+// The camera of pixel (x, y)'s sample at jitter (jx, jy) under the omni-directional stereo projection `od` (vpt_set_projection_ods):
+//   eye e (-1 left, +1 right), row y_e within the eye and the eye's height H_e from the layout (over-under: rows [H/2, H) are the left eye);
+//   (phi, theta) = pano_angles and b0 = pano_b0 at resolution (W, H_e), row y_e;
+//   k = 1 for |theta| <= merge_from, 0 for |theta| >= merge_to, (merge_to - |theta|) * inv_span in between (the pole merge);
+//   s = (e * ipd/2) * k, r = cos phi u + sin phi w (the viewer's right at azimuth phi; the __sinf / __cosf values pano_b0 takes);
+//   origin' = fma(s, r, origin), lower_left_corner' = origin' + b0, horizontal = vertical = 0, everything else the caller's camera.
+// generate_body traces that camera under the perspective rule, so every sample is the reference's camera::get_ray of it.  The operation
+// order is pinned: k_generate_ods (and its adaptive / region forms) and k_ods_cameras must get the same bits.
+struct OdsCamera { vpt_camera cam; float e, k; };
+VPT_DEV OdsCamera ods_camera(const vpt_camera& cam, const OdsParams& od, const vpt_u2 res, const int x, const int y, const float jx, const float jy)
+{
+    vpt_u2 re = res;
+    int ye = y;
+    float e = od.layout == kOdsRight ? 1.0f : -1.0f;
+    if (od.layout == kOdsOverUnder) {
+        re.y = res.y >> 1;
+        if (y >= (int)re.y) ye = y - (int)re.y;
+        else e = 1.0f;
+    }
+    Projection pj; pj.kind = kProjOds; pj.hfov = od.hfov; pj.vfov = od.vfov;
+    const float2 a = pano_angles(pj, re, x, ye, jx, jy);
+    const float3 b0 = pano_b0(cam, pj, re, x, ye, jx, jy);
+    const float at = fabsf(a.y);
+    const float k = at <= od.merge_from ? 1.0f : at >= od.merge_to ? 0.0f : pmul(psub(od.merge_to, at), od.inv_span);
+    const float s = pmul(e < 0.0f ? -od.half_ipd : od.half_ipd, k);
+    const float sp = __sinf(a.x), cp = __cosf(a.x);
+    OdsCamera o;
+    o.cam = cam; o.e = e; o.k = k;
+    o.cam.origin.x = pfma(s, pfma(cp, cam.u.x, pmul(sp, cam.w.x)), cam.origin.x);
+    o.cam.origin.y = pfma(s, pfma(cp, cam.u.y, pmul(sp, cam.w.y)), cam.origin.y);
+    o.cam.origin.z = pfma(s, pfma(cp, cam.u.z, pmul(sp, cam.w.z)), cam.origin.z);
+    o.cam.lower_left_corner.x = padd(o.cam.origin.x, b0.x);
+    o.cam.lower_left_corner.y = padd(o.cam.origin.y, b0.y);
+    o.cam.lower_left_corner.z = padd(o.cam.origin.z, b0.z);
+    o.cam.horizontal.x = o.cam.horizontal.y = o.cam.horizontal.z = 0.0f;
+    o.cam.vertical.x = o.cam.vertical.y = o.cam.vertical.z = 0.0f;
+    return o;
+}
+
 // the pinhole camera: what k_generate and k_miss_cull test before taking the pinhole branch (an origin component of exactly 0 could meet a
 // signed zero of the lens offset, so those cameras take the literal order)
 VPT_DEV bool pinhole_camera(const vpt_camera& cam)

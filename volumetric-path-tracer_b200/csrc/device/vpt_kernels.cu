@@ -28,6 +28,8 @@
 //                     (vpt_set_projection) -- the same kernels with the camera ray of pano_b0; k_camera_rays: vpt_debug_camera_rays
 //   k_generate_motion, k_generate_adaptive_motion, k_generate_region_motion : camera motion (vpt_set_camera_motion) -- k_generate with each
 //                     sample's camera placed between two poses by its shutter draw (motion_camera); k_motion_cameras: vpt_debug_motion_cameras
+//   k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods : omni-directional stereo (vpt_set_projection_ods) -- k_generate with each
+//                     sample's camera on its eye's viewing circle (ods_camera); k_ods_cameras: vpt_debug_ods_cameras, and the ODS camera rays
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -119,9 +121,11 @@ __global__ void k_prepare_scene(const vpt_gpu_vdb* __restrict__ vols, const vpt_
 // draw, whose index depends on how many trials the lens loop took, so every sample runs the loop first, takes xi where the static kernels
 // skip the shutter draw, and builds its ray from motion_camera(xi) in the thin-lens order (a pinhole's rd is +-0).  No pre-step: queue_aux
 // carries the per-ray origin (the host sets thin_lens), and the host runs no miss cull.
-template <bool kAdaptive, bool kRegion = false, bool kPano = false, bool kMotion = false>
+// kOds (k_generate_ods, ...): each sample's camera is ods_camera's under `od` (its own origin, horizontal = vertical = 0), traced by the
+// perspective rule below as the reference camera it is.  No pre-step and no miss cull, as for motion: queue_aux carries the origin.
+template <bool kAdaptive, bool kRegion = false, bool kPano = false, bool kMotion = false, bool kOds = false>
 __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptArgs* ad, const RenderRegion* rg = nullptr, const Projection* pj = nullptr,
-                                              const CameraMotion* mo = nullptr)
+                                              const CameraMotion* mo = nullptr, const OdsParams* od = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -165,7 +169,7 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
     load_frame_shared(fs, fa.scene);
     __shared__ EmptyAhead ea;
     __shared__ AheadScratch eas;
-    if constexpr (!kMotion) build_empty_ahead(ea, eas, fs.oct, fa.empty_ahead != 0);   // the pre-step's table (no pre-step under motion)
+    if constexpr (!kMotion && !kOds) build_empty_ahead(ea, eas, fs.oct, fa.empty_ahead != 0);   // the pre-step's table (none under motion / ODS)
     const SceneTables& sc = fs.sc;
     uint32_t n_pre = 0, n_hop = 0, n_ahead = 0;                 // statistics of the pre-step: rays, hops, rays ended by "empty ahead"
 
@@ -234,10 +238,13 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
             dir = normalize(f3(psub(b0.x, offset.x), psub(b0.y, offset.y), psub(b0.z, offset.z)));
             kdraws = rng.k;
         } else {
-            const bool pinhole = pinhole_camera(cam);
-            const float3 b0 = camera_b0(cam, kp.resolution, x, y, bnv.x, bnv.y);
+            vpt_camera ocam;
+            if constexpr (kOds) ocam = ods_camera(cam, *od, kp.resolution, x, y, bnv.x, bnv.y).cam;
+            const vpt_camera& pc = kOds ? ocam : cam;         // the camera whose ray the sample is
+            const bool pinhole = pinhole_camera(pc);
+            const float3 b0 = camera_b0(pc, kp.resolution, x, y, bnv.x, bnv.y);
             if (pinhole && b0.x != 0.0f && b0.y != 0.0f && b0.z != 0.0f) {
-                org = ld3(cam.origin);
+                org = ld3(pc.origin);
                 dir = normalize(b0);
                 lens_pending = true;
             } else {
@@ -247,10 +254,10 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
                     const float b = vdc3[int(rng.next() * 100)];
                     p = f3(pfma(a, 2.0f, -1.0f), pfma(b, 2.0f, -1.0f), 0.0f);
                 } while (pfma(p.x, p.x, pmul(p.y, p.y)) >= 1.0f);
-                const float3 rd = f3(pmul(cam.lens_radius, p.x), pmul(cam.lens_radius, p.y), 0.0f);
-                const float3 offset = f3(pfma(cam.u.x, rd.x, pmul(cam.v.x, rd.y)), pfma(cam.u.y, rd.x, pmul(cam.v.y, rd.y)), pfma(cam.u.z, rd.x, pmul(cam.v.z, rd.y)));
+                const float3 rd = f3(pmul(pc.lens_radius, p.x), pmul(pc.lens_radius, p.y), 0.0f);
+                const float3 offset = f3(pfma(pc.u.x, rd.x, pmul(pc.v.x, rd.y)), pfma(pc.u.y, rd.x, pmul(pc.v.y, rd.y)), pfma(pc.u.z, rd.x, pmul(pc.v.z, rd.y)));
                 ++rng.k;                                                 // shutter time draw: consumed, value unused by the path
-                org = f3(padd(cam.origin.x, offset.x), padd(cam.origin.y, offset.y), padd(cam.origin.z, offset.z));
+                org = f3(padd(pc.origin.x, offset.x), padd(pc.origin.y, offset.y), padd(pc.origin.z, offset.z));
                 dir = normalize(f3(psub(b0.x, offset.x), psub(b0.y, offset.y), psub(b0.z, offset.z)));
                 kdraws = rng.k;
             }
@@ -266,7 +273,7 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         // leaves the box without ever meeting a populated leaf contributes exactly what a miss does and never enters the
         // queue, the others are queued at the position where stepping really starts.  (Pinhole camera and a ray whose line
         // provably misses the sphere only; everything else takes the generic route.)
-        if (!kMotion && obj == 1 && kp.ray_depth >= 1 && kp.volume_depth >= 1 && cam.lens_radius == 0.0f && sphere_clear) {
+        if (!kMotion && !kOds && obj == 1 && kp.ray_depth >= 1 && kp.volume_depth >= 1 && cam.lens_radius == 0.0f && sphere_clear) {
             float3 p = madd3(org, dir, padd(t_min, VPT_EPS));
             int leaf = -2;
             if (!aabb_contains(sc.root_pmin, sc.root_pmax, p)) leaf = -1;
@@ -356,6 +363,17 @@ k_generate_adaptive_motion(const FrameArgs fa, const AdaptArgs ad, const CameraM
 __global__ void __launch_bounds__(128)
 k_generate_region_motion(const FrameArgs fa, const RenderRegion rg, const CameraMotion mo) { generate_body<false, true, false, true>(fa, nullptr, &rg, nullptr, &mo); }
 
+__global__ void __launch_bounds__(128)
+k_generate_ods(const FrameArgs fa, const OdsParams od) { generate_body<false, false, false, false, true>(fa, nullptr, nullptr, nullptr, nullptr, &od); }
+
+__global__ void __launch_bounds__(128)
+k_generate_adaptive_ods(const FrameArgs fa, const AdaptArgs ad, const OdsParams od)
+{ generate_body<true, false, false, false, true>(fa, &ad, nullptr, nullptr, nullptr, &od); }
+
+__global__ void __launch_bounds__(128)
+k_generate_region_ods(const FrameArgs fa, const RenderRegion rg, const OdsParams od)
+{ generate_body<false, true, false, false, true>(fa, nullptr, &rg, nullptr, nullptr, &od); }
+
 // =====================================================================================================
 // k_miss_cull
 // =====================================================================================================
@@ -383,6 +401,14 @@ __device__ __forceinline__ double3 box_corner(const double pmin[3], const double
 }
 __device__ __forceinline__ double dot_d(const double3 a, const double3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 __device__ __forceinline__ double len_d(const double3 a) { return sqrt(dot_d(a, a)); }
+// ODS: the squared radius of the sphere grown as line_misses_sphere grows it for an origin up to R from the camera origin (distance <= L + R),
+// then by R
+__device__ __forceinline__ double ods_grown_r2(const float radius, const double L2, const double R)
+{
+    const double L = sqrt(L2) + R;
+    const double rb = sqrt(1.02 * (double)radius * (double)radius + 2e-3 * L * L + 1e-6) + R;
+    return rb * rb;
+}
 
 // The equirectangular strip x0 .. x1 - 1 of global row y (tests (a) - (d) of miss_cull_body, kPano).  The float angles of its samples lie in
 // [phi(x0 + 0), phi(x1 + 0)] x [theta(y + 0), theta(y + 1)] (pano_angles is monotone), computed here by the same helper (the same bits).  In
@@ -392,9 +418,10 @@ __device__ __forceinline__ double len_d(const double3 a) { return sqrt(dot_d(a, 
 // to float rounding: with every entry of M^T M - I (M = [u v w]) at most e, M's condition number k has k^2 <= (1 + 3e) / (1 - 3e), and M
 // moves no angle by more than 2 asin((k - 1) / (k + 1)), which alpha takes in.  The float rounding of __sinf / __cosf, pano_b0 and normalize
 // (about 1e-6 rad) is far below kCullSlack.
+template <bool kOds = false>
 __device__ __forceinline__ bool pano_strip_culled(const vpt_camera& cam, const Projection& pj, const vpt_u2 res, const int x0, const int x1,
                                                   const int y, const double3* planes, const int n_planes, const double3 sa, const double L2,
-                                                  const double r2)
+                                                  const double r2, const double ods_delta = 0.0)
 {
     const double3 U = make_double3(cam.u.x, cam.u.y, cam.u.z), V = make_double3(cam.v.x, cam.v.y, cam.v.z), Wd = make_double3(cam.w.x, cam.w.y, cam.w.z);
     const double e = fmax(fmax(fmax(fabs(dot_d(U, U) - 1.0), fabs(dot_d(V, V) - 1.0)), fmax(fabs(dot_d(Wd, Wd) - 1.0), fabs(dot_d(U, V)))),
@@ -405,12 +432,19 @@ __device__ __forceinline__ bool pano_strip_culled(const vpt_camera& cam, const P
     const double p0 = lo.x, p1 = hi.x, t0 = lo.y, t1 = hi.y;
     const double pc = (p0 + p1) / 2, tc = (t0 + t1) / 2;
     const double cmax = (t0 <= 0.0 && t1 >= 0.0) ? 1.0 : fmax(cos(t0), cos(t1));
-    const double alpha = (t1 - t0) / 2 + cmax * (p1 - p0) / 2 + 2.0 * asin((k - 1.0) / (k + 1.0));
+    double alpha = (t1 - t0) / 2 + cmax * (p1 - p0) / 2 + 2.0 * asin((k - 1.0) / (k + 1.0));
+    if constexpr (kOds) alpha += ods_delta;
     if (!(alpha + kCullSlack < 1.5707963267948966)) return false;
     const double ct = cos(tc), st = sin(tc), sp = sin(pc), cp = cos(pc);
     double3 f = make_double3(ct * (sp * U.x - cp * Wd.x) + st * V.x, ct * (sp * U.y - cp * Wd.y) + st * V.y, ct * (sp * U.z - cp * Wd.z) + st * V.z);
     const double fl = len_d(f);
     f = make_double3(f.x / fl, f.y / fl, f.z / fl);
+    // ODS: every component of every ray direction is away from 0 (a unit vector within alpha of f moves each component by at most alpha),
+    // so k_generate_ods takes the pinhole order for every sample and k_resolve_ods rebuilds it as normalize(camera_b0)
+    if constexpr (kOds) {
+        const double m = alpha + kCullSlack;
+        if (!(fabs(f.x) > m && fabs(f.y) > m && fabs(f.z) > m)) return false;
+    }
     // (c)
     const double lim = -sin(alpha + kCullSlack);
     bool box_miss = false;
@@ -420,13 +454,45 @@ __device__ __forceinline__ bool pano_strip_culled(const vpt_camera& cam, const P
     return dot_d(f, sa) / sqrt(L2) < cos(alpha + asin(sqrt(r2 / L2)) + kCullSlack);
 }
 
+// The ODS cull's bounds (k_miss_cull_ods), in double, or a negative R when the camera cannot be culled:
+//   R, the radius of a ball around the camera origin that holds every origin' of the frame: |s| <= ipd/2, |r| <= sqrt((1 + 2e)(1 + 1e-5))
+//     + sqrt(3) 2^-23 (the float basis' error e as in pano_strip_culled, __sinf / __cosf within 2.5e-6 of the unit circle, the rounding of
+//     r's components), and the fma rounds each component of origin' by at most 2^-24 |origin'|;
+//   delta, the angle between llc' - origin' and b0: llc' and the subtraction round each component by at most 2^-24 (|origin'| + |b0|)
+//     and 2^-24 |llc' - origin'|, against |b0| >= 0.9.
+// Every origin component must be further than R from 0, so that no origin' component is 0 and the pinhole order is taken.
+struct OdsCullBounds { double R, delta; };
+__device__ __forceinline__ OdsCullBounds ods_cull_bounds(const vpt_camera& cam, const OdsParams& od)
+{
+    const double3 U = make_double3(cam.u.x, cam.u.y, cam.u.z), V = make_double3(cam.v.x, cam.v.y, cam.v.z), Wd = make_double3(cam.w.x, cam.w.y, cam.w.z);
+    const double e = fmax(fmax(fmax(fabs(dot_d(U, U) - 1.0), fabs(dot_d(V, V) - 1.0)), fmax(fabs(dot_d(Wd, Wd) - 1.0), fabs(dot_d(U, V)))),
+                          fmax(fabs(dot_d(U, Wd)), fabs(dot_d(V, Wd))));
+    OdsCullBounds b; b.R = -1.0; b.delta = 0.0;
+    if (!(e < 1e-4)) return b;
+    const double u24 = 5.9604644775390625e-8, s3 = 1.7320508075688772;
+    const double rb = sqrt((1.0 + 2.0 * e) * (1.0 + 1e-5)) + s3 * 2.0 * u24;
+    const double h = fabs((double)od.half_ipd);
+    const double omax = fmax(fmax(fabs((double)cam.origin.x), fabs((double)cam.origin.y)), fabs((double)cam.origin.z));
+    const double R = (h * rb + s3 * u24 * (omax + h * rb)) * (1.0 + 1e-12);
+    const double omin = fmin(fmin(fabs((double)cam.origin.x), fabs((double)cam.origin.y)), fabs((double)cam.origin.z));
+    const double err = s3 * 2.0 * u24 * (omax + R + 2.0);
+    if (!(isfinite(R) && omin > R && err < 0.45)) return b;
+    b.R = R; b.delta = asin(fmin(1.0, err / (0.9 - err)));
+    return b;
+}
+
 // kRegion (k_miss_cull_region): only the strips that hold a pixel of R -- the same strips, on the same kCullStrip grid, as a full frame.
 // kPano (k_miss_cull_equirect, k_miss_cull_region_equirect): the equirectangular projection `pj`, whose rays all start at the camera
 // origin.  (a) and (b) become: the camera has no lens, and the strip's directions lie in a cone of half-angle alpha < pi / 2 - kCullSlack
 // around the direction f of the centre of its (phi, theta) range (see below).  (c) holds when f . n < -sin(alpha + kCullSlack) for a
 // candidate plane n: every direction of the cone is then more than kCullSlack past the plane.  (d) is the test above with that cone.
-template <bool kRegion, bool kPano = false>
-__device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __restrict__ mask, const RenderRegion* rg, const Projection* pj = nullptr)
+// kOds (k_miss_cull_ods, k_miss_cull_region_ods): the ODS projection `od`.  Every origin' lies within R of the camera origin (ods_cull_bounds),
+// and a ray from origin' meets the root box (the sphere) only if the same ray from the origin meets the box grown by R on every axis (the
+// sphere grown by R).  So the panorama test runs from the origin with the grown box and sphere, on the strip's eye row, with alpha widened
+// by delta; the sphere's growth of line_misses_sphere is taken at distance L + R.
+template <bool kRegion, bool kPano = false, bool kOds = false>
+__device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __restrict__ mask, const RenderRegion* rg, const Projection* pj = nullptr,
+                                               const OdsParams* od = nullptr)
 {
     __shared__ double3 planes[kCullPlanes];
     __shared__ int n_planes;
@@ -435,11 +501,17 @@ __device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __r
     const double3 o = make_double3(cam.origin.x, cam.origin.y, cam.origin.z);
     double pmin[3], pmax[3];
     bool ok;
-    if constexpr (kPano) ok = cam.lens_radius == 0.0f;
+    if constexpr (kPano || kOds) ok = cam.lens_radius == 0.0f;
     else ok = pinhole_camera(cam);
     for (int a = 0; a < 3; ++a) {
         pmin[a] = fa.scene->root_pmin[a]; pmax[a] = fa.scene->root_pmax[a];
         ok = ok && isfinite(pmin[a]) && isfinite(pmax[a]) && pmin[a] <= pmax[a];       // an empty or broken root box culls nothing
+    }
+    OdsCullBounds ob; ob.R = 0.0; ob.delta = 0.0;
+    if constexpr (kOds) {
+        ob = ods_cull_bounds(cam, *od);
+        ok = ok && ob.R >= 0.0;
+        for (int a = 0; a < 3; ++a) { pmin[a] -= ob.R; pmax[a] += ob.R; }
     }
     if (threadIdx.x == 0) n_planes = 0;
     __syncthreads();
@@ -485,7 +557,17 @@ __device__ __forceinline__ void miss_cull_body(const FrameArgs& fa, uint8_t* __r
     bool culled = false;
     const SphereRec sph = load_sphere(fa.sphere);
     const double3 sa = make_double3(sph.center.x - o.x, sph.center.y - o.y, sph.center.z - o.z);
-    const double L2 = dot_d(sa, sa), r2 = 1.02 * (double)sph.radius * (double)sph.radius + 2e-3 * L2 + 1e-6;
+    const double L2 = dot_d(sa, sa), r2 = kOds ? ods_grown_r2(sph.radius, L2, ob.R) : 1.02 * (double)sph.radius * (double)sph.radius + 2e-3 * L2 + 1e-6;
+    if constexpr (kOds) {
+        if (ok && y < g.height && L2 > r2) {
+            // the strip's eye row, as ods_camera takes it (one strip lies in one row, so in one eye)
+            vpt_u2 re = fa.kp.resolution;
+            int ye = y;
+            if (od->layout == kOdsOverUnder) { re.y = fa.kp.resolution.y >> 1; if (y >= (int)re.y) ye = y - (int)re.y; }
+            Projection pe; pe.kind = kProjOds; pe.hfov = od->hfov; pe.vfov = od->vfov;
+            culled = pano_strip_culled<true>(cam, pe, re, x0, x1, ye, planes, n_planes, sa, L2, r2, ob.delta);
+        }
+    } else
     if constexpr (kPano) {
         if (ok && y < g.height && L2 > r2) culled = pano_strip_culled(cam, *pj, fa.kp.resolution, x0, x1, y, planes, n_planes, sa, L2, r2);
     } else
@@ -551,6 +633,15 @@ __global__ void __launch_bounds__(256)
 k_miss_cull_region_equirect(const FrameArgs fa, uint8_t* __restrict__ mask, const RenderRegion rg, const Projection pj)
 {
     miss_cull_body<true, true>(fa, mask, &rg, &pj);
+}
+
+__global__ void __launch_bounds__(256)
+k_miss_cull_ods(const FrameArgs fa, uint8_t* __restrict__ mask, const OdsParams od) { miss_cull_body<false, false, true>(fa, mask, nullptr, nullptr, &od); }
+
+__global__ void __launch_bounds__(256)
+k_miss_cull_region_ods(const FrameArgs fa, uint8_t* __restrict__ mask, const RenderRegion rg, const OdsParams od)
+{
+    miss_cull_body<true, false, true>(fa, mask, &rg, nullptr, &od);
 }
 
 
@@ -647,11 +738,11 @@ __device__ __forceinline__ void deep_end(const DeepSlices& dp, const uint8_t* do
 // the compositing AOVs in `aov` (DESIGN.md section 8c).  kGroups: also the running means of the light groups in `lg` (section 8d).
 // kPano (k_resolve_equirect, ...; HDRI frames): a culled pixel's miss samples are the equirectangular rays of the projection `pj`.
 // kDeep: the deep slices in `dp` (section 8h), updated lazily in their buffer, and no other store (see deep_pass).
-template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false, bool kDeep = false>
+template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false, bool kDeep = false, bool kOds = false>
 __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                               const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
                                               const AdaptArgs* ad, const AovBuffers* aov, const LightGroups* lg = nullptr,
-                                              const Projection* pj = nullptr, const DeepSlices* dp = nullptr)
+                                              const Projection* pj = nullptr, const DeepSlices* dp = nullptr, const OdsParams* od = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
@@ -824,7 +915,8 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         for (int p = 0; p < n_passes; ++p) {
             const float2 j = __ldg(fa.bn_table + (size_t)p * 65536 + (y % 256) * 256 + px % 256);
             float3 d;
-            if constexpr (kPano) d = normalize(pano_b0(cam, *pj, kp.resolution, px, y, j.x, j.y));
+            if constexpr (kOds) d = normalize(camera_b0(ods_camera(cam, *od, kp.resolution, px, y, j.x, j.y).cam, kp.resolution, px, y, j.x, j.y));
+            else if constexpr (kPano) d = normalize(pano_b0(cam, *pj, kp.resolution, px, y, j.x, j.y));
             else d = pinhole_dir(cam, kp.resolution, px, y, j.x, j.y);
             one_pass(p, make_float4(d.x, d.y, d.z, __uint_as_float(kMissSentinel)), zero4, zero4);
         }
@@ -893,10 +985,12 @@ __device__ __forceinline__ const DeepSlices* deep_of(const AovBuffers&, const De
 __device__ __forceinline__ const DeepSlices* deep_of(const LightGroups&, const DeepSlices& d) { return &d; }
 __device__ __forceinline__ const DeepSlices* deep_of(const AovBuffers&, const LightGroups&, const DeepSlices& d) { return &d; }
 
-// The thread's pixel and its resolve_pixel, shared by k_resolve and k_resolve_equirect (kPano: the projection `pj`)
-template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
+// The thread's pixel and its resolve_pixel, shared by k_resolve, k_resolve_equirect and k_resolve_ods (kProj: 0 the perspective camera,
+// 1 the equirectangular projection `pj`, 2 the ODS projection `od`)
+template <int kSky, bool kAov, bool kGroups, int kProj, class... Ext>
 __device__ __forceinline__ void resolve_body(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
-                                             const int write_display, const PeerFrames& peers, const Projection* pj, const Ext&... ext)
+                                             const int write_display, const PeerFrames& peers, const Projection* pj, const OdsParams* od,
+                                             const Ext&... ext)
 {
     const FrameGeom& g = fa.geom;
     const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
@@ -910,8 +1004,8 @@ __device__ __forceinline__ void resolve_body(const FrameArgs& fa, const SkyArg<k
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
     if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups, kPano, has_deep<Ext...>>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y, nullptr, ap, gp,
-                                                                       pj, dq);
+    resolve_pixel<kSky, false, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y,
+                                                                                         nullptr, ap, gp, pj, dq, od);
 }
 
 template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
@@ -920,16 +1014,16 @@ k_resolve(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const
           const Ext... ext)
 {
     static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
-    resolve_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, sampled, write_display, peers, nullptr, ext...);
+    resolve_body<kSky, kAov, kGroups, 0>(fa, atmo, n_passes, sampled, write_display, peers, nullptr, nullptr, ext...);
 }
 
 // k_resolve over R only: one thread per pixel of R on this rank, region row by region row (rg.lr0 .. rg.lr1 - 1, columns rg.x0 .. rg.x1 - 1),
 // so a warp reads and writes consecutive pixels of one row as k_resolve does.  Every pixel it visits is a pixel of R.  Shared by
 // k_resolve_region and k_resolve_region_equirect.
-template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
+template <int kSky, bool kAov, bool kGroups, int kProj, class... Ext>
 __device__ __forceinline__ void resolve_region_body(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                                     const int write_display, const PeerFrames& peers, const RenderRegion& rg, const Projection* pj,
-                                                    const Ext&... ext)
+                                                    const OdsParams* od, const Ext&... ext)
 {
     const FrameGeom& g = fa.geom;
     const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
@@ -944,8 +1038,8 @@ __device__ __forceinline__ void resolve_region_body(const FrameArgs& fa, const S
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
     if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups, kPano, has_deep<Ext...>>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, global_row(g, lr),
-                                                                       nullptr, ap, gp, pj, dq);
+    resolve_pixel<kSky, false, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr,
+                                                                                         global_row(g, lr), nullptr, ap, gp, pj, dq, od);
 }
 
 template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
@@ -954,7 +1048,7 @@ k_resolve_region(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes
                  const RenderRegion rg, const Ext... ext)
 {
     static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_region<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
-    resolve_region_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, sampled, write_display, peers, rg, nullptr, ext...);
+    resolve_region_body<kSky, kAov, kGroups, 0>(fa, atmo, n_passes, sampled, write_display, peers, rg, nullptr, nullptr, ext...);
 }
 
 // The equirectangular frames of the HDRI environment (sky 0): k_resolve, k_resolve_region and k_resolve_adaptive with the projection `pj` as
@@ -965,7 +1059,7 @@ k_resolve_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, con
                    const Projection pj, const Ext... ext)
 {
     static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
-    resolve_body<0, kAov, kGroups, true>(fa, atmo, n_passes, sampled, write_display, peers, &pj, ext...);
+    resolve_body<0, kAov, kGroups, 1>(fa, atmo, n_passes, sampled, write_display, peers, &pj, nullptr, ext...);
 }
 
 template <bool kAov = false, bool kGroups = false, class... Ext>
@@ -974,7 +1068,27 @@ k_resolve_region_equirect(const FrameArgs fa, const NoSky atmo, const int n_pass
                           const RenderRegion rg, const Projection pj, const Ext... ext)
 {
     static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_region_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
-    resolve_region_body<0, kAov, kGroups, true>(fa, atmo, n_passes, sampled, write_display, peers, rg, &pj, ext...);
+    resolve_region_body<0, kAov, kGroups, 1>(fa, atmo, n_passes, sampled, write_display, peers, rg, &pj, nullptr, ext...);
+}
+
+// The ODS frames of the HDRI environment (sky 0): the same with the ODS projection `od`, whose culled pixels' miss samples are rebuilt from
+// ods_camera (k_miss_cull_ods guarantees they took the pinhole order)
+template <bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve_ods(const FrameArgs fa, const NoSky atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+              const OdsParams od, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_ods<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
+    resolve_body<0, kAov, kGroups, 2>(fa, atmo, n_passes, sampled, write_display, peers, nullptr, &od, ext...);
+}
+
+template <bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(256)
+k_resolve_region_ods(const FrameArgs fa, const NoSky atmo, const int n_passes, const int sampled, const int write_display, const PeerFrames peers,
+                     const RenderRegion rg, const OdsParams od, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_region_ods<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
+    resolve_region_body<0, kAov, kGroups, 2>(fa, atmo, n_passes, sampled, write_display, peers, rg, nullptr, &od, ext...);
 }
 
 // 32x4 pixel tile and the lane's pixel in it, for the per-tile adaptive kernels (a warp covers one row of 32 pixels)
@@ -990,9 +1104,9 @@ __device__ __forceinline__ TilePixel tile_pixel(const FrameGeom& g, const int ti
 
 // One block of 128 per active tile: the running mean of the pixels that have not stopped, every pass of the chunk sampled; at the end of the
 // chunk their display / raw words, pass count and relative error (so a pixel keeps those of the last pass it took).  kAov: as k_resolve.
-template <int kSky, bool kAov, bool kGroups, bool kPano, class... Ext>
+template <int kSky, bool kAov, bool kGroups, int kProj, class... Ext>
 __device__ __forceinline__ void resolve_adaptive_body(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const AdaptArgs& ad,
-                                                      const Projection* pj, const Ext&... ext)
+                                                      const Projection* pj, const OdsParams* od, const Ext&... ext)
 {
     const FrameGeom& g = fa.geom;
     const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
@@ -1005,8 +1119,8 @@ __device__ __forceinline__ void resolve_adaptive_body(const FrameArgs& fa, const
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
     if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
-    resolve_pixel<kSky, true, kAov, kGroups, kPano, has_deep<Ext...>>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr, global_row(g, t.lr), &ad, ap,
-                                                                      gp, pj, dq);
+    resolve_pixel<kSky, true, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr,
+                                                                                        global_row(g, t.lr), &ad, ap, gp, pj, dq, od);
 }
 
 template <int kSky, bool kAov = false, bool kGroups = false, class... Ext>
@@ -1014,7 +1128,7 @@ __global__ void __launch_bounds__(128)
 k_resolve_adaptive(const FrameArgs fa, const SkyArg<kSky> atmo, const int n_passes, const AdaptArgs ad, const Ext... ext)
 {
     static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_adaptive<kSky, kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
-    resolve_adaptive_body<kSky, kAov, kGroups, false>(fa, atmo, n_passes, ad, nullptr, ext...);
+    resolve_adaptive_body<kSky, kAov, kGroups, 0>(fa, atmo, n_passes, ad, nullptr, nullptr, ext...);
 }
 
 template <bool kAov = false, bool kGroups = false, class... Ext>
@@ -1022,7 +1136,15 @@ __global__ void __launch_bounds__(128)
 k_resolve_adaptive_equirect(const FrameArgs fa, const NoSky atmo, const int n_passes, const AdaptArgs ad, const Projection pj, const Ext... ext)
 {
     static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_adaptive_equirect<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
-    resolve_adaptive_body<0, kAov, kGroups, true>(fa, atmo, n_passes, ad, &pj, ext...);
+    resolve_adaptive_body<0, kAov, kGroups, 1>(fa, atmo, n_passes, ad, &pj, nullptr, ext...);
+}
+
+template <bool kAov = false, bool kGroups = false, class... Ext>
+__global__ void __launch_bounds__(128)
+k_resolve_adaptive_ods(const FrameArgs fa, const NoSky atmo, const int n_passes, const AdaptArgs ad, const OdsParams od, const Ext... ext)
+{
+    static_assert(sizeof...(Ext) == (kAov ? 1 : 0) + (kGroups ? 1 : 0) + (has_deep<Ext...> ? 1 : 0),"k_resolve_adaptive_ods<kAov, kGroups> takes an AovBuffers if kAov, then a LightGroups if kGroups, then a DeepSlices for the deep slices");
+    resolve_adaptive_body<0, kAov, kGroups, 2>(fa, atmo, n_passes, ad, nullptr, &od, ext...);
 }
 
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
@@ -1305,6 +1427,30 @@ __global__ void k_motion_cameras(const vpt_camera cam, const CameraMotion mo, co
     o[19] = 0.f;
 }
 
+// vpt_debug_ods_cameras / vpt_debug_camera_rays on an ODS frame: every local pixel's ods_camera at the jitter `bn` holds now (read only).
+// rays == 0: origin', lower_left_corner', e, k (8 floats); rays == 1: (camera_b0 of that camera, 0), the ray direction before normalize
+__global__ void k_ods_cameras(const vpt_camera cam, const OdsParams od, const vpt_u2 res, const FrameGeom g, const float3* __restrict__ bn,
+                              const int rays, float* out)
+{
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= (uint32_t)g.n_local) return;
+    const int lr = lp / g.width, x = lp - lr * g.width;
+    const int y = global_row(g, lr);
+    const int n = rays ? 4 : 8;
+    float* o = out + (size_t)lp * n;
+    if (y >= g.height) { for (int i = 0; i < n; ++i) o[i] = 0.f; return; }
+    const float3 j = bn[(y % 256) * 256 + x % 256];
+    const OdsCamera c = ods_camera(cam, od, res, x, y, j.x, j.y);
+    if (rays) {
+        const float3 b = camera_b0(c.cam, res, x, y, j.x, j.y);
+        o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = 0.f;
+        return;
+    }
+    o[0] = c.cam.origin.x; o[1] = c.cam.origin.y; o[2] = c.cam.origin.z;
+    o[3] = c.cam.lower_left_corner.x; o[4] = c.cam.lower_left_corner.y; o[5] = c.cam.lower_left_corner.z;
+    o[6] = c.e; o[7] = c.k;
+}
+
 // =====================================================================================================
 // host-callable launchers
 // =====================================================================================================
@@ -1337,55 +1483,61 @@ static dim3 generate_grid(FrameArgs& a, long long tiles, int n_passes)
     return dim3((unsigned)((tiles + tpb - 1) / tpb), 1, (unsigned)((n_passes + ppb - 1) / ppb));
 }
 
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, cudaStream_t s)
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, const OdsParams* od, cudaStream_t s)
 {
     FrameArgs a = fa;
     const long long tiles = (long long)((fa.geom.width + 31) / 32) * ((fa.geom.local_rows + 3) / 4);
     const dim3 grid = generate_grid(a, tiles, n_passes);
     if (mo) k_generate_motion<<<grid, 128, 0, s>>>(a, *mo);
+    else if (od) k_generate_ods<<<grid, 128, 0, s>>>(a, *od);
     else if (equirect(pj)) k_generate_equirect<<<grid, 128, 0, s>>>(a, pj);
     else k_generate<<<grid, 128, 0, s>>>(a);
     return cudaGetLastError();
 }
 
-cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s)
+cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s, const OdsParams* od)
 {
     if (fa.geom.n_local <= 0) return cudaSuccess;
     const long long strips = (long long)fa.geom.local_rows * ((fa.geom.width + kCullStrip - 1) / kCullStrip);
-    if (equirect(pj)) k_miss_cull_equirect<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, pj);
+    if (od) k_miss_cull_ods<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, *od);
+    else if (equirect(pj)) k_miss_cull_equirect<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, pj);
     else k_miss_cull<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask);
     return cudaGetLastError();
 }
 
 cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, const CameraMotion* mo,
-                                   cudaStream_t s)
+                                   const OdsParams* od, cudaStream_t s)
 {
     const long long tiles = region_tiles(rg);
     if (tiles <= 0) return cudaSuccess;
     FrameArgs a = fa;
     const dim3 grid = generate_grid(a, tiles, n_passes);
     if (mo) k_generate_region_motion<<<grid, 128, 0, s>>>(a, rg, *mo);
+    else if (od) k_generate_region_ods<<<grid, 128, 0, s>>>(a, rg, *od);
     else if (equirect(pj)) k_generate_region_equirect<<<grid, 128, 0, s>>>(a, rg, pj);
     else k_generate_region<<<grid, 128, 0, s>>>(a, rg);
     return cudaGetLastError();
 }
 
-cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s)
+cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s,
+                                    const OdsParams* od)
 {
     if (rg.lr1 <= rg.lr0) return cudaSuccess;
     const long long strips = (long long)(rg.lr1 - rg.lr0) * ((rg.x1 + kCullStrip - 1) / kCullStrip - rg.x0 / kCullStrip);
-    if (equirect(pj)) k_miss_cull_region_equirect<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg, pj);
+    if (od) k_miss_cull_region_ods<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg, *od);
+    else if (equirect(pj)) k_miss_cull_region_equirect<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg, pj);
     else k_miss_cull_region<<<(unsigned)((strips + 255) / 256), 256, 0, s>>>(fa, mask, rg);
     return cudaGetLastError();
 }
 
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, const CameraMotion* mo,
-                                     cudaStream_t s)
+                                     const OdsParams* od, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
     FrameArgs a = fa;
     const dim3 grid = generate_grid(a, ad.n_tiles, n_passes);
     if (mo) k_generate_adaptive_motion<<<grid, 128, 0, s>>>(a, ad, *mo);
+    else if (od) k_generate_adaptive_ods<<<grid, 128, 0, s>>>(a, ad, *od);
     else if (equirect(pj)) k_generate_adaptive_equirect<<<grid, 128, 0, s>>>(a, ad, pj);
     else k_generate_adaptive<<<grid, 128, 0, s>>>(a, ad);
     return cudaGetLastError();
@@ -1497,6 +1649,34 @@ static cudaError_t resolve_kernels_equirect(const ResolveKey& r, const AovBuffer
     }
 }
 
+template <bool A, bool G, class F, class... E>
+static cudaError_t resolve_kernels_ods_deep(F&& f, const NoSky& sky, const E&... e)
+{
+    return f(+k_resolve_ods<A, G, E...>, +k_resolve_adaptive_ods<A, G, E...>, +k_resolve_region_ods<A, G, E...>, sky, e...);
+}
+
+// The ODS resolve kernels of the HDRI frames, in the form of resolve_kernels_equirect
+template <class F>
+static cudaError_t resolve_kernels_ods(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, F&& f)
+{
+    const NoSky hdri{};
+    if (r.sky != 0) return cudaErrorInvalidValue;
+    if (r.deep) switch (r.aov * 2 + r.groups) {
+    case 0:  return resolve_kernels_ods_deep<false, false>(f, hdri, dp);
+    case 1:  return resolve_kernels_ods_deep<false, true>(f, hdri, lg, dp);
+    case 2:  return resolve_kernels_ods_deep<true, false>(f, hdri, aov, dp);
+    case 3:  return resolve_kernels_ods_deep<true, true>(f, hdri, aov, lg, dp);
+    default: return cudaErrorInvalidValue;
+    }
+    switch (r.aov * 2 + r.groups) {
+    case 0:  return f(k_resolve_ods<false, false>, k_resolve_adaptive_ods<false, false>, k_resolve_region_ods<false, false>, hdri);
+    case 1:  return f(+k_resolve_ods<false, true, LightGroups>, +k_resolve_adaptive_ods<false, true, LightGroups>, +k_resolve_region_ods<false, true, LightGroups>, hdri, lg);
+    case 2:  return f(+k_resolve_ods<true, false, AovBuffers>, +k_resolve_adaptive_ods<true, false, AovBuffers>, +k_resolve_region_ods<true, false, AovBuffers>, hdri, aov);
+    case 3:  return f(+k_resolve_ods<true, true, AovBuffers, LightGroups>, +k_resolve_adaptive_ods<true, true, AovBuffers, LightGroups>, +k_resolve_region_ods<true, true, AovBuffers, LightGroups>, hdri, aov, lg);
+    default: return cudaErrorInvalidValue;
+    }
+}
+
 cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const float* brick_pool,
                          const int brick_dims[3], int n_ctas, cudaStream_t s)
 {
@@ -1549,12 +1729,15 @@ cudaError_t exchange_kernels_preload()
                     const cudaError_t ep = resolve_kernels_equirect(key, {}, {}, {},
                                                                     [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
                     if (ep != cudaSuccess) return ep;
+                    const cudaError_t eo = resolve_kernels_ods(key, {}, {}, {},
+                                                               [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
+                    if (eo != cudaSuccess) return eo;
                 }
     return load(k_prepare_scene, k_bn_prepare, k_bn_advance, k_miss_cull, k_generate, k_generate_adaptive, k_adapt_init, k_adapt, k_adapt_halo,
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
                 k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish, k_generate_motion, k_generate_adaptive_motion,
-                k_generate_region_motion);
+                k_generate_region_motion, k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_miss_cull_ods, k_miss_cull_region_ods);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1565,11 +1748,16 @@ cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, co
 
 static cudaError_t resolve_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                                   const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                                  cudaStream_t s)
+                                  const OdsParams* od, cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
+    if (od && key.sky == 0)
+        return resolve_kernels_ods(key, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+            kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, *od, ext...);
+            return cudaGetLastError();
+        });
     if (equirect(pj) && key.sky == 0)
         return resolve_kernels_equirect(key, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
             kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, pj, ext...);
@@ -1585,12 +1773,17 @@ static cudaError_t resolve_launch(const FrameArgs& fa, const ResolveKey& key, co
 
 static cudaError_t resolve_region_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled,
                                          int write_display, const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp,
-                                         const RenderRegion& rg, const Projection& pj, cudaStream_t s)
+                                         const RenderRegion& rg, const Projection& pj, const OdsParams* od, cudaStream_t s)
 {
     const long long n = region_pixels(rg);
     if (n <= 0) return cudaSuccess;
     const int threads = 256;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
+    if (od && key.sky == 0)
+        return resolve_kernels_ods(key, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+            kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, *od, ext...);
+            return cudaGetLastError();
+        });
     if (equirect(pj) && key.sky == 0)
         return resolve_kernels_equirect(key, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
             kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, pj, ext...);
@@ -1603,9 +1796,15 @@ static cudaError_t resolve_region_launch(const FrameArgs& fa, const ResolveKey& 
 }
 
 static cudaError_t resolve_adaptive_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                           const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s)
+                                           const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
+                                           const OdsParams* od, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
+    if (od && key.sky == 0)
+        return resolve_kernels_ods(key, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+            kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, *od, ext...);
+            return cudaGetLastError();
+        });
     if (equirect(pj) && key.sky == 0)
         return resolve_kernels_equirect(key, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
             kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, pj, ext...);
@@ -1623,34 +1822,35 @@ static ResolveKey without_deep(const ResolveKey& key) { ResolveKey k = key; k.de
 
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                            const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                           cudaStream_t s)
+                           cudaStream_t s, const OdsParams* od)
 {
     if (key.deep) {
-        const cudaError_t e = resolve_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, pj, s);
+        const cudaError_t e = resolve_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, pj, od, s);
         if (e != cudaSuccess) return e;
     }
-    return resolve_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, pj, s);
+    return resolve_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, pj, od, s);
 }
 
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                                   const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,
-                                  const Projection& pj, cudaStream_t s)
+                                  const Projection& pj, cudaStream_t s, const OdsParams* od)
 {
     if (key.deep) {
-        const cudaError_t e = resolve_region_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, rg, pj, s);
+        const cudaError_t e = resolve_region_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, rg, pj, od, s);
         if (e != cudaSuccess) return e;
     }
-    return resolve_region_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, rg, pj, s);
+    return resolve_region_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, rg, pj, od, s);
 }
 
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s)
+                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s,
+                                    const OdsParams* od)
 {
     if (key.deep) {
-        const cudaError_t e = resolve_adaptive_launch(fa, key, atm, n_passes, ad, aov, lg, dp, pj, s);
+        const cudaError_t e = resolve_adaptive_launch(fa, key, atm, n_passes, ad, aov, lg, dp, pj, od, s);
         if (e != cudaSuccess) return e;
     }
-    return resolve_adaptive_launch(fa, without_deep(key), atm, n_passes, ad, aov, lg, dp, pj, s);
+    return resolve_adaptive_launch(fa, without_deep(key), atm, n_passes, ad, aov, lg, dp, pj, od, s);
 }
 
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s)
@@ -1755,6 +1955,14 @@ cudaError_t launch_motion_cameras(const vpt_camera& cam, const CameraMotion& mo,
 {
     if (g.n_local <= 0) return cudaSuccess;
     k_motion_cameras<<<(g.n_local + 255) / 256, 256, 0, s>>>(cam, mo, g, iteration, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ods_cameras(const vpt_camera& cam, const OdsParams& od, const vpt_u2 res, const FrameGeom& g, const void* bn, int rays, float* out,
+                               cudaStream_t s)
+{
+    if (g.n_local <= 0) return cudaSuccess;
+    k_ods_cameras<<<(g.n_local + 255) / 256, 256, 0, s>>>(cam, od, res, g, reinterpret_cast<const float3*>(bn), rays, out);
     return cudaGetLastError();
 }
 

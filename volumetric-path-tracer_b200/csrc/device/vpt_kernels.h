@@ -123,15 +123,28 @@ inline bool equirect(const Projection& p) { return p.kind == kProjEquirect; }
 // pick them for a non-null CameraMotion), as Projection is.
 struct CameraMotion { vpt_f3 origin, lower_left_corner, horizontal, vertical, u, v; };
 
+// Omni-directional stereo (vpt_set_projection_ods): Projection::kind is kProjOds, and these are the rest of the projection.  Each sample's
+// camera is ods_camera's (vpt_frame.cuh): the panorama of (hfov, vfov) per eye, its origin moved by +-half_ipd * k along the viewer's
+// right, k the pole merge (1 up to |theta| = merge_from, 0 from merge_to on, (merge_to - |theta|) * inv_span in between; angles in
+// radians).  A kernel argument of the ODS kernels only (k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_ods_cameras: the
+// launchers below pick them for a non-null OdsParams), as Projection is.
+constexpr int kProjOds = 2;                                       // VPT_PROJECTION_ODS of vpt_b200.h
+constexpr int kOdsLeft = 0, kOdsRight = 1, kOdsOverUnder = 2;     // VPT_ODS_LEFT, VPT_ODS_RIGHT, VPT_ODS_OVER_UNDER
+struct OdsParams { float hfov = 0.f, vfov = 0.f, half_ipd = 0.f; int layout = kOdsOverUnder; float merge_from = 0.f, merge_to = 0.f, inv_span = 0.f; };
+inline bool ods(const Projection& p) { return p.kind == kProjOds; }
+
 cudaError_t launch_prepare_scene(const vpt_gpu_vdb* vols, const vpt_octnode* root, SceneTables* out, OctInternal* internal,
                                  uint2* leaf_list, int* leaf_indices, VolumeRec* vrec, int max_volumes, cudaStream_t s);
 cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& hdr, SceneTables* out, VolumeRec* vrec, cudaStream_t s);
 // pj: the frame's projection -- the launchers below run the equirectangular kernels when equirect(pj); mo: the frame's shutter-close pose
-// (null: no motion) -- the generate launchers run the motion kernels when it is set (never together with equirect(pj): the host refuses that)
-cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, cudaStream_t s);
+// (null: no motion) -- the generate launchers run the motion kernels when it is set (never together with equirect(pj): the host refuses that);
+// od: the frame's ODS projection (null unless ods(pj)) -- the generate, cull and resolve launchers run the ODS kernels when it is set (never
+// with motion)
+cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, const OdsParams* od, cudaStream_t s);
 // once per render call, before the first chunk: mask[local pixel] = 1 where every jitter misses the root box and the sphere (pinhole
 // and equirectangular cameras; a thin lens or a root box that is empty or not finite culls nothing)
-cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s);
+// od: the frame's ODS projection (null unless ods(pj)) -- the cull and resolve launchers below run the ODS kernels when it is set
+cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
 struct LightGroups;
 // The trace kernels, with their instantiations in trace_kernel (vpt_kernels.cu): generic / lean / volumetric path at 3 rays per lane,
 // k_trace_brick, generic / lean at 2, lean at 2 on the cell table, generic / volumetric path keeping the light-group planes.
@@ -187,7 +200,7 @@ struct DeepSlices { float4* out = nullptr; int n = 0; float z[kDeepMaxSlices + 1
 struct ResolveKey { int sky = 0; bool aov = false, groups = false, deep = false; };
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                            const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                           cudaStream_t s);
+                           cudaStream_t s, const OdsParams* od = nullptr);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -217,12 +230,18 @@ cudaError_t launch_camera_rays(const vpt_camera& cam, const vpt_u2 res, const Fr
 // vpt_debug_motion_cameras: out[local pixel * 20 ..] = xi, then origin, lower_left_corner, horizontal, vertical, u, v of motion_camera at the
 // shutter draw of the pixel's first pass at `iteration` (19 floats, padded with 0; padding rows all 0)
 cudaError_t launch_motion_cameras(const vpt_camera& cam, const CameraMotion& mo, const FrameGeom& g, uint32_t iteration, float* out, cudaStream_t s);
+// vpt_debug_ods_cameras (rays == 0): out[local pixel * 8 ..] = origin', lower_left_corner', e, k of ods_camera for the next render call's
+// first pass; vpt_debug_camera_rays on an ODS frame (rays == 1): out[local pixel * 4 ..] = (camera_b0 of that camera, 0).  Both at the jitter
+// the blue-noise buffer `bn` holds now (read only); padding rows all 0
+cudaError_t launch_ods_cameras(const vpt_camera& cam, const OdsParams& od, const vpt_u2 res, const FrameGeom& g, const void* bn, int rays, float* out,
+                               cudaStream_t s);
 // adaptive frame: k_generate / k_resolve over the tiles of ad.tiles only (stopped pixels sample nothing and keep their buffers); the resolve
 // also updates the Welford state and writes pass_count, rel_error, display and raw of the pixels it visits
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, const CameraMotion* mo,
-                                     cudaStream_t s);
+                                     const OdsParams* od, cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s);
+                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s,
+                                    const OdsParams* od = nullptr);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);
@@ -233,11 +252,12 @@ cudaError_t launch_adapt_init(const FrameGeom& g, uint8_t* stopped, unsigned* ti
 // Adaptive, one rank: the tile list starts as R's tiles with every pixel outside R stopped, and k_adapt_region clips the 3x3 neighbourhood
 // at R's edge.
 cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const RenderRegion& rg, const Projection& pj, const CameraMotion* mo,
-                                   cudaStream_t s);
-cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s);
+                                   const OdsParams* od, cudaStream_t s);
+cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s,
+                                    const OdsParams* od = nullptr);
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                                   const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,
-                                  const Projection& pj, cudaStream_t s);
+                                  const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
 cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s);
 cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s);
 

@@ -194,21 +194,63 @@ int vpt_set_render_region(vpt_context* c, unsigned x0, unsigned y0, unsigned x1,
     return VPT_OK;
 }
 
-static_assert(vpt::kProjPerspective == VPT_PROJECTION_PERSPECTIVE && vpt::kProjEquirect == VPT_PROJECTION_EQUIRECT, "projection kinds");
+static_assert(vpt::kProjPerspective == VPT_PROJECTION_PERSPECTIVE && vpt::kProjEquirect == VPT_PROJECTION_EQUIRECT &&
+              vpt::kProjOds == VPT_PROJECTION_ODS, "projection kinds");
+static_assert(vpt::kOdsLeft == VPT_ODS_LEFT && vpt::kOdsRight == VPT_ODS_RIGHT && vpt::kOdsOverUnder == VPT_ODS_OVER_UNDER, "ODS layouts");
+
+// the field of view of a panorama (equirectangular, or each eye of an ODS frame), in float radians
+static int panorama_fov(vpt_context* c, const char* fn, double hfov_deg, double vfov_deg, vpt::Projection* p) {
+    if (!(hfov_deg > 0.0 && hfov_deg <= 360.0)) return fail(c, VPT_ERR_INVALID, std::string(fn) + ": hfov_deg must be in (0, 360], got " + std::to_string(hfov_deg));
+    if (!(vfov_deg > 0.0 && vfov_deg <= 180.0)) return fail(c, VPT_ERR_INVALID, std::string(fn) + ": vfov_deg must be in (0, 180], got " + std::to_string(vfov_deg));
+    p->hfov = (float)(hfov_deg * (3.14159265358979323846 / 180.0));
+    p->vfov = (float)(vfov_deg * (3.14159265358979323846 / 180.0));
+    return VPT_OK;
+}
 
 int vpt_set_projection(vpt_context* c, int kind, double hfov_deg, double vfov_deg) {
     if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_projection: null context");
     vpt::Projection p;
     if (kind == VPT_PROJECTION_EQUIRECT) {
-        if (!(hfov_deg > 0.0 && hfov_deg <= 360.0)) return fail(c, VPT_ERR_INVALID, "vpt_set_projection: hfov_deg must be in (0, 360], got " + std::to_string(hfov_deg));
-        if (!(vfov_deg > 0.0 && vfov_deg <= 180.0)) return fail(c, VPT_ERR_INVALID, "vpt_set_projection: vfov_deg must be in (0, 180], got " + std::to_string(vfov_deg));
+        const int rc = panorama_fov(c, "vpt_set_projection", hfov_deg, vfov_deg, &p);
+        if (rc != VPT_OK) return rc;
         p.kind = kind;
-        p.hfov = (float)(hfov_deg * (3.14159265358979323846 / 180.0));
-        p.vfov = (float)(vfov_deg * (3.14159265358979323846 / 180.0));
+    } else if (kind == VPT_PROJECTION_ODS) {
+        return fail(c, VPT_ERR_INVALID, "vpt_set_projection: VPT_PROJECTION_ODS needs its options: use vpt_set_projection_ods");
     } else if (kind != VPT_PROJECTION_PERSPECTIVE) {
         return fail(c, VPT_ERR_INVALID, "vpt_set_projection: unknown projection kind " + std::to_string(kind));
     }
     c->proj_req = p;                // taken at the next iteration-0 call
+    return VPT_OK;
+}
+
+void vpt_ods_options_defaults(vpt_ods_options* opt) {
+    if (!opt) return;
+    opt->ipd = 0.064f; opt->layout = VPT_ODS_OVER_UNDER; opt->pole_merge_from_deg = 60.0f; opt->pole_merge_to_deg = 75.0f;
+}
+
+int vpt_set_projection_ods(vpt_context* c, double hfov_deg, double vfov_deg, const vpt_ods_options* opt) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_projection_ods: null context");
+    vpt_ods_options o;
+    vpt_ods_options_defaults(&o);
+    if (opt) o = *opt;
+    vpt::Projection p;
+    const int rc = panorama_fov(c, "vpt_set_projection_ods", hfov_deg, vfov_deg, &p);
+    if (rc != VPT_OK) return rc;
+    if (!(std::isfinite(o.ipd) && o.ipd >= 0.0f)) return fail(c, VPT_ERR_INVALID, "vpt_set_projection_ods: ipd must be finite and >= 0, got " + std::to_string(o.ipd));
+    if (o.layout != VPT_ODS_LEFT && o.layout != VPT_ODS_RIGHT && o.layout != VPT_ODS_OVER_UNDER)
+        return fail(c, VPT_ERR_INVALID, "vpt_set_projection_ods: unknown layout " + std::to_string(o.layout));
+    const double from = o.pole_merge_from_deg, to = o.pole_merge_to_deg;
+    if (!(from >= 0.0 && from <= to && to <= 90.0))
+        return fail(c, VPT_ERR_INVALID, "vpt_set_projection_ods: the pole merge needs 0 <= from <= to <= 90, got from " + std::to_string(from) + ", to " + std::to_string(to));
+    p.kind = VPT_PROJECTION_ODS;
+    vpt::OdsParams d;
+    d.hfov = p.hfov; d.vfov = p.vfov;
+    d.half_ipd = (float)((double)o.ipd / 2.0);
+    d.layout = o.layout;
+    d.merge_from = (float)(from * (3.14159265358979323846 / 180.0));
+    d.merge_to = (float)(to * (3.14159265358979323846 / 180.0));
+    d.inv_span = to > from ? (float)(1.0 / ((to - from) * (3.14159265358979323846 / 180.0))) : 0.0f;   // from == to: k is a step, inv_span unread
+    c->proj_req = p; c->ods_req = d;          // taken at the next iteration-0 call
     return VPT_OK;
 }
 
@@ -302,6 +344,8 @@ struct FramePlan {
     bool motion = false;                  // camera motion: the motion generate kernels with the shutter-close pose mo
     vpt::CameraMotion mo;
     const vpt::CameraMotion* motion_arg() const { return motion ? &mo : nullptr; }
+    vpt::OdsParams ods;                   // the ODS projection when ods(proj): the ODS generate kernels
+    const vpt::OdsParams* ods_arg() const { return vpt::ods(proj) ? &ods : nullptr; }
 };
 
 // Under option "profile": brackets the launches of fn with CUDA events of the given kind (0 generate, 1 trace, 2 resolve, 3 blue noise).
@@ -425,6 +469,14 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     const bool motion = kp.iteration == 0 ? c->motion_req : c->motion_cur;
     if (motion && vpt::equirect(proj))
         return fail(c, VPT_ERR_UNSUPPORTED, "camera motion (vpt_set_camera_motion) is not supported with the equirectangular projection");
+    const vpt::OdsParams& ods = kp.iteration == 0 ? c->ods_req : c->ods_cur;
+    if (vpt::ods(proj)) {
+        if (fa.cam.lens_radius != 0.0f)
+            return fail(c, VPT_ERR_UNSUPPORTED, "the ODS projection has no lens: camera.lens_radius must be 0 (got " + std::to_string(fa.cam.lens_radius) + ")");
+        if (motion) return fail(c, VPT_ERR_UNSUPPORTED, "camera motion (vpt_set_camera_motion) is not supported with the ODS projection");
+        if (ods.layout == vpt::kOdsOverUnder && (kp.resolution.y & 1u))
+            return fail(c, VPT_ERR_UNSUPPORTED, "the over-under ODS layout needs an even height, got " + std::to_string(kp.resolution.y));
+    }
 
     // ---- scene tables ---------------------------------------------------------------------------------------
     // Octrees built by vpt_octree_build are registered with their flat tables and instance count: nothing is read
@@ -529,7 +581,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         VPT_CUDA(c, cudaMalloc(&c->d_bn_table, sizeof(float2) * 65536 * (size_t)chunk));
         c->cap_chunk = chunk;
     }
-    fa.queue_dir = c->d_queue; fa.queue_id = c->d_queue_id; fa.queue_aux = c->d_queue_org; fa.thin_lens = (fa.cam.lens_radius != 0.0f || motion) ? 1 : 0;
+    fa.queue_dir = c->d_queue; fa.queue_id = c->d_queue_id; fa.queue_aux = c->d_queue_org; fa.thin_lens = (fa.cam.lens_radius != 0.0f || motion || vpt::ods(proj)) ? 1 : 0;
     fa.bn_table = c->d_bn_table; fa.debug_flags = c->debug_flags;
     fa.queue_count = c->d_counters; fa.queue_head = c->d_counters + 1;
     fa.planeA = c->d_planeA;
@@ -537,7 +589,8 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     fa.plane_tr = wide ? nullptr : c->d_plane_tr;
     // pixels no jitter can take to the root box or the sphere (pinhole and equirectangular HDRI frames that sample): k_miss_cull marks them once per call, and
     // k_generate / k_resolve skip their sample records.  Frames that end on the precomputed sky keep every record (see resolve_pixel), and
-    // so do motion frames: the cull assumes one camera per strip, and k_resolve rebuilds a culled sample without the lens loop.
+    // so do motion frames: the cull assumes one camera per strip, and k_resolve rebuilds a culled sample without the lens loop.  ODS frames
+    // cull with k_miss_cull_ods, whose bound takes in every origin' of a strip.
     fa.miss_mask = nullptr;
     if (c->miss_cull && n_sampled && !sky_env && fa.cam.lens_radius == 0.0f && !motion && fa.geom.n_local > 0) {
         if ((size_t)fa.geom.n_local > c->cap_miss_mask) {
@@ -597,10 +650,11 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     }
     plan.resolve.deep = plan.deep.out != nullptr;
     plan.proj = proj;
+    plan.ods = ods;
     plan.motion = motion;
     plan.mo = kp.iteration == 0 ? c->motion_close_req : c->motion_close_cur;
     if (kp.iteration == 0) {
-        memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req;
+        memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req; c->ods_cur = c->ods_req;
         c->motion_cur = c->motion_req; c->motion_close_cur = c->motion_close_req;
     }
     plan.region = region;
@@ -658,8 +712,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
     const bool region = plan.region;
     const vpt::RenderRegion& rg = plan.rg;
     if (fa.miss_mask) {
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, rg, plan.proj, stream)
-                                                            : vpt::launch_miss_cull(fa, c->d_miss_mask, plan.proj, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, rg, plan.proj, stream, plan.ods_arg())
+                                                            : vpt::launch_miss_cull(fa, c->d_miss_mask, plan.proj, stream, plan.ods_arg()); }));
         c->launches++;
     }
     unsigned done = 0;
@@ -667,8 +721,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
         fa.kp.iteration = it0 + done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, plan.proj, plan.motion_arg(), stream)
-                                                            : vpt::launch_generate(fa, (int)np, plan.proj, plan.motion_arg(), stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, plan.proj, plan.motion_arg(), plan.ods_arg(), stream)
+                                                            : vpt::launch_generate(fa, (int)np, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
         VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
@@ -676,9 +730,9 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
             return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, rg,
-                                                       plan.proj, stream)
+                                                       plan.proj, stream, plan.ods_arg())
                           : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep,
-                                                plan.proj, stream); }));
+                                                plan.proj, stream, plan.ods_arg()); }));
         c->launches += 4 + (plan.resolve.deep ? 1 : 0);            // with deep slices the resolve is two kernels
         done += np;
     }
@@ -689,8 +743,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
         if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, rg,
-                                                           plan.proj, stream));
-        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.proj, stream));
+                                                           plan.proj, stream, plan.ods_arg()));
+        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.proj, stream, plan.ods_arg()));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
         c->launches += 2 + (plan.resolve.deep ? 1 : 0);
     }
@@ -800,8 +854,8 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         c->launches++;
     }
     if (fa.miss_mask) {
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return plan.region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, plan.rg, plan.proj, stream)
-                                                                 : vpt::launch_miss_cull(fa, c->d_miss_mask, plan.proj, stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return plan.region ? vpt::launch_miss_cull_region(fa, c->d_miss_mask, plan.rg, plan.proj, stream, plan.ods_arg())
+                                                                 : vpt::launch_miss_cull(fa, c->d_miss_mask, plan.proj, stream, plan.ods_arg()); }));
         c->launches++;
     }
     const void* bn = (const void*)(uintptr_t)kp0.blue_noise_buffer;
@@ -816,9 +870,9 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)bn, c->d_bn_table, (int)np, plan.bn_limit, c->d_counters, stream); }));
         c->launches++;
         if (ad.n_tiles > 0) {
-            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, plan.motion_arg(), stream); }));
+            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.proj, stream); }));
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.proj, stream, plan.ods_arg()); }));
             c->launches += 3 + (plan.resolve.deep ? 1 : 0);
         }
         done += np;
@@ -950,6 +1004,17 @@ int vpt_render_pass(vpt_context* c, void* const params[VPT_NUM_ARGS], void* stre
     return vpt_render_passes(c, params, 1, stream);
 }
 
+// k_ods_cameras for the next render call (ods_req at iteration 0, else ods_cur) at the jitter the blue-noise buffer holds now, on the default
+// stream; rays: camera_b0 of each pixel's camera (4 floats) instead of the camera (8 floats)
+static int ods_cameras(vpt_context* c, const char* fn, const vpt_camera& cam, const vpt_kernel_params& kp, int rays, float* d_out) {
+    const vpt::OdsParams& od = kp.iteration == 0 ? c->ods_req : c->ods_cur;
+    if (od.layout == vpt::kOdsOverUnder && (kp.resolution.y & 1u))
+        return fail(c, VPT_ERR_UNSUPPORTED, std::string(fn) + ": the over-under ODS layout needs an even height, got " + std::to_string(kp.resolution.y));
+    VPT_CUDA(c, vpt::launch_ods_cameras(cam, od, kp.resolution, make_geom(c, kp.resolution.x, kp.resolution.y), (const void*)(uintptr_t)kp.blue_noise_buffer,
+                                        rays, d_out, 0));
+    return VPT_OK;
+}
+
 // b0 of every local pixel at the next render call's first pass: the projection that call takes (proj_req at iteration 0, else proj_cur)
 // at the jitter the blue-noise buffer holds now, on the default stream.  Reads the camera, Kernel_params and the blue noise; writes d_out_f4 only.
 int vpt_debug_camera_rays(vpt_context* c, void* const params[VPT_NUM_ARGS], float* d_out_f4) {
@@ -964,10 +1029,32 @@ int vpt_debug_camera_rays(vpt_context* c, void* const params[VPT_NUM_ARGS], floa
         return fail(c, VPT_ERR_UNSUPPORTED, "vpt_debug_camera_rays: the next call is a camera-motion frame, whose rays depend on each sample's "
                                             "shutter draw; use vpt_debug_motion_cameras");
     const vpt::Projection& pj = kp.iteration == 0 ? c->proj_req : c->proj_cur;
+    if (vpt::ods(pj)) {                       // camera_b0 of each pixel's ODS camera
+        const int rc = ods_cameras(c, "vpt_debug_camera_rays", cam, kp, 1, d_out_f4);
+        if (rc == VPT_OK) c->launches++;
+        return rc;
+    }
     VPT_CUDA(c, vpt::launch_camera_rays(cam, kp.resolution, make_geom(c, kp.resolution.x, kp.resolution.y), pj, (const void*)(uintptr_t)kp.blue_noise_buffer,
                                         reinterpret_cast<float4*>(d_out_f4), 0));
     c->launches++;
     return VPT_OK;
+}
+
+// The ODS camera of every local pixel's first sample of the next render call (the projection it takes must be ODS).  Reads the camera,
+// Kernel_params and the blue noise; writes d_out only.
+int vpt_debug_ods_cameras(vpt_context* c, void* const params[VPT_NUM_ARGS], float* d_out) {
+    if (!c || !params || !d_out || !params[VPT_ARG_CAMERA] || !params[VPT_ARG_KERNEL_PARAMS])
+        return fail(c, VPT_ERR_INVALID, "vpt_debug_ods_cameras: null argument");
+    vpt_camera cam; vpt_kernel_params kp;
+    memcpy(&cam, params[VPT_ARG_CAMERA], sizeof(cam));
+    memcpy(&kp, params[VPT_ARG_KERNEL_PARAMS], sizeof(kp));
+    if (!kp.blue_noise_buffer) return fail(c, VPT_ERR_INVALID, "vpt_debug_ods_cameras: Kernel_params.blue_noise_buffer is null");
+    if (kp.resolution.x == 0 || kp.resolution.y == 0) return fail(c, VPT_ERR_INVALID, "vpt_debug_ods_cameras: resolution is zero");
+    if (!vpt::ods(kp.iteration == 0 ? c->proj_req : c->proj_cur))
+        return fail(c, VPT_ERR_INVALID, "vpt_debug_ods_cameras: the next call has no ODS projection (vpt_set_projection_ods)");
+    const int rc = ods_cameras(c, "vpt_debug_ods_cameras", cam, kp, 0, d_out);
+    if (rc == VPT_OK) c->launches++;
+    return rc;
 }
 
 // The camera of every local pixel's first sample of the next render call under camera motion (motion_req at iteration 0, else motion_cur):

@@ -108,6 +108,8 @@ struct vpt_context {
     // camera projection (vpt_set_projection), checked when set: proj_req is what the caller set last; it becomes proj_cur at the next render
     // call with iteration == 0, so a running mean never continues under another projection
     vpt::Projection proj_req, proj_cur;
+    // the rest of an ODS projection (vpt_set_projection_ods), read where proj_req / proj_cur is of kind kProjOds, and taken over with it
+    vpt::OdsParams ods_req, ods_cur;
     // camera motion (vpt_set_camera_motion), checked when set: the shutter-close pose the caller set last (motion_req false: none); it becomes
     // motion_cur at the next render call with iteration == 0, so a running mean never continues under another pose
     bool      motion_req = false, motion_cur = false;

@@ -237,15 +237,41 @@ class Renderer:
         """Render the whole frame again from the next call with kp.iteration == 0 on."""
         check(lib.vpt_set_render_region(self.ctx, 0, 0, 0, 0), self.ctx, "vpt_set_render_region")
 
-    def set_projection(self, kind, hfov=360.0, vfov=180.0):
+    def set_projection(self, kind, hfov=360.0, vfov=180.0, ipd=None, layout=None, pole_merge=None):
         """Camera projection (vpt_set_projection) from the next call with kp.iteration == 0 on: "perspective", the reference camera (the
         default), or "equirect", a latitude-longitude panorama of hfov x vfov degrees (hfov in (0, 360], vfov in (0, 180]) around the
-        camera's origin, oriented by its u, v, w (forward -w).  A bad kind or field of view raises VptError here; an equirectangular frame
-        with a lens (cam.lens_radius != 0) is refused by the render call."""
-        kinds = {"perspective": N.VPT_PROJECTION_PERSPECTIVE, "equirect": N.VPT_PROJECTION_EQUIRECT}
+        camera's origin, oriented by its u, v, w (forward -w).  "ods" (vpt_set_projection_ods) is the omni-directional stereo panorama of
+        hfov x vfov per eye: interocular distance `ipd` in scene units (None: 0.064), layout "over_under" (left eye on top; the default),
+        "left" or "right", and the eye separation merged to 0 between the |elevation| angles pole_merge = (from, to) in degrees (None:
+        (60, 75); DESIGN.md section 8k).  A bad kind, field of view or ODS option, or an ODS option given with another kind, raises
+        VptError here; a panorama with a lens (cam.lens_radius != 0) is refused by the render call, and so is an over-under frame of odd
+        height."""
+        kinds = {"perspective": N.VPT_PROJECTION_PERSPECTIVE, "equirect": N.VPT_PROJECTION_EQUIRECT, "ods": N.VPT_PROJECTION_ODS}
         if kind not in kinds:
             raise N.VptError(f"Renderer.set_projection: unknown projection {kind!r} (one of {', '.join(kinds)})")
-        check(lib.vpt_set_projection(self.ctx, kinds[kind], float(hfov), float(vfov)), self.ctx, "vpt_set_projection")
+        if kind != "ods":
+            if ipd is not None or layout is not None or pole_merge is not None:
+                raise N.VptError(f"Renderer.set_projection: ipd, layout and pole_merge are options of the 'ods' projection, not of {kind!r}")
+            check(lib.vpt_set_projection(self.ctx, kinds[kind], float(hfov), float(vfov)), self.ctx, "vpt_set_projection")
+            return
+        layouts = {"left": N.VPT_ODS_LEFT, "right": N.VPT_ODS_RIGHT, "over_under": N.VPT_ODS_OVER_UNDER}
+        layout = "over_under" if layout is None else layout
+        if layout not in layouts:
+            raise N.VptError(f"Renderer.set_projection: unknown ODS layout {layout!r} (one of {', '.join(layouts)})")
+        opt = N.ods_options()
+        lib.vpt_ods_options_defaults(C.byref(opt))
+        if ipd is not None: opt.ipd = float(ipd)
+        opt.layout = layouts[layout]
+        if pole_merge is not None: opt.pole_merge_from_deg, opt.pole_merge_to_deg = (float(a) for a in pole_merge)
+        check(lib.vpt_set_projection_ods(self.ctx, float(hfov), float(vfov), C.byref(opt)), self.ctx, "vpt_set_projection_ods")
+
+    def ods_cameras(self):
+        """(local_rows, W, 8) float32: per local pixel the camera of its sample in the next render call's first pass under the ODS
+        projection -- origin' (3), lower_left_corner' (3), the eye e (-1 left, +1 right) and the pole merge k (vpt_debug_ods_cameras).
+        Writes nothing else and leaves the blue noise as it is.  Raises VptError when the next call has no ODS projection."""
+        out = torch.empty(self.n_local, 8, dtype=torch.float32, device=self.buffers.accum.device)
+        check(lib.vpt_debug_ods_cameras(self.ctx, self.params.array, C.c_void_p(out.data_ptr())), self.ctx, "vpt_debug_ods_cameras")
+        return out.view(self.n_local // self.width, self.width, 8)
 
     def camera_rays(self):
         """(n_local, 4) float32: per local pixel (b0, 0), the ray direction before normalize that the next render call's first pass takes
@@ -570,9 +596,9 @@ class DistributedRenderer:
     def clear_region(self):
         self.r.clear_region()
 
-    def set_projection(self, kind, hfov=360.0, vfov=180.0):
+    def set_projection(self, kind, hfov=360.0, vfov=180.0, ipd=None, layout=None, pole_merge=None):
         """Renderer.set_projection on this rank; every rank sets the same projection."""
-        self.r.set_projection(kind, hfov=hfov, vfov=vfov)
+        self.r.set_projection(kind, hfov=hfov, vfov=vfov, ipd=ipd, layout=layout, pole_merge=pole_merge)
 
     def set_camera_motion(self, cam_close):
         """Renderer.set_camera_motion on this rank; every rank sets the same poses."""
