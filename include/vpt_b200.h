@@ -286,6 +286,47 @@ int  vpt_set_light_group_buffers(vpt_context* ctx, float* d_sun_f3, float* d_poi
 #define VPT_DEEP_MAX_SLICES 32
 int  vpt_set_deep_buffers(vpt_context* ctx, float* d_slices_f4, unsigned n_slices, const float* h_bounds /* n_slices + 1 */);
 
+/* ---- instance mattes: the compositing AOVs split by the volume instance of each camera ray's first collision ---------------------
+ * alpha and volume flatten every instance into one coverage.  With a matte buffer set, every render call also keeps the two AOVs split by
+ * WHICH volume the camera ray collided with first (an ID matte), so one cloud of a cloudscape can be isolated, graded or held out without
+ * rendering it alone -- which would change the octree, the majorant walk and every draw after it.
+ *
+ *   Id of a sample.  A pass sample whose collision decision c = depth > 0 holds (as for the AOVs; a NaN depth is none) gets an id: the
+ *     sphere when the camera ray hit the reference sphere before the volume box; otherwise the volume instance of the first walk's accepted
+ *     collision (the collision depth measures).  The walk accepts where sigma_max^-1 * density > u, density the float sum over the start
+ *     leaf's instance list in list order at the collision point; the instance is the first list entry i whose prefix sum over entries 0..i
+ *     (the same additions, point and u) passes the same test.  The last prefix is the density itself, so an accepted collision always finds
+ *     an instance (with negative densities too).  No draw is added: paths are those of a render without mattes.  Each overlapping
+ *     instance takes a collision with probability density_i / density while sigma_max^-1 * density <= 1.  The root majorant is a maximum
+ *     over instances, not a sum, so where overlapping instances add up past it every step is accepted and the first list entries are
+ *     favoured.  A single-volume scene's id is always instance 0.
+ *   Mattes.  h_matte_of_instance[i] (copied at the call) maps instance i to one of K = n_mattes mattes or to none (-1); sphere_matte maps the
+ *     sphere.  Per matte and pixel one float4: (r, g, b) the premultiplied colour, w the coverage, defined exactly as a deep slice with "its
+ *     id maps to matte k" for "falls in slice k": coverage sample 1 or 0 (not guarded); colour sample the sample as the volume AOV takes it,
+ *     or +0 (a select); a sample the guard replaced gives every matte its own mean; accum's rule and arithmetic; a pass that samples nothing
+ *     gives coverage 0 and colour +0.  So K = 1 with every instance and the sphere in matte 0 is (volume, alpha) bit for bit; matte k of
+ *     any K is bit for bit the single matte of a K = 1 frame whose map selects the same set; with every id mapped the mattes sum to the AOVs
+ *     up to the rounding of the separate means.
+ *   Buffer.  Caller-owned device memory of K * vpt_local_pixels() float4, matte-major [K][local pixel] (rank-local order on a partitioned
+ *     context), 16-byte aligned.  A NULL buffer turns the mattes off at once (the other arguments are then ignored).  Buffer, K and map take
+ *     over at the next render call whose Kernel_params.iteration is 0; calls before that leave the buffer untouched.
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active mattes, as they do the deep slices (adaptive frames, render
+ *     regions, panoramas with the miss cull).  Every other output is bit for bit what the same call gives without mattes.  Level (A) has
+ *     none.  On a partitioned context the mattes are rank-local; neither exchange carries them.
+ *   Cost.  The trace kernel writes 4 B per sample whose camera ray collided (generic kernels: one pass over the leaf list per first
+ *     collision), and a resolve kernel more per chunk reads the records again.  The trace kernel keeps the rays per lane of
+ *     the frame without mattes (DESIGN.md section 8l).
+ *   Refused when set (VPT_ERR_INVALID), with a non-NULL buffer: a buffer not 16-byte aligned, n_mattes outside 1..VPT_MATTE_MAX, a NULL map
+ *     with n_instances > 0, a map entry or sphere_matte outside -1..n_mattes - 1.  A refused call changes nothing.  A NULL map with
+ *     n_instances == 0 is an empty map, accepted when set on purpose: every scene has at least one instance, so the first render call
+ *     refuses it for its instance count.
+ *   Refused at render time: n_instances other than the scene's instance count (VPT_ERR_INVALID); a matte buffer that overlaps accum, depth,
+ *     cost, raw or display, an AOV, light-group or deep-slice buffer (VPT_ERR_INVALID, naming the buffer); brick or cell mode
+ *     (VPT_ERR_UNSUPPORTED). */
+#define VPT_MATTE_MAX 32
+int  vpt_set_instance_mattes(vpt_context* ctx, float* d_mattes_f4, unsigned n_mattes, const int* h_matte_of_instance, unsigned n_instances,
+                             int sphere_matte);
+
 /* ---- render region: sample and write only a rectangle of the frame ------------------------------------------------------------
  * A viewer that tunes the density, the phase or a light on part of a volume re-renders only that part.  The region R is the half-open
  * rectangle [x0, x1) x [y0, y1) in pixels of the full frame, also on a partitioned context; (0, 0, 0, 0) clears it.

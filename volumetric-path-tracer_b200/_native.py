@@ -164,6 +164,7 @@ EXPORTED_SYMBOLS = [
     "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
     "vpt_set_deep_buffers", "vpt_set_camera_motion", "vpt_debug_motion_cameras",
     "vpt_ods_options_defaults", "vpt_set_projection_ods", "vpt_debug_ods_cameras",
+    "vpt_set_instance_mattes",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -196,6 +197,9 @@ lib.vpt_set_aov_buffers.argtypes = [_vp, _vp, _vp]; lib.vpt_set_aov_buffers.rest
 lib.vpt_set_light_group_buffers.argtypes = [_vp, _vp, _vp, _vp, _vp]; lib.vpt_set_light_group_buffers.restype = C.c_int
 VPT_DEEP_MAX_SLICES = 32                                            # vpt_set_deep_buffers: most slices
 lib.vpt_set_deep_buffers.argtypes = [_vp, _vp, C.c_uint, C.POINTER(C.c_float)]; lib.vpt_set_deep_buffers.restype = C.c_int
+VPT_MATTE_MAX = 32                                                  # vpt_set_instance_mattes: most mattes
+lib.vpt_set_instance_mattes.argtypes = [_vp, _vp, C.c_uint, C.POINTER(C.c_int), C.c_uint, C.c_int]
+lib.vpt_set_instance_mattes.restype = C.c_int
 lib.vpt_set_render_region.argtypes = [_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint]; lib.vpt_set_render_region.restype = C.c_int
 VPT_PROJECTION_PERSPECTIVE, VPT_PROJECTION_EQUIRECT, VPT_PROJECTION_ODS = 0, 1, 2   # vpt_set_projection kinds
 lib.vpt_set_projection.argtypes = [_vp, C.c_int, C.c_double, C.c_double]; lib.vpt_set_projection.restype = C.c_int

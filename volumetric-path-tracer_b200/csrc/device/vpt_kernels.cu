@@ -694,9 +694,23 @@ __device__ __forceinline__ float4 deep_step(const float4 x, const float3 s, cons
 // tonemap arithmetic differently once the slice code is in the kernel, inlined or behind a call.)
 struct DeepPixel { uint32_t lp, n_local, it0, max_interactions; };
 
+// The instance mattes (section 8l) are the same running means with another bin: the instantiations whose pack ends with a Mattes run these
+// functions on it (`Bins` = DeepSlices or Mattes; both have out and n).
+// the bin of pass p's sample of depth d: its deep slice, or the matte its id maps to (the id plane is read only where d > 0, where the trace
+// kernel wrote it); -1: none
+__device__ __forceinline__ int sample_bin(const DeepSlices& dp, const float d, const DeepPixel&, const int) { return deep_slice(dp, d); }
+__device__ __forceinline__ int sample_bin(const Mattes& mt, const float d, const DeepPixel& px, const int p)
+{
+    if (!(d > 0.0f)) return -1;
+    const uint32_t id = mt.id[(size_t)p * px.n_local + px.lp];
+    if (id == kMatteSphereId) return mt.sphere;
+    return id < mt.n_ids ? (int)mt.map[id] : -1;
+}
+
 // slice k's means after the chunk's passes before `upto`, none of which since done[k] put a sample in it (at iteration 0 the zero sample
 // is assigned, so the buffer is not read)
-__device__ __forceinline__ float4 deep_catch_up(const DeepSlices& dp, const uint8_t* done, const DeepPixel& px, const int k, const int upto)
+template <class Bins>
+__device__ __forceinline__ float4 deep_catch_up(const Bins& dp, const uint8_t* done, const DeepPixel& px, const int k, const int upto)
 {
     int q = done[k];
     float4 x;
@@ -709,11 +723,12 @@ __device__ __forceinline__ float4 deep_catch_up(const DeepSlices& dp, const uint
 // pass p of the chunk with the sample `value` (as it entered accum) of depth `depth`: its slice takes (value, 1) as the volume AOV takes
 // it; a sample the guard replaced gives every slice its own mean as colour (at iteration 0: the buffer's previous content) and its slice
 // the coverage 1 (coverage is not guarded)
-__device__ __forceinline__ void deep_pass(const DeepSlices& dp, uint8_t* done, const DeepPixel px, const int p, const float3 value, const float depth,
+template <class Bins>
+__device__ __forceinline__ void deep_pass(const Bins& dp, uint8_t* done, const DeepPixel px, const int p, const float3 value, const float depth,
                                           const bool guarded)
 {
     const uint32_t iteration = px.it0 + (uint32_t)p;
-    const int b = deep_slice(dp, depth);
+    const int b = sample_bin(dp, depth, px, p);
     if (guarded) {
         for (int k = 0; k < dp.n; ++k) {
             const float4 x = deep_catch_up(dp, done, px, k, p);
@@ -727,7 +742,8 @@ __device__ __forceinline__ void deep_pass(const DeepSlices& dp, uint8_t* done, c
 }
 
 // the end of a chunk of n_passes passes: every slice catches up
-__device__ __forceinline__ void deep_end(const DeepSlices& dp, const uint8_t* done, const DeepPixel px, const int n_passes)
+template <class Bins>
+__device__ __forceinline__ void deep_end(const Bins& dp, const uint8_t* done, const DeepPixel px, const int n_passes)
 {
     for (int k = 0; k < dp.n; ++k)
         if (done[k] < n_passes) dp.out[(size_t)k * px.n_local + px.lp] = deep_catch_up(dp, done, px, k, n_passes);
@@ -737,12 +753,14 @@ __device__ __forceinline__ void deep_end(const DeepSlices& dp, const uint8_t* do
 // pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.  kAov: also the running means of
 // the compositing AOVs in `aov` (DESIGN.md section 8c).  kGroups: also the running means of the light groups in `lg` (section 8d).
 // kPano (k_resolve_equirect, ...; HDRI frames): a culled pixel's miss samples are the equirectangular rays of the projection `pj`.
-// kDeep: the deep slices in `dp` (section 8h), updated lazily in their buffer, and no other store (see deep_pass).
-template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false, bool kDeep = false, bool kOds = false>
+// kDeep: the deep slices in `dp` (section 8h), updated lazily in their buffer, and no other store (see deep_pass); with Bins = Mattes the
+// instance mattes (section 8l) in their place.
+template <int kSky, bool kAdaptive, bool kAov, bool kGroups = false, bool kPano = false, bool kDeep = false, bool kOds = false,
+          class Bins = DeepSlices>
 __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<kSky>& atmo, const int n_passes, const int sampled,
                                               const int write_display, const PeerFrames& peers, const uint32_t lp, const int lr, const int y,
                                               const AdaptArgs* ad, const AovBuffers* aov, const LightGroups* lg = nullptr,
-                                              const Projection* pj = nullptr, const DeepSlices* dp = nullptr, const OdsParams* od = nullptr)
+                                              const Projection* pj = nullptr, const Bins* dp = nullptr, const OdsParams* od = nullptr)
 {
     const FrameGeom& g = fa.geom;
     const vpt_kernel_params& kp = fa.kp;
@@ -979,11 +997,18 @@ __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const D
 __device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const LightGroups&, const DeepSlices&) { return &a; }
 __device__ __forceinline__ const LightGroups* lg_of(const LightGroups& l, const DeepSlices&) { return &l; }
 __device__ __forceinline__ const LightGroups* lg_of(const AovBuffers&, const LightGroups& l, const DeepSlices&) { return &l; }
-template <class... Ext> constexpr bool has_deep = (std::is_same<Ext, DeepSlices>::value || ... || false);
-__device__ __forceinline__ const DeepSlices* deep_of(const DeepSlices& d) { return &d; }
-__device__ __forceinline__ const DeepSlices* deep_of(const AovBuffers&, const DeepSlices& d) { return &d; }
-__device__ __forceinline__ const DeepSlices* deep_of(const LightGroups&, const DeepSlices& d) { return &d; }
-__device__ __forceinline__ const DeepSlices* deep_of(const AovBuffers&, const LightGroups&, const DeepSlices& d) { return &d; }
+__device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const Mattes&) { return &a; }
+__device__ __forceinline__ const AovBuffers* aov_of(const AovBuffers& a, const LightGroups&, const Mattes&) { return &a; }
+__device__ __forceinline__ const LightGroups* lg_of(const LightGroups& l, const Mattes&) { return &l; }
+__device__ __forceinline__ const LightGroups* lg_of(const AovBuffers&, const LightGroups& l, const Mattes&) { return &l; }
+// The matte instantiations end the pack with a Mattes instead: the deep code runs on it (bins_of), binned by id.
+template <class... Ext> constexpr bool has_mattes = (std::is_same<Ext, Mattes>::value || ... || false);
+template <class... Ext> constexpr bool has_deep = (std::is_same<Ext, DeepSlices>::value || ... || false) || has_mattes<Ext...>;
+template <class... Ext> using bins_of = typename std::conditional<has_mattes<Ext...>, Mattes, DeepSlices>::type;
+template <class B> __device__ __forceinline__ const B* deep_of(const B& d) { return &d; }
+template <class B> __device__ __forceinline__ const B* deep_of(const AovBuffers&, const B& d) { return &d; }
+template <class B> __device__ __forceinline__ const B* deep_of(const LightGroups&, const B& d) { return &d; }
+template <class B> __device__ __forceinline__ const B* deep_of(const AovBuffers&, const LightGroups&, const B& d) { return &d; }
 
 // The thread's pixel and its resolve_pixel, shared by k_resolve, k_resolve_equirect and k_resolve_ods (kProj: 0 the perspective camera,
 // 1 the equirectangular projection `pj`, 2 the ODS projection `od`)
@@ -1000,11 +1025,11 @@ __device__ __forceinline__ void resolve_body(const FrameArgs& fa, const SkyArg<k
     if (y >= g.height) return;
     const AovBuffers* ap = nullptr;
     const LightGroups* gp = nullptr;
-    const DeepSlices* dq = nullptr;
+    const bins_of<Ext...>* dq = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
     if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y,
+    resolve_pixel<kSky, false, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2, bins_of<Ext...>>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr, y,
                                                                                          nullptr, ap, gp, pj, dq, od);
 }
 
@@ -1034,11 +1059,11 @@ __device__ __forceinline__ void resolve_region_body(const FrameArgs& fa, const S
     const uint32_t lp = (uint32_t)lr * (uint32_t)g.width + (uint32_t)rg.x0 + (i - r * w);
     const AovBuffers* ap = nullptr;
     const LightGroups* gp = nullptr;
-    const DeepSlices* dq = nullptr;
+    const bins_of<Ext...>* dq = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
     if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
-    resolve_pixel<kSky, false, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr,
+    resolve_pixel<kSky, false, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2, bins_of<Ext...>>(fa, atmo, n_passes, sampled, write_display, peers, lp, lr,
                                                                                          global_row(g, lr), nullptr, ap, gp, pj, dq, od);
 }
 
@@ -1115,11 +1140,11 @@ __device__ __forceinline__ void resolve_adaptive_body(const FrameArgs& fa, const
     if (ad.stopped[lp]) return;
     const AovBuffers* ap = nullptr;
     const LightGroups* gp = nullptr;
-    const DeepSlices* dq = nullptr;
+    const bins_of<Ext...>* dq = nullptr;
     if constexpr (kAov) ap = aov_of(ext...);
     if constexpr (kGroups) gp = lg_of(ext...);
     if constexpr (has_deep<Ext...>) dq = deep_of(ext...);
-    resolve_pixel<kSky, true, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr,
+    resolve_pixel<kSky, true, kAov, kGroups, kProj == 1, has_deep<Ext...>, kProj == 2, bins_of<Ext...>>(fa, atmo, n_passes, 1, 1, PeerFrames{}, lp, t.lr,
                                                                                         global_row(g, t.lr), &ad, ap, gp, pj, dq, od);
 }
 
@@ -1557,9 +1582,16 @@ static BrickArgs brick_args(const float* pool, const int dims[3])
 // memory opt-in, occupancy and preload all go through this list and resolve_kernels below.  (A unary + forms the pointer of an
 // instantiation with a pack argument: inside a template, g++ cannot deduce the lambda's parameter from that template-id.)
 template <class F>
-static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const BrickArgs& ba, F&& f)
+static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const MatteIds& mi, const BrickArgs& ba, F&& f)
 {
     switch (k) {
+    case TK_LEAN_3_MATTES:           return f(+k_trace<0, true, 3, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, mi);
+    case TK_LEAN_2_MATTES:           return f(+k_trace<0, true, 2, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(2), NoAtmo{}, mi);
+    case TK_GENERIC_3_MATTES:        return f(+k_trace<0, false, 3, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, mi);
+    case TK_GENERIC_2_MATTES:        return f(+k_trace<0, false, 2, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(2), NoAtmo{}, mi);
+    case TK_VOL_3_MATTES:            return f(+k_trace<1, false, 3, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(3), atm, mi);
+    case TK_GENERIC_3_GROUPS_MATTES: return f(+k_trace<0, false, 3, false, true, LightGroups, MatteIds>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, lg, mi);
+    case TK_VOL_3_GROUPS_MATTES:     return f(+k_trace<1, false, 3, false, true, LightGroups, MatteIds>, kTraceThreads, trace_smem_bytes(3), atm, lg, mi);
     case TK_GENERIC_3:        return f(k_trace<0, false, 3>, kTraceThreads, trace_smem_bytes(3), NoAtmo{});
     case TK_LEAN_3:           return f(k_trace<0, true, 3>, kTraceThreads, trace_smem_bytes(3), NoAtmo{});
     case TK_VOL_3:            return f(k_trace<1, false, 3>, kTraceThreads, trace_smem_bytes(3), atm);
@@ -1580,14 +1612,13 @@ static cudaError_t resolve_kernels_deep(F&& f, const Sky& sky, const E&... e)
     return f(+k_resolve<S, A, G, E...>, +k_resolve_adaptive<S, A, G, E...>, +k_resolve_region<S, A, G, E...>, sky, e...);
 }
 
-// The resolve kernels: f(k_resolve<S, A, G>, k_resolve_adaptive<S, A, G>, k_resolve_region<S, A, G>, the sky argument, the trailing
-// AovBuffers / LightGroups / DeepSlices) for key {S, A, G, D}, case S * 4 + A * 2 + G of the table without (D false) or with the deep slices.
-template <class F>
-static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp,
-                                   F&& f)
+// The table of resolve_kernels whose pack ends with `dp`: the deep slices (a DeepSlices) or the instance mattes (a Mattes)
+template <class F, class Bins>
+static cudaError_t resolve_kernels_binned(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, const Bins& dp,
+                                          F&& f)
 {
     const NoSky hdri{};
-    if (r.deep) switch (r.sky * 4 + r.aov * 2 + r.groups) {
+    switch (r.sky * 4 + r.aov * 2 + r.groups) {
     case 0:  return resolve_kernels_deep<0, false, false>(f, hdri, dp);
     case 1:  return resolve_kernels_deep<0, false, true>(f, hdri, lg, dp);
     case 2:  return resolve_kernels_deep<0, true, false>(f, hdri, aov, dp);
@@ -1602,6 +1633,18 @@ static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& at
     case 11: return resolve_kernels_deep<2, true, true>(f, atm, aov, lg, dp);
     default: return cudaErrorInvalidValue;
     }
+}
+
+// The resolve kernels: f(k_resolve<S, A, G>, k_resolve_adaptive<S, A, G>, k_resolve_region<S, A, G>, the sky argument, the trailing
+// AovBuffers / LightGroups / DeepSlices or Mattes) for key {S, A, G, D, M}, case S * 4 + A * 2 + G of the table without (D, M false), with
+// the deep slices (D) or with the instance mattes (M; D false).
+template <class F>
+static cudaError_t resolve_kernels(const ResolveKey& r, const vpt_atmosphere& atm, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp,
+                                   const Mattes& mt, F&& f)
+{
+    const NoSky hdri{};
+    if (r.deep) return resolve_kernels_binned(r, atm, aov, lg, dp, f);
+    if (r.mattes) return resolve_kernels_binned(r, atm, aov, lg, mt, f);
     switch (r.sky * 4 + r.aov * 2 + r.groups) {
     case 0:  return f(k_resolve<0>, k_resolve_adaptive<0>, k_resolve_region<0>, hdri);
     case 1:  return f(+k_resolve<0, false, true, LightGroups>, +k_resolve_adaptive<0, false, true, LightGroups>, +k_resolve_region<0, false, true, LightGroups>, hdri, lg);
@@ -1625,21 +1668,30 @@ static cudaError_t resolve_kernels_equirect_deep(F&& f, const NoSky& sky, const 
     return f(+k_resolve_equirect<A, G, E...>, +k_resolve_adaptive_equirect<A, G, E...>, +k_resolve_region_equirect<A, G, E...>, sky, e...);
 }
 
-// The equirectangular resolve kernels of the HDRI frames, in the form of resolve_kernels: f(k_resolve_equirect<A, G>,
-// k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G>, the sky argument, the trailing AovBuffers / LightGroups / DeepSlices),
-// case A * 2 + G of the table without or with the deep slices.
-template <class F>
-static cudaError_t resolve_kernels_equirect(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, F&& f)
+template <class F, class Bins>
+static cudaError_t resolve_kernels_equirect_binned(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const Bins& dp, F&& f)
 {
     const NoSky hdri{};
-    if (r.sky != 0) return cudaErrorInvalidValue;
-    if (r.deep) switch (r.aov * 2 + r.groups) {
+    switch (r.aov * 2 + r.groups) {
     case 0:  return resolve_kernels_equirect_deep<false, false>(f, hdri, dp);
     case 1:  return resolve_kernels_equirect_deep<false, true>(f, hdri, lg, dp);
     case 2:  return resolve_kernels_equirect_deep<true, false>(f, hdri, aov, dp);
     case 3:  return resolve_kernels_equirect_deep<true, true>(f, hdri, aov, lg, dp);
     default: return cudaErrorInvalidValue;
     }
+}
+
+// The equirectangular resolve kernels of the HDRI frames, in the form of resolve_kernels: f(k_resolve_equirect<A, G>,
+// k_resolve_adaptive_equirect<A, G>, k_resolve_region_equirect<A, G>, the sky argument, the trailing AovBuffers / LightGroups / DeepSlices or
+// Mattes), case A * 2 + G of the table without, with the deep slices or with the instance mattes.
+template <class F>
+static cudaError_t resolve_kernels_equirect(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                                            F&& f)
+{
+    const NoSky hdri{};
+    if (r.sky != 0) return cudaErrorInvalidValue;
+    if (r.deep) return resolve_kernels_equirect_binned(r, aov, lg, dp, f);
+    if (r.mattes) return resolve_kernels_equirect_binned(r, aov, lg, mt, f);
     switch (r.aov * 2 + r.groups) {
     case 0:  return f(k_resolve_equirect<false, false>, k_resolve_adaptive_equirect<false, false>, k_resolve_region_equirect<false, false>, hdri);
     case 1:  return f(+k_resolve_equirect<false, true, LightGroups>, +k_resolve_adaptive_equirect<false, true, LightGroups>, +k_resolve_region_equirect<false, true, LightGroups>, hdri, lg);
@@ -1655,19 +1707,27 @@ static cudaError_t resolve_kernels_ods_deep(F&& f, const NoSky& sky, const E&...
     return f(+k_resolve_ods<A, G, E...>, +k_resolve_adaptive_ods<A, G, E...>, +k_resolve_region_ods<A, G, E...>, sky, e...);
 }
 
-// The ODS resolve kernels of the HDRI frames, in the form of resolve_kernels_equirect
-template <class F>
-static cudaError_t resolve_kernels_ods(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, F&& f)
+template <class F, class Bins>
+static cudaError_t resolve_kernels_ods_binned(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const Bins& dp, F&& f)
 {
     const NoSky hdri{};
-    if (r.sky != 0) return cudaErrorInvalidValue;
-    if (r.deep) switch (r.aov * 2 + r.groups) {
+    switch (r.aov * 2 + r.groups) {
     case 0:  return resolve_kernels_ods_deep<false, false>(f, hdri, dp);
     case 1:  return resolve_kernels_ods_deep<false, true>(f, hdri, lg, dp);
     case 2:  return resolve_kernels_ods_deep<true, false>(f, hdri, aov, dp);
     case 3:  return resolve_kernels_ods_deep<true, true>(f, hdri, aov, lg, dp);
     default: return cudaErrorInvalidValue;
     }
+}
+
+// The ODS resolve kernels of the HDRI frames, in the form of resolve_kernels_equirect
+template <class F>
+static cudaError_t resolve_kernels_ods(const ResolveKey& r, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt, F&& f)
+{
+    const NoSky hdri{};
+    if (r.sky != 0) return cudaErrorInvalidValue;
+    if (r.deep) return resolve_kernels_ods_binned(r, aov, lg, dp, f);
+    if (r.mattes) return resolve_kernels_ods_binned(r, aov, lg, mt, f);
     switch (r.aov * 2 + r.groups) {
     case 0:  return f(k_resolve_ods<false, false>, k_resolve_adaptive_ods<false, false>, k_resolve_region_ods<false, false>, hdri);
     case 1:  return f(+k_resolve_ods<false, true, LightGroups>, +k_resolve_adaptive_ods<false, true, LightGroups>, +k_resolve_region_ods<false, true, LightGroups>, hdri, lg);
@@ -1677,10 +1737,10 @@ static cudaError_t resolve_kernels_ods(const ResolveKey& r, const AovBuffers& ao
     }
 }
 
-cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const float* brick_pool,
-                         const int brick_dims[3], int n_ctas, cudaStream_t s)
+cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const MatteIds& mi,
+                         const float* brick_pool, const int brick_dims[3], int n_ctas, cudaStream_t s)
 {
-    return trace_kernel(k, atm, lg, brick_args(brick_pool, brick_dims), [&](auto kernel, int threads, size_t smem, const auto&... args) {
+    return trace_kernel(k, atm, lg, mi, brick_args(brick_pool, brick_dims), [&](auto kernel, int threads, size_t smem, const auto&... args) {
         kernel<<<n_ctas, threads, smem, s>>>(fa, args...);
         return cudaGetLastError();
     });
@@ -1688,10 +1748,10 @@ cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmospher
 
 // Once per context (= per device): opt the trace kernels into their dynamic shared memory and record how many CTAs of each fit
 // on an SM.  The attribute is a per-device property of the function, so this must not be a process-wide static.
-cudaError_t trace_kernels_init(int max_ctas[kTraceKernels])
+cudaError_t trace_kernels_init(int max_ctas[kTraceKernelsAll])
 {
-    for (int k = 0; k < kTraceKernels; ++k) {
-        const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, [&](auto kernel, int threads, size_t smem, const auto&...) {
+    for (int k = 0; k < kTraceKernelsAll; ++k) {
+        const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, {}, [&](auto kernel, int threads, size_t smem, const auto&...) {
             const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             return r != cudaSuccess ? r : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[k], kernel, threads, smem);
         });
@@ -1713,23 +1773,23 @@ cudaError_t exchange_kernels_preload()
         }
         return cudaSuccess;
     };
-    for (int k = 0; k < kTraceKernels; ++k) {
-        const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, [&](auto kernel, int, size_t, const auto&...) { return load(kernel); });
+    for (int k = 0; k < kTraceKernelsAll; ++k) {
+        const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, {}, [&](auto kernel, int, size_t, const auto&...) { return load(kernel); });
         if (e != cudaSuccess) return e;
     }
     for (int sky = 0; sky < 3; ++sky)
         for (bool aov : {false, true})
             for (bool groups : {false, true})
-                for (bool deep : {false, true}) {
-                    const ResolveKey key{sky, aov, groups, deep};
-                    const cudaError_t e = resolve_kernels(key, {}, {}, {}, {},
+                for (int bins = 0; bins < 3; ++bins) {                 // none, the deep slices, the instance mattes
+                    const ResolveKey key{sky, aov, groups, bins == 1, bins == 2};
+                    const cudaError_t e = resolve_kernels(key, {}, {}, {}, {}, {},
                                                           [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
                     if (e != cudaSuccess) return e;
                     if (sky != 0) continue;
-                    const cudaError_t ep = resolve_kernels_equirect(key, {}, {}, {},
+                    const cudaError_t ep = resolve_kernels_equirect(key, {}, {}, {}, {},
                                                                     [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
                     if (ep != cudaSuccess) return ep;
-                    const cudaError_t eo = resolve_kernels_ods(key, {}, {}, {},
+                    const cudaError_t eo = resolve_kernels_ods(key, {}, {}, {}, {},
                                                                [&](auto fixed, auto adaptive, auto region, const auto&...) { return load(fixed, adaptive, region); });
                     if (eo != cudaSuccess) return eo;
                 }
@@ -1747,25 +1807,25 @@ cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, co
 }
 
 static cudaError_t resolve_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                                  const OdsParams* od, cudaStream_t s)
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                                  const Projection& pj, const OdsParams* od, cudaStream_t s)
 {
     const int threads = 256;
     const int blocks = (fa.geom.n_local + threads - 1) / threads;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     if (od && key.sky == 0)
-        return resolve_kernels_ods(key, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+        return resolve_kernels_ods(key, aov, lg, dp, mt, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
             kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, *od, ext...);
             return cudaGetLastError();
         });
     if (equirect(pj) && key.sky == 0)
-        return resolve_kernels_equirect(key, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+        return resolve_kernels_equirect(key, aov, lg, dp, mt, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
             kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, pj, ext...);
             return cudaGetLastError();
         });
     // (tried for frames of less than two waves of blocks -- multi-GPU shards: fetching the records of four passes at once before the
     // order-dependent running mean; slower there too)
-    return resolve_kernels(key, atm, aov, lg, dp, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, dp, mt, [&](auto kernel, auto, auto, const auto& sky, const auto&... ext) {
         kernel<<<blocks, threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, ext...);
         return cudaGetLastError();
     });
@@ -1773,84 +1833,99 @@ static cudaError_t resolve_launch(const FrameArgs& fa, const ResolveKey& key, co
 
 static cudaError_t resolve_region_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled,
                                          int write_display, const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp,
-                                         const RenderRegion& rg, const Projection& pj, const OdsParams* od, cudaStream_t s)
+                                         const Mattes& mt, const RenderRegion& rg, const Projection& pj, const OdsParams* od, cudaStream_t s)
 {
     const long long n = region_pixels(rg);
     if (n <= 0) return cudaSuccess;
     const int threads = 256;
     const PeerFrames pf = peers ? *peers : PeerFrames{};
     if (od && key.sky == 0)
-        return resolve_kernels_ods(key, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+        return resolve_kernels_ods(key, aov, lg, dp, mt, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
             kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, *od, ext...);
             return cudaGetLastError();
         });
     if (equirect(pj) && key.sky == 0)
-        return resolve_kernels_equirect(key, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+        return resolve_kernels_equirect(key, aov, lg, dp, mt, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
             kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, pj, ext...);
             return cudaGetLastError();
         });
-    return resolve_kernels(key, atm, aov, lg, dp, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, dp, mt, [&](auto, auto, auto kernel, const auto& sky, const auto&... ext) {
         kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, s>>>(fa, sky, n_passes, sampled, write_display, pf, rg, ext...);
         return cudaGetLastError();
     });
 }
 
 static cudaError_t resolve_adaptive_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                           const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                                           const OdsParams* od, cudaStream_t s)
+                                           const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                                           const Projection& pj, const OdsParams* od, cudaStream_t s)
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
     if (od && key.sky == 0)
-        return resolve_kernels_ods(key, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+        return resolve_kernels_ods(key, aov, lg, dp, mt, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
             kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, *od, ext...);
             return cudaGetLastError();
         });
     if (equirect(pj) && key.sky == 0)
-        return resolve_kernels_equirect(key, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+        return resolve_kernels_equirect(key, aov, lg, dp, mt, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
             kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, pj, ext...);
             return cudaGetLastError();
         });
-    return resolve_kernels(key, atm, aov, lg, dp, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
+    return resolve_kernels(key, atm, aov, lg, dp, mt, [&](auto, auto kernel, auto, const auto& sky, const auto&... ext) {
         kernel<<<ad.n_tiles, 128, 0, s>>>(fa, sky, n_passes, ad, ext...);
         return cudaGetLastError();
     });
 }
 
 // With deep slices (key.deep) a resolve is two launches: the deep instantiation, which keeps the slices only and reads accum and the AOVs
-// before they change, then the frame's own kernel, the very one without slices -- so every other output is bit for bit the same.
-static ResolveKey without_deep(const ResolveKey& key) { ResolveKey k = key; k.deep = false; return k; }
+// before they change, then the frame's own kernel, the very one without slices -- so every other output is bit for bit the same.  The
+// instance mattes (key.mattes) take one more launch of the same kind, after the deep one.
+static ResolveKey only_deep(const ResolveKey& key) { ResolveKey k = key; k.mattes = false; return k; }
+static ResolveKey only_mattes(const ResolveKey& key) { ResolveKey k = key; k.deep = false; return k; }
+static ResolveKey without_deep(const ResolveKey& key) { ResolveKey k = key; k.deep = false; k.mattes = false; return k; }
 
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                           cudaStream_t s, const OdsParams* od)
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                           const Projection& pj, cudaStream_t s, const OdsParams* od)
 {
     if (key.deep) {
-        const cudaError_t e = resolve_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, pj, od, s);
+        const cudaError_t e = resolve_launch(fa, only_deep(key), atm, n_passes, sampled, 0, nullptr, aov, lg, dp, mt, pj, od, s);
         if (e != cudaSuccess) return e;
     }
-    return resolve_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, pj, od, s);
+    if (key.mattes) {
+        const cudaError_t e = resolve_launch(fa, only_mattes(key), atm, n_passes, sampled, 0, nullptr, aov, lg, dp, mt, pj, od, s);
+        if (e != cudaSuccess) return e;
+    }
+    return resolve_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, mt, pj, od, s);
 }
 
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,
-                                  const Projection& pj, cudaStream_t s, const OdsParams* od)
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                                  const RenderRegion& rg, const Projection& pj, cudaStream_t s, const OdsParams* od)
 {
     if (key.deep) {
-        const cudaError_t e = resolve_region_launch(fa, key, atm, n_passes, sampled, 0, nullptr, aov, lg, dp, rg, pj, od, s);
+        const cudaError_t e = resolve_region_launch(fa, only_deep(key), atm, n_passes, sampled, 0, nullptr, aov, lg, dp, mt, rg, pj, od, s);
         if (e != cudaSuccess) return e;
     }
-    return resolve_region_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, rg, pj, od, s);
+    if (key.mattes) {
+        const cudaError_t e = resolve_region_launch(fa, only_mattes(key), atm, n_passes, sampled, 0, nullptr, aov, lg, dp, mt, rg, pj, od, s);
+        if (e != cudaSuccess) return e;
+    }
+    return resolve_region_launch(fa, without_deep(key), atm, n_passes, sampled, write_display, peers, aov, lg, dp, mt, rg, pj, od, s);
 }
 
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s,
-                                    const OdsParams* od)
+                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt, const Projection& pj,
+                                    cudaStream_t s, const OdsParams* od)
 {
     if (key.deep) {
-        const cudaError_t e = resolve_adaptive_launch(fa, key, atm, n_passes, ad, aov, lg, dp, pj, od, s);
+        const cudaError_t e = resolve_adaptive_launch(fa, only_deep(key), atm, n_passes, ad, aov, lg, dp, mt, pj, od, s);
         if (e != cudaSuccess) return e;
     }
-    return resolve_adaptive_launch(fa, without_deep(key), atm, n_passes, ad, aov, lg, dp, pj, od, s);
+    if (key.mattes) {
+        const cudaError_t e = resolve_adaptive_launch(fa, only_mattes(key), atm, n_passes, ad, aov, lg, dp, mt, pj, od, s);
+        if (e != cudaSuccess) return e;
+    }
+    return resolve_adaptive_launch(fa, without_deep(key), atm, n_passes, ad, aov, lg, dp, mt, pj, od, s);
 }
 
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s)

@@ -148,12 +148,24 @@ cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projectio
 struct LightGroups;
 // The trace kernels, with their instantiations in trace_kernel (vpt_kernels.cu): generic / lean / volumetric path at 3 rays per lane,
 // k_trace_brick, generic / lean at 2, lean at 2 on the cell table, generic / volumetric path keeping the light-group planes.
+// kTraceKernels counts those; the *_MATTES kernels after them are the same with the instance mattes' id plane (MatteIds, below), and
+// kTraceKernelsAll counts every trace kernel.
 enum TraceKernel : int { TK_GENERIC_3, TK_LEAN_3, TK_VOL_3, TK_BRICK, TK_GENERIC_2, TK_LEAN_2, TK_LEAN_2_CELLS, TK_GENERIC_3_GROUPS,
-                         TK_VOL_3_GROUPS, kTraceKernels };
+                         TK_VOL_3_GROUPS, kTraceKernels,
+                         TK_LEAN_3_MATTES = kTraceKernels, TK_LEAN_2_MATTES, TK_GENERIC_3_MATTES, TK_VOL_3_MATTES, TK_GENERIC_3_GROUPS_MATTES,
+                         TK_VOL_3_GROUPS_MATTES, TK_GENERIC_2_MATTES, kTraceKernelsAll };
 // The trace kernel of a frame.  brick / cells: volume 0 is read from a brick pool / a cell table (lean scenes only); vol_integ: the volumetric
-// path integrator; group_planes: a generic kernel keeps the light-group planes; slots: rays per lane, 2 or 3 (the group kernels run 3).
-inline TraceKernel pick_trace_kernel(bool brick, bool cells, bool vol_integ, bool lean, bool group_planes, int slots)
+// path integrator; group_planes: a generic kernel keeps the light-group planes; slots: rays per lane, 2 or 3 (the group kernels run 3);
+// mattes: the kernel writes the instance mattes' id plane (never with brick or cell mode: the host refuses that), at the rays per lane of
+// the same frame without mattes.
+inline TraceKernel pick_trace_kernel(bool brick, bool cells, bool vol_integ, bool lean, bool group_planes, int slots, bool mattes = false)
 {
+    if (mattes) {
+        if (group_planes) return vol_integ ? TK_VOL_3_GROUPS_MATTES : TK_GENERIC_3_GROUPS_MATTES;
+        if (vol_integ) return TK_VOL_3_MATTES;
+        if (slots == 2) return lean ? TK_LEAN_2_MATTES : TK_GENERIC_2_MATTES;
+        return lean ? TK_LEAN_3_MATTES : TK_GENERIC_3_MATTES;
+    }
     if (group_planes) return vol_integ ? TK_VOL_3_GROUPS : TK_GENERIC_3_GROUPS;
     if (brick) return TK_BRICK;
     if (cells) return TK_LEAN_2_CELLS;
@@ -162,13 +174,19 @@ inline TraceKernel pick_trace_kernel(bool brick, bool cells, bool vol_integ, boo
     return lean ? TK_LEAN_3 : TK_GENERIC_3;
 }
 // default of option "sched_min_lanes": lanes an operation must gather before it pre-empts stepping (26 helps only the lean kernel at 3)
-inline int trace_sched_min_lanes(TraceKernel k) { return k == TK_LEAN_3 ? 26 : 20; }
+inline int trace_sched_min_lanes(TraceKernel k) { return k == TK_LEAN_3 || k == TK_LEAN_3_MATTES ? 26 : 20; }
 // per device: dynamic shared memory opt-in of every trace kernel, and how many CTAs of each fit on an SM
-cudaError_t trace_kernels_init(int max_ctas[kTraceKernels]);
+cudaError_t trace_kernels_init(int max_ctas[kTraceKernelsAll]);
+// Instance mattes, trace side (vpt_set_instance_mattes): id[pass * n_local + local pixel] = the id of a sample whose camera ray collided
+// (depth > 0): kMatteSphereId when the camera ray hit the sphere before the volume box, else the volume instance of the first walk's
+// accepted collision (the first leaf-list entry whose density prefix passes the acceptance test).  Written only where depth > 0 will hold.
+// A kernel argument of the matte instantiations of k_trace only (the last of the pack), as LightGroups is.
+constexpr uint32_t kMatteSphereId = 0xffffffffu;
+struct MatteIds { uint32_t* id = nullptr; };
 // kernel k on n_ctas persistent CTAs.  atm: the caller's AtmosphereParameters (volumetric path kernels); lg: the light groups (group
-// kernels); brick_pool / brick_dims: the brick pool of volume 0 and its voxels per axis (k_trace_brick)
-cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const float* brick_pool,
-                         const int brick_dims[3], int n_ctas, cudaStream_t s);
+// kernels); mi: the id plane (matte kernels); brick_pool / brick_dims: the brick pool of volume 0 and its voxels per axis (k_trace_brick)
+cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const MatteIds& mi,
+                         const float* brick_pool, const int brick_dims[3], int n_ctas, cudaStream_t s);
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s);
 cudaError_t launch_fill_perlin(float* d_buffer, int dx, int dy, int dz, float scale, int seed, cudaStream_t s);
 cudaError_t launch_build_bricks(const float* d_dense, int dx, int dy, int dz, float* d_bricks, cudaStream_t s);
@@ -194,13 +212,19 @@ struct LightGroups { float3* out[kLightGroups] = {}; float* planes = nullptr; un
 // argument of the deep instantiations of k_resolve / k_resolve_adaptive / k_resolve_region only (the last of the pack), as AovBuffers is.
 constexpr int kDeepMaxSlices = 32;                    // VPT_DEEP_MAX_SLICES of vpt_b200.h
 struct DeepSlices { float4* out = nullptr; int n = 0; float z[kDeepMaxSlices + 1] = {}; };
+// Instance mattes, resolve side (vpt_set_instance_mattes): out[k * n_local + local pixel] = matte k's running means {premultiplied colour,
+// coverage}, defined as a deep slice's with "its id maps to matte k" for "its depth falls in slice k": a sample with d > 0 and id i lands in
+// map[i] (i < n_ids) or `sphere` (i == kMatteSphereId), none where that is -1.  id: the trace's id plane (MatteIds); map: device memory.
+// A kernel argument of the matte instantiations of the resolve kernels only (the last of the pack, in place of a DeepSlices).
+constexpr int kMatteMax = 32;                         // VPT_MATTE_MAX of vpt_b200.h
+struct Mattes { float4* out = nullptr; int n = 0; const uint32_t* id = nullptr; const int8_t* map = nullptr; uint32_t n_ids = 0; int sphere = -1; };
 // Which k_resolve / k_resolve_adaptive a frame runs (instantiations: resolve_kernels in vpt_kernels.cu).  sky: 0 HDRI, 1 the precomputed
 // sky, 2 the volumetric path integrator (ends on that sky; atm: the caller's AtmosphereParameters); with the AOVs; with the light groups;
-// with the deep slices.
-struct ResolveKey { int sky = 0; bool aov = false, groups = false, deep = false; };
+// with the deep slices; with the instance mattes.
+struct ResolveKey { int sky = 0; bool aov = false, groups = false, deep = false, mattes = false; };
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj,
-                           cudaStream_t s, const OdsParams* od = nullptr);
+                           const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                           const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);
@@ -240,8 +264,8 @@ cudaError_t launch_ods_cameras(const vpt_camera& cam, const OdsParams& od, const
 cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const AdaptArgs& ad, const Projection& pj, const CameraMotion* mo,
                                      const OdsParams* od, cudaStream_t s);
 cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, const AdaptArgs& ad,
-                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Projection& pj, cudaStream_t s,
-                                    const OdsParams* od = nullptr);
+                                    const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt, const Projection& pj,
+                                    cudaStream_t s, const OdsParams* od = nullptr);
 // convergence test over ad.tiles: stops every active pixel whose 3x3 neighbourhood (global rows) has err < threshold, lists the tiles still
 // active.  halo: the local exchange block's full-frame err plane, read for neighbour rows of other ranks (null for one rank)
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s);
@@ -256,8 +280,8 @@ cudaError_t launch_generate_region(const FrameArgs& fa, int n_passes, const Rend
 cudaError_t launch_miss_cull_region(const FrameArgs& fa, uint8_t* mask, const RenderRegion& rg, const Projection& pj, cudaStream_t s,
                                     const OdsParams* od = nullptr);
 cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
-                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const RenderRegion& rg,
-                                  const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
+                                  const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
+                                  const RenderRegion& rg, const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
 cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s);
 cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s);
 

@@ -97,6 +97,7 @@ VPT_DEV void reset_path(PathState& st)
 // into the following add, and a product used for L AND for the group is no longer single-use, so both updates are pinned to the fma the
 // instantiation without groups compiles to: L + a * b -> fma(a, b, L).
 VPT_DEV const LightGroups* lg_of(const LightGroups& a) { return &a; }
+VPT_DEV const LightGroups* lg_of(const LightGroups& a, const MatteIds&) { return &a; }
 VPT_DEV float3 pfma3(const float3 a, const float3 b, const float3 c) { return f3(pfma(a.x, b.x, c.x), pfma(a.y, b.y, c.y), pfma(a.z, b.z, c.z)); }
 VPT_DEV size_t group_slot(const PathState& st, const FrameArgs& fa) { return (size_t)st.pass * fa.geom.n_local + ray_local_pixel(fa.geom, st.lp); }
 VPT_DEV void group_fma(const LightGroups* lg, const size_t s, const int group, const float3 a, const float3 b) {
@@ -108,6 +109,31 @@ VPT_DEV void group_add(const LightGroups* lg, const size_t s, const int group, c
     float* p = lg->planes + (size_t)(group * 3) * lg->stride + s;
     const size_t n = lg->stride;
     p[0] = padd(p[0], a.x); p[n] = padd(p[n], a.y); p[2 * n] = padd(p[2 * n], a.z);
+}
+
+// ---- instance mattes (the instantiations whose pack ends with a MatteIds; DESIGN.md section 8l) ------------------------------------
+// The id of the camera ray's first collision goes to the id plane at the ray's sample slot.  The walks, their draws and walk_step itself
+// are those of the instantiations without mattes (a template parameter more on walk_step moved a stack store of the group and volumetric
+// kernels): the instance comes from the acceptance draw u the walk already made, regenerated from the counter-based stream.
+VPT_DEV const MatteIds* mt_of(const MatteIds& m) { return &m; }
+VPT_DEV const MatteIds* mt_of(const LightGroups&, const MatteIds& m) { return &m; }
+VPT_DEV const MatteIds* matte_ids(const MatteIds* m) { return m; }
+// the last draw of the stream: at PH_AFTER_DELTA / VP_AFTER_DELTA after an accepted collision, the u of the accepting test (walk_step ends
+// the walk there, and nothing draws before the id is taken).  Philox is counter-based: the copy re-evaluates draw k - 1, and `rng` is untouched.
+VPT_DEV float last_draw(const Rng& rng) { Rng r = rng; r.k -= 1u; return r.next(); }
+// the instance of an accepted collision at p in `leaf` with acceptance draw u: the first entry i of the leaf's list whose density prefix
+// (the float sum over entries 0..i in list order, as leaf_density adds them) passes the walk's test pmul(inv_max, prefix) > u.  The last
+// prefix is the density the walk accepted, bit for bit, so some entry always passes (negative densities included).
+VPT_DEV uint32_t collision_instance(const SceneTables& sc, const int leaf, const float3 p, const float u, const float inv_max)
+{
+    if (sc.single_volume) return 0u;
+    const LeafList lst = leaf_list_of(sc, leaf);
+    float prefix = 0.0f;
+    for (uint32_t i = 0; i < lst.n; ++i) {
+        prefix += volume_density(sc.volumes[lst.idx[i]], p);
+        if (pmul(inv_max, prefix) > u) return (uint32_t)lst.idx[i];
+    }
+    return lst.n ? (uint32_t)lst.idx[lst.n - 1] : 0u;           // not reached after an accepted collision
 }
 
 // ---- ray record <-> registers ------------------------------------------------------------------------------
@@ -344,10 +370,11 @@ VPT_DEV void begin_ratio_walk(PathState& st, const FrameShared& fs, const TraceC
 VPT_DEV float finish_ratio_walk(const PathState& st) { return clampf(st.trv * st.T_c, .0f, 1.0f); }
 
 // ---- the integrator's control flow between heavy operations -------------------------------------------------
-// kGroups (generic instantiation only): every L += also goes to the ray's light-group sums in lg->planes
-template <bool kLean, bool kGroups = false>
+// kGroups (generic instantiation only): every L += also goes to the ray's light-group sums in lg->planes.  Mattes (the pack `mt`, one
+// MatteIds pointer or empty): the id of the camera ray's first collision goes to the id plane (a lean kernel's volume is instance 0)
+template <bool kLean, bool kGroups = false, class... Mt>
 VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, const TraceConsts& tc, const SphereRec& sph,
-                     const LightGroups* lg = nullptr)
+                     const LightGroups* lg = nullptr, const Mt*... mt)
 {
     const SceneTables& sc = fs.sc;
     const vpt_kernel_params& kp = fa.kp;
@@ -361,7 +388,10 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
             break;
         case PH_TOP_HAVE:
             if (st.first_walk && st.obj_c != 1) {                   // depth pass without a volume walk (:1883-1888)
-                if (st.obj_c == 2) st.depth = length(st.org - (st.pos + st.dir * st.tmin_c));
+                if (st.obj_c == 2) {
+                    st.depth = length(st.org - (st.pos + st.dir * st.tmin_c));
+                    if constexpr (sizeof...(Mt) > 0) matte_ids(mt...)->id[group_slot(st, fa)] = kMatteSphereId;
+                }
                 st.first_walk = false;
             }
             if (st.obj_c == 0) { st.op = OP_FINISH; return; }       // nothing ahead: every later bounce is a no-op
@@ -391,6 +421,9 @@ VPT_DEV void advance(PathState& st, const FrameShared& fs, const FrameArgs& fa, 
             if (st.exit_reason == EX_DISTANCE) obj = 2;             // compiled reference: obj = 2 on every distance exit (Q4)
             if (st.first_walk) {
                 st.depth = st.mi ? length(st.org - st.pos) : .0f;
+                if constexpr (sizeof...(Mt) > 0) {
+                    if (st.mi) matte_ids(mt...)->id[group_slot(st, fa)] = kLean ? 0u : collision_instance(sc, __float_as_int(st.aux.x), st.pos, last_draw(st.rng), tc.inv_max);
+                }
                 // the reference runs this identical walk twice (depth pass + integrator) and accumulates `tr` in
                 // both; the replay adds the same densities again while tr < 1
                 if (st.alpha < 1.0f) st.alpha += st.alpha;
@@ -578,13 +611,17 @@ VPT_DEV void write_sample(const PathState& st, const FrameArgs& fa)
 struct NoAtmo { int pad[4]; };
 
 // kGroups (generic kernels): the light-group instantiation, which takes the LightGroups as one more argument (the pack `lgs`, empty
-// otherwise), so the kernels without groups keep their parameter block
+// otherwise), so the kernels without groups keep their parameter block.  The matte instantiations end the pack with a MatteIds; it is the
+// pack, not a template flag, that selects them, so every kernel without mattes keeps its name as well.
+template <class... Lg> constexpr bool has_matte_ids = (std::is_same<Lg, MatteIds>::value || ... || false);
 template <int kInteg, bool kLean, int kSlots, bool kCells = false, bool kGroups = false, class... Lg>
 __global__ void __launch_bounds__(kTraceThreads, trace_min_ctas(kSlots))
 k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atmosphere, NoAtmo>::type atm, const Lg... lgs)
 {
-    static_assert(sizeof...(Lg) == (kGroups ? 1 : 0), "k_trace<..., true> takes one LightGroups, the other instantiations none");
+    static_assert(sizeof...(Lg) == (kGroups ? 1 : 0) + (has_matte_ids<Lg...> ? 1 : 0),
+                  "k_trace<..., true> takes one LightGroups, then a MatteIds for the mattes; the other instantiations only the MatteIds or none");
     static_assert(!kGroups || !kLean, "lean kernels keep their light groups in the wide records (L is the sun group)");
+    static_assert(!has_matte_ids<Lg...> || !kCells, "cell mode has no mattes");
     // (the LightGroups are reached through lg_of(lgs...) where they are used: a pointer variable in every instantiation, even unused,
     // moved two stack stores of k_trace<1, false, 3>)
     __shared__ FrameShared fs;
@@ -659,7 +696,13 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
                     st.have_closest = true; st.op = OP_GLUE;
                 }
                 if (st.op == OP_GLUE) {
-                    if constexpr (kInteg != 0 && kGroups) advance_vol<true>(st, fs, fa, atm, tc, sph, lg_of(lgs...));
+                    if constexpr (has_matte_ids<Lg...>) {
+                        const LightGroups* lgp = nullptr;
+                        if constexpr (kGroups) lgp = lg_of(lgs...);
+                        if constexpr (kInteg != 0) advance_vol<kGroups>(st, fs, fa, atm, tc, sph, lgp, mt_of(lgs...));
+                        else advance<kLean, kGroups>(st, fs, fa, tc, sph, lgp, mt_of(lgs...));
+                    }
+                    else if constexpr (kInteg != 0 && kGroups) advance_vol<true>(st, fs, fa, atm, tc, sph, lg_of(lgs...));
                     else if constexpr (kInteg != 0) advance_vol(st, fs, fa, atm, tc, sph);
                     else if constexpr (kGroups) advance<kLean, true>(st, fs, fa, tc, sph, lg_of(lgs...));
                     else advance<kLean>(st, fs, fa, tc, sph);

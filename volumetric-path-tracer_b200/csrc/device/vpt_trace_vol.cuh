@@ -114,9 +114,10 @@ VPT_DEV float3 vol_env_radiance(const FrameArgs& fa, const vpt_atmosphere& atm, 
 
 // kGroups: every L += also goes to the ray's light-group sums in lg->planes.  The class of a light estimate is the last transmittance
 // walk's tr_kind: uniform_sample_one_light leaves aux at 0 when it ran no walk, and then the group gains an exact zero.
-template <bool kGroups = false>
+// mt: the mattes, as advance's
+template <bool kGroups = false, class... Mt>
 VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& fa, const vpt_atmosphere& atm, const TraceConsts& tc, const SphereRec& sph,
-                         const LightGroups* lg = nullptr)
+                         const LightGroups* lg = nullptr, const Mt*... mt)
 {
     const SceneTables& sc = fs.sc;
     const vpt_kernel_params& kp = fa.kp;
@@ -125,7 +126,10 @@ VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& 
         switch (st.phase) {
         case VP_START: {
             // depth pass (:1859-1889): walks only when the box is the closest object; the sphere alone sets the depth
-            if (st.obj_c == 2) st.depth = length(st.org - (st.pos + st.dir * st.tmin_c));
+            if (st.obj_c == 2) {
+                st.depth = length(st.org - (st.pos + st.dir * st.tmin_c));
+                if constexpr (sizeof...(Mt) > 0) matte_ids(mt...)->id[group_slot(st, fa)] = kMatteSphereId;
+            }
             if (st.obj_c != 1) st.first_walk = false;
             float t, tmax;
             if (!aabb_intersect(sc.root_pmin, sc.root_pmax, st.pos, st.dir, t, tmax)) { st.op = OP_FINISH; return; }   // :1731
@@ -151,6 +155,9 @@ VPT_DEV void advance_vol(PathState& st, const FrameShared& fs, const FrameArgs& 
             if (st.exit_reason == EX_SCATTER) { scatter_event(st, fs, fa, tc); st.mi = true; }
             if (st.first_walk) {                                    // this walk is also the depth pass's (same start, same draws)
                 st.depth = st.mi ? length(st.org - st.pos) : .0f;
+                if constexpr (sizeof...(Mt) > 0) {
+                    if (st.mi) matte_ids(mt...)->id[group_slot(st, fa)] = collision_instance(sc, __float_as_int(st.aux.x), st.pos, last_draw(st.rng), tc.inv_max);
+                }
                 if (st.alpha < 1.0f) st.alpha += st.alpha;
                 st.first_walk = false;
             }

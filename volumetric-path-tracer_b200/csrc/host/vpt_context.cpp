@@ -79,7 +79,7 @@ static void free_context(vpt_context* c) {
     for (auto& e : c->events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     cudaFree(c->d_queue_id); cudaFree(c->d_queue_org); cudaFree(c->d_bn_table);
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
-    cudaFree(c->d_plane_tr); cudaFree(c->d_lg_planes); cudaFree(c->d_miss_mask);
+    cudaFree(c->d_plane_tr); cudaFree(c->d_lg_planes); cudaFree(c->d_miss_mask); cudaFree(c->d_matte_map); cudaFree(c->d_matte_ids);
     cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
     cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz);
     delete c;
@@ -188,6 +188,42 @@ int vpt_set_deep_buffers(vpt_context* c, float* d_slices_f4, unsigned n_slices, 
     return VPT_OK;
 }
 
+static_assert(vpt::kMatteMax == VPT_MATTE_MAX, "matte limit");
+
+int vpt_set_instance_mattes(vpt_context* c, float* d_mattes_f4, unsigned n_mattes, const int* h_matte_of_instance, unsigned n_instances,
+                            int sphere_matte) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_instance_mattes: null context");
+    vpt::Mattes m;
+    std::vector<int8_t> map;
+    if (d_mattes_f4) {
+        if (n_mattes < 1 || n_mattes > VPT_MATTE_MAX)
+            return fail(c, VPT_ERR_INVALID, "vpt_set_instance_mattes: n_mattes must be in 1.." + std::to_string(VPT_MATTE_MAX) + ", got " + std::to_string(n_mattes));
+        if ((uintptr_t)d_mattes_f4 % 16 != 0)
+            return fail(c, VPT_ERR_INVALID, "vpt_set_instance_mattes: the matte buffer must be 16-byte aligned (the kernels move float4)");
+        if (!h_matte_of_instance && n_instances > 0) return fail(c, VPT_ERR_INVALID, "vpt_set_instance_mattes: null instance map");
+        const auto in_range = [&](int k) { return k >= -1 && k < (int)n_mattes; };
+        map.resize(n_instances);
+        for (unsigned i = 0; i < n_instances; ++i) {
+            const int k = h_matte_of_instance[i];
+            if (!in_range(k))
+                return fail(c, VPT_ERR_INVALID, "vpt_set_instance_mattes: instance " + std::to_string(i) + " maps to " + std::to_string(k) +
+                                                ", outside -1.." + std::to_string((int)n_mattes - 1));
+            map[i] = (int8_t)k;
+        }
+        if (!in_range(sphere_matte))
+            return fail(c, VPT_ERR_INVALID, "vpt_set_instance_mattes: sphere_matte " + std::to_string(sphere_matte) + " is outside -1.." +
+                                            std::to_string((int)n_mattes - 1));
+        m.out = reinterpret_cast<float4*>(d_mattes_f4);
+        m.n = (int)n_mattes;
+        m.n_ids = n_instances;
+        m.sphere = sphere_matte;
+    }
+    c->matte_req = m;
+    c->matte_map_req.swap(map);
+    c->matte_active = false;        // null: off from now on; otherwise the mattes take over at the next call with iteration == 0
+    return VPT_OK;
+}
+
 int vpt_set_render_region(vpt_context* c, unsigned x0, unsigned y0, unsigned x1, unsigned y1) {
     if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_render_region: null context");
     c->region_req[0] = x0; c->region_req[1] = y0; c->region_req[2] = x1; c->region_req[3] = y1;   // checked and taken at the next iteration-0 call
@@ -293,8 +329,8 @@ int vpt_get_stats(vpt_context* c, unsigned long long* launches, unsigned* last_q
 
 // Scratch of one round: the ray queue and plane A per sample, then either planes B, C (and D) per sample (wide records) or the tr plane
 // per pixel (compact records).  A change of record layout reallocates, so the scratch never holds another layout's planes.  Light groups
-// traced by a generic kernel also need their 12 float planes per sample, which are kept once grown.
-static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixels, bool wide, bool planeD, bool groups) {
+// traced by a generic kernel also need their 12 float planes per sample, and the instance mattes their id plane, which are kept once grown.
+static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixels, bool wide, bool planeD, bool groups, bool mattes) {
     if (n_samples > c->cap_samples || wide != c->cap_wide || planeD != c->cap_planeD) {
         cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
         cudaFree(c->d_queue_id); cudaFree(c->d_queue_org);
@@ -315,6 +351,11 @@ static int ensure_frame_buffers(vpt_context* c, size_t n_samples, size_t n_pixel
         cudaFree(c->d_lg_planes); c->d_lg_planes = nullptr; c->cap_lg_samples = 0;
         VPT_CUDA(c, cudaMalloc(&c->d_lg_planes, n_samples * 12 * sizeof(float)));
         c->cap_lg_samples = n_samples;
+    }
+    if (mattes && n_samples > c->cap_matte_samples) {
+        cudaFree(c->d_matte_ids); c->d_matte_ids = nullptr; c->cap_matte_samples = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_matte_ids, n_samples * sizeof(uint32_t)));
+        c->cap_matte_samples = n_samples;
     }
     if (!wide && n_pixels > c->cap_tr) {
         cudaFree(c->d_plane_tr); c->d_plane_tr = nullptr; c->cap_tr = 0;
@@ -338,6 +379,8 @@ struct FramePlan {
     vpt::AovBuffers aov;                  // the active compositing AOVs (both null: off)
     vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
     vpt::DeepSlices deep;                 // the active deep slices (out null: off)
+    vpt::Mattes mattes;                   // the active instance mattes (out null: off)
+    vpt::MatteIds matte_ids;              // their id plane, for the trace kernel
     bool region = false;                  // a render region is active: the region kernels over rg
     vpt::RenderRegion rg;
     vpt::Projection proj;                 // the frame's projection: the equirectangular kernels when equirect(proj)
@@ -416,6 +459,22 @@ static int check_deep_buffers(vpt_context* c, const vpt_kernel_params& kp, size_
     for (const auto& o : others)
         if (byte_ranges_overlap(c->deep_req.out, 16 * n * (size_t)c->deep_req.n, o.p, o.bytes))
             return fail(c, VPT_ERR_INVALID, std::string("vpt_set_deep_buffers: the slice buffer overlaps ") + o.name);
+    return VPT_OK;
+}
+
+// The matte buffer may not share a byte with a Kernel_params output buffer, an AOV, light-group or deep-slice buffer (n = local pixels).
+static int check_matte_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    const struct { const char* name; const void* p; size_t bytes; } others[] = {
+        { "Kernel_params.accum_buffer", (const void*)(uintptr_t)kp.accum_buffer, 12 * n }, { "Kernel_params.depth_buffer", (const void*)(uintptr_t)kp.depth_buffer, 4 * n },
+        { "Kernel_params.cost_buffer", (const void*)(uintptr_t)kp.cost_buffer, 12 * n }, { "Kernel_params.raw_buffer", (const void*)(uintptr_t)kp.raw_buffer, 16 * n },
+        { "Kernel_params.display_buffer", (const void*)(uintptr_t)kp.display_buffer, 4 * n },
+        { "the alpha AOV buffer", c->aov_alpha, 4 * n }, { "the volume AOV buffer", c->aov_volume, 12 * n },
+        { "the sun light-group buffer", c->lg_out[0], 12 * n }, { "the point light-group buffer", c->lg_out[1], 12 * n },
+        { "the emission light-group buffer", c->lg_out[2], 12 * n }, { "the environment light-group buffer", c->lg_out[3], 12 * n },
+        { "the deep slice buffer", c->deep_req.out, 16 * n * (size_t)c->deep_req.n } };
+    for (const auto& o : others)
+        if (byte_ranges_overlap(c->matte_req.out, 16 * n * (size_t)c->matte_req.n, o.p, o.bytes))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_instance_mattes: the matte buffer overlaps ") + o.name);
     return VPT_OK;
 }
 
@@ -503,6 +562,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
                 hdr.internal = ent.d_internal; hdr.leaf_list = ent.d_leaf_list; hdr.leaf_indices = ent.d_leaf_indices; hdr.volumes = c->d_vrec; hdr.leaf_nodes = nullptr;
                 VPT_CUDA(c, vpt::launch_prepare_volumes(reinterpret_cast<const vpt_gpu_vdb*>(d_volumes), hdr, c->d_scene, c->d_vrec, stream));
                 c->scene_single_volume = ent.n == 1;
+                c->scene_instances = ent.n;
             } else {
                 if (!c->d_internal) {
                     VPT_CUDA(c, cudaMalloc(&c->d_internal, sizeof(vpt::OctInternal) * vpt::kOctInternalNodes));
@@ -516,10 +576,12 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
                 }
                 VPT_CUDA(c, vpt::launch_prepare_scene(reinterpret_cast<const vpt_gpu_vdb*>(d_volumes), reinterpret_cast<const vpt_octnode*>(d_root),
                                                       c->d_scene, c->d_internal, c->d_leaf_list, c->d_leaf_indices, c->d_vrec, VPT_OCT_MAX_VOLUMES, stream));
-                VPT_CUDA(c, cudaMemcpyAsync(c->h_pinned, reinterpret_cast<const char*>(c->d_scene) + offsetof(vpt::SceneTables, single_volume), sizeof(int),
+                static_assert(offsetof(vpt::SceneTables, single_volume) == offsetof(vpt::SceneTables, num_volumes) + sizeof(int), "instance count, then single_volume");
+                VPT_CUDA(c, cudaMemcpyAsync(c->h_pinned, reinterpret_cast<const char*>(c->d_scene) + offsetof(vpt::SceneTables, num_volumes), 2 * sizeof(int),
                                             cudaMemcpyDeviceToHost, stream));
                 VPT_CUDA(c, cudaStreamSynchronize(stream));
-                c->scene_single_volume = c->h_pinned[0] != 0;
+                c->scene_instances = c->h_pinned[0];
+                c->scene_single_volume = c->h_pinned[1] != 0;
             }
             c->launches++;
             c->cached_volumes = d_volumes; c->cached_root = d_root; c->cached_generation = registered ? ent.generation : 0ull;
@@ -562,18 +624,29 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         if (rc != VPT_OK) return rc;
     }
     const bool group_planes = groups && !lean;
+    // instance mattes, decided with the groups: registered mattes take over at the first call of a frame (iteration == 0) and are checked on
+    // every call.  The trace kernel writes one id per sample (4 B more per sample)
+    const bool mattes = c->matte_active || (kp.iteration == 0 && c->matte_req.out);
+    if (mattes) {
+        if (c->brick_pool || c->cell_table) return fail(c, VPT_ERR_UNSUPPORTED, "instance mattes (vpt_set_instance_mattes) are not supported in brick or cell mode");
+        if (c->matte_req.n_ids != (uint32_t)c->scene_instances)
+            return fail(c, VPT_ERR_INVALID, "vpt_set_instance_mattes: the map covers " + std::to_string(c->matte_req.n_ids) + " instances, the scene has " +
+                                            std::to_string(c->scene_instances));
+        int rc = check_matte_buffers(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+    }
     const bool planeD = sky_env;
     const bool wide = sky_env || !lean || groups;
     int chunk = c->passes_per_chunk;
     if (c->chunk_auto) chunk = (size_t)fa.geom.n_local <= ((size_t)1 << 20) ? 64 : 32;
     {
-        const size_t per_sample = (wide ? 88 + (planeD ? 16 : 0) : 56) + (group_planes ? 48 : 0);
+        const size_t per_sample = (wide ? 88 + (planeD ? 16 : 0) : 56) + (group_planes ? 48 : 0) + (mattes ? 4 : 0);
         const size_t fit = c->max_scratch_bytes / (per_sample * (size_t)(fa.geom.n_local > 0 ? fa.geom.n_local : 1));
         if ((size_t)chunk > fit) chunk = fit < 1 ? 1 : (int)fit;
     }
     if (n_sampled) {
         const size_t per_chunk = (size_t)fa.geom.n_local * (size_t)(n_sampled < (unsigned)chunk ? n_sampled : (unsigned)chunk);
-        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD, group_planes);
+        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD, group_planes, mattes);
         if (rc != VPT_OK) return rc;
     }
     if (c->cap_chunk < chunk) {
@@ -613,7 +686,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
             if (vpt::scene_registry_find(d_root, &ent) && (ent.max_grid_bytes > 2ull * c->l2_bytes || ent.n >= 64)) slots = 2;
         }
     }
-    const vpt::TraceKernel trace = vpt::pick_trace_kernel(c->brick_pool != nullptr, c->cell_table != nullptr, vol_integ, lean, group_planes, slots);
+    const vpt::TraceKernel trace = vpt::pick_trace_kernel(c->brick_pool != nullptr, c->cell_table != nullptr, vol_integ, lean, group_planes, slots, mattes);
     fa.sched_min_lanes = c->sched_min_lanes > 0 ? c->sched_min_lanes : vpt::trace_sched_min_lanes(trace);
     int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm : c->max_ctas[trace];
     if (ctas_per_sm < 1) ctas_per_sm = 1;
@@ -649,6 +722,24 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         plan.deep = c->deep_req;
     }
     plan.resolve.deep = plan.deep.out != nullptr;
+    // instance mattes: the map goes to the device when they take over
+    if (mattes) {
+        if (!c->matte_active) {
+            const size_t n = c->matte_map_req.size();
+            if (n > c->cap_matte_map) {
+                cudaFree(c->d_matte_map); c->d_matte_map = nullptr; c->cap_matte_map = 0;
+                VPT_CUDA(c, cudaMalloc(&c->d_matte_map, n));
+                c->cap_matte_map = n;
+            }
+            if (n) VPT_CUDA(c, cudaMemcpyAsync(c->d_matte_map, c->matte_map_req.data(), n, cudaMemcpyHostToDevice, stream));
+            c->matte_active = true;
+        }
+        plan.mattes = c->matte_req;
+        plan.mattes.map = c->d_matte_map;
+        plan.mattes.id = c->d_matte_ids;
+        plan.matte_ids.id = c->d_matte_ids;
+    }
+    plan.resolve.mattes = mattes;
     plan.proj = proj;
     plan.ods = ods;
     plan.motion = motion;
@@ -676,7 +767,7 @@ static vpt::LayerSources layer_sources(const FramePlan& plan) {
 static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, unsigned np, cudaStream_t stream) {
     vpt::FrameArgs fa = plan.fa;
     fa.n_passes = (int)np;
-    return vpt::launch_trace(fa, plan.trace, plan.atmo, plan.lg, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
+    return vpt::launch_trace(fa, plan.trace, plan.atmo, plan.lg, plan.matte_ids, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
 }
 
 extern "C" {
@@ -729,11 +820,11 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
-            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, rg,
+            return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
                                                        plan.proj, stream, plan.ods_arg())
-                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep,
+                          : vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, plan.mattes,
                                                 plan.proj, stream, plan.ods_arg()); }));
-        c->launches += 4 + (plan.resolve.deep ? 1 : 0);            // with deep slices the resolve is two kernels
+        c->launches += 4 + (plan.resolve.deep ? 1 : 0) + (plan.resolve.mattes ? 1 : 0);   // deep slices and mattes: one more resolve kernel each
         done += np;
     }
     if (n_sampled < n_passes) {
@@ -742,11 +833,11 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
-        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, rg,
+        if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
                                                            plan.proj, stream, plan.ods_arg()));
-        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.proj, stream, plan.ods_arg()));
+        else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.mattes, plan.proj, stream, plan.ods_arg()));
         VPT_CUDA(c, vpt::launch_bn_advance((void*)kp.blue_noise_buffer, (int)(n_passes - n_sampled), bn_limit, stream));
-        c->launches += 2 + (plan.resolve.deep ? 1 : 0);
+        c->launches += 2 + (plan.resolve.deep ? 1 : 0) + (plan.resolve.mattes ? 1 : 0);
     }
     // multi-GPU: the one exchange of the path.  Peer-memory mode: the last resolve above already stored every pixel into every rank's
     // frame, the exported layers follow; publish and wait for the peers.  NCCL mode: all-gather of the rank-local frame into the caller's
@@ -872,8 +963,8 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
-            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.proj, stream, plan.ods_arg()); }));
-            c->launches += 3 + (plan.resolve.deep ? 1 : 0);
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.mattes, plan.proj, stream, plan.ods_arg()); }));
+            c->launches += 3 + (plan.resolve.deep ? 1 : 0) + (plan.resolve.mattes ? 1 : 0);
         }
         done += np;
         if (done == next_test && done < n_total) {

@@ -24,7 +24,7 @@ struct vpt_context {
     bool   scene_single_volume = false;
     size_t cap_vrec = 0;              // VolumeRec capacity (grows with the instance count)
     int*   h_pinned = nullptr;        // eight pinned words: the read-back a foreign octree needs, the tile counts of an adaptive test
-    int    max_ctas[vpt::kTraceKernels] = {};   // trace kernel occupancy (CTAs per SM), by vpt::TraceKernel
+    int    max_ctas[vpt::kTraceKernelsAll] = {};   // trace kernel occupancy (CTAs per SM), by vpt::TraceKernel
     size_t l2_fetch_default = 0; int l2_sector_fetch = 0;     // option "l2_sector_fetch" (cell mode)
     const float4* cell_table = nullptr; int cell_dims[3] = {0, 0, 0};   // vpt_set_cell_volume
     int    trace_slots = 0;              // option "trace_slots": rays per lane of k_trace, 0 = by grid size (2 when the grid is larger than twice the L2)
@@ -101,6 +101,17 @@ struct vpt_context {
     // (deep_req.out null: off) and activated like the AOVs
     vpt::DeepSlices deep_req;
     bool      deep_active = false;
+    // instance mattes (vpt_set_instance_mattes): a caller-owned [matte][local pixel] float4 buffer, its matte count and the host copy of the
+    // instance -> matte map, checked when set (matte_req.out null: off) and activated like the AOVs; the map goes to d_matte_map then.
+    // d_matte_ids: the trace kernels' id plane (one uint32 per sample), allocated with the other frame buffers
+    vpt::Mattes matte_req;
+    std::vector<int8_t> matte_map_req;
+    bool      matte_active = false;
+    int8_t*   d_matte_map = nullptr;
+    size_t    cap_matte_map = 0;
+    uint32_t* d_matte_ids = nullptr;
+    size_t    cap_matte_samples = 0;
+    int       scene_instances = 0;    // instances of the cached scene
     // render region (vpt_set_render_region): global pixels [x0, x1) x [y0, y1), all 0 = the whole frame.  region_req is what the caller
     // set last; it becomes region_cur at the next render call with iteration == 0, so a running mean never continues under another region
     unsigned  region_req[4] = {0, 0, 0, 0};

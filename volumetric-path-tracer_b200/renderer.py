@@ -24,7 +24,8 @@ class FrameBuffers:
     """accum/cost (float3), depth (float), raw (float4), display (uint32) for `n_pixels` pixels; alpha (float) and volume (float3),
     the compositing AOVs, once Renderer.enable_aovs() has allocated them (None until then); `groups`, the light groups (name -> float3
     tensor, LIGHT_GROUPS order), once Renderer.enable_light_groups() has allocated them (None until then); `deep`, the deep slices
-    ((K, n, 4) float32), once Renderer.enable_deep() has allocated them (None until then)."""
+    ((K, n, 4) float32), once Renderer.enable_deep() has allocated them (None until then); `mattes`, the instance mattes ((K, n, 4) float32),
+    once Renderer.enable_mattes() has allocated them (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -37,9 +38,10 @@ class FrameBuffers:
         self.volume = None
         self.groups = None
         self.deep = None
+        self.mattes = None
 
     def zero_(self):
-        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep,
+        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep, self.mattes,
                   *(self.groups.values() if self.groups else ())):
             if t is not None:
                 t.zero_()
@@ -225,6 +227,43 @@ class Renderer:
         if self.buffers.deep is None:
             raise N.VptError("Renderer.deep_image: deep slices are not enabled (Renderer.enable_deep(bounds))")
         return self.buffers.deep.view(self.buffers.deep.shape[0], self.n_local // self.width, self.width, 4)
+
+    def enable_mattes(self, sets, sphere=None):
+        """Allocate and register the instance mattes (vpt_set_instance_mattes): `sets` is a list of K iterables of instance indices
+        (K = 1..VPT_MATTE_MAX), matte k selecting the instances of sets[k]; `sphere` is the matte of the reference sphere (None: none).
+        buffers.mattes (K, n, 4) float32 holds per matte and pixel the running means (premultiplied colour, coverage) of the samples whose
+        camera ray collided first with an instance of the set: the compositing AOVs split by instance.  They take over at the next render
+        call with kp.iteration == 0 (DESIGN.md section 8l).  An index in two sets, or outside the scene's instances, raises VptError and
+        leaves the mattes as they were.  n is the renderer's local pixel count (rank-local rows on a partitioned renderer)."""
+        sets = [sorted({int(i) for i in s}) for s in sets]
+        k = len(sets)
+        if not 1 <= k <= N.VPT_MATTE_MAX:
+            raise N.VptError(f"Renderer.enable_mattes: {k} sets (1..{N.VPT_MATTE_MAX})")
+        n_inst = len(self.scene.instances)
+        matte_of = np.full(n_inst, -1, dtype=np.int32)
+        for m, s in enumerate(sets):
+            for i in s:
+                if not 0 <= i < n_inst:
+                    raise N.VptError(f"Renderer.enable_mattes: instance {i} of set {m} is outside the scene's {n_inst} instances")
+                if matte_of[i] >= 0:
+                    raise N.VptError(f"Renderer.enable_mattes: instance {i} is in set {int(matte_of[i])} and set {m}")
+                matte_of[i] = m
+        if sphere is not None and not 0 <= int(sphere) < k:
+            raise N.VptError(f"Renderer.enable_mattes: sphere matte {sphere} is outside 0..{k - 1}")
+        mattes = torch.zeros(k, self.n_local, 4, dtype=torch.float32, device=self.buffers.accum.device)
+        check(lib.vpt_set_instance_mattes(self.ctx, C.c_void_p(mattes.data_ptr()), k, matte_of.ctypes.data_as(C.POINTER(C.c_int)), n_inst,
+                                          -1 if sphere is None else int(sphere)), self.ctx, "vpt_set_instance_mattes")
+        self.buffers.mattes, self.matte_sets = mattes, tuple(tuple(s) for s in sets)
+
+    def disable_mattes(self):
+        """Turn the instance mattes off at once; buffers.mattes keeps what it holds."""
+        check(lib.vpt_set_instance_mattes(self.ctx, None, 0, None, 0, -1), self.ctx, "vpt_set_instance_mattes")
+
+    def matte_image(self):
+        """(K, H, W, 4) float32 view of buffers.mattes ((K, local rows, W, 4) on a partitioned renderer); the sets are matte_sets."""
+        if self.buffers.mattes is None:
+            raise N.VptError("Renderer.matte_image: instance mattes are not enabled (Renderer.enable_mattes(sets))")
+        return self.buffers.mattes.view(self.buffers.mattes.shape[0], self.n_local // self.width, self.width, 4)
 
     def set_region(self, x0, y0, x1, y1):
         """Render only the full-frame pixels [x0, x1) x [y0, y1) (vpt_set_render_region) from the next call with kp.iteration == 0 on:
@@ -587,6 +626,19 @@ class DistributedRenderer:
                 rel_error = torch.as_tensor(_DeviceView(pe.value, (self.r.height, self.r.width), "<f4"), device=self.full.device)
         return self.r.denoise(color=self.full_accum(), depth=depth if depth is not None else False, rel_error=rel_error, out=out,
                               display=display, iterations=iterations, sigma_luminance=sigma_luminance, sigma_depth=sigma_depth, stream=stream)
+
+    def enable_mattes(self, sets, sphere=None):
+        """Renderer.enable_mattes on this rank; every rank enables the same sets.  The mattes stay rank-local: neither exchange carries
+        them, so matte_image() holds this rank's stripes of rows (the whole frame on one rank)."""
+        self.r.enable_mattes(sets, sphere)
+
+    def disable_mattes(self):
+        """Renderer.disable_mattes on this rank."""
+        self.r.disable_mattes()
+
+    def matte_image(self):
+        """Renderer.matte_image of this rank: (K, local rows, W, 4), the rows of stripe_rows_of_rank(H, rank, world, stripe_rows)."""
+        return self.r.matte_image()
 
     def set_region(self, x0, y0, x1, y1):
         """Renderer.set_region on this rank; every rank sets the same region.  The peer-memory exchange then stores only the region's
