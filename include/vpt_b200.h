@@ -142,6 +142,34 @@ int  vpt_comm_p2p_export_layers(vpt_context* ctx, int rank, int n_ranks, int str
 int  vpt_comm_p2p_layer(vpt_context* ctx, unsigned layer, vpt_devptr_t* d_full);
 int  vpt_comm_p2p_block_bytes(unsigned width, unsigned height, int with_display, unsigned layers, size_t* out);
 
+/* Binned exchange layers: the deep slices (vpt_set_deep_buffers) and the instance mattes (vpt_set_instance_mattes) full-frame on every rank.
+ *   Export.  vpt_comm_p2p_export_binned is vpt_comm_p2p_export_layers with n_slices (0 or 1..VPT_DEEP_MAX_SLICES) and n_mattes (0 or
+ *     1..VPT_MATTE_MAX); 0 leaves that layer out.  vpt_comm_p2p_export_layers is this call with 0, 0: same block, same behaviour.  After the
+ *     seven layer planes the block holds the deep slices [n_slices][H][W] float4, then the mattes [n_mattes][H][W] float4, each array on a
+ *     256-byte boundary: slice-major and matte-major like the rank-local buffers, at global pixels.  Counts out of range are refused
+ *     (VPT_ERR_INVALID).  vpt_comm_p2p_block_bytes_binned sizes the block (pure host code; with both counts 0 it is vpt_comm_p2p_block_bytes).
+ *     The block header records the two counts, and vpt_comm_p2p_import / _import_local refuse a peer whose counts differ (VPT_ERR_INVALID,
+ *     naming the rank and both counts) and map nothing, as for the layer mask.
+ *   Layout and content.  Ranks agree on the layout (the counts, checked at import); the caller on the content: the slice bounds and the
+ *     instance -> matte map are not in the block, so every rank sets the same ones, like every other option of a sharded call.
+ *   Calls.  Once the exchange is active, a render call whose deep slices are active (registered, and taken over by an iteration-0 call) on a
+ *     block that carries deep slices must have exactly n_slices slices, and likewise for the mattes; otherwise the call is refused
+ *     (VPT_ERR_INVALID, naming both counts) before it enqueues anything, so no peer is left waiting for it.  To change K, tear the exchange
+ *     down (vpt_comm_destroy) and export again.  Every vpt_render_pass(es) and sharded vpt_render_adaptive call then ends, right after the
+ *     layer copy, with a copy of the active slices and mattes into every rank's arrays, so after the call vpt_comm_p2p_binned's array holds
+ *     the single-context frame's buffer bit for bit on every rank.  Padding rows are not stored; with a render region only R's pixels are.  A
+ *     binned layer that is exported but not active on the call keeps its array as it is.  Nothing is copied while the exchange is suspended
+ *     or on one rank.  The NCCL exchange does not carry them.
+ *   vpt_comm_p2p_binned returns the full-frame array of `which` (VPT_BINNED_DEEP or VPT_BINNED_MATTES) and its count K (k may be NULL); a
+ *     layer the block was exported without is refused (VPT_ERR_INVALID). */
+#define VPT_BINNED_DEEP    1u   /* the deep slices: [n_slices][H][W] float4 */
+#define VPT_BINNED_MATTES  2u   /* the instance mattes: [n_mattes][H][W] float4 */
+int  vpt_comm_p2p_export_binned(vpt_context* ctx, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
+                                unsigned layers, unsigned n_slices, unsigned n_mattes, unsigned char handle_out[VPT_P2P_HANDLE_BYTES]);
+int  vpt_comm_p2p_binned(vpt_context* ctx, unsigned which, vpt_devptr_t* d_full, unsigned* k);
+int  vpt_comm_p2p_block_bytes_binned(unsigned width, unsigned height, int with_display, unsigned layers, unsigned n_slices, unsigned n_mattes,
+                                     size_t* out);
+
 /* ---- the hot path --------------------------------------------------------------------------------
  * vpt_render_pass   replaces ONE launch of the reference `volume_rt_kernel` (render_kernel.cu:2216):
  *                   same inputs, same buffer updates (accum/depth/cost running means, display, raw,
@@ -276,7 +304,8 @@ int  vpt_set_light_group_buffers(vpt_context* ctx, float* d_sun_f3, float* d_poi
  *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active slices.  An adaptive frame's stopped pixels keep theirs, and every
  *     pixel's slices are bit for bit what a fixed-count frame of its own pass count leaves there.  A render region writes no slice outside
  *     it.  Every other output is bit for bit what the same call gives without slices.  Level (A) has none.  On a partitioned context the
- *     slices are rank-local; neither exchange carries them.
+ *     buffer is rank-local; the peer-memory exchange carries the slices full-frame to every rank when the block is exported with n_slices =
+ *     K (vpt_comm_p2p_export_binned, which then refuses a call with another active K).  The NCCL exchange does not carry them.
  *   Cost.  A second resolve kernel per chunk: it reads the chunk's sample records again, reads and writes each slice once per pixel
  *     (K * 32 B) plus once per sample that lands in a slice, and updates every slice once per pass (DESIGN.md section 8h).
  *   Refused when set (VPT_ERR_INVALID), with a non-NULL buffer: a buffer not 16-byte aligned, n_slices outside 1..VPT_DEEP_MAX_SLICES,
@@ -312,7 +341,9 @@ int  vpt_set_deep_buffers(vpt_context* ctx, float* d_slices_f4, unsigned n_slice
  *     over at the next render call whose Kernel_params.iteration is 0; calls before that leave the buffer untouched.
  *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active mattes, as they do the deep slices (adaptive frames, render
  *     regions, panoramas with the miss cull).  Every other output is bit for bit what the same call gives without mattes.  Level (A) has
- *     none.  On a partitioned context the mattes are rank-local; neither exchange carries them.
+ *     none.  On a partitioned context the buffer is rank-local; the peer-memory exchange carries the mattes full-frame to every rank when
+ *     the block is exported with n_mattes = K (vpt_comm_p2p_export_binned, which then refuses a call with another active K).  The NCCL
+ *     exchange does not carry them.
  *   Cost.  The trace kernel writes 4 B per sample whose camera ray collided (generic kernels: one pass over the leaf list per first
  *     collision), and a resolve kernel more per chunk reads the records again.  The trace kernel keeps the rays per lane of
  *     the frame without mattes (DESIGN.md section 8l).

@@ -165,6 +165,7 @@ EXPORTED_SYMBOLS = [
     "vpt_set_deep_buffers", "vpt_set_camera_motion", "vpt_debug_motion_cameras",
     "vpt_ods_options_defaults", "vpt_set_projection_ods", "vpt_debug_ods_cameras",
     "vpt_set_instance_mattes",
+    "vpt_comm_p2p_export_binned", "vpt_comm_p2p_binned", "vpt_comm_p2p_block_bytes_binned",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -258,6 +259,13 @@ lib.vpt_comm_p2p_export_layers.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_u
 lib.vpt_comm_p2p_export_layers.restype = C.c_int
 lib.vpt_comm_p2p_layer.argtypes = [_vp, C.c_uint, C.POINTER(C.c_uint64)]; lib.vpt_comm_p2p_layer.restype = C.c_int
 lib.vpt_comm_p2p_block_bytes.argtypes = [C.c_uint, C.c_uint, C.c_int, C.c_uint, C.POINTER(C.c_size_t)]; lib.vpt_comm_p2p_block_bytes.restype = C.c_int
+VPT_BINNED_DEEP, VPT_BINNED_MATTES = 1, 2                          # vpt_comm_p2p_binned: which binned layer
+lib.vpt_comm_p2p_export_binned.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_int, C.c_uint, C.c_uint, C.c_uint,
+                                           C.POINTER(C.c_ubyte)]
+lib.vpt_comm_p2p_export_binned.restype = C.c_int
+lib.vpt_comm_p2p_binned.argtypes = [_vp, C.c_uint, C.POINTER(C.c_uint64), C.POINTER(C.c_uint)]; lib.vpt_comm_p2p_binned.restype = C.c_int
+lib.vpt_comm_p2p_block_bytes_binned.argtypes = [C.c_uint, C.c_uint, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.POINTER(C.c_size_t)]
+lib.vpt_comm_p2p_block_bytes_binned.restype = C.c_int
 
 
 lib.vpt_texture_create_3d_from_device.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.POINTER(_vp)]

@@ -21,6 +21,7 @@
 //   k_adapt_halo, k_adapt_count_publish, k_adapt_tally, k_adapt_publish : the same frame sharded over the peer-memory exchange -- stripe-edge
 //                     errors, the agreement on when to stop, and the final full-frame stores
 //   k_layers_publish : depth, the compositing AOVs and the light groups into every rank's full-frame planes (vpt_comm_p2p_export_layers)
+//   k_binned_publish : the deep slices or the instance mattes into every rank's full-frame [K][H][W] arrays (vpt_comm_p2p_export_binned)
 //   k_generate_region, k_miss_cull_region, k_resolve_region<S, A, G>, k_adapt_init_region, k_adapt_region : render regions
 //                     (vpt_set_render_region) -- the same per-pixel work over the pixels of one rectangle of the frame
 //   k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect, k_miss_cull_equirect, k_miss_cull_region_equirect,
@@ -1333,6 +1334,27 @@ k_layers_publish(const FrameGeom g, const RenderRegion rg, const LayerSources sr
     }
 }
 
+// Binned exchange layers, one thread per (bin k = blockIdx.y, pixel of the rectangle rg), pixels row by row as k_layers_publish walks
+// them: bin k of the pixel as one float4 at its global position in every rank's [K][H][W] array.  Adjacent threads take adjacent x, so
+// the load and each peer store are coalesced 16-byte accesses.  A copy of its own rather than wider deep / matte resolve kernels: their
+// parameter blocks stay as they are.
+__global__ void __launch_bounds__(256)
+k_binned_publish(const FrameGeom g, const RenderRegion rg, const float4* __restrict__ src, const BinnedPlanes dst)
+{
+    const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= w * (uint32_t)(rg.lr1 - rg.lr0)) return;
+    const uint32_t r = i / w;
+    const int lr = rg.lr0 + (int)r, x = rg.x0 + (int)(i - r * w);
+    const int y = global_row(g, lr);
+    if (y >= g.height) return;                                    // padding row
+    const size_t k = blockIdx.y;
+    const float4 v = src[k * (size_t)g.n_local + (size_t)lr * g.width + x];
+    const size_t gp = k * ((size_t)g.width * g.height) + (size_t)y * g.width + x;
+    #pragma unroll
+    for (int p = 0; p < kMaxPeers; ++p) if (p < dst.n) dst.plane[p][gp] = v;
+}
+
 __global__ void k_peer_signal(PeerFlagPtrs fl, int n, int rank, int which, unsigned long long epoch)
 {
     const int p = threadIdx.x;
@@ -1797,7 +1819,8 @@ cudaError_t exchange_kernels_preload()
                 k_adapt_count_publish, k_adapt_tally, k_adapt_publish, k_peer_signal, k_peer_wait, k_generate_region, k_miss_cull_region,
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
                 k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish, k_generate_motion, k_generate_adaptive_motion,
-                k_generate_region_motion, k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_miss_cull_ods, k_miss_cull_region_ods);
+                k_generate_region_motion, k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_miss_cull_ods, k_miss_cull_region_ods,
+                k_binned_publish);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1971,6 +1994,17 @@ cudaError_t launch_layers_publish(const FrameGeom& g, const RenderRegion* rg, co
     const long long n = region_pixels(r);
     if (n <= 0 || dst.n <= 0) return cudaSuccess;
     k_layers_publish<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(g, r, src, dst);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_binned_publish(const FrameGeom& g, const RenderRegion* rg, const float4* src, int n_bins, const BinnedPlanes& dst, cudaStream_t s)
+{
+    RenderRegion all;                                             // the whole local frame
+    all.x1 = g.width; all.lr1 = g.local_rows;
+    const RenderRegion& r = rg ? *rg : all;
+    const long long n = region_pixels(r);
+    if (n <= 0 || n_bins <= 0 || dst.n <= 0 || !src) return cudaSuccess;
+    k_binned_publish<<<dim3((unsigned)((n + 255) / 256), (unsigned)n_bins), 256, 0, s>>>(g, r, src, dst);
     return cudaGetLastError();
 }
 

@@ -231,7 +231,7 @@ cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], 
 cudaError_t launch_peer_wait(unsigned long long* local_flags, int n, int which, unsigned long long epoch, cudaStream_t s);
 // loads every kernel a render call may issue (lazy module loading): no first launch may have to wait behind a peer's spinning flag wait
 cudaError_t exchange_kernels_preload();
-constexpr int kPeerFlagStride = 16;                   // u64 slots per flag array; layout of a block header: ready[16] done[16] error[1] layout[1] (+14 unused) adapt[16]
+constexpr int kPeerFlagStride = 16;                   // u64 slots per flag array; layout of a block header: ready[16] done[16] error[1] layout[1] binned[1] (+13 unused) adapt[16]
 constexpr int kPeerFlagsAdapt = 3;                    // flag array of the two barriers of every convergence test of a sharded adaptive frame
 // Exchange layers (vpt_comm_p2p_export_layers): full-frame planes [H][W] of depth and the compositing layers in every rank's block, in the
 // order of the VPT_LAYER_* bits (bit l = 1 << l).  Depth and alpha are float, the others float3.
@@ -243,6 +243,12 @@ struct LayerPlanes { int n = 0; float* plane[kExchangeLayers][kMaxPeers] = {}; }
 // after the call's last resolve (or k_adapt_publish): every active, exported layer of every local pixel at its global position in every rank's
 // planes; rg: the frame's render region (null: the whole frame).  Padding rows and pixels outside R are not written.
 cudaError_t launch_layers_publish(const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, const LayerPlanes& dst, cudaStream_t s);
+// Binned exchange layers (vpt_comm_p2p_export_binned): the deep slices and the instance mattes, one [K][H][W] float4 array each in every
+// rank's block after the layer planes.  plane[p]: rank p's array of one binned layer as mapped here.  A kernel argument of k_binned_publish only.
+struct BinnedPlanes { int n = 0; float4* plane[kMaxPeers] = {}; };
+// right after launch_layers_publish: src[k * n_local + local pixel] (a deep-slice or matte buffer, k < n_bins) of every local pixel at
+// plane[p][k * W * H + global pixel] in every rank's array; rg as for launch_layers_publish.  Padding rows and pixels outside R are not written.
+cudaError_t launch_binned_publish(const FrameGeom& g, const RenderRegion* rg, const float4* src, int n_bins, const BinnedPlanes& dst, cudaStream_t s);
 // limit = min(W*H, 65536) entries are advanced (the reference updates entry y*W + x from pixel (x, y))
 cudaError_t launch_bn_prepare(void* bn, float2* table, int np, int limit, unsigned* queue_counters, cudaStream_t s);   // also zeroes queue_counters[0..1]
 cudaError_t launch_bn_advance(void* bn, int n, int limit, cudaStream_t s);

@@ -108,22 +108,31 @@ int comm_gather_frame(vpt_context* c, const FrameGeom& g, const void* d_local_ac
 // Block layout: header (u64 flag arrays: ready[16] done[16] error[1], adapt[16] at kPeerFlagsAdapt) | float3 accum [H][W] | u32 display
 // [H][W] (exported with display only) | u32 pass counts [H][W] | f32 relative errors [H][W] | u32 active-tile count per rank [16].
 // The last three serve vpt_render_adaptive.  Then, in VPT_LAYER_* bit order, one [H][W] plane of each exported layer (f32 depth and alpha,
-// float3 the others).  Each part starts on a 256-byte boundary.
+// float3 the others), then the binned layers: deep slices [n_slices][H][W] float4 and mattes [n_mattes][H][W] float4.  Each part starts on
+// a 256-byte boundary.  Sizes and offsets are size_t: K x H x W x 16 passes 32 bits at modest frames.
 static constexpr size_t kP2pHeader = 512;
 static size_t p2p_round(size_t b) { return (b + 255) & ~(size_t)255; }
 static size_t p2p_accum_bytes(size_t px) { return p2p_round(px * 12); }
 static size_t p2p_plane_bytes(size_t px) { return p2p_round(px * 4); }
 static size_t p2p_tiles_offset(size_t px, bool display) { return kP2pHeader + p2p_accum_bytes(px) + (display ? p2p_plane_bytes(px) : 0) + 2 * p2p_plane_bytes(px); }
-// the block of a w x h frame; layer_off[l] (may be null) = byte offset of layer l's plane, 0 for a layer not in `layers`
-static size_t p2p_block_layout(size_t w, size_t h, bool display, unsigned layers, size_t layer_off[kExchangeLayers])
+enum BinnedLayer : int { BL_DEEP = 0, BL_MATTES = 1, kBinnedLayers = 2 };
+// the block of a w x h frame; layer_off[l] (may be null) = byte offset of layer l's plane, 0 for a layer not in `layers`; bin_off[b] (may
+// be null) = byte offset of the deep-slice (BL_DEEP) and matte (BL_MATTES) arrays, 0 for a count of 0
+static size_t p2p_block_layout(size_t w, size_t h, bool display, unsigned layers, unsigned n_slices, unsigned n_mattes,
+                               size_t layer_off[kExchangeLayers], size_t bin_off[kBinnedLayers] = nullptr)
 {
     const size_t px = w * h;
     size_t end = p2p_tiles_offset(px, display) + sizeof(unsigned) * kPeerFlagStride;
-    if (layers) end = p2p_round(end);
+    if (layers || n_slices || n_mattes) end = p2p_round(end);
     for (int l = 0; l < kExchangeLayers; ++l) {
         const bool on = (layers >> l) & 1u;
         if (layer_off) layer_off[l] = on ? end : 0;
         if (on) end += p2p_round(px * (l < XL_VOLUME ? 4 : 12));
+    }
+    const unsigned bins[kBinnedLayers] = {n_slices, n_mattes};
+    for (int b = 0; b < kBinnedLayers; ++b) {
+        if (bin_off) bin_off[b] = bins[b] ? end : 0;
+        end += p2p_round(px * bins[b] * sizeof(float4));
     }
     return end;
 }
@@ -149,18 +158,31 @@ static std::string p2p_layout_text(unsigned long long w)
     return std::to_string(w & 0xfffffffull) + " x " + std::to_string((w >> 28) & 0xfffffffull) + ", display " + std::to_string((w >> 56) & 1ull) +
            ", layers " + hex2((unsigned)(w >> 57));
 }
-// every mapped peer block must carry this rank's layout word
+// The header slot after the layout word: the binned layers' counts -- deep slices (bits 0-31) and mattes (32-63).  The layout word is full,
+// and the counts must agree for the same reason: a rank exported with more slices would store past the end of its peers' blocks.
+static constexpr int kP2pBinnedSlot = kP2pLayoutSlot + 1;
+static_assert(kP2pBinnedSlot < 3 * kPeerFlagStride, "the binned counts live in an unused slot of the header, before the adapt flags");
+static unsigned long long p2p_binned_word(const vpt_context* c) { return (unsigned long long)c->p2p_slices | ((unsigned long long)c->p2p_mattes << 32); }
+static std::string p2p_binned_text(unsigned long long w)
+{
+    return std::to_string(w & 0xffffffffull) + " deep slices and " + std::to_string(w >> 32) + " mattes";
+}
+// every mapped peer block must carry this rank's layout word and binned counts
 static int p2p_check_layouts(vpt_context* c, const char* fn)
 {
-    const unsigned long long mine = p2p_layout_word(c);
+    const unsigned long long mine = p2p_layout_word(c), mine_bins = p2p_binned_word(c);
     for (int p = 0; p < c->p2p_n; ++p) {
         if (p == c->rank) continue;
-        unsigned long long w = 0;
-        VPT_CU(c, cudaMemcpy(&w, p2p_flags(c->p2p_peer[p]) + kP2pLayoutSlot, sizeof(w), cudaMemcpyDefault));
-        if (w != mine)
-            return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block for " + p2p_layout_text(w) +
+        unsigned long long w[2] = {0, 0};
+        VPT_CU(c, cudaMemcpy(w, p2p_flags(c->p2p_peer[p]) + kP2pLayoutSlot, sizeof(w), cudaMemcpyDefault));
+        if (w[0] != mine)
+            return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block for " + p2p_layout_text(w[0]) +
                                                 ", this rank (" + std::to_string(c->rank) + ") for " + p2p_layout_text(mine) +
                                                 "; every rank must export the same frame size, display and layers");
+        if (w[1] != mine_bins)
+            return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block with " + p2p_binned_text(w[1]) +
+                                                ", this rank (" + std::to_string(c->rank) + ") with " + p2p_binned_text(mine_bins) +
+                                                "; every rank must export the same deep-slice and matte counts (vpt_comm_p2p_export_binned)");
     }
     return VPT_OK;
 }
@@ -202,13 +224,30 @@ int comm_p2p_end(vpt_context* c, cudaStream_t stream) {
 int comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream) {
     if (!c->p2p_on || c->p2p_n < 2 || !c->p2p_layers) return VPT_OK;
     size_t off[kExchangeLayers];
-    p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, off);
+    p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, off);
     LayerPlanes dst;
     dst.n = c->p2p_n;
     for (int l = 0; l < kExchangeLayers; ++l)
         for (int p = 0; off[l] && p < c->p2p_n; ++p) dst.plane[l][p] = reinterpret_cast<float*>(reinterpret_cast<char*>(c->p2p_peer[p]) + off[l]);
     VPT_CU(c, launch_layers_publish(g, rg, src, dst, stream));
     c->launches++;
+    return VPT_OK;
+}
+
+int comm_p2p_binned(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const float4* deep, const float4* mattes, cudaStream_t stream) {
+    if (!c->p2p_on || c->p2p_n < 2 || !(c->p2p_slices || c->p2p_mattes)) return VPT_OK;
+    size_t off[kBinnedLayers];
+    p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, nullptr, off);
+    const float4* src[kBinnedLayers] = {deep, mattes};
+    const unsigned n[kBinnedLayers] = {c->p2p_slices, c->p2p_mattes};
+    for (int b = 0; b < kBinnedLayers; ++b) {
+        if (!n[b] || !src[b]) continue;                               // not exported / not active on this call: the arrays keep what they hold
+        BinnedPlanes dst;
+        dst.n = c->p2p_n;
+        for (int p = 0; p < c->p2p_n; ++p) dst.plane[p] = reinterpret_cast<float4*>(reinterpret_cast<char*>(c->p2p_peer[p]) + off[b]);
+        VPT_CU(c, launch_binned_publish(g, rg, src[b], (int)n[b], dst, stream));
+        c->launches++;
+    }
     return VPT_OK;
 }
 
@@ -250,10 +289,26 @@ int vpt_comm_p2p_export(vpt_context* c, int rank, int n_ranks, int stripe_rows, 
 
 int vpt_comm_p2p_export_layers(vpt_context* c, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
                                unsigned layers, unsigned char handle_out[VPT_P2P_HANDLE_BYTES]) {
+    return vpt_comm_p2p_export_binned(c, rank, n_ranks, stripe_rows, width, height, with_display, layers, 0u, 0u, handle_out);
+}
+
+static_assert(vpt::kDeepMaxSlices == VPT_DEEP_MAX_SLICES && vpt::kMatteMax == VPT_MATTE_MAX, "binned layer limits");
+// n_slices / n_mattes within 0..VPT_DEEP_MAX_SLICES / 0..VPT_MATTE_MAX; "" when they are
+static std::string binned_count_error(unsigned n_slices, unsigned n_mattes) {
+    if (n_slices > VPT_DEEP_MAX_SLICES)
+        return "n_slices must be 0 or 1.." + std::to_string(VPT_DEEP_MAX_SLICES) + ", got " + std::to_string(n_slices);
+    if (n_mattes > VPT_MATTE_MAX) return "n_mattes must be 0 or 1.." + std::to_string(VPT_MATTE_MAX) + ", got " + std::to_string(n_mattes);
+    return "";
+}
+
+int vpt_comm_p2p_export_binned(vpt_context* c, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
+                               unsigned layers, unsigned n_slices, unsigned n_mattes, unsigned char handle_out[VPT_P2P_HANDLE_BYTES]) {
     if (!c || !handle_out || n_ranks < 1 || n_ranks > vpt::kMaxPeers || rank < 0 || rank >= n_ranks || stripe_rows < 1 || !width || !height)
         return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export: bad arguments (at most 8 ranks: one NVSwitch domain)");
     if (layers & ~vpt::kLayerMask)
         return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export_layers: unknown layer bits " + vpt::hex2(layers & ~vpt::kLayerMask));
+    if (const std::string e = binned_count_error(n_slices, n_mattes); !e.empty())
+        return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export_binned: " + e);
     if (c->p2p_block) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_export: already exported");
     static_assert(sizeof(cudaIpcMemHandle_t) == VPT_P2P_HANDLE_BYTES, "IPC handle size");
     static_assert(VPT_LAYER_DEPTH == 1u << vpt::XL_DEPTH && VPT_LAYER_ALPHA == 1u << vpt::XL_ALPHA && VPT_LAYER_VOLUME == 1u << vpt::XL_VOLUME &&
@@ -264,11 +319,13 @@ int vpt_comm_p2p_export_layers(vpt_context* c, int rank, int n_ranks, int stripe
     if (rc != VPT_OK) return rc;
     VPT_CU(c, vpt::exchange_kernels_preload());
     c->p2p_w = (int)width; c->p2p_h = (int)height; c->p2p_display = with_display != 0; c->p2p_n = n_ranks; c->p2p_layers = layers;
-    c->p2p_bytes = vpt::p2p_block_layout(width, height, c->p2p_display, layers, nullptr);
+    c->p2p_slices = n_slices; c->p2p_mattes = n_mattes;
+    c->p2p_bytes = vpt::p2p_block_layout(width, height, c->p2p_display, layers, n_slices, n_mattes, nullptr);
     VPT_CU(c, cudaMalloc(&c->p2p_block, c->p2p_bytes));
     VPT_CU(c, cudaMemset(c->p2p_block, 0, c->p2p_bytes));
-    const unsigned long long word = vpt::p2p_layout_word(c);
-    VPT_CU(c, cudaMemcpy(vpt::p2p_flags(c->p2p_block) + vpt::kP2pLayoutSlot, &word, sizeof(word), cudaMemcpyHostToDevice));
+    const unsigned long long words[2] = {vpt::p2p_layout_word(c), vpt::p2p_binned_word(c)};
+    static_assert(vpt::kP2pBinnedSlot == vpt::kP2pLayoutSlot + 1, "layout word, then the binned counts");
+    VPT_CU(c, cudaMemcpy(vpt::p2p_flags(c->p2p_block) + vpt::kP2pLayoutSlot, words, sizeof(words), cudaMemcpyHostToDevice));
     VPT_CU(c, cudaDeviceSynchronize());
     cudaIpcMemHandle_t h;
     VPT_CU(c, cudaIpcGetMemHandle(&h, c->p2p_block));
@@ -279,7 +336,33 @@ int vpt_comm_p2p_export_layers(vpt_context* c, int rank, int n_ranks, int stripe
 int vpt_comm_p2p_block_bytes(unsigned width, unsigned height, int with_display, unsigned layers, size_t* out) {
     if (!out || !width || !height) return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes: bad arguments");
     if (layers & ~vpt::kLayerMask) return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes: unknown layer bits");
-    *out = vpt::p2p_block_layout(width, height, with_display != 0, layers, nullptr);
+    *out = vpt::p2p_block_layout(width, height, with_display != 0, layers, 0u, 0u, nullptr);
+    return VPT_OK;
+}
+
+int vpt_comm_p2p_block_bytes_binned(unsigned width, unsigned height, int with_display, unsigned layers, unsigned n_slices, unsigned n_mattes,
+                                    size_t* out) {
+    if (!out || !width || !height) return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes_binned: bad arguments");
+    if (layers & ~vpt::kLayerMask) return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes_binned: unknown layer bits");
+    if (const std::string e = binned_count_error(n_slices, n_mattes); !e.empty())
+        return vpt::fail_global(VPT_ERR_INVALID, "vpt_comm_p2p_block_bytes_binned: " + e);
+    *out = vpt::p2p_block_layout(width, height, with_display != 0, layers, n_slices, n_mattes, nullptr);
+    return VPT_OK;
+}
+
+int vpt_comm_p2p_binned(vpt_context* c, unsigned which, vpt_devptr_t* d_full, unsigned* k) {
+    if (!c || !d_full || !c->p2p_block) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_binned: no exchange block");
+    if (which != VPT_BINNED_DEEP && which != VPT_BINNED_MATTES)
+        return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_binned: " + std::to_string(which) + " is neither VPT_BINNED_DEEP nor VPT_BINNED_MATTES");
+    const int b = which == VPT_BINNED_DEEP ? vpt::BL_DEEP : vpt::BL_MATTES;
+    const unsigned n = b == vpt::BL_DEEP ? c->p2p_slices : c->p2p_mattes;
+    if (!n)
+        return vpt::fail_ctx(c, VPT_ERR_INVALID, std::string("vpt_comm_p2p_binned: the block was exported without ") +
+                                                 (b == vpt::BL_DEEP ? "deep slices" : "mattes") + " (vpt_comm_p2p_export_binned)");
+    size_t off[vpt::kBinnedLayers];
+    vpt::p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, nullptr, off);
+    *d_full = (vpt_devptr_t)(reinterpret_cast<char*>(c->p2p_block) + off[b]);
+    if (k) *k = n;
     return VPT_OK;
 }
 
@@ -291,7 +374,7 @@ int vpt_comm_p2p_layer(vpt_context* c, unsigned layer, vpt_devptr_t* d_full) {
     if (!(c->p2p_layers & layer))
         return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: the block was exported without layer " + std::to_string(layer) + " (vpt_comm_p2p_export_layers)");
     size_t off[vpt::kExchangeLayers];
-    vpt::p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, off);
+    vpt::p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, off);
     *d_full = (vpt_devptr_t)(reinterpret_cast<char*>(c->p2p_block) + off[l]);
     return VPT_OK;
 }
@@ -423,7 +506,7 @@ int vpt_comm_destroy(vpt_context* c) {
     if (c->p2p_block) {
         cudaDeviceSynchronize();
         if (!c->p2p_local) for (int p = 0; p < c->p2p_n; ++p) if (p != c->rank && c->p2p_peer[p]) cudaIpcCloseMemHandle(c->p2p_peer[p]);
-        cudaFree(c->p2p_block); c->p2p_block = nullptr; c->p2p_on = false; c->p2p_n = 0; c->p2p_layers = 0;
+        cudaFree(c->p2p_block); c->p2p_block = nullptr; c->p2p_on = false; c->p2p_n = 0; c->p2p_layers = 0; c->p2p_slices = c->p2p_mattes = 0;
         for (auto& q : c->p2p_peer) q = nullptr;
     }
     return VPT_OK;

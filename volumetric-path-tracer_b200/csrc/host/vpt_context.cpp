@@ -635,6 +635,19 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         int rc = check_matte_buffers(c, kp, (size_t)fa.geom.n_local);
         if (rc != VPT_OK) return rc;
     }
+    const bool deep = c->deep_active || (kp.iteration == 0 && c->deep_req.out);
+    // an active exchange whose block carries deep slices or mattes: this call's count must be the exported one, or k_binned_publish would
+    // store another layout.  Checked before any state changes and before the call enqueues its first flag signal
+    if (c->p2p_on) {
+        const struct { bool on; unsigned have, exported; const char *what, *setter; } bins[2] = {
+            { deep, (unsigned)c->deep_req.n, c->p2p_slices, "deep slices", "vpt_set_deep_buffers" },
+            { mattes, (unsigned)c->matte_req.n, c->p2p_mattes, "mattes", "vpt_set_instance_mattes" } };
+        for (const auto& b : bins)
+            if (b.on && b.exported && b.have != b.exported)
+                return fail(c, VPT_ERR_INVALID, std::string("the peer exchange block was exported with ") + std::to_string(b.exported) + " " + b.what +
+                                                " (vpt_comm_p2p_export_binned), this call's " + b.what + " (" + b.setter + ") are " + std::to_string(b.have) +
+                                                "; set " + std::to_string(b.exported) + ", or tear the exchange down (vpt_comm_destroy) and export again");
+    }
     const bool planeD = sky_env;
     const bool wide = sky_env || !lean || groups;
     int chunk = c->passes_per_chunk;
@@ -715,7 +728,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     plan.resolve.aov = plan.aov.alpha || plan.aov.volume;
     plan.resolve.groups = plan.lg.out[0] || plan.lg.out[1] || plan.lg.out[2] || plan.lg.out[3];
     // deep slices: the buffer, its slice count and bounds take over at the first call of a frame (iteration == 0), checked on every call
-    if (c->deep_active || (kp.iteration == 0 && c->deep_req.out)) {
+    if (deep) {
         int rc = check_deep_buffers(c, kp, (size_t)fa.geom.n_local);
         if (rc != VPT_OK) return rc;
         c->deep_active = true;
@@ -843,6 +856,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
     // frame, the exported layers follow; publish and wait for the peers.  NCCL mode: all-gather of the rank-local frame into the caller's
     // full-frame buffers.
     { int rc = vpt::comm_p2p_layers(c, fa.geom, region ? &rg : nullptr, layer_sources(plan), stream); if (rc != VPT_OK) return rc; }
+    { int rc = vpt::comm_p2p_binned(c, fa.geom, region ? &rg : nullptr, plan.deep.out, plan.mattes.out, stream); if (rc != VPT_OK) return rc; }
     { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     if (c->nccl_comm && (c->d_full_accum || c->d_full_display)) {
         int rc = vpt::comm_gather_frame(c, fa.geom, (const void*)kp.accum_buffer, (const void*)kp.display_buffer, stream);
@@ -1003,6 +1017,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         VPT_CUDA(c, vpt::launch_adapt_publish(g, fa.kp, ad, peers, stream));
         c->launches++;
         { int rc = vpt::comm_p2p_layers(c, g, nullptr, layer_sources(plan), stream); if (rc != VPT_OK) return rc; }
+        { int rc = vpt::comm_p2p_binned(c, g, nullptr, plan.deep.out, plan.mattes.out, stream); if (rc != VPT_OK) return rc; }
         { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }
     if (passes_run) *passes_run = done;

@@ -71,6 +71,7 @@ struct vpt_context {
     int    p2p_n = 0; bool p2p_on = false, p2p_display = false, p2p_local = false; unsigned long long p2p_epoch = 0;
     unsigned long long p2p_adapt_epoch = 0;                     // barriers of the convergence tests of sharded adaptive frames (flag array kPeerFlagsAdapt)
     unsigned p2p_layers = 0;                                    // VPT_LAYER_* mask the block was exported with (vpt_comm_p2p_export_layers)
+    unsigned p2p_slices = 0, p2p_mattes = 0;                    // deep slices / mattes the block carries, 0: none (vpt_comm_p2p_export_binned)
     int    gather_async = 0;                                    // option "gather_async": gather on the side stream (see vpt_comm_wait)
     bool   gather_pending = false;
     size_t max_scratch_bytes = (size_t)12 << 30;                // cap of the per-chunk ray queue + sample planes
@@ -170,6 +171,10 @@ int  comm_p2p_end(vpt_context* c, cudaStream_t stream);                         
 // right before comm_p2p_end: the exported layers that src holds into every rank's planes (k_layers_publish); nothing when the exchange is
 // suspended, on one rank or without layers.  rg: the frame's render region, null for the whole frame
 int  comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream);
+// right after comm_p2p_layers: the frame's active deep slices and mattes (null: not active) into every rank's binned arrays
+// (k_binned_publish); nothing when the exchange is suspended, on one rank, or for a layer the block does not carry.  The caller has checked
+// that an active layer's count is the exported one (frame_setup)
+int  comm_p2p_binned(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const float4* deep, const float4* mattes, cudaStream_t stream);
 // sharded adaptive frames: every rank's planes as mapped here, and the local block's halo (err plane), count slots and error word
 struct P2pAdaptLocal { const float* halo = nullptr; const unsigned* tiles = nullptr; const unsigned long long* error_word = nullptr; };
 void comm_p2p_adapt_views(vpt_context* c, AdaptPeers* out, P2pAdaptLocal* local);

@@ -427,6 +427,16 @@ def _layer_mask(names):
     return m
 
 
+def _binned_counts(deep_slices, n_mattes):
+    """The binned layers asked for: 0 (not carried) or 1..VPT_DEEP_MAX_SLICES / 1..VPT_MATTE_MAX."""
+    d, m = int(deep_slices), int(n_mattes)
+    if not 0 <= d <= N.VPT_DEEP_MAX_SLICES:
+        raise N.VptError(f"DistributedRenderer: deep_slices={d} (0 or 1..{N.VPT_DEEP_MAX_SLICES})")
+    if not 0 <= m <= N.VPT_MATTE_MAX:
+        raise N.VptError(f"DistributedRenderer: n_mattes={m} (0 or 1..{N.VPT_MATTE_MAX})")
+    return d, m
+
+
 class _DeviceView:
     """Zero-copy torch view of library-owned device memory (__cuda_array_interface__)."""
     def __init__(self, ptr, shape, typestr):
@@ -446,16 +456,21 @@ class DistributedRenderer:
 
     layers: names of N.LAYER_BITS -- "depth", "alpha", "volume" and the LIGHT_GROUPS -- that the peer-memory exchange also carries full-frame
     to every rank (vpt_comm_p2p_export_layers): full_depth(), full_alpha(), full_volume(), full_light_group(name).  The AOVs and groups must
-    be enabled on every rank (enable_aovs(), enable_light_groups()) and take over at the next call with kp.iteration == 0."""
+    be enabled on every rank (enable_aovs(), enable_light_groups()) and take over at the next call with kp.iteration == 0.
+
+    deep_slices, n_mattes: the binned layers the peer-memory exchange also carries full-frame (vpt_comm_p2p_export_binned): K deep slices
+    (full_deep()) and K mattes (full_mattes()), 0 = not carried.  Every rank enables exactly that many (enable_deep(bounds) with K + 1
+    bounds, enable_mattes(sets) with K sets), with the same bounds and sets; changing K needs a new DistributedRenderer."""
 
     def __init__(self, scene: Scene, width, height, cam=None, kp=None, stripe_rows=16, options=None, gather_display=False, exchange="p2p",
-                 layers=()):
+                 layers=(), deep_slices=0, n_mattes=0):
         import torch.distributed as dist
         self.dist = dist
         self.rank, self.world = dist.get_rank(), dist.get_world_size()
         if self.world > 8 and exchange == "p2p": exchange = "nccl"
         self.exchange = exchange if self.world > 1 else "none"
         self.layers = _layer_names(layers)
+        self.deep_slices, self.n_mattes = _binned_counts(deep_slices, n_mattes)
         self.r = Renderer(scene, width, height, cam=cam, kp=kp, rank=self.rank, n_ranks=self.world,
                           stripe_rows=stripe_rows, options=options)
         self.last_adaptive = False; self._err1 = None
@@ -468,9 +483,9 @@ class DistributedRenderer:
             ok, err = 1, ""
             raw = (C.c_ubyte * 64)()
             try:
-                check(lib.vpt_comm_p2p_export_layers(self.r.ctx, self.rank, self.world, stripe_rows, self.r.width, self.r.height,
-                                                     1 if gather_display else 0, _layer_mask(self.layers), raw),
-                      self.r.ctx, "vpt_comm_p2p_export_layers")
+                check(lib.vpt_comm_p2p_export_binned(self.r.ctx, self.rank, self.world, stripe_rows, self.r.width, self.r.height,
+                                                     1 if gather_display else 0, _layer_mask(self.layers), self.deep_slices, self.n_mattes, raw),
+                      self.r.ctx, "vpt_comm_p2p_export_binned")
             except N.VptError as e:
                 ok, err = 0, str(e)
             mine = torch.tensor(list(raw), dtype=torch.uint8, device=scene.device)
@@ -509,18 +524,26 @@ class DistributedRenderer:
                                     "resolve kernel, + stripe un-permutation kernel")
 
     @classmethod
-    def over_exchange(cls, renderer: Renderer, layers=(), gather_display=False):
+    def over_exchange(cls, renderer: Renderer, layers=(), gather_display=False, deep_slices=0, n_mattes=0):
         """A DistributedRenderer over a partitioned `renderer` whose peer-memory exchange is already active (vpt_comm_p2p_export_layers with
-        the mask of `layers`, then vpt_comm_p2p_import or _import_local): what __init__ leaves after its torch.distributed bootstrap.  For one
-        process that drives several shards (one Renderer per GPU, or several on one GPU), each shard's calls on its own thread."""
+        the mask of `layers`, or vpt_comm_p2p_export_binned with that mask, deep_slices and n_mattes, then vpt_comm_p2p_import or
+        _import_local): what __init__ leaves after its torch.distributed bootstrap.  For one process that drives several shards (one Renderer
+        per GPU, or several on one GPU), each shard's calls on its own thread."""
         self = cls.__new__(cls)
         self.dist = None
         self.rank, self.world, self.r = renderer.rank, renderer.n_ranks, renderer
         self.exchange = "p2p" if self.world > 1 else "none"
         self.layers = _layer_names(layers)
+        self.deep_slices, self.n_mattes = _binned_counts(deep_slices, n_mattes)
         self.last_adaptive = False; self._err1 = None
         self.full = None; self.full_display = None
         self.collective_note = "peer-memory exchange set up by the caller"
+        if self.world > 1:
+            for which, want, name in ((N.VPT_BINNED_DEEP, self.deep_slices, "deep_slices"), (N.VPT_BINNED_MATTES, self.n_mattes, "n_mattes")):
+                p, k = C.c_uint64(0), C.c_uint(0)
+                have = int(k.value) if lib.vpt_comm_p2p_binned(renderer.ctx, which, C.byref(p), C.byref(k)) == 0 else 0
+                if have != want:
+                    raise N.VptError(f"DistributedRenderer.over_exchange: {name}={want}, but the exchange block was exported with {have}")
         self._map_frame(gather_display)
         return self
 
@@ -627,9 +650,30 @@ class DistributedRenderer:
         return self.r.denoise(color=self.full_accum(), depth=depth if depth is not None else False, rel_error=rel_error, out=out,
                               display=display, iterations=iterations, sigma_luminance=sigma_luminance, sigma_depth=sigma_depth, stream=stream)
 
+    def _check_binned_count(self, k, exported, what, caller):
+        """An exchange that carries a binned layer refuses a render call with another count: refuse it here already."""
+        if self.world > 1 and self.exchange == "p2p" and exported and k != exported:
+            raise N.VptError(f"DistributedRenderer.{caller}: {k} {what}, but the peer-memory exchange carries {exported} (set K = {exported}, "
+                             f"or make a new DistributedRenderer with another count)")
+
+    def enable_deep(self, bounds):
+        """Renderer.enable_deep on this rank; every rank enables the same bounds.  With deep_slices = K the peer-memory exchange carries
+        them (full_deep()), and len(bounds) - 1 must be K: another count raises VptError."""
+        self._check_binned_count(len(np.asarray(bounds).reshape(-1)) - 1, self.deep_slices, "deep slices", "enable_deep")
+        self.r.enable_deep(bounds)
+
+    def disable_deep(self):
+        """Renderer.disable_deep on this rank."""
+        self.r.disable_deep()
+
+    def deep_image(self):
+        """Renderer.deep_image of this rank: (K, local rows, W, 4), the rows of stripe_rows_of_rank(H, rank, world, stripe_rows)."""
+        return self.r.deep_image()
+
     def enable_mattes(self, sets, sphere=None):
-        """Renderer.enable_mattes on this rank; every rank enables the same sets.  The mattes stay rank-local: neither exchange carries
-        them, so matte_image() holds this rank's stripes of rows (the whole frame on one rank)."""
+        """Renderer.enable_mattes on this rank; every rank enables the same sets.  With n_mattes = K the peer-memory exchange carries
+        them (full_mattes()), and len(sets) must be K: another count raises VptError."""
+        self._check_binned_count(len(sets), self.n_mattes, "mattes", "enable_mattes")
         self.r.enable_mattes(sets, sphere)
 
     def disable_mattes(self):
@@ -637,8 +681,34 @@ class DistributedRenderer:
         self.r.disable_mattes()
 
     def matte_image(self):
-        """Renderer.matte_image of this rank: (K, local rows, W, 4), the rows of stripe_rows_of_rank(H, rank, world, stripe_rows)."""
+        """Renderer.matte_image of this rank: (K, local rows, W, 4), the rows of stripe_rows_of_rank(H, rank, world, stripe_rows).
+        full_mattes() is the whole frame."""
         return self.r.matte_image()
+
+    def _binned(self, which, caller):
+        """(K, H, W, 4) full frame of a binned layer: a view of this rank's exchange block, or on one rank a copy of the renderer's buffer."""
+        deep = which == N.VPT_BINNED_DEEP
+        what, count, arg = ("deep slices", self.deep_slices, "deep_slices") if deep else ("mattes", self.n_mattes, "n_mattes")
+        if not count:
+            raise N.VptError(f"DistributedRenderer.{caller}: {what} were not requested (DistributedRenderer(..., {arg}=K))")
+        if self.world == 1:
+            return (self.r.deep_image() if deep else self.r.matte_image()).clone()
+        if self.exchange != "p2p":
+            raise N.VptError(f"DistributedRenderer.{caller}: the {self.exchange} exchange does not carry {what}, they stay rank-local; the "
+                             f"peer-memory exchange could not be set up ({getattr(self, 'p2p_error', 'exchange=' + repr(self.exchange))})")
+        p, k = C.c_uint64(0), C.c_uint(0)
+        check(lib.vpt_comm_p2p_binned(self.r.ctx, which, C.byref(p), C.byref(k)), self.r.ctx, "vpt_comm_p2p_binned")
+        return torch.as_tensor(_DeviceView(p.value, (int(k.value), self.r.height, self.r.width, 4), "<f4"), device=self.full.device)
+
+    def full_deep(self):
+        """(K, H, W, 4) float32 deep slices of the whole frame, slice-major like Renderer.deep_image(): a view of this rank's exchange block
+        that the next call overwrites (a copy on one rank).  The bounds are those given to enable_deep (self.r.deep_bounds), so
+        deep.flatten / insert / exr_samples take it as they take a single context's deep_image()."""
+        return self._binned(N.VPT_BINNED_DEEP, "full_deep")
+
+    def full_mattes(self):
+        """(K, H, W, 4) float32 instance mattes of the whole frame, matte-major like Renderer.matte_image() (see full_deep)."""
+        return self._binned(N.VPT_BINNED_MATTES, "full_mattes")
 
     def set_region(self, x0, y0, x1, y1):
         """Renderer.set_region on this rank; every rank sets the same region.  The peer-memory exchange then stores only the region's
