@@ -542,6 +542,11 @@ int  vpt_get_counters(vpt_context* ctx, unsigned long long out[8], int reset);
  * walk, so out[2] stays 0), out[3] = k_trace walks ended by "empty ahead" (option "empty_ahead"), out[4..6] = rays that
  * entered k_generate's octree pre-step / its hops / those ended at once by "empty ahead"; out[7] = 0.  Synchronises the device. */
 int  vpt_get_hop_counters(vpt_context* ctx, unsigned long long out[8], int reset);
+/* The "empty ahead" table of the last render call (option "empty_ahead"; built once per call from the scene's octree): out[8 * i + c] is
+ * the entry of child c of internal node i (0..72), bit o set when no populated leaf lies in the orthant of the child's block for direction
+ * octant o (bit 0 x < 0, bit 1 y < 0, bit 2 z < 0); the last 8 bytes are 0.  Synchronises the device. */
+#define VPT_EMPTY_AHEAD_BYTES 592
+int  vpt_debug_empty_ahead(vpt_context* ctx, unsigned char out[VPT_EMPTY_AHEAD_BYTES]);
 int  vpt_get_kernel_times(vpt_context* ctx, float ms[4], int n[4]);
 
 /* ---- host-side scene helpers (what the reference does in main.cpp / gpu_vdb.cpp / bvh_builder.cpp) -- */

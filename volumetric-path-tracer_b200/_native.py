@@ -150,7 +150,7 @@ EXPORTED_SYMBOLS = [
     "vpt_local_pixels", "vpt_unpermute", "vpt_render_pass", "vpt_render_passes", "vpt_invalidate_scene", "vpt_get_stats",
     "vpt_texture_create_3d", "vpt_texture_create_env", "vpt_texture_destroy", "vpt_vdb_load", "vpt_hdr_load",
     "vpt_bmp_load_rbg", "vpt_exr_load_rgb", "vpt_free", "vpt_octree_build", "vpt_octree_destroy", "vpt_volume_bounds",
-    "vpt_camera_look_at", "vpt_kernel_params_defaults", "vpt_get_counters", "vpt_get_hop_counters", "vpt_get_kernel_times", "vpt_octree_read",
+    "vpt_camera_look_at", "vpt_kernel_params_defaults", "vpt_get_counters", "vpt_get_hop_counters", "vpt_debug_empty_ahead", "vpt_get_kernel_times", "vpt_octree_read",
     "vpt_env_tables_create", "vpt_ins_load", "vpt_env_sky_tabulate",
     "vpt_octree_info", "vpt_octree_read_flat", "vpt_bvh_build", "vpt_bvh_read", "vpt_bvh_destroy", "vpt_env_tables_compute",
     "vpt_comm_get_unique_id", "vpt_comm_init", "vpt_comm_set_gather", "vpt_comm_wait", "vpt_comm_info", "vpt_comm_destroy",
@@ -227,6 +227,7 @@ lib.vpt_denoise.restype = C.c_int
 lib.vpt_get_stats.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.POINTER(C.c_uint)]; lib.vpt_get_stats.restype = C.c_int
 lib.vpt_get_counters.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.c_int]; lib.vpt_get_counters.restype = C.c_int
 lib.vpt_get_hop_counters.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.c_int]; lib.vpt_get_hop_counters.restype = C.c_int
+lib.vpt_debug_empty_ahead.argtypes = [_vp, C.POINTER(C.c_uint8)]; lib.vpt_debug_empty_ahead.restype = C.c_int
 lib.vpt_get_kernel_times.argtypes = [_vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]; lib.vpt_get_kernel_times.restype = C.c_int
 lib.vpt_texture_create_3d.argtypes = [C.POINTER(C.c_float), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.POINTER(_vp)]
 lib.vpt_texture_create_3d.restype = C.c_int

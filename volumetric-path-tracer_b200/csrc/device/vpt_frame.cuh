@@ -71,7 +71,8 @@ struct FrameShared {
     VolumeRec   vol0;      // volume 0 staged for single-volume scenes (the headline case)
 };
 
-VPT_DEV void load_frame_shared(FrameShared& fs, const SceneTables* sc_dev) {
+// ea: also stage the render call's empty-ahead table (sc_dev is then the context's SceneAlloc); null for the kernels that do not read it
+VPT_DEV void load_frame_shared(FrameShared& fs, const SceneTables* sc_dev, EmptyAhead* ea = nullptr) {
     if (threadIdx.x == 0 && threadIdx.y == 0) fs.sc = *sc_dev;
     __syncthreads();
     // stage_octree assumes a 1-D thread index
@@ -83,6 +84,11 @@ VPT_DEV void load_frame_shared(FrameShared& fs, const SceneTables* sc_dev) {
         const uint4* vs = reinterpret_cast<const uint4*>(fs.sc.volumes);
         uint4* vd = reinterpret_cast<uint4*>(&fs.vol0);
         for (int i = t; i < (int)(sizeof(VolumeRec) / 16); i += nt) vd[i] = __ldg(vs + i);
+    }
+    if (ea) {
+        const uint4* es = reinterpret_cast<const uint4*>(&reinterpret_cast<const SceneAlloc*>(sc_dev)->ahead);
+        uint4* ed = reinterpret_cast<uint4*>(ea);
+        for (int i = t; i < (int)(sizeof(EmptyAhead) / 16); i += nt) ed[i] = __ldg(es + i);
     }
     __syncthreads();
 }

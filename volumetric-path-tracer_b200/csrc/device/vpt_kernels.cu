@@ -167,10 +167,8 @@ __device__ __forceinline__ void generate_body(const FrameArgs& fa, const AdaptAr
         { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 2; while (n) { denom *= 2; r = padd(r, __fdividef((float)(n % 2), denom)); n *= inv; } vdc2[threadIdx.x] = r; }
         { int n = threadIdx.x; float r = 0, denom = 1, inv = 1.f / 3; while (n) { denom *= 3; r = padd(r, __fdividef((float)(n % 3), denom)); n *= inv; } vdc3[threadIdx.x] = r; }
     }
-    load_frame_shared(fs, fa.scene);
     __shared__ EmptyAhead ea;
-    __shared__ AheadScratch eas;
-    if constexpr (!kMotion && !kOds) build_empty_ahead(ea, eas, fs.oct, fa.empty_ahead != 0);   // the pre-step's table (none under motion / ODS)
+    load_frame_shared(fs, fa.scene, (!kMotion && !kOds) ? &ea : nullptr);   // the pre-step's table (none under motion / ODS)
     const SceneTables& sc = fs.sc;
     uint32_t n_pre = 0, n_hop = 0, n_ahead = 0;                 // statistics of the pre-step: rays, hops, rays ended by "empty ahead"
 
@@ -374,6 +372,17 @@ k_generate_adaptive_ods(const FrameArgs fa, const AdaptArgs ad, const OdsParams 
 __global__ void __launch_bounds__(128)
 k_generate_region_ods(const FrameArgs fa, const RenderRegion rg, const OdsParams od)
 { generate_body<false, true, false, false, true>(fa, nullptr, &rg, nullptr, nullptr, &od); }
+
+// The render call's empty-ahead table, into the scene allocation (one CTA): the table depends only on the octree and the option, so it
+// is built once here instead of by every block of k_generate and k_trace
+__global__ void __launch_bounds__(128)
+k_empty_ahead(SceneAlloc* scene, int enable)
+{
+    __shared__ FrameShared fs;
+    __shared__ AheadScratch s;
+    load_frame_shared(fs, &scene->sc);
+    build_empty_ahead(scene->ahead, s, fs.oct, enable != 0);
+}
 
 // =====================================================================================================
 // k_miss_cull
@@ -1590,6 +1599,12 @@ cudaError_t launch_generate_adaptive(const FrameArgs& fa, int n_passes, const Ad
     return cudaGetLastError();
 }
 
+cudaError_t launch_empty_ahead(SceneTables* scene, int enable, cudaStream_t s)
+{
+    k_empty_ahead<<<1, 128, 0, s>>>(reinterpret_cast<SceneAlloc*>(scene), enable);
+    return cudaGetLastError();
+}
+
 static size_t trace_smem_bytes(int slots) { return (size_t)kTraceWarps * kRayWords * 32 * slots * sizeof(float); }
 
 static BrickArgs brick_args(const float* pool, const int dims[3])
@@ -1820,7 +1835,7 @@ cudaError_t exchange_kernels_preload()
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
                 k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish, k_generate_motion, k_generate_adaptive_motion,
                 k_generate_region_motion, k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_miss_cull_ods, k_miss_cull_region_ods,
-                k_binned_publish);
+                k_binned_publish, k_empty_ahead);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)

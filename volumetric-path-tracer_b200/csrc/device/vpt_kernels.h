@@ -35,11 +35,8 @@ struct FrameArgs {
     uint2*    queue_id;
     float4*   queue_aux;           // per-ray origin (thin lens or camera motion); pre-stepped ray (pinhole only): position where stepping starts
     int       thin_lens;           // per-ray origin: thin lens or camera motion (cam.lens_radius != 0 or a CameraMotion)
-    // option "empty_ahead": k_generate's pre-step and the lean k_trace end a walk at the first empty node from which no populated leaf lies
-    // ahead (build_empty_ahead, vpt_walk.cuh).  0: the table stays empty and every walk hops to the box exit.  (In the padding after
-    // thin_lens: the struct's size and every other offset stay as they were.)
-    int       empty_ahead;
-    const float2* bn_table;        // [pass][65536] blue-noise jitter of the chunk
+    // (option "empty_ahead" reaches the kernels through the table behind `scene`: SceneAlloc, launch_empty_ahead)
+    const float2* bn_table;       // [pass][65536] blue-noise jitter of the chunk
     int       n_passes;            // passes in this chunk (k_generate loops over them; k_trace keeps tr of the last one)
     int       passes_per_block;    // k_generate: passes handled by one block (blockIdx.z selects the run)
     int       debug_flags;         // development switches (0 in production)
@@ -141,6 +138,9 @@ cudaError_t launch_prepare_volumes(const vpt_gpu_vdb* vols, const SceneTables& h
 // od: the frame's ODS projection (null unless ods(pj)) -- the generate, cull and resolve launchers run the ODS kernels when it is set (never
 // with motion)
 cudaError_t launch_generate(const FrameArgs& fa, int n_passes, const Projection& pj, const CameraMotion* mo, const OdsParams* od, cudaStream_t s);
+// once per render call, after the scene tables: the empty-ahead table of option "empty_ahead" (enable) into the context's SceneAlloc,
+// whose first member `scene` is
+cudaError_t launch_empty_ahead(SceneTables* scene, int enable, cudaStream_t s);
 // once per render call, before the first chunk: mask[local pixel] = 1 where every jitter misses the root box and the sphere (pinhole
 // and equirectangular cameras; a thin lens or a root box that is empty or not finite culls nothing)
 // od: the frame's ODS projection (null unless ods(pj)) -- the cull and resolve launchers below run the ODS kernels when it is set

@@ -10,6 +10,7 @@
 //   * VolumeRec[N]      : world->texture affine as the reference's own adjugate/determinant split,
 //                         so the lookup coordinate is bit-identical to the reference's inline inverse.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 #include <cuda_runtime.h>
 
@@ -49,5 +50,16 @@ struct SceneTables {
     // Null everywhere else.  [512] pointers to the leaf nodes (null where the leaf does not exist).
     const void* const* leaf_nodes;
 };
+
+// "Nothing populated ahead" (DESIGN.md section 8j, build_empty_ahead in vpt_walk.cuh): one entry per (node, child) pair below the root,
+// entry of child c of internal node i at i * 8 + c.  Bit o of an entry: no populated leaf in the orthant of the entry's block for octant o.
+constexpr int kAheadEntries = 8 + 64 + 512;
+struct __align__(16) EmptyAhead { uint8_t bit[kAheadEntries + 8]; };
+
+// The context's scene allocation: the tables, then the empty-ahead table of the current render call.  k_empty_ahead writes the table
+// once per call; k_generate and the lean k_trace stage it into shared memory with the octree (load_frame_shared), reaching it through
+// FrameArgs::scene, so no kernel's parameter block changes.
+struct SceneAlloc { SceneTables sc; EmptyAhead ahead; };
+static_assert(sizeof(EmptyAhead) % 16 == 0 && offsetof(SceneAlloc, ahead) % 16 == 0, "the table is staged in 16-byte words");
 
 } // namespace vpt

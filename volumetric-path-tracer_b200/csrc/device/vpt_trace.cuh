@@ -5,7 +5,7 @@
 // instructions (closest-object test, tracking step, HG resampling, transmittance set-up, bookkeeping)
 // and walks have geometric length.  One-ray-per-lane designs leave most lanes of a warp idle on each
 // issued instruction.  Here every LANE owns kSlots = 3 rays, parked in shared memory (34 words each,
-// word-major so that lane l only ever touches bank l: conflict-free, no inter-lane hand-over) and tagged,
+// word-major so that lane l only ever touches bank l, or in 16-byte groups: conflict-free, no inter-lane hand-over) and tagged,
 // in registers, with the operation they wait for:
 //
 //     OP_STEP     one unified tracking step (delta / residual-ratio / emission walk)
@@ -226,6 +226,87 @@ VPT_DEV void store_walk(const PV& pv, int s, const PathState& st)
     pv.u(30, s) = (st.packed & ~kExitMask) | ((uint32_t)st.exit_reason << 6);
 }
 
+// The headline kernels (lean, 3 rays per lane) park the same 34 words in eight 16-byte groups and one 8-byte group, each moved by one
+// 128-bit / 64-bit shared-memory access (a service round moves 9 groups each way instead of 34 words, a walk swap 4 + 3 groups instead of 16 + 11 words):
+//   G_WPOS {wpos, t}   G_WDIR {wdir, distance}   G_AUX {aux, alpha}   G_WALK {trv, rng.k, lp, packed word}      (the walk's groups)
+//   G_POS {pos, depth}   G_DIR {dir, T_c}   G_L {L, tmin_c}   G_BETA {beta, qslot}   and the 8-byte {rd | vd, light word}
+// Group g of slot j of lane l at vector index (g * kSlots + j) * 32 + l of the warp's pool: a quarter-warp's 128-bit access covers 128
+// contiguous bytes (conflict-free).  The other kernels keep the word-major view above: with 128-bit moves the generic kernel ran slower on
+// the fireball (config 3) and the kernels at 2 rays per lane spilled more.
+enum RayGroup : int { G_WPOS = 0, G_WDIR, G_AUX, G_WALK, G_POS, G_DIR, G_L, G_BETA, kRayGroups4 };
+static_assert(kRayGroups4 * 4 + 2 == kRayWords, "eight 16-byte groups and one 8-byte group per ray");
+template <int kSlots>
+struct PoolGroups {
+    float4* q;                                                   // this warp's 16-byte groups, already offset by the lane
+    float2* h;                                                   // its 8-byte groups, already offset by the lane
+    VPT_DEV float4& g(int group, int slot) const { return q[(group * kSlots + slot) * 32]; }
+    VPT_DEV float2& g2(int slot) const { return h[slot * 32]; }
+};
+VPT_DEV float4 f4(const float3 v, const float w) { return make_float4(v.x, v.y, v.z, w); }
+VPT_DEV float3 xyz(const float4 v) { return f3(v.x, v.y, v.z); }
+
+template <int kSlots>
+VPT_DEV void store_ray(const PoolGroups<kSlots>& pv, int s, const PathState& st)
+{
+    const uint32_t a = (uint32_t)st.phase | ((uint32_t)st.mode << 4) | ((uint32_t)st.exit_reason << 6) | ((uint32_t)st.tr_kind << 9) |
+                       ((uint32_t)st.obj_c << 11) | ((uint32_t)st.mi << 13) | ((uint32_t)st.first_walk << 14) | ((uint32_t)st.have_closest << 15) |
+                       ((uint32_t)st.sphere_bounced << 16) | ((uint32_t)st.sphere_free << 17) | (st.pass << 18);
+    pv.g(G_WPOS, s) = f4(st.wpos, st.t);
+    pv.g(G_WDIR, s) = f4(st.wdir, st.distance);
+    pv.g(G_AUX, s) = f4(st.aux, st.alpha);
+    pv.g(G_WALK, s) = make_float4(st.trv, __uint_as_float(st.rng.k), __uint_as_float(st.lp), __uint_as_float(a));
+    pv.g(G_POS, s) = f4(st.pos, st.depth);
+    pv.g(G_DIR, s) = f4(st.dir, st.T_c);
+    pv.g(G_L, s) = f4(st.L, st.tmin_c);
+    pv.g(G_BETA, s) = f4(st.beta, __uint_as_float(st.qslot));
+    pv.g2(s) = make_float2(__uint_as_float((uint32_t)(st.rd & 0xffff) | ((uint32_t)(st.vd & 0xffff) << 16)),
+                           __uint_as_float((uint32_t)(st.light_budget & 0xff) | ((uint32_t)st.light_index << 8)));
+}
+
+template <int kSlots>
+VPT_DEV void load_ray(const PoolGroups<kSlots>& pv, int s, PathState& st, const FrameArgs& fa)
+{
+    const float4 gwp = pv.g(G_WPOS, s), gwd = pv.g(G_WDIR, s), gax = pv.g(G_AUX, s), gwk = pv.g(G_WALK, s);
+    const float4 gp = pv.g(G_POS, s), gd = pv.g(G_DIR, s), gl = pv.g(G_L, s), gb = pv.g(G_BETA, s);
+    const float2 gc = pv.g2(s);
+    st.pos = xyz(gp);    st.depth = gp.w;    st.dir = xyz(gd);   st.T_c = gd.w;
+    st.L = xyz(gl);      st.tmin_c = gl.w;   st.beta = xyz(gb);  st.qslot = __float_as_uint(gb.w);
+    st.wpos = xyz(gwp);  st.t = gwp.w;       st.wdir = xyz(gwd); st.distance = gwd.w;
+    st.aux = xyz(gax);   st.alpha = gax.w;
+    st.trv = gwk.x;
+    const uint32_t k = __float_as_uint(gwk.y); st.lp = __float_as_uint(gwk.z);
+    const uint32_t a = __float_as_uint(gwk.w), b = __float_as_uint(gc.x), c = __float_as_uint(gc.y);
+    st.phase = a & 15; st.mode = (a >> 4) & 3; st.exit_reason = (a >> 6) & 7; st.tr_kind = (a >> 9) & 3; st.obj_c = (a >> 11) & 3;
+    st.mi = (a >> 13) & 1; st.first_walk = (a >> 14) & 1; st.have_closest = (a >> 15) & 1; st.sphere_bounced = (a >> 16) & 1; st.sphere_free = (a >> 17) & 1; st.pass = a >> 18;
+    st.rd = b & 0xffff; st.vd = b >> 16;
+    st.light_budget = (int)(int8_t)(c & 0xff); st.light_index = c >> 8;
+    st.org = ray_origin(fa, st.qslot);
+    ray_rng_init(st, fa, k);
+}
+
+template <int kSlots>
+VPT_DEV void load_walk(const PoolGroups<kSlots>& pv, int s, PathState& st, const FrameArgs& fa)
+{
+    const float4 gwp = pv.g(G_WPOS, s), gwd = pv.g(G_WDIR, s), gax = pv.g(G_AUX, s), gwk = pv.g(G_WALK, s);
+    st.wpos = xyz(gwp); st.t = gwp.w; st.wdir = xyz(gwd); st.distance = gwd.w;
+    st.aux = xyz(gax);  st.alpha = gax.w;
+    st.trv = gwk.x;
+    const uint32_t k = __float_as_uint(gwk.y); st.lp = __float_as_uint(gwk.z);
+    const uint32_t a = __float_as_uint(gwk.w);
+    st.packed = a;
+    st.mode = (a >> 4) & 3; st.exit_reason = (a >> 6) & 7; st.sphere_free = (a >> 17) & 1; st.pass = a >> 18;
+    ray_rng_init(st, fa, k);
+}
+
+template <int kSlots>
+VPT_DEV void store_walk(const PoolGroups<kSlots>& pv, int s, const PathState& st)
+{
+    pv.g(G_WPOS, s) = f4(st.wpos, st.t);
+    pv.g(G_AUX, s) = f4(st.aux, st.alpha);
+    pv.g(G_WALK, s) = make_float4(st.trv, __uint_as_float(st.rng.k), __uint_as_float(st.lp),
+                                  __uint_as_float((st.packed & ~kExitMask) | ((uint32_t)st.exit_reason << 6)));
+}
+
 // Density of volume 0 from its cell table (vpt_cells_create): the eight corner texels of the cell under the point are 32 contiguous,
 // aligned bytes -- one DRAM sector per look-up instead of the four or five a 2x2x2 footprint costs in the tiled texture array --
 // blended with the texture unit's own arithmetic (vpt_texfilter.cuh).  On the 1024^3 grid DRAM traffic falls to the algorithmic 32 B per
@@ -258,7 +339,8 @@ struct HopStats { uint32_t delta, ratio, emit, ahead; };
 //   alpha update, then OP_FINISH.
 template <bool kLean, bool kCells = false, bool kAhead = false>
 VPT_DEV void walk_step(PathState& st, const FrameShared& fs, const FrameArgs& fa, const TraceConsts& tc, const SphereRec& sph, uint32_t& nlook,
-                       float* beta = nullptr, int beta_stride = 0,   // kLean: the path's throughput in the parked record (x, y, z one stride apart)
+                       float* beta = nullptr, int beta_stride = 0,   // kLean: the path's throughput in the parked record (x, y, z one stride
+                                                                     // apart; stride 1: a 16-byte group of PoolGroups)
                        const EmptyAhead* ea = nullptr, HopStats* hs = nullptr)
 {
     const SceneTables& sc = fs.sc;
@@ -317,9 +399,17 @@ VPT_DEV void walk_step(PathState& st, const FrameShared& fs, const FrameArgs& fa
                 const float3 Cd = fmax3(f3(0.0f), volume_color(fs.vol0, st.wpos));
                 const int index = int(floorf(fminf(fmaxf((density * tc.inv_max * 255.0f / kp.emission_pivot), 0.0f), 255.0f)));
                 const float3 density_color = reinterpret_cast<const float3*>(kp.density_color_texture)[index];
-                float3 b3 = f3(beta[0], beta[beta_stride], beta[2 * beta_stride]);
-                b3 *= (ld3(kp.albedo) * Cd * density_color / ld3(kp.extinction)) * float(kp.energy_inject);
-                beta[0] = b3.x; beta[beta_stride] = b3.y; beta[2 * beta_stride] = b3.z;
+                if (beta_stride == 1) {                             // one 128-bit read-modify-write of the group (qslot rides along)
+                    float4* g = reinterpret_cast<float4*>(beta);
+                    const float4 gb = *g;
+                    float3 b3 = f3(gb.x, gb.y, gb.z);
+                    b3 *= (ld3(kp.albedo) * Cd * density_color / ld3(kp.extinction)) * float(kp.energy_inject);
+                    *g = make_float4(b3.x, b3.y, b3.z, gb.w);
+                } else {
+                    float3 b3 = f3(beta[0], beta[beta_stride], beta[2 * beta_stride]);
+                    b3 *= (ld3(kp.albedo) * Cd * density_color / ld3(kp.extinction)) * float(kp.energy_inject);
+                    beta[0] = b3.x; beta[beta_stride] = b3.y; beta[2 * beta_stride] = b3.z;
+                }
             } else {
                 // instanced / emissive scenes: the per-leaf colour look-ups are deferred to scatter_event() in the service round, where
                 // many rays run them at once instead of one or two lanes of a stepping warp (faster on the fireball)
@@ -627,10 +717,9 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     __shared__ FrameShared fs;
     extern __shared__ float pool_smem[];                         // kTraceWarps x kRayWords x kPool words (opt-in dynamic shared memory)
     __shared__ EmptyAhead ea;
-    load_frame_shared(fs, fa.scene);
-    // the lean kernels end walks at "empty ahead"; the generic ones keep their hot loop as it was (on the fireball, config 3, the extra
-    // code of the shortcut cost more in the fetch-bound loop than its hops saved)
-    if constexpr (kLean) build_empty_ahead(ea, *reinterpret_cast<AheadScratch*>(pool_smem), fs.oct, fa.empty_ahead != 0);   // the ray pool is free until the first refill
+    // the lean kernels end walks at "empty ahead" (the render call's table, staged with the octree); the generic ones keep their hot loop
+    // as it was (on the fireball, config 3, the extra code of the shortcut cost more in the fetch-bound loop than its hops saved)
+    load_frame_shared(fs, fa.scene, kLean ? &ea : nullptr);
     const SceneTables& sc = fs.sc;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned lt_mask = (1u << lane) - 1u;
@@ -639,7 +728,13 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     const SphereRec sph = load_sphere(fa.sphere);
 
     constexpr int kPool = 32 * kSlots;
-    PoolView<kPool> pv; pv.w = pool_smem + (size_t)warp * kRayWords * kPool + lane;
+    constexpr bool kGroups16 = kLean && kSlots == 3;             // the headline kernels park their rays in 16-byte groups
+    typename std::conditional<kGroups16, PoolGroups<kSlots>, PoolView<kPool>>::type pv;
+    float* const pool_warp = pool_smem + (size_t)warp * kRayWords * kPool;   // this warp's kRayWords * kPool words
+    if constexpr (kGroups16) {
+        pv.q = reinterpret_cast<float4*>(pool_warp) + lane;
+        pv.h = reinterpret_cast<float2*>(pool_warp + kRayGroups4 * 4 * kPool) + lane;
+    } else pv.w = pool_warp + lane;
     constexpr int OP_NOSLOT = 15;                                 // third slot disabled when kSlots == 2
     int tag0 = OP_IDLE, tag1 = OP_IDLE, tag2 = (kSlots > 2) ? OP_IDLE : OP_NOSLOT;   // operation each of my rays waits for
 
@@ -734,7 +829,8 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
                     break;
                 }
                 if (cur >= 0) {
-                    walk_step<kLean, kCells, kLean>(st, fs, fa, tc, sph, nlook, &pv.f(9, cur), kPool, &ea, &hs); lane_steps++;
+                    if constexpr (kGroups16) walk_step<kLean, kCells, kLean>(st, fs, fa, tc, sph, nlook, &pv.g(G_BETA, cur).x, 1, &ea, &hs);
+                    else walk_step<kLean, kCells, kLean>(st, fs, fa, tc, sph, nlook, &pv.f(9, cur), kPool, &ea, &hs); lane_steps++;
                     if (st.op != OP_STEP) {                        // walk ended: park the ray with its new tag
                         store_walk(pv, cur, st);
                         if (cur == 0) tag0 = st.op; else if (cur == 1) tag1 = st.op; else tag2 = st.op;

@@ -142,8 +142,7 @@ VPT_DEV float oct_child_exit(const OctInternal& n, int c, float3 o, float3 d) {
 // (the orthant of N's block for the octant of d).  If no populated leaf lies there, the walk only hops over empty nodes until it
 // leaves the root box.  The table holds that answer for every (node, child) pair below the root and every octant: integer-only and
 // conservative, no float margin.
-constexpr int kAheadEntries = 8 + 64 + 512;       // entry of child c of internal node i: i * 8 + c
-struct EmptyAhead { uint8_t bit[kAheadEntries + 8]; };   // bit o of entry e: no populated leaf in the orthant of e's block for octant o
+// (kAheadEntries and EmptyAhead: vpt_scene.cuh)
 struct AheadScratch {
     unsigned long long occ[8];                    // [z] populated leaves, bit y * 8 + x (cell coordinates)
     unsigned long long sfx[8][8];                 // [octant][z] cells whose orthant holds a populated leaf
@@ -157,8 +156,8 @@ VPT_DEV bool empty_ahead(const EmptyAhead& ea, int entry, float3 d) { return (ea
 // upper-side bit of child c on axis a (y is reversed in the child order: bit 1 set means y-minus)
 VPT_DEV int child_upper(int c, int a) { return a == 1 ? ((c >> 1) & 1) ^ 1 : (c >> (a == 0 ? 0 : 2)) & 1; }
 
-// Built by the whole CTA from the staged internal nodes (`oct` must be complete; ends with a barrier).  enable == false leaves every
-// entry 0: the walks then hop exactly as without the table.
+// Built by the whole CTA from the staged internal nodes (`oct` must be complete; ends with a barrier), once per render call by
+// k_empty_ahead.  enable == false leaves every entry 0: the walks then hop exactly as without the table.
 VPT_DEV void build_empty_ahead(EmptyAhead& ea, AheadScratch& s, const OctShared& oct, bool enable)
 {
     const int t = threadIdx.y * blockDim.x + threadIdx.x, nt = blockDim.x * blockDim.y;

@@ -102,7 +102,7 @@ int vpt_create(vpt_context** out) {
     if (prop.major != 9 || prop.minor != 0) { std::string m = "vpt_create: device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ", kernels are built for sm_90a only"; free_context(c); return fail(nullptr, VPT_ERR_UNSUPPORTED, m); }
     c->num_sms = prop.multiProcessorCount;
     c->l2_bytes = (size_t)prop.l2CacheSize;
-    VPT_CREATE(cudaMalloc(&c->d_scene, sizeof(vpt::SceneTables)));
+    VPT_CREATE(cudaMalloc(&c->d_scene, sizeof(vpt::SceneAlloc)));      // the tables, then the render call's empty-ahead table
     VPT_CREATE(cudaMalloc(&c->d_counters, sizeof(unsigned) * 4));
     VPT_CREATE(cudaMalloc(&c->d_stats, sizeof(unsigned long long) * 16));
     VPT_CREATE(cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 16));
@@ -586,6 +586,9 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
             c->launches++;
             c->cached_volumes = d_volumes; c->cached_root = d_root; c->cached_generation = registered ? ent.generation : 0ull;
         }
+        // the call's empty-ahead table (option "empty_ahead"), from the octree just refreshed: k_generate and the lean k_trace stage it
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_empty_ahead(c->d_scene, c->empty_ahead, stream); }));
+        c->launches++;
     }
     if (c->brick_pool || c->cell_table) {
         // brick / cell mode read volume 0 from their own copy of the grid: only the lean case of the direct integrator is built for them
@@ -705,7 +708,6 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     if (ctas_per_sm < 1) ctas_per_sm = 1;
 
     fa.counters = c->count_stats ? c->d_stats : nullptr;
-    fa.empty_ahead = c->empty_ahead;
     fa.cell_table = c->cell_table; fa.cell_nx = c->cell_dims[0]; fa.cell_ny = c->cell_dims[1]; fa.cell_nz = c->cell_dims[2];
     const unsigned long long frame_px = (unsigned long long)kp.resolution.x * kp.resolution.y;
     plan.trace = trace; plan.trace_ctas = c->num_sms * ctas_per_sm;
@@ -1088,6 +1090,14 @@ int vpt_get_hop_counters(vpt_context* c, unsigned long long out[8], int reset) {
     VPT_CUDA(c, cudaDeviceSynchronize());
     VPT_CUDA(c, cudaMemcpy(out, c->d_stats + 8, sizeof(unsigned long long) * 8, cudaMemcpyDeviceToHost));
     if (reset) VPT_CUDA(c, cudaMemset(c->d_stats + 8, 0, sizeof(unsigned long long) * 8));
+    return VPT_OK;
+}
+
+int vpt_debug_empty_ahead(vpt_context* c, unsigned char out[VPT_EMPTY_AHEAD_BYTES]) {
+    static_assert(sizeof(vpt::EmptyAhead) == VPT_EMPTY_AHEAD_BYTES, "vpt_b200.h states the table's size");
+    if (!c || !out) return VPT_ERR_INVALID;
+    VPT_CUDA(c, cudaDeviceSynchronize());
+    VPT_CUDA(c, cudaMemcpy(out, &reinterpret_cast<const vpt::SceneAlloc*>(c->d_scene)->ahead, VPT_EMPTY_AHEAD_BYTES, cudaMemcpyDeviceToHost));
     return VPT_OK;
 }
 

@@ -380,6 +380,12 @@ class Renderer:
         return dict(hops_delta=v[0], hops_ratio=v[1], hops_emission=v[2], walks_ended_ahead=v[3],
                     prestep_rays=v[4], prestep_hops=v[5], prestep_ended_ahead=v[6])
 
+    def empty_ahead_table(self):
+        """The last render call's "empty ahead" table: 592 bytes, entry 8 * node + child of the 73 internal nodes, then 8 zero bytes."""
+        out = (C.c_uint8 * 592)()
+        check(lib.vpt_debug_empty_ahead(self.ctx, out), self.ctx, "vpt_debug_empty_ahead")
+        return bytes(out)
+
     def kernel_times(self):
         ms = (C.c_float * 4)(); n = (C.c_int * 4)()
         check(lib.vpt_get_kernel_times(self.ctx, ms, n), self.ctx, "vpt_get_kernel_times")
