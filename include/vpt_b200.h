@@ -49,8 +49,9 @@ int  vpt_abi_sizes(size_t* out, int n);
  * "gather_async" (see vpt_comm_*),
  * "sched_min_lanes" (1..32, lanes an operation must gather in a warp before it pre-empts stepping; 0 = by kernel, the default: 26 for the
  * lean kernel at 3 rays per lane, else 20),
- * "trace_slots" (rays per lane of the trace kernel: 0 = by scene, the default -- 2 when the density grid is larger than twice the L2 or
- * the scene has 64 or more instances, else 3; 2 or 3 to force it),
+ * "trace_slots" (rays per lane of the trace kernel: 0 = by scene, the default -- 2 for a frame with one volume, no emission and no point
+ * lights under the direct integrator, or when the density grid is larger than twice the L2 or the scene has 64 or more instances, else 3;
+ * 2 or 3 to force it),
  * "l2_sector_fetch" (0|1: while a cell table is set, ask the L2 for 32-byte DRAM fetches -- a device-wide hint, see vpt_set_cell_volume),
  * "ctas_per_sm" (0 = occupancy maximum), "generic_kernel" (1: never pick the lean instantiation), "debug_flags" (development),
  * "miss_cull" (1, the default: a pinhole HDRI frame first marks the pixels whose every jitter misses the volume's root box and the sphere,

@@ -690,13 +690,14 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         fa.miss_mask = c->d_miss_mask;
     }
 
-    // rays per lane: 3 by default; 2 (one more CTA per SM) when a look-up is a chain of cache misses -- a density grid that cannot live
-    // in L2 (every look-up a DRAM round trip) or long per-leaf instance lists (dependent loads): warps in flight then matter more than
-    // rays per warp; the L2-resident scenes lose with it (DESIGN.md section 4).
+    // rays per lane: 3 by default; 2 (one more CTA per SM) when warps in flight matter more than rays per warp -- a lean frame, whose
+    // stepping loop is bound by the latency of its look-ups even when they hit L2, or a look-up that is a chain of cache misses: a density
+    // grid that cannot live in L2 (every look-up a DRAM round trip) or long per-leaf instance lists (dependent loads) (DESIGN.md section 4).
     int slots = 3;
     if (c->cell_table) slots = 2;
     else if (!vol_integ && !c->brick_pool) {
         if (c->trace_slots) slots = c->trace_slots;
+        else if (lean) slots = 2;
         else {
             vpt::SceneEntry ent;
             if (vpt::scene_registry_find(d_root, &ent) && (ent.max_grid_bytes > 2ull * c->l2_bytes || ent.n >= 64)) slots = 2;

@@ -27,7 +27,7 @@ struct vpt_context {
     int    max_ctas[vpt::kTraceKernelsAll] = {};   // trace kernel occupancy (CTAs per SM), by vpt::TraceKernel
     size_t l2_fetch_default = 0; int l2_sector_fetch = 0;     // option "l2_sector_fetch" (cell mode)
     const float4* cell_table = nullptr; int cell_dims[3] = {0, 0, 0};   // vpt_set_cell_volume
-    int    trace_slots = 0;              // option "trace_slots": rays per lane of k_trace, 0 = by grid size (2 when the grid is larger than twice the L2)
+    int    trace_slots = 0;              // option "trace_slots": rays per lane of k_trace, 0 = by scene (2 for lean frames, grids larger than twice the L2, >= 64 instances)
     size_t l2_bytes = 0;
     const float* brick_pool = nullptr; int brick_dims[3] = {0, 0, 0};   // fast mode: density of volume 0 as a brick pool (vpt_set_brick_volume)
     int    force_generic = 0;        // option "generic_kernel": 1 = never use the lean trace instantiation (A/B and tests)
