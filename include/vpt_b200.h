@@ -521,6 +521,34 @@ int  vpt_denoise(vpt_context* ctx, unsigned width, unsigned height,
                  unsigned* d_out_display,         /* [H][W] BGRA words as k_resolve writes them, may be NULL */
                  void* stream);
 
+/* vpt_denoise_layers denoises the beauty exactly as vpt_denoise does and filters further layers (the compositing AOVs, light groups, deep
+ * slices, mattes, or any other full-frame planes) with the beauty's weights, so additive identities between the layers and the beauty
+ * (volume + (1 - alpha) k, the sum of the light groups, the sum of the deep slices) still hold after denoising, up to rounding.
+ *   Beauty.  d_out_f3 and d_out_display are vpt_denoise's outputs for the same arguments, bit for bit; n_layers == 0 is vpt_denoise.
+ *   Layers.  Each channel x of each plane of each layer is filtered at every level with the beauty's weights of that level:
+ *     x' = sum(h w x_q) / sum(h w), the same taps, the same h w, in the same order, with the same copy rule.  A pixel the beauty copies
+ *     (non-finite colour or luminance, or g == 0) keeps its layer values bit for bit at that level; a tap the beauty drops is dropped for
+ *     every layer.  A layer carries no variance of its own and does not guide.  A non-finite layer value in a tap that is used spreads to
+ *     the pixels that use it, like any other value.  A layer equal to the beauty's colour comes out equal to d_out_f3, bit for bit.
+ *   Contract.  As vpt_denoise's, and: a layer's dst may EQUAL its src (in place); any partial overlap of a dst with its own src, and any
+ *     overlap of a dst with another layer's src or dst, d_color_f3, d_out_f3, d_out_display, d_depth or d_rel_error, is refused.  A
+ *     layer's src may be any of the beauty's inputs (d_color_f3 passed as a layer gives the beauty's output).  The layer scratch (two sets
+ *     of 16 B per plane and pixel, 32 B * sum(count) per pixel, on top of vpt_denoise's 48 B) belongs to the context, is allocated on
+ *     first use and only grows.
+ *   Refused (VPT_ERR_INVALID, nothing enqueued): everything vpt_denoise refuses; n_layers > 0 with a NULL layers; a NULL src or dst;
+ *     channels outside 1..4; count 0; the overlaps above. */
+typedef struct vpt_denoise_layer {
+    const float* src;       /* [count][H][W][channels] float, full row-major frames in device memory */
+    float*       dst;       /* same shape; may EQUAL src (in place), no other overlap */
+    unsigned     channels;  /* 1..4 */
+    unsigned     count;     /* >= 1 planes of H*W pixels (K for deep slices / mattes, 1 otherwise) */
+} vpt_denoise_layer;
+int  vpt_denoise_layers(vpt_context* ctx, unsigned width, unsigned height,
+                        const float* d_color_f3, const float* d_depth, const float* d_rel_error,
+                        const vpt_denoise_options* opt, float exposure_scale,
+                        float* d_out_f3, unsigned* d_out_display,
+                        const vpt_denoise_layer* layers, unsigned n_layers, void* stream);
+
 /* The flattened scene tables are cached per (volumes pointer, octree root pointer, build generation of a vpt_octree_build
  * octree) and refreshed whenever a call arrives with Kernel_params.iteration == 0 (the reference application resets the
  * iteration on every scene edit, main.cpp:1667-1780).  Call this only if the GPU_VDB[] array or a foreign octree was

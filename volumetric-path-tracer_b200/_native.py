@@ -159,7 +159,7 @@ EXPORTED_SYMBOLS = [
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
     "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
-    "vpt_denoise_options_defaults", "vpt_denoise",
+    "vpt_denoise_options_defaults", "vpt_denoise", "vpt_denoise_layers",
     "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
     "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
     "vpt_set_deep_buffers", "vpt_set_camera_motion", "vpt_debug_motion_cameras",
@@ -224,6 +224,15 @@ class denoise_options(C.Structure):
 lib.vpt_denoise_options_defaults.argtypes = [C.POINTER(denoise_options)]; lib.vpt_denoise_options_defaults.restype = None
 lib.vpt_denoise.argtypes = [_vp, C.c_uint, C.c_uint, _vp, _vp, _vp, C.POINTER(denoise_options), C.c_float, _vp, _vp, _vp]
 lib.vpt_denoise.restype = C.c_int
+
+
+class denoise_layer(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("channels", C.c_uint), ("count", C.c_uint)]
+
+
+lib.vpt_denoise_layers.argtypes = [_vp, C.c_uint, C.c_uint, _vp, _vp, _vp, C.POINTER(denoise_options), C.c_float, _vp, _vp,
+                                   C.POINTER(denoise_layer), C.c_uint, _vp]
+lib.vpt_denoise_layers.restype = C.c_int
 lib.vpt_get_stats.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.POINTER(C.c_uint)]; lib.vpt_get_stats.restype = C.c_int
 lib.vpt_get_counters.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.c_int]; lib.vpt_get_counters.restype = C.c_int
 lib.vpt_get_hop_counters.argtypes = [_vp, C.POINTER(C.c_ulonglong), C.c_int]; lib.vpt_get_hop_counters.restype = C.c_int

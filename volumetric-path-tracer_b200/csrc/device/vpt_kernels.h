@@ -310,6 +310,13 @@ cudaError_t launch_adapt_publish(const FrameGeom& g, const vpt_kernel_params& kp
 
 // Denoiser (vpt_denoise, csrc/device/vpt_denoise.cu): k_denoise_prep fills plane pair 0, then one k_denoise_atrous per level ping-pongs
 // the pairs; the last level reads the planes only and writes out_f3 / out_display, so out_f3 may be the colour input itself.
+// vpt_denoise_layers adds layers: k_denoise_layer_gather copies each into its float4 planes of lp[0] (in order, count planes each) before
+// the first level, and after each k_denoise_atrous the planes take the same level, the last one scattering into each layer's dst.
+struct DenoiseLayer {
+    const float* src;                    // [count][H][W][channels]
+    float*       dst;                    // same shape, may equal src
+    unsigned     channels, count;        // 1..4, >= 1
+};
 struct DenoiseArgs {
     int          width, height, iterations;
     float        sigma_l, sigma_z, exposure_scale;
@@ -320,7 +327,12 @@ struct DenoiseArgs {
     unsigned*    out_display;            // [H][W], may be null
     float4*      cv[2];                  // scratch planes {r, g, b, v}, width * height each
     float2*      yz[2];                  // scratch planes {Y, z}
+    const DenoiseLayer* layers = nullptr; // host array of n_layers
+    int          n_layers = 0;
+    float4*      lp[2] = {};             // layer scratch planes, sum of the counts * width * height each
 };
+// launches of the layer planes per level: groups of 8, 4, 2 or 1 planes
+inline int denoise_layer_groups(size_t n_planes) { return (int)(n_planes / 8) + __builtin_popcountll(n_planes % 8); }
 cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t s);
 
 } // namespace vpt

@@ -81,7 +81,7 @@ static void free_context(vpt_context* c) {
     cudaFree(c->d_counters); cudaFree(c->d_queue); cudaFree(c->d_planeA); cudaFree(c->d_planeB); cudaFree(c->d_planeC); cudaFree(c->d_planeD);
     cudaFree(c->d_plane_tr); cudaFree(c->d_lg_planes); cudaFree(c->d_miss_mask); cudaFree(c->d_matte_map); cudaFree(c->d_matte_ids);
     cudaFree(c->d_adapt_stat); cudaFree(c->d_adapt_stopped); cudaFree(c->d_adapt_tiles);
-    cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz);
+    cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz); cudaFree(c->d_dn_layer);
     delete c;
 }
 
@@ -1032,43 +1032,119 @@ void vpt_denoise_options_defaults(vpt_denoise_options* opt) {
     opt->iterations = 5; opt->sigma_luminance = 4.0f; opt->sigma_depth = 0.2f;
 }
 
-// Denoiser: prep + one a-trous launch per level on `stream` (csrc/device/vpt_denoise.cu), no synchronisation.  The scratch planes are the
-// context's; the last level reads only them, which is what makes d_out_f3 == d_color_f3 safe.
-int vpt_denoise(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_depth, const float* d_rel_error,
-                const vpt_denoise_options* opt, float exposure_scale, float* d_out, unsigned* d_out_display, void* stream) {
-    if (!c || !d_color || !d_out) return fail(c, VPT_ERR_INVALID, "vpt_denoise: null context, colour or output");
-    if (width == 0 || height == 0) return fail(c, VPT_ERR_INVALID, "vpt_denoise: width and height must be >= 1");
-    if (width > 65535 || height > 65535) return fail(c, VPT_ERR_INVALID, "vpt_denoise: width and height must be <= 65535");
-    vpt_denoise_options o;
-    vpt_denoise_options_defaults(&o);
-    if (opt) o = *opt;
-    if (o.iterations < 1 || o.iterations > 10) return fail(c, VPT_ERR_INVALID, "vpt_denoise: iterations must be 1..10");
-    if (!(std::isfinite(o.sigma_luminance) && o.sigma_luminance > 0.0f))
-        return fail(c, VPT_ERR_INVALID, "vpt_denoise: sigma_luminance must be finite and > 0");
-    if (!(std::isfinite(o.sigma_depth) && o.sigma_depth > 0.0f)) return fail(c, VPT_ERR_INVALID, "vpt_denoise: sigma_depth must be finite and > 0");
+// The checks of vpt_denoise's arguments, for vpt_denoise and vpt_denoise_layers (`fn` names the caller in the messages): VPT_OK with the
+// options in *o, or the refusal.
+static int denoise_check(vpt_context* c, const char* fn, unsigned width, unsigned height, const float* d_color, const float* d_depth,
+                         const float* d_rel_error, const vpt_denoise_options* opt, float* d_out, unsigned* d_out_display, vpt_denoise_options* o) {
+    const std::string f(fn);
+    if (!c || !d_color || !d_out) return fail(c, VPT_ERR_INVALID, f + ": null context, colour or output");
+    if (width == 0 || height == 0) return fail(c, VPT_ERR_INVALID, f + ": width and height must be >= 1");
+    if (width > 65535 || height > 65535) return fail(c, VPT_ERR_INVALID, f + ": width and height must be <= 65535");
+    vpt_denoise_options_defaults(o);
+    if (opt) *o = *opt;
+    if (o->iterations < 1 || o->iterations > 10) return fail(c, VPT_ERR_INVALID, f + ": iterations must be 1..10");
+    if (!(std::isfinite(o->sigma_luminance) && o->sigma_luminance > 0.0f))
+        return fail(c, VPT_ERR_INVALID, f + ": sigma_luminance must be finite and > 0");
+    if (!(std::isfinite(o->sigma_depth) && o->sigma_depth > 0.0f)) return fail(c, VPT_ERR_INVALID, f + ": sigma_depth must be finite and > 0");
     const size_t px = (size_t)width * height;
     const size_t b3 = 3 * sizeof(float) * px, b1 = sizeof(float) * px;
     if (d_out != d_color && byte_ranges_overlap(d_out, b3, d_color, b3))
-        return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_f3 partially overlaps d_color_f3 (it may only be the very same buffer)");
+        return fail(c, VPT_ERR_INVALID, f + ": d_out_f3 partially overlaps d_color_f3 (it may only be the very same buffer)");
     if (byte_ranges_overlap(d_out, b3, d_depth, b1) || byte_ranges_overlap(d_out, b3, d_rel_error, b1))
-        return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_f3 overlaps d_depth or d_rel_error");
+        return fail(c, VPT_ERR_INVALID, f + ": d_out_f3 overlaps d_depth or d_rel_error");
     if (byte_ranges_overlap(d_out_display, b1, d_color, b3) || byte_ranges_overlap(d_out_display, b1, d_depth, b1) ||
         byte_ranges_overlap(d_out_display, b1, d_rel_error, b1))
-        return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_display overlaps an input");
-    if (byte_ranges_overlap(d_out_display, b1, d_out, b3)) return fail(c, VPT_ERR_INVALID, "vpt_denoise: d_out_display overlaps d_out_f3");
+        return fail(c, VPT_ERR_INVALID, f + ": d_out_display overlaps an input");
+    if (byte_ranges_overlap(d_out_display, b1, d_out, b3)) return fail(c, VPT_ERR_INVALID, f + ": d_out_display overlaps d_out_f3");
+    return VPT_OK;
+}
+
+// The beauty's scratch planes (48 B per pixel) for px pixels, allocated on first use, grown when a larger frame comes.
+static int denoise_scratch(vpt_context* c, size_t px) {
     if (px > c->cap_dn_px) {
         cudaFree(c->d_dn_cv); cudaFree(c->d_dn_yz); c->d_dn_cv = nullptr; c->d_dn_yz = nullptr; c->cap_dn_px = 0;
         VPT_CUDA(c, cudaMalloc(&c->d_dn_cv, 2 * px * sizeof(float4)));
         VPT_CUDA(c, cudaMalloc(&c->d_dn_yz, 2 * px * sizeof(float2)));
         c->cap_dn_px = px;
     }
+    return VPT_OK;
+}
+
+static vpt::DenoiseArgs denoise_args(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_depth,
+                                     const float* d_rel_error, const vpt_denoise_options& o, float exposure_scale, float* d_out,
+                                     unsigned* d_out_display) {
+    const size_t px = (size_t)width * height;
     vpt::DenoiseArgs a;
     a.width = (int)width; a.height = (int)height; a.iterations = (int)o.iterations;
     a.sigma_l = o.sigma_luminance; a.sigma_z = o.sigma_depth; a.exposure_scale = exposure_scale;
     a.color = d_color; a.depth = d_depth; a.rel_error = d_rel_error; a.out_f3 = d_out; a.out_display = d_out_display;
     a.cv[0] = c->d_dn_cv; a.cv[1] = c->d_dn_cv + px; a.yz[0] = c->d_dn_yz; a.yz[1] = c->d_dn_yz + px;
+    return a;
+}
+
+// Denoiser: prep + one a-trous launch per level on `stream` (csrc/device/vpt_denoise.cu), no synchronisation.  The scratch planes are the
+// context's; the last level reads only them, which is what makes d_out_f3 == d_color_f3 safe.
+int vpt_denoise(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_depth, const float* d_rel_error,
+                const vpt_denoise_options* opt, float exposure_scale, float* d_out, unsigned* d_out_display, void* stream) {
+    vpt_denoise_options o;
+    { int rc = denoise_check(c, "vpt_denoise", width, height, d_color, d_depth, d_rel_error, opt, d_out, d_out_display, &o); if (rc != VPT_OK) return rc; }
+    { int rc = denoise_scratch(c, (size_t)width * height); if (rc != VPT_OK) return rc; }
+    const vpt::DenoiseArgs a = denoise_args(c, width, height, d_color, d_depth, d_rel_error, o, exposure_scale, d_out, d_out_display);
     VPT_CUDA(c, vpt::launch_denoise(a, (cudaStream_t)stream));
     c->launches += 1 + o.iterations;
+    return VPT_OK;
+}
+
+// vpt_denoise plus layers filtered with the beauty's weights: the layers are gathered into the context's layer planes (two sets of
+// 16 B per plane and pixel) before the first level, so the last level may write a layer's source or the beauty's colour.
+int vpt_denoise_layers(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_depth, const float* d_rel_error,
+                       const vpt_denoise_options* opt, float exposure_scale, float* d_out, unsigned* d_out_display,
+                       const vpt_denoise_layer* layers, unsigned n_layers, void* stream) {
+    vpt_denoise_options o;
+    { int rc = denoise_check(c, "vpt_denoise_layers", width, height, d_color, d_depth, d_rel_error, opt, d_out, d_out_display, &o); if (rc != VPT_OK) return rc; }
+    if (n_layers > 0 && !layers) return fail(c, VPT_ERR_INVALID, "vpt_denoise_layers: n_layers > 0 with a null layers array");
+    const size_t px = (size_t)width * height;
+    const size_t b3 = 3 * sizeof(float) * px, b1 = sizeof(float) * px;
+    std::vector<vpt::DenoiseLayer> dl(n_layers);
+    size_t n_planes = 0;
+    for (unsigned l = 0; l < n_layers; ++l) {
+        const vpt_denoise_layer& L = layers[l];
+        const std::string at = "vpt_denoise_layers: layer " + std::to_string(l);
+        if (!L.src || !L.dst) return fail(c, VPT_ERR_INVALID, at + " has a null src or dst");
+        if (L.channels < 1 || L.channels > 4) return fail(c, VPT_ERR_INVALID, at + ": channels must be 1..4");
+        if (L.count == 0) return fail(c, VPT_ERR_INVALID, at + ": count must be >= 1");
+        dl[l] = vpt::DenoiseLayer{ L.src, L.dst, L.channels, L.count };
+        n_planes += L.count;
+    }
+    auto bytes = [&](unsigned l) { return (size_t)layers[l].count * layers[l].channels * sizeof(float) * px; };
+    for (unsigned l = 0; l < n_layers; ++l) {
+        const std::string at = "vpt_denoise_layers: layer " + std::to_string(l);
+        const float* dst = layers[l].dst;
+        const size_t n = bytes(l);
+        if (dst != layers[l].src && byte_ranges_overlap(dst, n, layers[l].src, n))
+            return fail(c, VPT_ERR_INVALID, at + ": dst partially overlaps its src (it may only be the very same buffer)");
+        for (unsigned m = 0; m < n_layers; ++m) {
+            if (m == l) continue;
+            if (byte_ranges_overlap(dst, n, layers[m].src, bytes(m)) || byte_ranges_overlap(dst, n, layers[m].dst, bytes(m)))
+                return fail(c, VPT_ERR_INVALID, at + ": dst overlaps the src or dst of layer " + std::to_string(m));
+        }
+        if (byte_ranges_overlap(dst, n, d_color, b3) || byte_ranges_overlap(dst, n, d_out, b3) || byte_ranges_overlap(dst, n, d_out_display, b1))
+            return fail(c, VPT_ERR_INVALID, at + ": dst overlaps d_color_f3, d_out_f3 or d_out_display");
+        if (byte_ranges_overlap(dst, n, d_depth, b1) || byte_ranges_overlap(dst, n, d_rel_error, b1))
+            return fail(c, VPT_ERR_INVALID, at + ": dst overlaps d_depth or d_rel_error");
+    }
+    { int rc = denoise_scratch(c, px); if (rc != VPT_OK) return rc; }
+    const size_t need = n_planes * px;
+    if (need > c->cap_dn_layer) {
+        cudaFree(c->d_dn_layer); c->d_dn_layer = nullptr; c->cap_dn_layer = 0;
+        VPT_CUDA(c, cudaMalloc(&c->d_dn_layer, 2 * need * sizeof(float4)));
+        c->cap_dn_layer = need;
+    }
+    vpt::DenoiseArgs a = denoise_args(c, width, height, d_color, d_depth, d_rel_error, o, exposure_scale, d_out, d_out_display);
+    a.layers = dl.data(); a.n_layers = (int)n_layers;
+    a.lp[0] = c->d_dn_layer; a.lp[1] = c->d_dn_layer + need;
+    VPT_CUDA(c, vpt::launch_denoise(a, (cudaStream_t)stream));
+    c->launches += 1 + o.iterations + n_layers + (unsigned long long)o.iterations * vpt::denoise_layer_groups(n_planes);
     return VPT_OK;
 }
 

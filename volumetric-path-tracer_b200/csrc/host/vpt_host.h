@@ -86,6 +86,9 @@ struct vpt_context {
     float4*   d_dn_cv = nullptr;                                // 2 * cap_dn_px
     float2*   d_dn_yz = nullptr;                                // 2 * cap_dn_px
     size_t    cap_dn_px = 0;
+    // vpt_denoise_layers, allocated on first use and only grown: two sets of float4 layer planes of cap_dn_layer (planes * pixels) each
+    float4*   d_dn_layer = nullptr;
+    size_t    cap_dn_layer = 0;
     // compositing AOVs (vpt_set_aov_buffers): caller-owned [local pixel] float / float3 buffers, either may be null; registered buffers
     // become active at the next render call with iteration == 0, so no running mean ever continues from what they held before
     float*    aov_alpha = nullptr;

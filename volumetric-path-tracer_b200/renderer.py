@@ -153,6 +153,79 @@ class Renderer:
         out = out.view(H, W, 3)
         return (out, words) if display else out
 
+    def denoise_layers(self, layers, color=None, depth=True, rel_error=None, iterations=5, sigma_luminance=4.0, sigma_depth=0.2,
+                       stream=None, display=False):
+        """Renderer.denoise of `color` together with layers filtered by the beauty's own weights (vpt_denoise_layers), so the denoised
+        layers still add up to the denoised frame (DESIGN.md section 8n).  Returns a dict of new tensors: "beauty" (H, W, 3), equal bit
+        for bit to Renderer.denoise with the same arguments, and one entry per layer: "alpha" (H, W); "volume" and each name of
+        LIGHT_GROUPS (H, W, 3); "deep" and "mattes" (K, H, W, 4).
+        layers: an iterable of those names, taken from this renderer's buffers (they must be enabled), or a dict mapping names to
+        full-frame tensors of those shapes (a partitioned renderer must pass a dict, e.g. DistributedRenderer.denoise_layers does).
+        color, depth, rel_error and the options are Renderer.denoise's; display=True adds "display", the (H, W) int32 display words
+        Renderer.denoise(..., display=True) returns."""
+        H, W = self.height, self.width
+        if color is None:
+            if self.n_ranks > 1:
+                raise N.VptError("Renderer.denoise_layers: a partitioned renderer holds no full frame; pass `color` "
+                                 "(e.g. DistributedRenderer.full_accum())")
+            color = self.buffers.accum
+        if depth is True:
+            depth = self.buffers.depth if self.n_ranks == 1 else None
+        elif depth is False:
+            depth = None
+        dev = color.device
+        color = _frame_tensor(color, H * W * 3, "color", dev)
+        depth = _frame_tensor(depth, H * W, "depth", dev)
+        rel_error = _frame_tensor(rel_error, H * W, "rel_error", dev)
+        if isinstance(layers, dict):
+            named = dict(layers)
+        else:
+            named = {name: None for name in layers}
+        srcs = {}
+        for name, t in named.items():
+            if name not in _DENOISE_LAYERS:
+                raise N.VptError(f"Renderer.denoise_layers: unknown layer {name!r} (one of {', '.join(_DENOISE_LAYERS)})")
+            if t is None:
+                if self.n_ranks > 1:
+                    raise N.VptError(f"Renderer.denoise_layers: a partitioned renderer holds no full frame of {name!r}; pass a dict of "
+                                     "full-frame tensors (e.g. DistributedRenderer.denoise_layers)")
+                t = self._layer_buffer(name)
+            k = t.shape[0] if name in ("deep", "mattes") else 1
+            ch = _DENOISE_LAYERS[name]
+            srcs[name] = (_frame_tensor(t, k * H * W * ch, name, dev), ch, k)
+        out = torch.empty(H, W, 3, dtype=torch.float32, device=dev)
+        words = torch.empty(H, W, dtype=torch.int32, device=dev) if display else None
+        res = {"beauty": out, **({"display": words} if display else {})}
+        descs = (N.denoise_layer * max(1, len(srcs)))()
+        for i, (name, (t, ch, k)) in enumerate(srcs.items()):
+            shape = (k, H, W, ch) if name in ("deep", "mattes") else (H, W) if ch == 1 else (H, W, ch)
+            res[name] = torch.empty(shape, dtype=torch.float32, device=dev)
+            descs[i] = N.denoise_layer(t.data_ptr(), res[name].data_ptr(), ch, k)
+        opt = N.denoise_options(int(iterations), float(sigma_luminance), float(sigma_depth))
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        check(lib.vpt_denoise_layers(self.ctx, W, H, ptr(color), ptr(depth), ptr(rel_error), C.byref(opt), float(self.kp.exposure_scale),
+                                     ptr(out), ptr(words), descs, len(srcs), C.c_void_p(stream or 0)), self.ctx, "vpt_denoise_layers")
+        return res
+
+    def _layer_buffer(self, name):
+        """This renderer's own buffer of denoise layer `name`, or VptError when it is not enabled."""
+        b = self.buffers
+        if name in ("alpha", "volume"):
+            if getattr(b, name) is None:
+                raise N.VptError(f"Renderer.denoise_layers: layer {name!r} needs the AOVs (Renderer.enable_aovs())")
+            return getattr(b, name)
+        if name in LIGHT_GROUPS:
+            if b.groups is None:
+                raise N.VptError(f"Renderer.denoise_layers: layer {name!r} needs the light groups (Renderer.enable_light_groups())")
+            return b.groups[name]
+        if name == "deep":
+            if b.deep is None:
+                raise N.VptError("Renderer.denoise_layers: layer 'deep' needs the deep slices (Renderer.enable_deep(bounds))")
+            return b.deep
+        if b.mattes is None:
+            raise N.VptError("Renderer.denoise_layers: layer 'mattes' needs the instance mattes (Renderer.enable_mattes(sets))")
+        return b.mattes
+
     def enable_aovs(self):
         """Allocate and register the compositing AOVs (vpt_set_aov_buffers): buffers.alpha (n,) float32, the running mean of the
         coverage [depth > 0], and buffers.volume (n, 3) float32, the volume's share of accum.  They take over at the next render call with
@@ -418,6 +491,10 @@ def _frame_tensor(t, numel, name, device):
     return t
 
 
+# the layers Renderer.denoise_layers takes by name, and their channels per pixel
+_DENOISE_LAYERS = {"alpha": 1, "volume": 3, **{g: 3 for g in LIGHT_GROUPS}, "deep": 4, "mattes": 4}
+
+
 def _layer_names(layers):
     """The exchange layers asked for, checked against N.LAYER_BITS, in bit order without repeats."""
     unknown = [n for n in layers if n not in N.LAYER_BITS]
@@ -645,16 +722,37 @@ class DistributedRenderer:
         adaptive frame, by its error map.  Returns what Renderer.denoise returns; equal bit for bit to Renderer.denoise of the same frame
         rendered on one context."""
         depth = self.full_depth() if depth else None
-        rel_error = None
-        if self.last_adaptive:
-            if self.world == 1:
-                rel_error = self._err1
-            else:
-                pe = C.c_uint64(0)
-                check(lib.vpt_comm_p2p_adaptive_frame(self.r.ctx, None, C.byref(pe)), self.r.ctx, "vpt_comm_p2p_adaptive_frame")
-                rel_error = torch.as_tensor(_DeviceView(pe.value, (self.r.height, self.r.width), "<f4"), device=self.full.device)
-        return self.r.denoise(color=self.full_accum(), depth=depth if depth is not None else False, rel_error=rel_error, out=out,
+        return self.r.denoise(color=self.full_accum(), depth=depth if depth is not None else False, rel_error=self._rel_error(), out=out,
                               display=display, iterations=iterations, sigma_luminance=sigma_luminance, sigma_depth=sigma_depth, stream=stream)
+
+    def denoise_layers(self, layers, depth=True, iterations=5, sigma_luminance=4.0, sigma_depth=0.2, stream=None, display=False):
+        """Renderer.denoise_layers of this rank's full frame: full_accum() guided by full_depth() (depth=False: no depth term) and, after
+        an adaptive frame, by its error map, with the layers named in `layers` taken from full_alpha(), full_volume(),
+        full_light_group(name), full_deep() and full_mattes().  A layer the exchange does not carry raises VptError.  Returns what
+        Renderer.denoise_layers returns; equal bit for bit to Renderer.denoise_layers of the same frame rendered on one context."""
+        full = {"alpha": self.full_alpha, "volume": self.full_volume, "deep": self.full_deep, "mattes": self.full_mattes}
+        frames = {}
+        for name in layers:
+            if name in LIGHT_GROUPS:
+                frames[name] = self.full_light_group(name)
+            elif name in full:
+                frames[name] = full[name]()
+            else:
+                raise N.VptError(f"DistributedRenderer.denoise_layers: unknown layer {name!r} (one of {', '.join(_DENOISE_LAYERS)})")
+        depth = self.full_depth() if depth else None
+        return self.r.denoise_layers(frames, color=self.full_accum(), depth=depth if depth is not None else False,
+                                     rel_error=self._rel_error(), iterations=iterations, sigma_luminance=sigma_luminance,
+                                     sigma_depth=sigma_depth, stream=stream, display=display)
+
+    def _rel_error(self):
+        """The error map of the last frame when it was adaptive (full frame), else None."""
+        if not self.last_adaptive:
+            return None
+        if self.world == 1:
+            return self._err1
+        pe = C.c_uint64(0)
+        check(lib.vpt_comm_p2p_adaptive_frame(self.r.ctx, None, C.byref(pe)), self.r.ctx, "vpt_comm_p2p_adaptive_frame")
+        return torch.as_tensor(_DeviceView(pe.value, (self.r.height, self.r.width), "<f4"), device=self.full.device)
 
     def _check_binned_count(self, k, exported, what, caller):
         """An exchange that carries a binned layer refuses a render call with another count: refuse it here already."""
