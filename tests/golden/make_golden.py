@@ -9,8 +9,9 @@ entry, SURVEY 8(c)(i)); octree built by the reference builder; environment = the
 `synthetic_env(512, 256)` so that the fixtures need no 13 MB HDRI.
 
 mixed_direct renders scene S1 of tests/mixed_scenes.py (the dragon and three synthetic volumes: a heat grid at its own resolution,
-a colour grid, different majorants) with emission, point lights and the sphere.  `make_golden.py OUT_DIR NAME ...` writes only the
-named fixtures.
+a colour grid, different majorants) with emission, point lights and the sphere.  mixed_params renders the same scene at volume, light and
+phase parameters away from their identity defaults (albedo, extinction, energy_inject, sun and sky colours, sun direction, g), so the
+CPU suite covers them too.  `make_golden.py OUT_DIR NAME ...` writes only the named fixtures.
 """
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -26,20 +27,30 @@ CASES = {
                           lights=[((9.0, 6.0, 2.0), (1.0, 0.8, 0.6), 40.0), ((-2.0, 3.0, 8.0), (0.5, 0.7, 1.0), 25.0)]),
     "mixed_direct":  dict(W=256, H=128, passes=2, kp=dict(ray_depth=3, volume_depth=2, emission_scale=1.0, emission_pivot=1.0),
                           lights=[((9.0, 6.0, 2.0), (1.0, 0.8, 0.6), 40.0), ((-2.0, 3.0, 8.0), (0.5, 0.7, 1.0), 25.0)], scene="S1"),   # = mixed_scenes.LIGHTS
+    "mixed_params":  dict(W=256, H=128, passes=2, kp=dict(ray_depth=3, volume_depth=2, emission_scale=1.0, emission_pivot=1.0,
+                                                          albedo=[0.9, 0.55, 0.3], extinction=[0.8, 1.25, 2.0], energy_inject=1.01234,
+                                                          sun_color=[1.0, 0.55, 0.2], sun_mult=2.5, sky_color=[0.3, 0.6, 1.2], sky_mult=0.7,
+                                                          azimuth=200.0, elevation=15.0, phase_g1=0.9),
+                          lights=[((9.0, 6.0, 2.0), (1.0, 0.8, 0.6), 40.0), ((-2.0, 3.0, 8.0), (0.5, 0.7, 1.0), 25.0)], scene="S1"),
 }
+
+
+def set_params(kp, over):
+    """Kernel_params fields from a fixture's meta; a list is a float3."""
+    for k, v in over.items(): setattr(kp, k, V.f3(*v) if isinstance(v, (list, tuple)) else v)
+    return kp
+
 
 def build(case):
     if case.get("scene") == "S1":
         import mixed_scenes
         scene = mixed_scenes.build_s1(mixed_scenes.Volumes())              # its own point lights and sphere
         kp = V.default_kernel_params(); kp.environment_type = 1; kp.max_interactions = 1000
-        for k, v in case["kp"].items(): setattr(kp, k, v)
-        return scene, kp
+        return scene, set_params(kp, case["kp"])
     vol = V.Volume.load_vdb(V.find_asset("dragon.vdb"))
     scene = V.Scene([vol.instance()], env=synthetic_env(512, 256), lights=case["lights"])
     kp = V.default_kernel_params(); kp.environment_type = 1; kp.max_interactions = 1000
-    for k, v in case["kp"].items(): setattr(kp, k, v)
-    return scene, kp
+    return scene, set_params(kp, case["kp"])
 
 def main():
     if len(sys.argv) < 2: raise SystemExit("usage: make_golden.py OUT_DIR [NAME ...]")

@@ -115,8 +115,12 @@ def _stored_names():
 
 class _Stored(str):
     def __getitem__(self, name):
-        with np.load(os.path.join(GOLDEN_DIR, _stored_names()[f"{self}.{name}"])) as z:
-            return z[f"{self}.{name}"]
+        full = f"{self}.{name}"
+        if full not in _stored_names():                  # stored once under another key (pack: SAME_AS)
+            with np.load(os.path.join(GOLDEN_DIR, _stored_names()[full + SAME_AS])) as z:
+                full = str(z[full + SAME_AS])
+        with np.load(os.path.join(GOLDEN_DIR, _stored_names()[full])) as z:
+            return z[full]
 
 
 def _load(key, digest):
@@ -135,22 +139,33 @@ class _NoLibrary:
         pytest.skip(f"oracle/_ref not built: {name} has no stored output")
 
 
+SAME_AS = "@"
+
+
 def pack(record_dir, out_dir=GOLDEN_DIR, limit=990_000, first=0):
     """Pack the per-array files of a recording run (<key>.<name>.npz) into as few files below 1 MB as the array sizes allow, numbered
-    from pack<first>: a run that recorded only some tests packs them after the existing packs."""
-    files = sorted(os.listdir(record_dir))
+    from pack<first>: a run that recorded only some tests packs them after the existing packs.  An array equal to one packed before it
+    (the blue-noise state after the same number of passes over the same frame size, say) is stored once: the later key holds only the
+    earlier key's name, under <key>.<name>@."""
+    entries, seen = [], {}                               # (array name, array, compressed size)
+    for f in sorted(os.listdir(record_dir)):
+        name, a = f[:-len(".npz")], np.load(os.path.join(record_dir, f))["a"]
+        h = (a.dtype.str, a.shape, hashlib.sha256(a.tobytes()).hexdigest())
+        if h in seen and a.nbytes > 1024:
+            entries.append((name + SAME_AS, np.array(seen[h]), 256))
+        else:
+            seen.setdefault(h, name)
+            entries.append((name, a, os.path.getsize(os.path.join(record_dir, f))))
     os.makedirs(out_dir, exist_ok=True)
     groups, cur, size = [], [], 0
-    for f in files:
-        s = os.path.getsize(os.path.join(record_dir, f))
-        if cur and size + s > limit:
+    for e in entries:
+        if cur and size + e[2] > limit:
             groups.append(cur); cur, size = [], 0
-        cur.append(f); size += s
+        cur.append(e); size += e[2]
     if cur: groups.append(cur)
     for i, g in enumerate(groups):
-        arrays = {f[:-len(".npz")]: np.load(os.path.join(record_dir, f))["a"] for f in g}
         path = os.path.join(out_dir, f"pack{first + i:02d}.npz")
-        np.savez_compressed(path, **arrays)
+        np.savez_compressed(path, **{name: a for name, a, _ in g})
         assert os.path.getsize(path) <= MAX_FILE_BYTES, path
 
 
