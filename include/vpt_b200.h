@@ -138,6 +138,7 @@ int  vpt_comm_p2p_status(vpt_context* ctx, unsigned long long* abandoned_waits);
 #define VPT_LAYER_POINT        0x10u   /* float3: light group point */
 #define VPT_LAYER_EMISSION     0x20u   /* float3: light group emission */
 #define VPT_LAYER_ENVIRONMENT  0x40u   /* float3: light group environment */
+#define VPT_LAYER_MOTION      0x100u   /* float3: the motion vectors (vpt_set_motion_vectors); its plane follows the seven above, 0x80 is unused */
 int  vpt_comm_p2p_export_layers(vpt_context* ctx, int rank, int n_ranks, int stripe_rows, unsigned width, unsigned height, int with_display,
                                 unsigned layers, unsigned char handle_out[VPT_P2P_HANDLE_BYTES]);
 int  vpt_comm_p2p_layer(vpt_context* ctx, unsigned layer, vpt_devptr_t* d_full);
@@ -479,6 +480,37 @@ int  vpt_set_camera_motion(vpt_context* ctx, const vpt_camera* shutter_close);
  * and leaves the blue noise as it is.  VPT_ERR_INVALID when the next call has no camera motion.  vpt_debug_camera_rays refuses such a
  * call (VPT_ERR_UNSUPPORTED): its rays depend on each sample's draw. */
 int  vpt_debug_motion_cameras(vpt_context* ctx, void* const params[VPT_NUM_ARGS], float* d_out);
+
+/* ---- motion vectors: each pixel's screen-space motion of the camera ray's first collision towards a second camera pose --------------
+ * With a vector buffer set, every render call also keeps, per pixel, where the point each sample's camera ray first collided with moves on
+ * the film when the camera goes from the frame's pose A (the Kernel_params camera; the shutter-open pose of a motion frame) to a target pose
+ * B -- the input of a vector blur in post, of retiming and of temporal filtering.
+ *
+ *   Definition.  For each pass a pixel takes, let c = (depth > 0) as for the alpha AOV (a NaN depth counts as false).  If c holds, the
+ *     sample's first collision is P = org + depth * dir, with (org, dir) the sample's camera ray exactly as the generator built it (pinhole:
+ *     the camera origin and normalize(llc + s horizontal + t vertical - origin) at the pass's jitter; thin lens: origin + the lens offset and
+ *     the lens loop's direction; camera motion: the ray of the sample's camera at its shutter draw).  The film projection pi_K(P) of a camera
+ *     K reads only its origin, lower_left_corner, horizontal and vertical: d = P - origin, e = llc - origin, n = cross(horizontal, vertical),
+ *     k = (e . n) / (d . n), q = k d - e, and (s, t) solving q = s horizontal + t vertical (the 2x2 normal equations; the dot-product form
+ *     when horizontal . vertical == 0); pi_K(P) = (s W, t H), the units of the film position (x + jx, y + jy): pixels along the column and
+ *     the buffer's row index.  A thin lens therefore projects through its lens centre.  The sample vector is pi_B(P) - pi_A(P), or (+0, +0)
+ *     when k <= 0 or the result is not finite for A or B (the point is not in front of that camera; the sample still counts as covered).
+ *   Buffer.  Per pixel one float3: the running means of (c vx, c vy, c) in accum's rule and arithmetic (iteration == 0 assigns,
+ *     iteration < max_interactions updates x + (s - x) / (iteration + 1), later passes change nothing), not guarded.  So z is the alpha AOV
+ *     bit for bit, xy / z is the unpremultiplied vector, B == A gives +0 in x and y everywhere, and a miss or a pass that samples nothing
+ *     adds exact zeros.  Caller-owned device memory of vpt_local_pixels() float3 (rank-local order on a partitioned context).
+ *   Activation.  As for the AOVs: a buffer and target set here take over at the next render call whose Kernel_params.iteration is 0; calls
+ *     before that leave the buffer untouched.  A NULL buffer turns the vectors off at once (target is then ignored).  The call copies target.
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active vectors (an adaptive frame's stopped pixels keep theirs; a render
+ *     region writes none outside it).  Every other output is bit for bit what the same call gives without vectors: a kernel of its own reads
+ *     each sample's depth word next to the frame's resolve.  On a partitioned context the buffer is rank-local; the peer-memory exchange
+ *     carries it full-frame to every rank when the block is exported with VPT_LAYER_MOTION.  The NCCL exchange does not carry it.  Level (A)
+ *     has no vectors.
+ *   Refused when set (VPT_ERR_INVALID; the vectors are left as they were): a NULL target with a buffer, a non-finite component of target's
+ *     origin, lower_left_corner, horizontal or vertical.  Refused at render time: VPT_PROJECTION_EQUIRECT and VPT_PROJECTION_ODS
+ *     (VPT_ERR_UNSUPPORTED); a buffer that overlaps accum, depth, cost, raw, display, an AOV, light-group, deep-slice or matte buffer
+ *     (VPT_ERR_INVALID, naming the buffer). */
+int  vpt_set_motion_vectors(vpt_context* ctx, float* d_vectors_f3, const vpt_camera* target);
 
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by

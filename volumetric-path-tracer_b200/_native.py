@@ -166,10 +166,12 @@ EXPORTED_SYMBOLS = [
     "vpt_ods_options_defaults", "vpt_set_projection_ods", "vpt_debug_ods_cameras",
     "vpt_set_instance_mattes",
     "vpt_comm_p2p_export_binned", "vpt_comm_p2p_binned", "vpt_comm_p2p_block_bytes_binned",
+    "vpt_set_motion_vectors",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
 LAYER_BITS = {"depth": 0x01, "alpha": 0x02, "volume": 0x04, "sun": 0x08, "point": 0x10, "emission": 0x20, "environment": 0x40}
+VPT_LAYER_MOTION = 0x100                                            # the motion vectors' exchange plane (after the seven above)
 
 # ---- prototypes ------------------------------------------------------------------------------------
 _vp = C.c_void_p
@@ -335,6 +337,7 @@ lib.vpt_camera_look_at.argtypes = [C.POINTER(camera), C.POINTER(C.c_float), C.PO
 lib.vpt_camera_look_at.restype = None
 lib.vpt_set_camera_motion.argtypes = [_vp, C.POINTER(camera)]; lib.vpt_set_camera_motion.restype = C.c_int
 lib.vpt_debug_motion_cameras.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_motion_cameras.restype = C.c_int
+lib.vpt_set_motion_vectors.argtypes = [_vp, _vp, C.POINTER(camera)]; lib.vpt_set_motion_vectors.restype = C.c_int
 lib.vpt_kernel_params_defaults.argtypes = [C.POINTER(Kernel_params)]; lib.vpt_kernel_params_defaults.restype = None
 
 

@@ -31,6 +31,8 @@
 //                     sample's camera placed between two poses by its shutter draw (motion_camera); k_motion_cameras: vpt_debug_motion_cameras
 //   k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods : omni-directional stereo (vpt_set_projection_ods) -- k_generate with each
 //                     sample's camera on its eye's viewing circle (ods_camera); k_ods_cameras: vpt_debug_ods_cameras, and the ODS camera rays
+//   k_motion_vectors, k_motion_vectors_region, k_motion_vectors_adaptive (and their _motion forms) : motion vectors (vpt_set_motion_vectors)
+//                     -- each sample's first collision projected through the frame camera and a second pose, next to the frame's resolve
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -1182,6 +1184,189 @@ k_resolve_adaptive_ods(const FrameArgs fa, const NoSky atmo, const int n_passes,
     resolve_adaptive_body<0, kAov, kGroups, 2>(fa, atmo, n_passes, ad, nullptr, &od, ext...);
 }
 
+// =====================================================================================================
+// k_motion_vectors: screen-space motion of each sample's first collision towards a second camera pose (DESIGN.md section 8o)
+// =====================================================================================================
+// The film projection pi_K of camera K: d = P - origin, e = lower_left_corner - origin, n = cross(horizontal, vertical), k = e.n / d.n,
+// q = k d - e, and (s, t) with q = s horizontal + t vertical (the 2x2 normal equations; the dot-product form when horizontal . vertical is 0),
+// in the units of camera_b0's (x + jx) / W, (y + jy) / H: (s W, t H).  FilmCam holds what depends on K alone.
+struct FilmCam { float3 o, e, h, v; float en, hh, hv, vv, det; };
+__device__ __forceinline__ FilmCam film_cam(const vpt_f3 origin, const vpt_f3 llc, const vpt_f3 horizontal, const vpt_f3 vertical)
+{
+    FilmCam K;
+    K.o = ld3(origin); K.h = ld3(horizontal); K.v = ld3(vertical);
+    K.e = f3(psub(llc.x, origin.x), psub(llc.y, origin.y), psub(llc.z, origin.z));
+    K.en = dot(K.e, cross(K.h, K.v));
+    K.hh = dot(K.h, K.h); K.hv = dot(K.h, K.v); K.vv = dot(K.v, K.v);
+    K.det = pfma(K.hh, K.vv, -pmul(K.hv, K.hv));
+    return K;
+}
+// pi_K(P) into *st; false when P is not in front of K (k <= 0, NaN) or the result is not finite
+__device__ __forceinline__ bool film_project(const FilmCam& K, const float3 P, const vpt_u2 res, float2* st)
+{
+    const float3 d = f3(psub(P.x, K.o.x), psub(P.y, K.o.y), psub(P.z, K.o.z));
+    const float k = __fdiv_rn(K.en, dot(d, cross(K.h, K.v)));
+    const float3 q = f3(pfma(k, d.x, -K.e.x), pfma(k, d.y, -K.e.y), pfma(k, d.z, -K.e.z));
+    const float qh = dot(q, K.h), qv = dot(q, K.v);
+    float s, t;
+    if (K.hv == 0.0f) { s = __fdiv_rn(qh, K.hh); t = __fdiv_rn(qv, K.vv); }
+    else {
+        s = __fdiv_rn(pfma(K.vv, qh, -pmul(K.hv, qv)), K.det);
+        t = __fdiv_rn(pfma(K.hh, qv, -pmul(K.hv, qh)), K.det);
+    }
+    st->x = pmul(s, (float)res.x); st->y = pmul(t, (float)res.y);
+    return k > 0.0f && isfinite(st->x) && isfinite(st->y);
+}
+
+// The accepted lens point of the rejection loop k_generate runs on the pixel's stream (two draws per trial through vanDerCorput in bases 2
+// and 3): the radical inverses k_generate tabulates, computed by the same operations
+__device__ __forceinline__ float2 lens_disk_point(Rng& rng)
+{
+    float2 p;
+    do {
+        const float a = van_der_corput<2>(rng);
+        const float b = van_der_corput<3>(rng);
+        p = make_float2(pfma(a, 2.0f, -1.0f), pfma(b, 2.0f, -1.0f));
+    } while (pfma(p.x, p.x, pmul(p.y, p.y)) >= 1.0f);
+    return p;
+}
+
+// The camera ray of pixel (x, global row y)'s sample at `iteration`, jitter j, as k_generate (kMotion: k_generate_motion) built it: the
+// pinhole order where k_generate takes it, else the thin-lens order with the loop's lens point (and, under motion, the camera of the shutter
+// draw that follows the loop)
+template <bool kMotion>
+__device__ __forceinline__ void sample_camera_ray(const FrameArgs& fa, const CameraMotion* mo, const int x, const int y, const uint32_t iteration,
+                                                  const float2 j, float3& org, float3& dir)
+{
+    const vpt_camera& cam = fa.cam;
+    const vpt_u2 res = fa.kp.resolution;
+    Rng rng; rng.init((uint32_t)y * (uint32_t)fa.geom.width + (uint32_t)x, iteration, 0u);
+    if constexpr (!kMotion) {
+        const float3 b0 = camera_b0(cam, res, x, y, j.x, j.y);
+        if (pinhole_camera(cam) && b0.x != 0.0f && b0.y != 0.0f && b0.z != 0.0f) { org = ld3(cam.origin); dir = normalize(b0); return; }
+    }
+    const float2 p = lens_disk_point(rng);
+    vpt_camera mc;
+    if constexpr (kMotion) mc = motion_camera(cam, *mo, rng.next());
+    const vpt_camera& pc = kMotion ? mc : cam;
+    const float3 rd = f3(pmul(cam.lens_radius, p.x), pmul(cam.lens_radius, p.y), 0.0f);
+    const float3 offset = f3(pfma(pc.u.x, rd.x, pmul(pc.v.x, rd.y)), pfma(pc.u.y, rd.x, pmul(pc.v.y, rd.y)), pfma(pc.u.z, rd.x, pmul(pc.v.z, rd.y)));
+    const float3 b0 = camera_b0(pc, res, x, y, j.x, j.y);
+    org = f3(padd(pc.origin.x, offset.x), padd(pc.origin.y, offset.y), padd(pc.origin.z, offset.z));
+    dir = normalize(f3(psub(b0.x, offset.x), psub(b0.y, offset.y), psub(b0.z, offset.z)));
+}
+
+// One pixel (local pixel lp, local row lr, global row y) over the chunk's passes.  Reads only each record's depth word (A.w of a compact
+// record, B.w of a wide one; a miss, or a pixel k_miss_cull removed, has none: c = 0), rebuilds the camera ray of the samples with c and keeps
+// the running means in accum's rule and arithmetic, written as the alpha AOV's, so z is alpha bit for bit.
+template <bool kMotion>
+__device__ __forceinline__ void motion_vectors_pixel(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
+                                                     const int sampled, const uint32_t lp, const int lr, const int y)
+{
+    const FrameGeom& g = fa.geom;
+    const vpt_kernel_params& kp = fa.kp;
+    const int x = (int)(lp - (uint32_t)lr * (uint32_t)g.width);
+    const FilmCam A = film_cam(fa.cam.origin, fa.cam.lower_left_corner, fa.cam.horizontal, fa.cam.vertical);
+    const FilmCam B = film_cam(mv.origin, mv.lower_left_corner, mv.horizontal, mv.vertical);
+    float3 m = kp.iteration > 0 ? mv.out[lp] : f3(0.f);
+    const bool records = sampled && !(fa.miss_mask && fa.miss_mask[lp]);
+    const bool compact = !fa.planeB;
+    for (int p = 0; p < n_passes; ++p) {
+        const uint32_t iteration = kp.iteration + (uint32_t)p;
+        float depth = 0.0f;
+        if (records) {
+            const size_t s = (size_t)p * g.n_local + lp;
+            const float4 a = fa.planeA[s];
+            if (__float_as_uint(a.w) != kMissSentinel) depth = compact ? a.w : fa.planeB[s].w;
+        }
+        const bool c = depth > 0.0f;
+        float vx = 0.0f, vy = 0.0f;
+        if (c) {
+            float3 org, dir;
+            const float2 j = __ldg(fa.bn_table + (size_t)p * 65536 + (y % 256) * 256 + x % 256);
+            sample_camera_ray<kMotion>(fa, mo, x, y, iteration, j, org, dir);
+            const float3 P = madd3(org, dir, depth);
+            float2 pa, pb;
+            if (film_project(A, P, kp.resolution, &pa) && film_project(B, P, kp.resolution, &pb)) { vx = psub(pb.x, pa.x); vy = psub(pb.y, pa.y); }
+        }
+        const float as = c ? 1.0f : 0.0f;
+        if (iteration == 0) m = f3(vx, vy, as);
+        else if (iteration < kp.max_interactions) {
+            m.x = m.x + (vx - m.x) / (float)(iteration + 1);
+            m.y = m.y + (vy - m.y) / (float)(iteration + 1);
+            m.z = m.z + (as - m.z) / (float)(iteration + 1);
+        }
+    }
+    mv.out[lp] = m;
+}
+
+// every local pixel of the frame (padding rows are skipped)
+template <bool kMotion>
+__device__ __forceinline__ void motion_vectors_frame(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
+                                                     const int sampled)
+{
+    const FrameGeom& g = fa.geom;
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= (uint32_t)g.n_local) return;
+    const int lr = lp / g.width;
+    const int y = global_row(g, lr);
+    if (y >= g.height) return;
+    motion_vectors_pixel<kMotion>(fa, mv, mo, n_passes, sampled, lp, lr, y);
+}
+
+// R's pixels on this rank, row by row as k_resolve_region walks them
+template <bool kMotion>
+__device__ __forceinline__ void motion_vectors_region(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
+                                                      const int sampled, const RenderRegion& rg)
+{
+    const FrameGeom& g = fa.geom;
+    const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= w * (uint32_t)(rg.lr1 - rg.lr0)) return;
+    const uint32_t r = i / w;
+    const int lr = rg.lr0 + (int)r;
+    const uint32_t lp = (uint32_t)lr * (uint32_t)g.width + (uint32_t)rg.x0 + (i - r * w);
+    motion_vectors_pixel<kMotion>(fa, mv, mo, n_passes, sampled, lp, lr, global_row(g, lr));
+}
+
+// the pixels of the active tiles that have not stopped, as k_resolve_adaptive visits them
+template <bool kMotion>
+__device__ __forceinline__ void motion_vectors_adaptive(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
+                                                        const AdaptArgs& ad)
+{
+    const FrameGeom& g = fa.geom;
+    const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
+    if (!t.inside) return;
+    const uint32_t lp = (uint32_t)t.lr * (uint32_t)g.width + (uint32_t)t.x;
+    if (ad.stopped[lp]) return;
+    motion_vectors_pixel<kMotion>(fa, mv, mo, n_passes, 1, lp, t.lr, global_row(g, t.lr));
+}
+
+__global__ void __launch_bounds__(256)
+k_motion_vectors(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled)
+{ motion_vectors_frame<false>(fa, mv, nullptr, n_passes, sampled); }
+
+__global__ void __launch_bounds__(256)
+k_motion_vectors_region(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled, const RenderRegion rg)
+{ motion_vectors_region<false>(fa, mv, nullptr, n_passes, sampled, rg); }
+
+__global__ void __launch_bounds__(128)
+k_motion_vectors_adaptive(const FrameArgs fa, const MotionVectors mv, const int n_passes, const AdaptArgs ad)
+{ motion_vectors_adaptive<false>(fa, mv, nullptr, n_passes, ad); }
+
+__global__ void __launch_bounds__(256)
+k_motion_vectors_motion(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled, const CameraMotion mo)
+{ motion_vectors_frame<true>(fa, mv, &mo, n_passes, sampled); }
+
+__global__ void __launch_bounds__(256)
+k_motion_vectors_region_motion(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled, const RenderRegion rg,
+                               const CameraMotion mo)
+{ motion_vectors_region<true>(fa, mv, &mo, n_passes, sampled, rg); }
+
+__global__ void __launch_bounds__(128)
+k_motion_vectors_adaptive_motion(const FrameArgs fa, const MotionVectors mv, const int n_passes, const AdaptArgs ad, const CameraMotion mo)
+{ motion_vectors_adaptive<true>(fa, mv, &mo, n_passes, ad); }
+
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
 // clipped at the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A neighbour row this
 // rank owns is read from ad.stat, a row of another rank from `halo` (the local exchange block's full-frame err plane, which k_adapt_halo of
@@ -1835,7 +2020,8 @@ cudaError_t exchange_kernels_preload()
                 k_adapt_init_region, k_adapt_region, k_generate_equirect, k_generate_adaptive_equirect, k_generate_region_equirect,
                 k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish, k_generate_motion, k_generate_adaptive_motion,
                 k_generate_region_motion, k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_miss_cull_ods, k_miss_cull_region_ods,
-                k_binned_publish, k_empty_ahead);
+                k_binned_publish, k_empty_ahead, k_motion_vectors, k_motion_vectors_region, k_motion_vectors_adaptive,
+                k_motion_vectors_motion, k_motion_vectors_region_motion, k_motion_vectors_adaptive_motion);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -1964,6 +2150,28 @@ cudaError_t launch_resolve_adaptive(const FrameArgs& fa, const ResolveKey& key, 
         if (e != cudaSuccess) return e;
     }
     return resolve_adaptive_launch(fa, without_deep(key), atm, n_passes, ad, aov, lg, dp, mt, pj, od, s);
+}
+
+cudaError_t launch_motion_vectors(const FrameArgs& fa, const MotionVectors& mv, int n_passes, int sampled, const RenderRegion* rg,
+                                  const AdaptArgs* ad, const CameraMotion* mo, cudaStream_t s)
+{
+    if (ad) {
+        if (ad->n_tiles <= 0) return cudaSuccess;
+        if (mo) k_motion_vectors_adaptive_motion<<<ad->n_tiles, 128, 0, s>>>(fa, mv, n_passes, *ad, *mo);
+        else k_motion_vectors_adaptive<<<ad->n_tiles, 128, 0, s>>>(fa, mv, n_passes, *ad);
+    } else if (rg) {
+        const long long n = region_pixels(*rg);
+        if (n <= 0) return cudaSuccess;
+        const unsigned blocks = (unsigned)((n + 255) / 256);
+        if (mo) k_motion_vectors_region_motion<<<blocks, 256, 0, s>>>(fa, mv, n_passes, sampled, *rg, *mo);
+        else k_motion_vectors_region<<<blocks, 256, 0, s>>>(fa, mv, n_passes, sampled, *rg);
+    } else {
+        if (fa.geom.n_local <= 0) return cudaSuccess;
+        const unsigned blocks = (unsigned)((fa.geom.n_local + 255) / 256);
+        if (mo) k_motion_vectors_motion<<<blocks, 256, 0, s>>>(fa, mv, n_passes, sampled, *mo);
+        else k_motion_vectors<<<blocks, 256, 0, s>>>(fa, mv, n_passes, sampled);
+    }
+    return cudaGetLastError();
 }
 
 cudaError_t launch_adapt(const FrameGeom& g, const AdaptArgs& ad, const float* halo, cudaStream_t s)

@@ -225,6 +225,16 @@ struct ResolveKey { int sky = 0; bool aov = false, groups = false, deep = false,
 cudaError_t launch_resolve(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                            const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
                            const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
+// Motion vectors (vpt_set_motion_vectors): out[local pixel] = running means of (c vx, c vy, c), c = [depth > 0] of the pass sample and
+// (vx, vy) = pi_B(P) - pi_A(P), P the sample's first collision on its camera ray, pi_K the film position (s W, t H) of camera K, A the frame
+// camera and B the pose below (origin, lower_left_corner, horizontal, vertical: the only fields pi reads).  Kept by k_motion_vectors* in a
+// launch of their own next to the frame's resolve (launch_motion_vectors), so no other kernel's parameter block changes.
+struct MotionVectors { float3* out = nullptr; vpt_f3 origin, lower_left_corner, horizontal, vertical; };
+// one chunk of n_passes passes (sampled 0: passes that sample nothing, every sample c = 0).  rg: the frame's render region (R's pixels only);
+// ad: an adaptive frame (the active tiles, stopped pixels keep their vectors); mo: the frame's camera motion (each sample's camera is
+// motion_camera's at its shutter draw).  At most one of rg and ad.
+cudaError_t launch_motion_vectors(const FrameArgs& fa, const MotionVectors& mv, int n_passes, int sampled, const RenderRegion* rg,
+                                  const AdaptArgs* ad, const CameraMotion* mo, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);

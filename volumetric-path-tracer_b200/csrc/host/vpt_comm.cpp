@@ -108,18 +108,23 @@ int comm_gather_frame(vpt_context* c, const FrameGeom& g, const void* d_local_ac
 // Block layout: header (u64 flag arrays: ready[16] done[16] error[1], adapt[16] at kPeerFlagsAdapt) | float3 accum [H][W] | u32 display
 // [H][W] (exported with display only) | u32 pass counts [H][W] | f32 relative errors [H][W] | u32 active-tile count per rank [16].
 // The last three serve vpt_render_adaptive.  Then, in VPT_LAYER_* bit order, one [H][W] plane of each exported layer (f32 depth and alpha,
-// float3 the others), then the binned layers: deep slices [n_slices][H][W] float4 and mattes [n_mattes][H][W] float4.  Each part starts on
-// a 256-byte boundary.  Sizes and offsets are size_t: K x H x W x 16 passes 32 bits at modest frames.
+// float3 the others), the motion vectors [H][W] float3 (VPT_LAYER_MOTION), then the binned layers: deep slices [n_slices][H][W] float4 and
+// mattes [n_mattes][H][W] float4.  Each part starts on a 256-byte boundary.  Sizes and offsets are size_t: K x H x W x 16 passes 32 bits at modest frames.
 static constexpr size_t kP2pHeader = 512;
 static size_t p2p_round(size_t b) { return (b + 255) & ~(size_t)255; }
 static size_t p2p_accum_bytes(size_t px) { return p2p_round(px * 12); }
 static size_t p2p_plane_bytes(size_t px) { return p2p_round(px * 4); }
 static size_t p2p_tiles_offset(size_t px, bool display) { return kP2pHeader + p2p_accum_bytes(px) + (display ? p2p_plane_bytes(px) : 0) + 2 * p2p_plane_bytes(px); }
 enum BinnedLayer : int { BL_DEEP = 0, BL_MATTES = 1, kBinnedLayers = 2 };
+// The motion-vector plane is not one of k_layers_publish's ExchangeLayer slots (its parameter block stays as it is): its bit lies past them,
+// bit 7 stays unknown, and comm_p2p_layers publishes it with a launch of its own.
+static constexpr unsigned kMotionLayerBit = VPT_LAYER_MOTION;
+static_assert(kMotionLayerBit > (1u << kExchangeLayers), "the motion bit lies past the k_layers_publish layers");
 // the block of a w x h frame; layer_off[l] (may be null) = byte offset of layer l's plane, 0 for a layer not in `layers`; bin_off[b] (may
-// be null) = byte offset of the deep-slice (BL_DEEP) and matte (BL_MATTES) arrays, 0 for a count of 0
+// be null) = byte offset of the deep-slice (BL_DEEP) and matte (BL_MATTES) arrays, 0 for a count of 0; motion_off (may be null) = byte
+// offset of the motion-vector plane, 0 without VPT_LAYER_MOTION
 static size_t p2p_block_layout(size_t w, size_t h, bool display, unsigned layers, unsigned n_slices, unsigned n_mattes,
-                               size_t layer_off[kExchangeLayers], size_t bin_off[kBinnedLayers] = nullptr)
+                               size_t layer_off[kExchangeLayers], size_t bin_off[kBinnedLayers] = nullptr, size_t* motion_off = nullptr)
 {
     const size_t px = w * h;
     size_t end = p2p_tiles_offset(px, display) + sizeof(unsigned) * kPeerFlagStride;
@@ -129,6 +134,8 @@ static size_t p2p_block_layout(size_t w, size_t h, bool display, unsigned layers
         if (layer_off) layer_off[l] = on ? end : 0;
         if (on) end += p2p_round(px * (l < XL_VOLUME ? 4 : 12));
     }
+    if (motion_off) *motion_off = (layers & kMotionLayerBit) ? end : 0;
+    if (layers & kMotionLayerBit) end += p2p_round(px * 12);
     const unsigned bins[kBinnedLayers] = {n_slices, n_mattes};
     for (int b = 0; b < kBinnedLayers; ++b) {
         if (bin_off) bin_off[b] = bins[b] ? end : 0;
@@ -142,7 +149,8 @@ static size_t p2p_count_offset(const vpt_context* c) { return kP2pHeader + p2p_a
 static size_t p2p_err_offset(const vpt_context* c) { return p2p_count_offset(c) + p2p_plane_bytes(c); }
 static size_t p2p_tiles_offset(const vpt_context* c) { return p2p_tiles_offset((size_t)c->p2p_w * c->p2p_h, c->p2p_display); }
 static unsigned long long* p2p_flags(void* block) { return reinterpret_cast<unsigned long long*>(block); }
-static constexpr unsigned kLayerMask = (1u << kExchangeLayers) - 1;
+static constexpr unsigned kPublishedLayers = (1u << kExchangeLayers) - 1;     // the layers k_layers_publish carries
+static constexpr unsigned kLayerMask = kPublishedLayers | kMotionLayerBit;
 // Header slot after the error word: what the block was exported for -- width (bits 0-27), height (28-55), display (56), layers (57-63).
 // Every rank's must equal every other's: a rank exported with more planes would store past the end of its peers' blocks.  28 bits hold
 // any size a partitioned frame can have (at most 65535 per side).
@@ -150,7 +158,7 @@ static constexpr int kP2pLayoutSlot = 2 * kPeerFlagStride + 1;
 static unsigned long long p2p_layout_word(const vpt_context* c)
 {
     return ((unsigned long long)c->p2p_w & 0xfffffffull) | (((unsigned long long)c->p2p_h & 0xfffffffull) << 28) |
-           ((unsigned long long)(c->p2p_display ? 1 : 0) << 56) | ((unsigned long long)c->p2p_layers << 57);
+           ((unsigned long long)(c->p2p_display ? 1 : 0) << 56) | ((unsigned long long)(c->p2p_layers & kPublishedLayers) << 57);
 }
 static std::string hex2(unsigned v) { char b[16]; snprintf(b, sizeof b, "0x%02x", v); return b; }
 static std::string p2p_layout_text(unsigned long long w)
@@ -163,6 +171,9 @@ static std::string p2p_layout_text(unsigned long long w)
 static constexpr int kP2pBinnedSlot = kP2pLayoutSlot + 1;
 static_assert(kP2pBinnedSlot < 3 * kPeerFlagStride, "the binned counts live in an unused slot of the header, before the adapt flags");
 static unsigned long long p2p_binned_word(const vpt_context* c) { return (unsigned long long)c->p2p_slices | ((unsigned long long)c->p2p_mattes << 32); }
+// The slot after the binned counts: the whole layer mask, whose motion bit the layout word has no room for
+static constexpr int kP2pLayersSlot = kP2pBinnedSlot + 1;
+static_assert(kP2pLayersSlot < 3 * kPeerFlagStride, "the layer mask lives in an unused slot of the header, before the adapt flags");
 static std::string p2p_binned_text(unsigned long long w)
 {
     return std::to_string(w & 0xffffffffull) + " deep slices and " + std::to_string(w >> 32) + " mattes";
@@ -173,7 +184,7 @@ static int p2p_check_layouts(vpt_context* c, const char* fn)
     const unsigned long long mine = p2p_layout_word(c), mine_bins = p2p_binned_word(c);
     for (int p = 0; p < c->p2p_n; ++p) {
         if (p == c->rank) continue;
-        unsigned long long w[2] = {0, 0};
+        unsigned long long w[3] = {0, 0, 0};
         VPT_CU(c, cudaMemcpy(w, p2p_flags(c->p2p_peer[p]) + kP2pLayoutSlot, sizeof(w), cudaMemcpyDefault));
         if (w[0] != mine)
             return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block for " + p2p_layout_text(w[0]) +
@@ -183,6 +194,10 @@ static int p2p_check_layouts(vpt_context* c, const char* fn)
             return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block with " + p2p_binned_text(w[1]) +
                                                 ", this rank (" + std::to_string(c->rank) + ") with " + p2p_binned_text(mine_bins) +
                                                 "; every rank must export the same deep-slice and matte counts (vpt_comm_p2p_export_binned)");
+        if (w[2] != c->p2p_layers)
+            return fail_ctx(c, VPT_ERR_INVALID, std::string(fn) + ": rank " + std::to_string(p) + " exported its block with layers " +
+                                                hex2((unsigned)w[2]) + ", this rank (" + std::to_string(c->rank) + ") with " + hex2(c->p2p_layers) +
+                                                "; every rank must export the same layers");
     }
     return VPT_OK;
 }
@@ -221,16 +236,28 @@ int comm_p2p_end(vpt_context* c, cudaStream_t stream) {
     return VPT_OK;
 }
 
-int comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream) {
+int comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream, const float3* motion) {
     if (!c->p2p_on || c->p2p_n < 2 || !c->p2p_layers) return VPT_OK;
-    size_t off[kExchangeLayers];
-    p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, off);
-    LayerPlanes dst;
-    dst.n = c->p2p_n;
-    for (int l = 0; l < kExchangeLayers; ++l)
-        for (int p = 0; off[l] && p < c->p2p_n; ++p) dst.plane[l][p] = reinterpret_cast<float*>(reinterpret_cast<char*>(c->p2p_peer[p]) + off[l]);
-    VPT_CU(c, launch_layers_publish(g, rg, src, dst, stream));
-    c->launches++;
+    size_t off[kExchangeLayers], motion_off = 0;
+    p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, off, nullptr, &motion_off);
+    if (c->p2p_layers & kPublishedLayers) {
+        LayerPlanes dst;
+        dst.n = c->p2p_n;
+        for (int l = 0; l < kExchangeLayers; ++l)
+            for (int p = 0; off[l] && p < c->p2p_n; ++p) dst.plane[l][p] = reinterpret_cast<float*>(reinterpret_cast<char*>(c->p2p_peer[p]) + off[l]);
+        VPT_CU(c, launch_layers_publish(g, rg, src, dst, stream));
+        c->launches++;
+    }
+    if (motion_off && motion) {
+        // k_layers_publish with the motion vectors in the slot of a float3 layer and every other slot empty
+        LayerSources ms;
+        ms.src[XL_VOLUME] = reinterpret_cast<const float*>(motion);
+        LayerPlanes dst;
+        dst.n = c->p2p_n;
+        for (int p = 0; p < c->p2p_n; ++p) dst.plane[XL_VOLUME][p] = reinterpret_cast<float*>(reinterpret_cast<char*>(c->p2p_peer[p]) + motion_off);
+        VPT_CU(c, launch_layers_publish(g, rg, ms, dst, stream));
+        c->launches++;
+    }
     return VPT_OK;
 }
 
@@ -323,8 +350,9 @@ int vpt_comm_p2p_export_binned(vpt_context* c, int rank, int n_ranks, int stripe
     c->p2p_bytes = vpt::p2p_block_layout(width, height, c->p2p_display, layers, n_slices, n_mattes, nullptr);
     VPT_CU(c, cudaMalloc(&c->p2p_block, c->p2p_bytes));
     VPT_CU(c, cudaMemset(c->p2p_block, 0, c->p2p_bytes));
-    const unsigned long long words[2] = {vpt::p2p_layout_word(c), vpt::p2p_binned_word(c)};
-    static_assert(vpt::kP2pBinnedSlot == vpt::kP2pLayoutSlot + 1, "layout word, then the binned counts");
+    const unsigned long long words[3] = {vpt::p2p_layout_word(c), vpt::p2p_binned_word(c), (unsigned long long)layers};
+    static_assert(vpt::kP2pBinnedSlot == vpt::kP2pLayoutSlot + 1 && vpt::kP2pLayersSlot == vpt::kP2pLayoutSlot + 2,
+                  "layout word, then the binned counts, then the layer mask");
     VPT_CU(c, cudaMemcpy(vpt::p2p_flags(c->p2p_block) + vpt::kP2pLayoutSlot, words, sizeof(words), cudaMemcpyHostToDevice));
     VPT_CU(c, cudaDeviceSynchronize());
     cudaIpcMemHandle_t h;
@@ -370,12 +398,13 @@ int vpt_comm_p2p_layer(vpt_context* c, unsigned layer, vpt_devptr_t* d_full) {
     if (!c || !d_full || !c->p2p_block) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: no exchange block");
     int l = 0;
     while (l < vpt::kExchangeLayers && layer != 1u << l) ++l;
-    if (l == vpt::kExchangeLayers) return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: " + std::to_string(layer) + " is not one VPT_LAYER_* bit");
+    if (l == vpt::kExchangeLayers && layer != vpt::kMotionLayerBit)
+        return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: " + std::to_string(layer) + " is not one VPT_LAYER_* bit");
     if (!(c->p2p_layers & layer))
         return vpt::fail_ctx(c, VPT_ERR_INVALID, "vpt_comm_p2p_layer: the block was exported without layer " + std::to_string(layer) + " (vpt_comm_p2p_export_layers)");
-    size_t off[vpt::kExchangeLayers];
-    vpt::p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, off);
-    *d_full = (vpt_devptr_t)(reinterpret_cast<char*>(c->p2p_block) + off[l]);
+    size_t off[vpt::kExchangeLayers], motion_off = 0;
+    vpt::p2p_block_layout((size_t)c->p2p_w, (size_t)c->p2p_h, c->p2p_display, c->p2p_layers, c->p2p_slices, c->p2p_mattes, off, nullptr, &motion_off);
+    *d_full = (vpt_devptr_t)(reinterpret_cast<char*>(c->p2p_block) + (l < vpt::kExchangeLayers ? off[l] : motion_off));
     return VPT_OK;
 }
 

@@ -306,6 +306,25 @@ int vpt_set_camera_motion(vpt_context* c, const vpt_camera* shutter_close) {
     return VPT_OK;
 }
 
+int vpt_set_motion_vectors(vpt_context* c, float* d_vectors_f3, const vpt_camera* target) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_motion_vectors: null context");
+    vpt::MotionVectors m;
+    if (d_vectors_f3) {
+        if (!target) return fail(c, VPT_ERR_INVALID, "vpt_set_motion_vectors: null target camera");
+        const struct { const char* name; vpt_f3 v; } fields[] = {
+            { "origin", target->origin }, { "lower_left_corner", target->lower_left_corner }, { "horizontal", target->horizontal },
+            { "vertical", target->vertical } };
+        for (const auto& f : fields)
+            if (!std::isfinite(f.v.x) || !std::isfinite(f.v.y) || !std::isfinite(f.v.z))
+                return fail(c, VPT_ERR_INVALID, std::string("vpt_set_motion_vectors: target.") + f.name + " is not finite");
+        m.out = reinterpret_cast<float3*>(d_vectors_f3);
+        m.origin = target->origin; m.lower_left_corner = target->lower_left_corner; m.horizontal = target->horizontal; m.vertical = target->vertical;
+    }
+    c->mv_req = m;
+    c->mv_active = false;           // null: off from now on; otherwise buffer and target take over at the next call with iteration == 0
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -381,6 +400,7 @@ struct FramePlan {
     vpt::DeepSlices deep;                 // the active deep slices (out null: off)
     vpt::Mattes mattes;                   // the active instance mattes (out null: off)
     vpt::MatteIds matte_ids;              // their id plane, for the trace kernel
+    vpt::MotionVectors mv;                // the active motion vectors (out null: off)
     bool region = false;                  // a render region is active: the region kernels over rg
     vpt::RenderRegion rg;
     vpt::Projection proj;                 // the frame's projection: the equirectangular kernels when equirect(proj)
@@ -478,6 +498,24 @@ static int check_matte_buffers(vpt_context* c, const vpt_kernel_params& kp, size
     return VPT_OK;
 }
 
+// The motion-vector buffer may not share a byte with a Kernel_params output buffer, an AOV, light-group, deep-slice or matte buffer
+// (n = local pixels).
+static int check_motion_vector_buffer(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    const struct { const char* name; const void* p; size_t bytes; } others[] = {
+        { "Kernel_params.accum_buffer", (const void*)(uintptr_t)kp.accum_buffer, 12 * n }, { "Kernel_params.depth_buffer", (const void*)(uintptr_t)kp.depth_buffer, 4 * n },
+        { "Kernel_params.cost_buffer", (const void*)(uintptr_t)kp.cost_buffer, 12 * n }, { "Kernel_params.raw_buffer", (const void*)(uintptr_t)kp.raw_buffer, 16 * n },
+        { "Kernel_params.display_buffer", (const void*)(uintptr_t)kp.display_buffer, 4 * n },
+        { "the alpha AOV buffer", c->aov_alpha, 4 * n }, { "the volume AOV buffer", c->aov_volume, 12 * n },
+        { "the sun light-group buffer", c->lg_out[0], 12 * n }, { "the point light-group buffer", c->lg_out[1], 12 * n },
+        { "the emission light-group buffer", c->lg_out[2], 12 * n }, { "the environment light-group buffer", c->lg_out[3], 12 * n },
+        { "the deep slice buffer", c->deep_req.out, 16 * n * (size_t)c->deep_req.n },
+        { "the matte buffer", c->matte_req.out, 16 * n * (size_t)c->matte_req.n } };
+    for (const auto& o : others)
+        if (byte_ranges_overlap(c->mv_req.out, 12 * n, o.p, o.bytes))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_motion_vectors: the motion-vector buffer overlaps ") + o.name);
+    return VPT_OK;
+}
+
 // The preamble of a render call of n_passes passes: validation, scene-table refresh, trace-kernel choice, chunk size and scratch buffers.
 static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned n_passes, cudaStream_t stream, FramePlan& plan) {
     vpt::FrameArgs& fa = plan.fa;
@@ -536,6 +574,10 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         if (ods.layout == vpt::kOdsOverUnder && (kp.resolution.y & 1u))
             return fail(c, VPT_ERR_UNSUPPORTED, "the over-under ODS layout needs an even height, got " + std::to_string(kp.resolution.y));
     }
+    // motion vectors: the buffer and target set last take over at a call with iteration == 0 (the rule of the AOVs)
+    const bool vectors = c->mv_active || (kp.iteration == 0 && c->mv_req.out);
+    if (vectors && (vpt::equirect(proj) || vpt::ods(proj)))
+        return fail(c, VPT_ERR_UNSUPPORTED, "motion vectors (vpt_set_motion_vectors) are not supported with the equirectangular or ODS projection");
 
     // ---- scene tables ---------------------------------------------------------------------------------------
     // Octrees built by vpt_octree_build are registered with their flat tables and instance count: nothing is read
@@ -738,6 +780,12 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         plan.deep = c->deep_req;
     }
     plan.resolve.deep = plan.deep.out != nullptr;
+    if (vectors) {
+        int rc = check_motion_vector_buffer(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+        c->mv_active = true;
+        plan.mv = c->mv_req;
+    }
     // instance mattes: the map goes to the device when they take over
     if (mattes) {
         if (!c->matte_active) {
@@ -835,6 +883,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         if (last) { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
+        if (plan.mv.out) {
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_motion_vectors(fa, plan.mv, (int)np, 1, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream); }));
+            c->launches++;
+        }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
             return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
                                                        plan.proj, stream, plan.ods_arg())
@@ -849,6 +901,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
         vpt::PeerFrames peers;
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
+        if (plan.mv.out) {
+            VPT_CUDA(c, vpt::launch_motion_vectors(fa, plan.mv, (int)(n_passes - n_sampled), 0, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream));
+            c->launches++;
+        }
         if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
                                                            plan.proj, stream, plan.ods_arg()));
         else VPT_CUDA(c, vpt::launch_resolve(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.mattes, plan.proj, stream, plan.ods_arg()));
@@ -858,7 +914,7 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
     // multi-GPU: the one exchange of the path.  Peer-memory mode: the last resolve above already stored every pixel into every rank's
     // frame, the exported layers follow; publish and wait for the peers.  NCCL mode: all-gather of the rank-local frame into the caller's
     // full-frame buffers.
-    { int rc = vpt::comm_p2p_layers(c, fa.geom, region ? &rg : nullptr, layer_sources(plan), stream); if (rc != VPT_OK) return rc; }
+    { int rc = vpt::comm_p2p_layers(c, fa.geom, region ? &rg : nullptr, layer_sources(plan), stream, plan.mv.out); if (rc != VPT_OK) return rc; }
     { int rc = vpt::comm_p2p_binned(c, fa.geom, region ? &rg : nullptr, plan.deep.out, plan.mattes.out, stream); if (rc != VPT_OK) return rc; }
     { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     if (c->nccl_comm && (c->d_full_accum || c->d_full_display)) {
@@ -980,6 +1036,10 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         if (ad.n_tiles > 0) {
             VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
+            if (plan.mv.out) {
+                VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_motion_vectors(fa, plan.mv, (int)np, 1, nullptr, &ad, plan.motion_arg(), stream); }));
+                c->launches++;
+            }
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.mattes, plan.proj, stream, plan.ods_arg()); }));
             c->launches += 3 + (plan.resolve.deep ? 1 : 0) + (plan.resolve.mattes ? 1 : 0);
         }
@@ -1019,7 +1079,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         { int rc = await_peers(); if (rc != VPT_OK) return rc; }
         VPT_CUDA(c, vpt::launch_adapt_publish(g, fa.kp, ad, peers, stream));
         c->launches++;
-        { int rc = vpt::comm_p2p_layers(c, g, nullptr, layer_sources(plan), stream); if (rc != VPT_OK) return rc; }
+        { int rc = vpt::comm_p2p_layers(c, g, nullptr, layer_sources(plan), stream, plan.mv.out); if (rc != VPT_OK) return rc; }
         { int rc = vpt::comm_p2p_binned(c, g, nullptr, plan.deep.out, plan.mattes.out, stream); if (rc != VPT_OK) return rc; }
         { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }

@@ -129,6 +129,10 @@ struct vpt_context {
     // motion_cur at the next render call with iteration == 0, so a running mean never continues under another pose
     bool      motion_req = false, motion_cur = false;
     vpt::CameraMotion motion_close_req, motion_close_cur;
+    // motion vectors (vpt_set_motion_vectors): a caller-owned [local pixel] float3 buffer and the target pose, checked when set (mv_req.out
+    // null: off) and activated like the AOVs, so a frame in progress keeps the target it started with (setting clears mv_active)
+    vpt::MotionVectors mv_req;
+    bool      mv_active = false;
 };
 
 
@@ -173,7 +177,8 @@ int  comm_p2p_peers(vpt_context* c, cudaStream_t stream, PeerFrames* out);      
 int  comm_p2p_end(vpt_context* c, cudaStream_t stream);                                          // after it: publish, and wait until every peer has published
 // right before comm_p2p_end: the exported layers that src holds into every rank's planes (k_layers_publish); nothing when the exchange is
 // suspended, on one rank or without layers.  rg: the frame's render region, null for the whole frame
-int  comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream);
+int  comm_p2p_layers(vpt_context* c, const FrameGeom& g, const RenderRegion* rg, const LayerSources& src, cudaStream_t stream,
+                     const float3* motion = nullptr);   // motion: the frame's active motion-vector buffer (VPT_LAYER_MOTION), null: none
 // right after comm_p2p_layers: the frame's active deep slices and mattes (null: not active) into every rank's binned arrays
 // (k_binned_publish); nothing when the exchange is suspended, on one rank, or for a layer the block does not carry.  The caller has checked
 // that an active layer's count is the exported one (frame_setup)

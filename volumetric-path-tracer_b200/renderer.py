@@ -25,7 +25,8 @@ class FrameBuffers:
     the compositing AOVs, once Renderer.enable_aovs() has allocated them (None until then); `groups`, the light groups (name -> float3
     tensor, LIGHT_GROUPS order), once Renderer.enable_light_groups() has allocated them (None until then); `deep`, the deep slices
     ((K, n, 4) float32), once Renderer.enable_deep() has allocated them (None until then); `mattes`, the instance mattes ((K, n, 4) float32),
-    once Renderer.enable_mattes() has allocated them (None until then)."""
+    once Renderer.enable_mattes() has allocated them (None until then); `motion`, the motion vectors ((n, 3) float32: the means of c vx,
+    c vy and c), once Renderer.enable_motion_vectors() has allocated them (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -39,9 +40,10 @@ class FrameBuffers:
         self.groups = None
         self.deep = None
         self.mattes = None
+        self.motion = None
 
     def zero_(self):
-        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep, self.mattes,
+        for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep, self.mattes, self.motion,
                   *(self.groups.values() if self.groups else ())):
             if t is not None:
                 t.zero_()
@@ -338,6 +340,27 @@ class Renderer:
             raise N.VptError("Renderer.matte_image: instance mattes are not enabled (Renderer.enable_mattes(sets))")
         return self.buffers.mattes.view(self.buffers.mattes.shape[0], self.n_local // self.width, self.width, 4)
 
+    def enable_motion_vectors(self, target_cam: N.camera):
+        """Allocate and register the motion vectors (vpt_set_motion_vectors): buffers.motion (n, 3) float32 holds per pixel the running
+        means of (c vx, c vy, c), c the coverage [depth > 0] and (vx, vy) the film motion in pixels of each sample's first collision from
+        this renderer's camera to `target_cam` (e.g. the next frame's look_at camera; copied).  They take over at the next render call with
+        kp.iteration == 0 (DESIGN.md section 8o).  A non-finite field of the target raises VptError and leaves the vectors as they were.
+        n is the renderer's local pixel count (rank-local rows on a partitioned renderer)."""
+        motion = torch.zeros(self.n_local, 3, dtype=torch.float32, device=self.buffers.accum.device)
+        check(lib.vpt_set_motion_vectors(self.ctx, C.c_void_p(motion.data_ptr()), C.byref(target_cam)), self.ctx, "vpt_set_motion_vectors")
+        self.buffers.motion = motion
+
+    def disable_motion_vectors(self):
+        """Turn the motion vectors off at once; buffers.motion keeps what it holds."""
+        check(lib.vpt_set_motion_vectors(self.ctx, None, None), self.ctx, "vpt_set_motion_vectors")
+
+    def motion_vector_image(self):
+        """(vectors, coverage): (H, W, 2) float32 unpremultiplied vectors xy / z in pixels (0 where the coverage z is 0) and the (H, W)
+        coverage z, which is the alpha AOV ((local rows, ...) on a partitioned renderer)."""
+        if self.buffers.motion is None:
+            raise N.VptError("Renderer.motion_vector_image: motion vectors are not enabled (Renderer.enable_motion_vectors(target_cam))")
+        return unpremultiply_vectors(self.buffers.motion.view(self.n_local // self.width, self.width, 3))
+
     def set_region(self, x0, y0, x1, y1):
         """Render only the full-frame pixels [x0, x1) x [y0, y1) (vpt_set_render_region) from the next call with kp.iteration == 0 on:
         inside it every buffer gets what a full-frame render gives there, bit for bit; outside it nothing is written, so the display keeps
@@ -491,22 +514,32 @@ def _frame_tensor(t, numel, name, device):
     return t
 
 
+def unpremultiply_vectors(m):
+    """(vectors, coverage) of a (..., 3) motion-vector buffer (c vx, c vy, c): xy / z where z > 0, else 0, and z."""
+    z = m[..., 2]
+    v = torch.where((z > 0).unsqueeze(-1), m[..., :2] / torch.where(z > 0, z, torch.ones_like(z)).unsqueeze(-1), torch.zeros_like(m[..., :2]))
+    return v, z
+
+
+# the layers DistributedRenderer(..., layers=...) takes: the exchange layers of vpt_comm_p2p_export_layers in block order
+_EXCHANGE_LAYERS = {**N.LAYER_BITS, "motion": N.VPT_LAYER_MOTION}
+
 # the layers Renderer.denoise_layers takes by name, and their channels per pixel
 _DENOISE_LAYERS = {"alpha": 1, "volume": 3, **{g: 3 for g in LIGHT_GROUPS}, "deep": 4, "mattes": 4}
 
 
 def _layer_names(layers):
-    """The exchange layers asked for, checked against N.LAYER_BITS, in bit order without repeats."""
-    unknown = [n for n in layers if n not in N.LAYER_BITS]
+    """The exchange layers asked for, checked against _EXCHANGE_LAYERS, in bit order without repeats."""
+    unknown = [n for n in layers if n not in _EXCHANGE_LAYERS]
     if unknown:
-        raise N.VptError(f"DistributedRenderer: unknown layer(s) {', '.join(map(repr, unknown))} (one of {', '.join(N.LAYER_BITS)})")
-    return tuple(n for n in N.LAYER_BITS if n in layers)
+        raise N.VptError(f"DistributedRenderer: unknown layer(s) {', '.join(map(repr, unknown))} (one of {', '.join(_EXCHANGE_LAYERS)})")
+    return tuple(n for n in _EXCHANGE_LAYERS if n in layers)
 
 
 def _layer_mask(names):
     m = 0
     for n in names:
-        m |= N.LAYER_BITS[n]
+        m |= _EXCHANGE_LAYERS[n]
     return m
 
 
@@ -537,9 +570,10 @@ class DistributedRenderer:
     Pixels are independent and every Philox stream is keyed by the GLOBAL pixel index, so the gathered frame is bit-identical to a
     single-GPU render whatever the partition (SURVEY 8(e)).
 
-    layers: names of N.LAYER_BITS -- "depth", "alpha", "volume" and the LIGHT_GROUPS -- that the peer-memory exchange also carries full-frame
-    to every rank (vpt_comm_p2p_export_layers): full_depth(), full_alpha(), full_volume(), full_light_group(name).  The AOVs and groups must
-    be enabled on every rank (enable_aovs(), enable_light_groups()) and take over at the next call with kp.iteration == 0.
+    layers: names of N.LAYER_BITS -- "depth", "alpha", "volume" and the LIGHT_GROUPS -- and "motion" that the peer-memory exchange also
+    carries full-frame to every rank (vpt_comm_p2p_export_layers): full_depth(), full_alpha(), full_volume(), full_light_group(name),
+    full_motion_vectors().  The AOVs, groups and vectors must be enabled on every rank (enable_aovs(), enable_light_groups(),
+    enable_motion_vectors(target)) and take over at the next call with kp.iteration == 0.
 
     deep_slices, n_mattes: the binned layers the peer-memory exchange also carries full-frame (vpt_comm_p2p_export_binned): K deep slices
     (full_deep()) and K mattes (full_mattes()), 0 = not carried.  Every rank enables exactly that many (enable_deep(bounds) with K + 1
@@ -687,16 +721,17 @@ class DistributedRenderer:
         k = 1 if name in ("depth", "alpha") else 3
         if self.world == 1:
             b = self.r.buffers
-            src = b.depth if name == "depth" else getattr(b, name) if name in ("alpha", "volume") else (b.groups or {}).get(name)
+            src = b.depth if name == "depth" else getattr(b, name) if name in ("alpha", "volume", "motion") else (b.groups or {}).get(name)
             if src is None:
-                what = "AOVs are" if name in ("alpha", "volume") else "light groups are"
-                raise N.VptError(f"DistributedRenderer.{caller}: {what} not enabled (enable_aovs() / enable_light_groups())")
+                what = "AOVs are" if name in ("alpha", "volume") else "motion vectors are" if name == "motion" else "light groups are"
+                raise N.VptError(f"DistributedRenderer.{caller}: {what} not enabled (enable_aovs() / enable_light_groups() / "
+                                 "enable_motion_vectors(target))")
             return src.reshape(n_px, k).clone()
         if self.exchange != "p2p":
             raise N.VptError(f"DistributedRenderer.{caller}: the {self.exchange} exchange does not carry layers, they stay rank-local; the "
                              f"peer-memory exchange could not be set up ({getattr(self, 'p2p_error', 'exchange=' + repr(self.exchange))})")
         p = C.c_uint64(0)
-        check(lib.vpt_comm_p2p_layer(self.r.ctx, N.LAYER_BITS[name], C.byref(p)), self.r.ctx, "vpt_comm_p2p_layer")
+        check(lib.vpt_comm_p2p_layer(self.r.ctx, _EXCHANGE_LAYERS[name], C.byref(p)), self.r.ctx, "vpt_comm_p2p_layer")
         return torch.as_tensor(_DeviceView(p.value, (n_px, k), "<f4"), device=self.full.device)
 
     def full_depth(self):
@@ -716,6 +751,18 @@ class DistributedRenderer:
         if name not in LIGHT_GROUPS:
             raise N.VptError(f"DistributedRenderer.full_light_group: unknown light group {name!r} (one of {', '.join(LIGHT_GROUPS)})")
         return self._layer(name, "full_light_group").view(self.r.height, self.r.width, 3)
+
+    def enable_motion_vectors(self, target_cam):
+        """Renderer.enable_motion_vectors on this rank; every rank sets the same target.  With layer "motion" the exchange carries them."""
+        self.r.enable_motion_vectors(target_cam)
+
+    def disable_motion_vectors(self):
+        self.r.disable_motion_vectors()
+
+    def full_motion_vectors(self):
+        """(H, W, 3) float32 motion-vector buffer (c vx, c vy, c) of the whole frame (see full_depth); unpremultiply_vectors() of it gives
+        what Renderer.motion_vector_image() gives on one context."""
+        return self._layer("motion", "full_motion_vectors").view(self.r.height, self.r.width, 3)
 
     def denoise(self, depth=True, out=None, display=False, iterations=5, sigma_luminance=4.0, sigma_depth=0.2, stream=None):
         """Renderer.denoise of this rank's full frame: full_accum() guided by full_depth() (depth=False: no depth term) and, after an
