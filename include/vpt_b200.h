@@ -636,13 +636,19 @@ int  vpt_procedural_fill(float* d_buffer, int dim_x, int dim_y, int dim_z, int n
  * rounded sum.  99.6 % of the fetches are bit-identical to tex3D, the rest one ulp off; rendered frames meet the same
  * per-pixel tolerance as the texture path (tests/test_bricks_gpu.py).  Supported: a vpt_octree_build scene of one volume
  * without colour grid, direct integrator, no emission, no point lights; anything else is refused with VPT_ERR_UNSUPPORTED.
- * d_pool = 0 returns the context to the texture path. */
+ * dim_* must be the dimensions of volume 0's density grid (vdb_info.dim of the scene's octree build): a render whose scene differs
+ * fails with VPT_ERR_INVALID, naming both, and launches nothing.  d_pool = 0 returns the context to the texture path. */
 int  vpt_bricks_create(const float* d_dense, int dim_x, int dim_y, int dim_z, vpt_devptr_t* d_pool_out, unsigned long long* bytes_out);
 int  vpt_bricks_read(vpt_devptr_t d_pool, unsigned long long first_brick, unsigned long long n_bricks, float* h_out);   /* 128 floats per brick */
 /* Diagnostic: the software filter under three weight rules (m = 0 the texture unit's integer corner weights -- the production rule --,
  * 1 per-axis weights truncated to 1/256, 2 per-axis full fp32 fractions), reading the bricks from global memory, against tex3D on n pseudo-random points: out12[m*4 + 0..3] = max |d|, sum |d|,
  * number of bit-identical results, n. */
 int  vpt_debug_sampler_compare(vpt_tex_t tex, vpt_devptr_t d_pool, int dim_x, int dim_y, int dim_z, int n_points, unsigned seed, double out12[12]);
+/* Diagnostic: the production brick and cell samplers (the look-ups of k_trace_brick and of the lean k_trace in cell mode) at n chosen
+ * normalised points, host arrays uvw[n][3] in [0, 1] (anything else is refused) -> out2[n][2] = { brick value, cell value }, on the default
+ * stream.  d_pool (vpt_bricks_create) or d_cells (vpt_cells_create) may be 0, its value is then 0; dim_* are the grid's dimensions.  Bricks
+ * are staged through a per-thread shared-memory slot exactly as in the trace, each thread taking 32 consecutive points. */
+int  vpt_debug_software_sample(vpt_devptr_t d_pool, vpt_devptr_t d_cells, int dim_x, int dim_y, int dim_z, const float* uvw, int n, float* out2);
 int  vpt_bricks_destroy(vpt_devptr_t d_pool);
 int  vpt_set_brick_volume(vpt_context* ctx, vpt_devptr_t d_pool, int dim_x, int dim_y, int dim_z);
 
@@ -652,7 +658,8 @@ int  vpt_set_brick_volume(vpt_context* ctx, vpt_devptr_t d_pool, int dim_x, int 
  * times the memory of the grid (1024^3: 32 GiB -- sized for 180 GB of HBM), and ONE sector per look-up where the 2x2x2
  * footprint costs four or five in the tiled array of the texture path.  vpt_set_cell_volume makes the trace kernel read volume
  * 0 from it (lean instantiation, 2 rays per lane, the texture unit's arithmetic in software as in brick mode: same per-pixel
- * tolerance, tests/test_bricks_gpu.py); same scene restrictions as brick mode; d_cells = 0 returns to the texture path. */
+ * tolerance, tests/test_bricks_gpu.py); same scene restrictions as brick mode, and the same dimension rule: dim_* must be those of
+ * volume 0's density grid or the render fails with VPT_ERR_INVALID and launches nothing; d_cells = 0 returns to the texture path. */
 int  vpt_cells_create(const float* d_dense, int dim_x, int dim_y, int dim_z, vpt_devptr_t* d_cells_out, unsigned long long* bytes_out);
 int  vpt_cells_read(vpt_devptr_t d_cells, unsigned long long first_cell, unsigned long long n_cells, float* h_out);       /* 8 floats per cell */
 int  vpt_cells_destroy(vpt_devptr_t d_cells);

@@ -154,7 +154,7 @@ EXPORTED_SYMBOLS = [
     "vpt_env_tables_create", "vpt_ins_load", "vpt_env_sky_tabulate",
     "vpt_octree_info", "vpt_octree_read_flat", "vpt_bvh_build", "vpt_bvh_read", "vpt_bvh_destroy", "vpt_env_tables_compute",
     "vpt_comm_get_unique_id", "vpt_comm_init", "vpt_comm_set_gather", "vpt_comm_wait", "vpt_comm_info", "vpt_comm_destroy",
-    "vpt_texture_create_3d_from_device", "vpt_procedural_fill", "vpt_bricks_create", "vpt_bricks_destroy", "vpt_set_brick_volume", "vpt_bricks_read", "vpt_debug_sampler_compare", "vpt_atmosphere_options_defaults", "vpt_atmosphere_precompute", "vpt_atmosphere_destroy",
+    "vpt_texture_create_3d_from_device", "vpt_procedural_fill", "vpt_bricks_create", "vpt_bricks_destroy", "vpt_set_brick_volume", "vpt_bricks_read", "vpt_debug_sampler_compare", "vpt_debug_software_sample", "vpt_atmosphere_options_defaults", "vpt_atmosphere_precompute", "vpt_atmosphere_destroy",
     "vpt_texture_read_f4", "vpt_debug_texture_sample",
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
@@ -287,6 +287,8 @@ lib.vpt_bricks_create.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_
 lib.vpt_bricks_read.argtypes = [C.c_uint64, C.c_ulonglong, C.c_ulonglong, C.POINTER(C.c_float)]; lib.vpt_bricks_read.restype = C.c_int
 lib.vpt_debug_sampler_compare.argtypes = [C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint, C.POINTER(C.c_double)]
 lib.vpt_debug_sampler_compare.restype = C.c_int
+lib.vpt_debug_software_sample.argtypes = [C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_float)]
+lib.vpt_debug_software_sample.restype = C.c_int
 lib.vpt_bricks_destroy.argtypes = [C.c_uint64]; lib.vpt_bricks_destroy.restype = C.c_int
 lib.vpt_cells_create.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_ulonglong)]; lib.vpt_cells_create.restype = C.c_int
 lib.vpt_cells_read.argtypes = [C.c_uint64, C.c_ulonglong, C.c_ulonglong, C.POINTER(C.c_float)]; lib.vpt_cells_read.restype = C.c_int

@@ -2030,6 +2030,13 @@ cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, co
     return cudaGetLastError();
 }
 
+cudaError_t launch_software_sample(const float* pool, const float4* cells, const int dims[3], const float* d_uvw, int n, float* d_out2, cudaStream_t s)
+{
+    const int per_block = kSampleThreads * kSamplePointsPerLane;
+    k_software_sample<<<(n + per_block - 1) / per_block, kSampleThreads, (size_t)kSampleThreads * kBrickBytes, s>>>(brick_args(pool, dims), cells, d_uvw, n, d_out2);
+    return cudaGetLastError();
+}
+
 static cudaError_t resolve_launch(const FrameArgs& fa, const ResolveKey& key, const vpt_atmosphere& atm, int n_passes, int sampled, int write_display,
                                   const PeerFrames* peers, const AovBuffers& aov, const LightGroups& lg, const DeepSlices& dp, const Mattes& mt,
                                   const Projection& pj, const OdsParams* od, cudaStream_t s)

@@ -188,6 +188,8 @@ struct MatteIds { uint32_t* id = nullptr; };
 cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const MatteIds& mi,
                          const float* brick_pool, const int brick_dims[3], int n_ctas, cudaStream_t s);
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s);
+// brick_sample / cell_sample at n points d_uvw [n][3] in [0, 1]: d_out2 [n][2] (k_software_sample); pool or cells may be null
+cudaError_t launch_software_sample(const float* pool, const float4* cells, const int dims[3], const float* d_uvw, int n, float* d_out2, cudaStream_t s);
 cudaError_t launch_fill_perlin(float* d_buffer, int dx, int dy, int dz, float scale, int seed, cudaStream_t s);
 cudaError_t launch_build_bricks(const float* d_dense, int dx, int dy, int dz, float* d_bricks, cudaStream_t s);
 cudaError_t launch_build_cells(const float* d_dense, int dx, int dy, int dz, float4* d_cells, cudaStream_t s);

@@ -16,6 +16,8 @@
 //     8-bit-weight emulation agrees with tex3D on ~0.2 % of the fetches, and this rule on 99.997 % of 60 000 probed weight sets)
 //  3. the blend is the exactly-rounded sum of weight * texel (evaluated in double here: 8-bit x 24-bit products are exact): bit-identical to
 //     tex3D<float> on 99.8 % of random fetches of a random-valued texture, within 1 ulp on the rest.
+// tests/test_texfilter_gpu.py holds brick_sample and cell_sample to an exact restatement of this rule (tests/texfilter_ref.py) bit for bit,
+// at the faces, clamp bands, ties and carries of grids from 1x1x1 to 2047 texels on an axis.
 // kWeightMode: 0 = this rule (production), 1 = per-axis weights truncated to 1/256, 2 = full-precision per-axis weights (fp32 blend) --
 // vpt_debug_sampler_compare reports all three against tex3D.
 #ifndef VPT_BRICK_WEIGHT_MODE

@@ -310,15 +310,21 @@ VPT_DEV void store_walk(const PoolGroups<kSlots>& pv, int s, const PathState& st
 // Density of volume 0 from its cell table (vpt_cells_create): the eight corner texels of the cell under the point are 32 contiguous,
 // aligned bytes -- one DRAM sector per look-up instead of the four or five a 2x2x2 footprint costs in the tiled texture array --
 // blended with the texture unit's own arithmetic (vpt_texfilter.cuh).  On the 1024^3 grid DRAM traffic falls to the algorithmic 32 B per
-// look-up (DESIGN.md 3a): an experiment kept as an instrument, not a faster path.
+// look-up (DESIGN.md 3a): an experiment kept as an instrument, not a faster path.  cell_sample: the look-up at a normalised coordinate in a
+// table of dims texels (also vpt_debug_software_sample's); cell_density: at a world point.
+VPT_DEV float cell_sample(const float4* table, int3 dims, float3 uvw)
+{
+    const TexCell q = tex_cell<0>(uvw, dims.x, dims.y, dims.z);
+    const float4* c = table + 2 * (((size_t)q.k * (size_t)dims.y + (size_t)q.j) * (size_t)dims.x + (size_t)q.i);
+    const float4 lo = __ldg(c), hi = __ldg(c + 1);
+    return tex_blend<0>(q, lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w);
+}
+
 VPT_DEV float cell_density(const FrameArgs& fa, const VolumeRec& v, float3 p)
 {
     float3 uvw;
     if (!volume_coord(v, p, uvw)) return .0f;
-    const TexCell q = tex_cell<0>(uvw, fa.cell_nx, fa.cell_ny, fa.cell_nz);
-    const float4* c = fa.cell_table + 2 * (((size_t)q.k * (size_t)fa.cell_ny + (size_t)q.j) * (size_t)fa.cell_nx + (size_t)q.i);
-    const float4 lo = __ldg(c), hi = __ldg(c + 1);
-    return tex_blend<0>(q, lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w);
+    return cell_sample(fa.cell_table, make_int3(fa.cell_nx, fa.cell_ny, fa.cell_nz), uvw);
 }
 
 // ---- OP_STEP -------------------------------------------------------------------------------------------------

@@ -70,10 +70,9 @@ VPT_DEV float brick_blend(const float* brick, const BrickCell& q)
     return tex_blend<kWeightMode>(q, s[0], s[1], s[5], s[6], s[25], s[26], s[30], s[31]);
 }
 
-VPT_DEV float brick_density(const VolumeRec& v, float3 p, const BrickArgs& ba, BrickSlot& bs, uint32_t& nfetch)
+// the look-up at a normalised coordinate: stage the brick under it into the lane's slot unless it is the resident one, then blend
+VPT_DEV float brick_sample(float3 uvw, const BrickArgs& ba, BrickSlot& bs, uint32_t& nfetch)
 {
-    float3 uvw;
-    if (!volume_coord(v, p, uvw)) return 0.0f;
     const BrickCell q = brick_cell<kBrickWeightMode>(uvw, ba);
     const int id = brick_id(q, ba);
     if (id != bs.resident) {
@@ -82,6 +81,13 @@ VPT_DEV float brick_density(const VolumeRec& v, float3 p, const BrickArgs& ba, B
         nfetch++;
     }
     return brick_blend<kBrickWeightMode>(bs.data, q);
+}
+
+VPT_DEV float brick_density(const VolumeRec& v, float3 p, const BrickArgs& ba, BrickSlot& bs, uint32_t& nfetch)
+{
+    float3 uvw;
+    if (!volume_coord(v, p, uvw)) return 0.0f;
+    return brick_sample(uvw, ba, bs, nfetch);
 }
 
 // Diagnostic: software filter (three weight rules, bricks read straight from global memory) against the texture unit on `n`
@@ -117,6 +123,37 @@ __global__ void k_sampler_compare(cudaTextureObject_t tex, const BrickArgs ba, i
             atomicAdd(out + m * 4 + 1, sum[m]);
             atomicAdd(out + m * 4 + 2, (double)same[m]);
         }
+    }
+}
+
+// Diagnostic (vpt_debug_software_sample): the brick and cell samplers of the trace kernels at caller-chosen normalised points in [0, 1]^3.
+// out2[2 p] = brick_sample (pool != 0), out2[2 p + 1] = cell_sample (cells != 0), 0 for the sampler not asked for.  Every thread owns a
+// 512-byte slot and an mbarrier as in k_trace_brick and takes kSamplePointsPerLane CONSECUTIVE points, so a point list whose neighbours
+// alternate between staying in a brick and leaving it runs both sides of the residency test.  64 slots = 32 KB of dynamic shared memory.
+constexpr int kSampleThreads = 64;
+constexpr int kSamplePointsPerLane = 32;
+
+__global__ void __launch_bounds__(kSampleThreads)
+k_software_sample(const BrickArgs ba, const float4* __restrict__ cells, const float* __restrict__ uvw, int n, float* __restrict__ out2)
+{
+    __shared__ __align__(8) unsigned long long bars[kSampleThreads];
+    extern __shared__ __align__(128) float slots[];               // kSampleThreads x 128 floats
+    BrickSlot bs;
+    bs.data = slots + threadIdx.x * kBrickFloats; bs.smem = smem_addr(bs.data);
+    bs.bar = smem_addr(&bars[threadIdx.x]); bs.resident = -1; bs.phase = 0u;
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bs.bar) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+
+    const int3 dims = make_int3(ba.dimx, ba.dimy, ba.dimz);
+    const long long first = ((long long)blockIdx.x * kSampleThreads + threadIdx.x) * kSamplePointsPerLane;
+    const long long last = min(first + kSamplePointsPerLane, (long long)n);
+    uint32_t nfetch = 0;
+    for (long long p = first; p < last; ++p) {
+        const float3 q = f3(uvw[3 * p], uvw[3 * p + 1], uvw[3 * p + 2]);
+        out2[2 * p] = ba.pool ? brick_sample(q, ba, bs, nfetch) : 0.0f;
+        out2[2 * p + 1] = cells ? cell_sample(cells, dims, q) : 0.0f;
     }
 }
 

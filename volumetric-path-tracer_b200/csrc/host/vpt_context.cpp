@@ -579,6 +579,22 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     if (vectors && (vpt::equirect(proj) || vpt::ods(proj)))
         return fail(c, VPT_ERR_UNSUPPORTED, "motion vectors (vpt_set_motion_vectors) are not supported with the equirectangular or ODS projection");
 
+    if (c->brick_pool || c->cell_table) {
+        // brick / cell mode read volume 0 from their own copy of the grid: only the lean case of the direct integrator is built for them,
+        // and that copy must have the dimensions of volume 0's density grid -- the samplers index it with the scene's coordinates
+        vpt::SceneEntry ent;
+        const bool ok = vpt::scene_registry_find(d_root, &ent) && ent.n == 1 && !(ent.any_flags & 1u) && !(kp.emission_scale > 0.0f) &&
+                        fa.lights.num_lights == 0 && kp.integrator == 0 && !c->force_generic;
+        if (!ok) return fail(c, VPT_ERR_UNSUPPORTED, "brick / cell mode needs a vpt_octree_build scene of ONE volume without colour grid, the direct integrator, no emission and no point lights");
+        if (c->brick_pool && c->cell_table) return fail(c, VPT_ERR_INVALID, "brick mode and cell mode are both set");
+        const int* have = c->brick_pool ? c->brick_dims : c->cell_dims;
+        if (have[0] != ent.dim0[0] || have[1] != ent.dim0[1] || have[2] != ent.dim0[2]) {
+            auto dims = [](const int* d) { return std::to_string(d[0]) + "x" + std::to_string(d[1]) + "x" + std::to_string(d[2]); };
+            return fail(c, VPT_ERR_INVALID, std::string(c->brick_pool ? "the brick pool (vpt_set_brick_volume)" : "the cell table (vpt_set_cell_volume)") +
+                                            " was set with dimensions " + dims(have) + ", volume 0's density grid is " + dims(ent.dim0));
+        }
+    }
+
     // ---- scene tables ---------------------------------------------------------------------------------------
     // Octrees built by vpt_octree_build are registered with their flat tables and instance count: nothing is read
     // back and nothing blocks.  A foreign (reference-built, pointer-linked) octree is flattened on the device and
@@ -631,14 +647,6 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         // the call's empty-ahead table (option "empty_ahead"), from the octree just refreshed: k_generate and the lean k_trace stage it
         VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_empty_ahead(c->d_scene, c->empty_ahead, stream); }));
         c->launches++;
-    }
-    if (c->brick_pool || c->cell_table) {
-        // brick / cell mode read volume 0 from their own copy of the grid: only the lean case of the direct integrator is built for them
-        vpt::SceneEntry ent;
-        const bool ok = vpt::scene_registry_find(d_root, &ent) && ent.n == 1 && !(ent.any_flags & 1u) && !(kp.emission_scale > 0.0f) &&
-                        fa.lights.num_lights == 0 && kp.integrator == 0 && !c->force_generic;
-        if (!ok) return fail(c, VPT_ERR_UNSUPPORTED, "brick / cell mode needs a vpt_octree_build scene of ONE volume without colour grid, the direct integrator, no emission and no point lights");
-        if (c->brick_pool && c->cell_table) return fail(c, VPT_ERR_INVALID, "brick mode and cell mode are both set");
     }
     // "lean" = nothing but one volume, sun and environment in play (the headline configuration)
     const bool lean = c->scene_single_volume && !(kp.emission_scale > 0.0f) && fa.lights.num_lights == 0 && kp.integrator == 0 && !c->force_generic;
@@ -1417,6 +1425,26 @@ int vpt_debug_sampler_compare(vpt_tex_t tex, vpt_devptr_t d_pool, int dx, int dy
     cudaFree(d_out);
     if (e != cudaSuccess) return fail(nullptr, VPT_ERR_CUDA, std::string("vpt_debug_sampler_compare: ") + cudaGetErrorString(e));
     for (int m = 0; m < 3; ++m) out12[m * 4 + 3] = (double)n_points;
+    return VPT_OK;
+}
+
+int vpt_debug_software_sample(vpt_devptr_t d_pool, vpt_devptr_t d_cells, int dx, int dy, int dz, const float* uvw, int n, float* out2) {
+    if ((!d_pool && !d_cells) || dx < 1 || dy < 1 || dz < 1 || !uvw || n < 1 || !out2)
+        return fail(nullptr, VPT_ERR_INVALID, "vpt_debug_software_sample: bad arguments");
+    // the samplers' cell arithmetic is defined on [0, 1] (what volume_coord hands them); NaN fails this test too
+    for (size_t i = 0; i < 3 * (size_t)n; ++i)
+        if (!(uvw[i] >= 0.0f && uvw[i] <= 1.0f))
+            return fail(nullptr, VPT_ERR_INVALID, "vpt_debug_software_sample: coordinate " + std::to_string(i) + " is not in [0, 1]");
+    float *d_in = nullptr, *d_out = nullptr;
+    cudaError_t e = cudaMalloc(&d_in, sizeof(float) * 3 * (size_t)n);
+    if (e == cudaSuccess) e = cudaMalloc(&d_out, sizeof(float) * 2 * (size_t)n);
+    if (e == cudaSuccess) e = cudaMemcpy(d_in, uvw, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice);
+    const int dims[3] = { dx, dy, dz };
+    if (e == cudaSuccess) e = vpt::launch_software_sample(reinterpret_cast<const float*>((uintptr_t)d_pool), reinterpret_cast<const float4*>((uintptr_t)d_cells),
+                                                          dims, d_in, n, d_out, 0);
+    if (e == cudaSuccess) e = cudaMemcpy(out2, d_out, sizeof(float) * 2 * (size_t)n, cudaMemcpyDeviceToHost);
+    cudaFree(d_in); cudaFree(d_out);
+    if (e != cudaSuccess) return fail(nullptr, VPT_ERR_CUDA, std::string("vpt_debug_software_sample: ") + cudaGetErrorString(e));
     return VPT_OK;
 }
 

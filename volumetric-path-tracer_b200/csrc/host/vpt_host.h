@@ -165,6 +165,7 @@ struct SceneEntry {
     int          max_leaf_count = 0;
     unsigned     any_flags = 0;              // bit0: some instance has a colour grid, bit1: some instance has an emission grid
     unsigned long long max_grid_bytes = 0;   // density grid of the largest instance (float voxels): picks the trace kernel's rays per lane
+    int          dim0[3] = {0, 0, 0};        // voxels per axis of volume 0's density grid: what a brick pool or cell table must cover
 };
 bool scene_registry_find(vpt_devptr_t d_root, SceneEntry* out);
 

@@ -92,6 +92,7 @@ int vpt_octree_build(const vpt_gpu_vdb* h_volumes, int n, vpt_devptr_t* d_root_o
     ent.root6[0] = root->bbox.pmin.x; ent.root6[1] = root->bbox.pmin.y; ent.root6[2] = root->bbox.pmin.z;
     ent.root6[3] = root->bbox.pmax.x; ent.root6[4] = root->bbox.pmax.y; ent.root6[5] = root->bbox.pmax.z;
     ent.max_extinction = root->max_extinction; ent.min_extinction = root->min_extinction; ent.any_flags = any_flags; ent.max_grid_bytes = max_grid_bytes;
+    ent.dim0[0] = h_volumes[0].vdb_info.dim.x; ent.dim0[1] = h_volumes[0].vdb_info.dim.y; ent.dim0[2] = h_volumes[0].vdb_info.dim.z;
     std::vector<int> counts(585);
     std::vector<vpt::OctInternal> internal(vpt::kOctInternalNodes);
     std::vector<uint2> leaf_list(vpt::kOctLeaves);
