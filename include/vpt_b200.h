@@ -512,6 +512,18 @@ int  vpt_debug_motion_cameras(vpt_context* ctx, void* const params[VPT_NUM_ARGS]
  *     (VPT_ERR_INVALID, naming the buffer). */
 int  vpt_set_motion_vectors(vpt_context* ctx, float* d_vectors_f3, const vpt_camera* target);
 
+/* ---- sample-stream offset: a fresh Philox stream for every frame of a restarted accumulation ----------------------------------------
+ * Pass p of a render call at Kernel_params.iteration = i draws the Philox stream the reference draws at iteration offset + i + p (32-bit
+ * unsigned arithmetic, wrapping as iteration * 4096 does).  Everything else keyed by the iteration keeps the caller's i: the running-mean
+ * arithmetic, the iteration < max_interactions gate and the "iteration 0 assigns" rule.  So a viewer that restarts every frame at
+ * iteration 0 (the reference application does on every camera move) draws new samples each frame when it advances the offset, and a
+ * one-pass frame at iteration 0 and offset k is the progressive render's pass k sample.  Offset 0, the default, is the reference stream.
+ *   Activation.  The offset takes effect at the next render call whose Kernel_params.iteration is 0; a continued frame keeps its own.
+ *   Works with every frame kind: vpt_render_pass(es), vpt_render_adaptive, render regions, both panoramas, camera motion, brick and cell
+ *     mode, both integrators, partitioned contexts and both exchanges; vpt_set_motion_vectors and vpt_debug_motion_cameras follow it.
+ *     Level (A) has none (its ABI is fixed). */
+int  vpt_set_sample_offset(vpt_context* ctx, uint32_t offset);
+
 /* ---- denoising: an edge-avoiding a-trous filter of a finished frame ------------------------------------------------------
  * vpt_denoise filters an HDR float3 frame (accum_buffer, or a full frame of the exchange block) guided by the noise of each pixel and by
  * the depth buffer -- the replacement for the reference application's Denoise button, which runs OIDN in place on accum_buffer.
@@ -580,6 +592,57 @@ int  vpt_denoise_layers(vpt_context* ctx, unsigned width, unsigned height,
                         const vpt_denoise_options* opt, float exposure_scale,
                         float* d_out_f3, unsigned* d_out_display,
                         const vpt_denoise_layer* layers, unsigned n_layers, void* stream);
+
+/* ---- temporal accumulation: a moving camera's frames averaged through the motion vectors ------------------------------------------
+ * vpt_temporal blends the current frame C into the previous output H, carried to each pixel along the pixel's motion towards the
+ * previous camera, so a viewer keeps converging while the camera moves.  For perspective frames (panoramas have no motion vectors).
+ * Per pixel (x, y) of W x H (tests/temporal_ref.py restates it):
+ *   1. Motion.  M = (c vx, c vy, c), the premultiplied vectors of vpt_set_motion_vectors rendered with target = `previous` (B); A is
+ *      `current`, the frame camera (the shutter-open pose of a motion frame).  When M.z < 1 the uncovered share moves like the environment,
+ *      a direction at infinity: d = e_A + s h_A + t v_A with s = (x + 1/2) / W, t = (y + 1/2) / H, e = llc - origin, h = horizontal,
+ *      v = vertical (d = fma(t, v, fma(s, h, e)) per component), and v_env = pi_B(d) - pi_A(d), pi the film projection of
+ *      vpt_set_motion_vectors with d in place of P - origin.  The pixel's motion is v = M.xy + (1 - M.z) v_env (per component
+ *      fma(1 - M.z, v_env, M.xy)); with M.z >= 1 (or NaN) v = M.xy.  So B == A gives v = +0 exactly, as the vectors do.  If the
+ *      projection of d fails for A or B (k <= 0 or a result not finite) while M.z < 1, the pixel has no history.
+ *   2. History.  q = (x + 1/2 + v.x, y + 1/2 + v.y).  No history if v is not finite or q lies outside [0, W] x [0, H].  Otherwise the
+ *      bilinear taps of H around q - 1/2, in the order (x0, y0), (x0 + 1, y0), (x0, y0 + 1), (x0 + 1, y0 + 1): taps outside the frame, of
+ *      weight 0 or with a non-finite colour are dropped, the rest renormalised (sum(w h) / sum(w)); none left: no history.  L_hist is the
+ *      least L among the taps used.  An integer-aligned q reads its one texel bit for bit.
+ *   3. Clip.  mu and sigma are the per-channel mean and population standard deviation of C over the 3x3 window (clipped at the frame
+ *      edge, non-finite neighbours dropped); h' = min(max(h, mu - clip_sigma sigma), mu + clip_sigma sigma).  clip_sigma = +inf skips it.
+ *   4. Blend.  L_new = min(L_hist + 1, max_history) and out = h' + (C - h') / (float)L_new, accum's running-mean expression of k_resolve
+ *      (the reference's render_kernel.cu:2284).  With no history, no history buffers, or a non-finite C: out = C bit for bit, L_new = 1.
+ *      d_out_display, if given, gets the display word of out exactly as k_resolve packs it (ACES, exposure_scale, gamma 2.2, BGRA).
+ *   Guarantee.  A still camera, clip_sigma = +inf, max_history >= F and F one-pass frames rendered at iteration 0 with sample offsets
+ *     0 .. F-1 (vpt_set_sample_offset), each filtered against the previous call's outputs: out is accum of one F-pass progressive render
+ *     bit for bit, and so is the display word -- unless a sample of those frames was replaced by the reference's NaN / Inf guard, which at
+ *     iteration 0 keeps the buffer's previous content instead of the running mean.
+ *   Contract.  Enqueued asynchronously on `stream`, no synchronisation, no scratch; touches no render state.  All buffers are full
+ *     row-major [H][W] frames in device memory; on a partitioned context pass the exchange block's full frames (vpt_comm_p2p_frame, the
+ *     VPT_LAYER_MOTION plane).  Deterministic: no atomics.  The fetch and the clip read neighbours, so the call cannot work in place: the
+ *     caller ping-pongs two history buffers.
+ *   Refused (VPT_ERR_INVALID, nothing enqueued): a NULL ctx, colour, vectors, camera, d_out_f3 or d_out_len; width or height 0 or above
+ *     65535; exactly one of d_history_f3 and d_history_len NULL; max_history outside 1..2^24; clip_sigma NaN or <= 0; a non-finite
+ *     component of origin, lower_left_corner, horizontal or vertical of either camera; any overlap of an output with an input or with
+ *     another output.  opt == NULL takes the defaults. */
+typedef struct vpt_temporal_options {
+    unsigned max_history;  /* cap on the history length L, 1 .. 2^24 (default 16) */
+    float    clip_sigma;   /* > 0: clip width in standard deviations of the 3x3 window; +INFINITY: no clip (default +INFINITY) */
+} vpt_temporal_options;
+void vpt_temporal_options_defaults(vpt_temporal_options* opt);
+int  vpt_temporal(vpt_context* ctx, unsigned width, unsigned height,
+                  const float* d_color_f3,        /* C: [H][W] float3, this frame (e.g. accum_buffer) */
+                  const float* d_vectors_f3,      /* M: [H][W] float3, vpt_set_motion_vectors' buffer rendered with target = previous */
+                  const vpt_camera* current,      /* A: the frame camera */
+                  const vpt_camera* previous,     /* B: the camera of the history */
+                  const float* d_history_f3,      /* H: [H][W] float3, the previous call's d_out_f3; NULL with d_history_len: no history */
+                  const float* d_history_len,     /* L: [H][W] float, the previous call's d_out_len */
+                  const vpt_temporal_options* opt,  /* NULL = defaults */
+                  float exposure_scale,           /* only read when d_out_display != NULL */
+                  float* d_out_f3,                /* [H][W] float3 */
+                  float* d_out_len,               /* [H][W] float, the history length of each pixel */
+                  unsigned* d_out_display,        /* [H][W] BGRA words as k_resolve writes them, may be NULL */
+                  void* stream);
 
 /* The flattened scene tables are cached per (volumes pointer, octree root pointer, build generation of a vpt_octree_build
  * octree) and refreshed whenever a call arrives with Kernel_params.iteration == 0 (the reference application resets the

@@ -166,7 +166,7 @@ EXPORTED_SYMBOLS = [
     "vpt_ods_options_defaults", "vpt_set_projection_ods", "vpt_debug_ods_cameras",
     "vpt_set_instance_mattes",
     "vpt_comm_p2p_export_binned", "vpt_comm_p2p_binned", "vpt_comm_p2p_block_bytes_binned",
-    "vpt_set_motion_vectors",
+    "vpt_set_motion_vectors", "vpt_set_sample_offset", "vpt_temporal_options_defaults", "vpt_temporal",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -340,6 +340,24 @@ lib.vpt_camera_look_at.restype = None
 lib.vpt_set_camera_motion.argtypes = [_vp, C.POINTER(camera)]; lib.vpt_set_camera_motion.restype = C.c_int
 lib.vpt_debug_motion_cameras.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_motion_cameras.restype = C.c_int
 lib.vpt_set_motion_vectors.argtypes = [_vp, _vp, C.POINTER(camera)]; lib.vpt_set_motion_vectors.restype = C.c_int
+lib.vpt_set_sample_offset.argtypes = [_vp, C.c_uint32]; lib.vpt_set_sample_offset.restype = C.c_int
+
+
+class temporal_options(C.Structure):
+    _fields_ = [("max_history", C.c_uint), ("clip_sigma", C.c_float)]
+
+
+lib.vpt_temporal_options_defaults.argtypes = [C.POINTER(temporal_options)]; lib.vpt_temporal_options_defaults.restype = None
+lib.vpt_temporal.argtypes = [_vp, C.c_uint, C.c_uint, _vp, _vp, C.POINTER(camera), C.POINTER(camera), _vp, _vp, C.POINTER(temporal_options),
+                             C.c_float, _vp, _vp, _vp, _vp]
+lib.vpt_temporal.restype = C.c_int
+
+
+def temporal_defaults():
+    """(max_history, clip_sigma) of vpt_temporal_options_defaults"""
+    o = temporal_options()
+    lib.vpt_temporal_options_defaults(C.byref(o))
+    return int(o.max_history), float(o.clip_sigma)
 lib.vpt_kernel_params_defaults.argtypes = [C.POINTER(Kernel_params)]; lib.vpt_kernel_params_defaults.restype = None
 
 

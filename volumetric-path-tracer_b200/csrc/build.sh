@@ -11,6 +11,8 @@ $NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC ${VPT_KERN
 $NVCC $ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_bricks.cu" -o "$HERE/_obj/vpt_bricks.o"
 # denoiser: the same flags as vpt_kernels.cu, so its display words come out of the very same tonemap code as k_resolve's
 $NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_denoise.cu" -o "$HERE/_obj/vpt_denoise.o"
+# temporal filter: the same flags again, so its blend is accum's running-mean arithmetic and its display words k_resolve's, bit for bit
+$NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_temporal.cu" -o "$HERE/_obj/vpt_temporal.o"
 $NVCC $ARCH -O3 --use_fast_math -lineinfo -std=c++17 -Xcompiler -fPIC -c "$HERE/device/vpt_bruneton.cu" -o "$HERE/_obj/vpt_bruneton.o"
 # octree build: plain IEEE flags, as the reference's bvh object
 $NVCC $ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-ffp-contract=off -c "$HERE/device/vpt_octree.cu" -o "$HERE/_obj/vpt_octree.o"

@@ -37,6 +37,7 @@
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
 #include "vpt_frame.cuh"
+#include "vpt_film.cuh"
 
 namespace vpt {
 
@@ -1187,36 +1188,7 @@ k_resolve_adaptive_ods(const FrameArgs fa, const NoSky atmo, const int n_passes,
 // =====================================================================================================
 // k_motion_vectors: screen-space motion of each sample's first collision towards a second camera pose (DESIGN.md section 8o)
 // =====================================================================================================
-// The film projection pi_K of camera K: d = P - origin, e = lower_left_corner - origin, n = cross(horizontal, vertical), k = e.n / d.n,
-// q = k d - e, and (s, t) with q = s horizontal + t vertical (the 2x2 normal equations; the dot-product form when horizontal . vertical is 0),
-// in the units of camera_b0's (x + jx) / W, (y + jy) / H: (s W, t H).  FilmCam holds what depends on K alone.
-struct FilmCam { float3 o, e, h, v; float en, hh, hv, vv, det; };
-__device__ __forceinline__ FilmCam film_cam(const vpt_f3 origin, const vpt_f3 llc, const vpt_f3 horizontal, const vpt_f3 vertical)
-{
-    FilmCam K;
-    K.o = ld3(origin); K.h = ld3(horizontal); K.v = ld3(vertical);
-    K.e = f3(psub(llc.x, origin.x), psub(llc.y, origin.y), psub(llc.z, origin.z));
-    K.en = dot(K.e, cross(K.h, K.v));
-    K.hh = dot(K.h, K.h); K.hv = dot(K.h, K.v); K.vv = dot(K.v, K.v);
-    K.det = pfma(K.hh, K.vv, -pmul(K.hv, K.hv));
-    return K;
-}
-// pi_K(P) into *st; false when P is not in front of K (k <= 0, NaN) or the result is not finite
-__device__ __forceinline__ bool film_project(const FilmCam& K, const float3 P, const vpt_u2 res, float2* st)
-{
-    const float3 d = f3(psub(P.x, K.o.x), psub(P.y, K.o.y), psub(P.z, K.o.z));
-    const float k = __fdiv_rn(K.en, dot(d, cross(K.h, K.v)));
-    const float3 q = f3(pfma(k, d.x, -K.e.x), pfma(k, d.y, -K.e.y), pfma(k, d.z, -K.e.z));
-    const float qh = dot(q, K.h), qv = dot(q, K.v);
-    float s, t;
-    if (K.hv == 0.0f) { s = __fdiv_rn(qh, K.hh); t = __fdiv_rn(qv, K.vv); }
-    else {
-        s = __fdiv_rn(pfma(K.vv, qh, -pmul(K.hv, qv)), K.det);
-        t = __fdiv_rn(pfma(K.hh, qv, -pmul(K.hv, qh)), K.det);
-    }
-    st->x = pmul(s, (float)res.x); st->y = pmul(t, (float)res.y);
-    return k > 0.0f && isfinite(st->x) && isfinite(st->y);
-}
+// The film projection pi_K of camera K (FilmCam, film_cam, film_project): vpt_film.cuh
 
 // The accepted lens point of the rejection loop k_generate runs on the pixel's stream (two draws per trial through vanDerCorput in bases 2
 // and 3): the radical inverses k_generate tabulates, computed by the same operations
@@ -1231,7 +1203,7 @@ __device__ __forceinline__ float2 lens_disk_point(Rng& rng)
     return p;
 }
 
-// The camera ray of pixel (x, global row y)'s sample at `iteration`, jitter j, as k_generate (kMotion: k_generate_motion) built it: the
+// The camera ray of pixel (x, global row y)'s sample on the Philox stream of `iteration` (the sample offset included), jitter j, as k_generate (kMotion: k_generate_motion) built it: the
 // pinhole order where k_generate takes it, else the thin-lens order with the loop's lens point (and, under motion, the camera of the shutter
 // draw that follows the loop)
 template <bool kMotion>
@@ -1284,7 +1256,7 @@ __device__ __forceinline__ void motion_vectors_pixel(const FrameArgs& fa, const 
         if (c) {
             float3 org, dir;
             const float2 j = __ldg(fa.bn_table + (size_t)p * 65536 + (y % 256) * 256 + x % 256);
-            sample_camera_ray<kMotion>(fa, mo, x, y, iteration, j, org, dir);
+            sample_camera_ray<kMotion>(fa, mo, x, y, fa.sample_offset + iteration, j, org, dir);
             const float3 P = madd3(org, dir, depth);
             float2 pa, pb;
             if (film_project(A, P, kp.resolution, &pa) && film_project(B, P, kp.resolution, &pb)) { vx = psub(pb.x, pa.x); vy = psub(pb.y, pa.y); }

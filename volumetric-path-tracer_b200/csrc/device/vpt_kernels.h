@@ -35,6 +35,12 @@ struct FrameArgs {
     uint2*    queue_id;
     float4*   queue_aux;           // per-ray origin (thin lens or camera motion); pre-stepped ray (pinhole only): position where stepping starts
     int       thin_lens;           // per-ray origin: thin lens or camera motion (cam.lens_radius != 0 or a CameraMotion)
+    // vpt_set_sample_offset: pass p of the call draws the Philox stream of iteration sample_offset + kp.iteration + p (everything else keeps
+    // kp.iteration).  Read by the motion-vector kernels, which need both; k_generate* and k_trace* read kp.iteration only as the stream key,
+    // so the host hands them the stream iteration in kp.iteration instead (stream_args in vpt_context.cpp) and their code stays as it was.
+    // In the 4-byte hole after thin_lens: the block has no tail padding, so a field at its end would move the kernel parameters that follow
+    // FrameArgs in every kernel, while the hole moves no offset at all.
+    uint32_t  sample_offset;
     // (option "empty_ahead" reaches the kernels through the table behind `scene`: SceneAlloc, launch_empty_ahead)
     const float2* bn_table;       // [pass][65536] blue-noise jitter of the chunk
     int       n_passes;            // passes in this chunk (k_generate loops over them; k_trace keeps tr of the last one)
@@ -346,5 +352,23 @@ struct DenoiseArgs {
 // launches of the layer planes per level: groups of 8, 4, 2 or 1 planes
 inline int denoise_layer_groups(size_t n_planes) { return (int)(n_planes / 8) + __builtin_popcountll(n_planes % 8); }
 cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t s);
+
+// Temporal filter (vpt_temporal, csrc/device/vpt_temporal.cu): k_temporal, one thread per pixel of full [H][W] frames.  history and
+// history_len are both null (no history) or both set; out_display may be null; no output overlaps an input or another output.
+struct TemporalArgs {
+    int          width, height;
+    unsigned     max_history;
+    float        clip_sigma, exposure_scale;       // clip_sigma +inf: no clip
+    vpt_f3       a_origin, a_llc, a_horizontal, a_vertical;   // A, the frame camera
+    vpt_f3       b_origin, b_llc, b_horizontal, b_vertical;   // B, the camera of the history
+    const float* color;                  // [H][W] float3
+    const float* vectors;                // [H][W] float3, vpt_set_motion_vectors' (c vx, c vy, c) towards B
+    const float* history;                // [H][W] float3
+    const float* history_len;            // [H][W]
+    float*       out;                    // [H][W] float3
+    float*       out_len;                // [H][W]
+    unsigned*    out_display;            // [H][W]
+};
+cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s);
 
 } // namespace vpt

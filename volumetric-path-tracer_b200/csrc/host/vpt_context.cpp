@@ -325,6 +325,12 @@ int vpt_set_motion_vectors(vpt_context* c, float* d_vectors_f3, const vpt_camera
     return VPT_OK;
 }
 
+int vpt_set_sample_offset(vpt_context* c, uint32_t offset) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_sample_offset: null context");
+    c->sample_offset_req = offset;  // taken at the next iteration-0 call
+    return VPT_OK;
+}
+
 int vpt_unpermute(vpt_context* c, const void* d_gathered, void* d_full, unsigned width, unsigned height, int elem_bytes, void* stream) {
     if (!c || !d_gathered || !d_full || elem_bytes <= 0 || (elem_bytes & 3)) return fail(c, VPT_ERR_INVALID, "vpt_unpermute: bad arguments");
     const vpt::FrameGeom g = make_geom(c, width, height);
@@ -816,9 +822,11 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     plan.ods = ods;
     plan.motion = motion;
     plan.mo = kp.iteration == 0 ? c->motion_close_req : c->motion_close_cur;
+    fa.sample_offset = kp.iteration == 0 ? c->sample_offset_req : c->sample_offset_cur;
     if (kp.iteration == 0) {
         memcpy(c->region_cur, c->region_req, sizeof(c->region_cur)); c->proj_cur = c->proj_req; c->ods_cur = c->ods_req;
         c->motion_cur = c->motion_req; c->motion_close_cur = c->motion_close_req;
+        c->sample_offset_cur = c->sample_offset_req;
     }
     plan.region = region;
     if (region) plan.rg = vpt::region_geometry(fa.geom, (int)reg[0], (int)reg[1], (int)reg[2], (int)reg[3]);
@@ -835,9 +843,17 @@ static vpt::LayerSources layer_sources(const FramePlan& plan) {
     return s;
 }
 
+// The arguments of k_generate* and k_trace*: they read Kernel_params.iteration only as the Philox stream key, so they get the stream
+// iteration (vpt_set_sample_offset's offset added, 32-bit wrap) in its place and keep their code; every other kernel keeps the caller's.
+static vpt::FrameArgs stream_args(const vpt::FrameArgs& fa) {
+    vpt::FrameArgs s = fa;
+    s.kp.iteration = fa.kp.iteration + fa.sample_offset;
+    return s;
+}
+
 // the frame's trace kernel over whatever k_generate queued for a chunk of np passes
 static cudaError_t launch_trace_of(vpt_context* c, const FramePlan& plan, unsigned np, cudaStream_t stream) {
-    vpt::FrameArgs fa = plan.fa;
+    vpt::FrameArgs fa = stream_args(plan.fa);
     fa.n_passes = (int)np;
     return vpt::launch_trace(fa, plan.trace, plan.atmo, plan.lg, plan.matte_ids, c->brick_pool, c->brick_dims, plan.trace_ctas, stream);
 }
@@ -884,8 +900,8 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         const unsigned np = (n_sampled - done) < (unsigned)chunk ? (n_sampled - done) : (unsigned)chunk;
         fa.kp.iteration = it0 + done;
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)kp.blue_noise_buffer, c->d_bn_table, (int)np, bn_limit, c->d_counters, stream); }));   // jitter table + advance + queue reset
-        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(fa, (int)np, rg, plan.proj, plan.motion_arg(), plan.ods_arg(), stream)
-                                                            : vpt::launch_generate(fa, (int)np, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
+        VPT_CUDA(c, timed(c, stream, 0, [&] { return region ? vpt::launch_generate_region(stream_args(fa), (int)np, rg, plan.proj, plan.motion_arg(), plan.ods_arg(), stream)
+                                                            : vpt::launch_generate(stream_args(fa), (int)np, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
         VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
         const bool last = (done + np == n_passes);
         if (c->gather_pending) { int rc = vpt::comm_before_accum_write(c, stream); if (rc != VPT_OK) return rc; }
@@ -1042,7 +1058,7 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         VPT_CUDA(c, timed(c, stream, 3, [&] { return vpt::launch_bn_prepare((void*)bn, c->d_bn_table, (int)np, plan.bn_limit, c->d_counters, stream); }));
         c->launches++;
         if (ad.n_tiles > 0) {
-            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(fa, (int)np, ad, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
+            VPT_CUDA(c, timed(c, stream, 0, [&] { return vpt::launch_generate_adaptive(stream_args(fa), (int)np, ad, plan.proj, plan.motion_arg(), plan.ods_arg(), stream); }));
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
             if (plan.mv.out) {
                 VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_motion_vectors(fa, plan.mv, (int)np, 1, nullptr, &ad, plan.motion_arg(), stream); }));
@@ -1216,6 +1232,59 @@ int vpt_denoise_layers(vpt_context* c, unsigned width, unsigned height, const fl
     return VPT_OK;
 }
 
+void vpt_temporal_options_defaults(vpt_temporal_options* opt) {
+    if (!opt) return;
+    opt->max_history = 16; opt->clip_sigma = INFINITY;   // DESIGN.md section 8p: the sweep
+}
+
+// Temporal filter: one k_temporal launch on `stream` (csrc/device/vpt_temporal.cu), no synchronisation, no scratch.  The fetch reads
+// neighbouring pixels of the history and the clip those of the colour, so no output may share a byte with any input.
+int vpt_temporal(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_vectors, const vpt_camera* current,
+                 const vpt_camera* previous, const float* d_history, const float* d_history_len, const vpt_temporal_options* opt,
+                 float exposure_scale, float* d_out, float* d_out_len, unsigned* d_out_display, void* stream) {
+    const std::string f("vpt_temporal");
+    if (!c || !d_color || !d_vectors || !current || !previous || !d_out || !d_out_len)
+        return fail(c, VPT_ERR_INVALID, f + ": null context, colour, vectors, camera or output");
+    if (width == 0 || height == 0) return fail(c, VPT_ERR_INVALID, f + ": width and height must be >= 1");
+    if (width > 65535 || height > 65535) return fail(c, VPT_ERR_INVALID, f + ": width and height must be <= 65535");
+    if (!d_history != !d_history_len) return fail(c, VPT_ERR_INVALID, f + ": d_history_f3 and d_history_len must both be set or both be NULL");
+    vpt_temporal_options o;
+    vpt_temporal_options_defaults(&o);
+    if (opt) o = *opt;
+    if (o.max_history < 1 || o.max_history > (1u << 24)) return fail(c, VPT_ERR_INVALID, f + ": max_history must be 1..2^24");
+    if (!(o.clip_sigma > 0.0f)) return fail(c, VPT_ERR_INVALID, f + ": clip_sigma must be > 0 (+inf: no clip)");
+    const struct { const char* cam; const vpt_camera* k; } cams[] = { { "current", current }, { "previous", previous } };
+    for (const auto& k : cams) {
+        const struct { const char* name; vpt_f3 v; } fields[] = {
+            { "origin", k.k->origin }, { "lower_left_corner", k.k->lower_left_corner }, { "horizontal", k.k->horizontal }, { "vertical", k.k->vertical } };
+        for (const auto& fl : fields)
+            if (!std::isfinite(fl.v.x) || !std::isfinite(fl.v.y) || !std::isfinite(fl.v.z))
+                return fail(c, VPT_ERR_INVALID, f + ": " + k.cam + "." + fl.name + " is not finite");
+    }
+    const size_t px = (size_t)width * height;
+    const size_t b3 = 3 * sizeof(float) * px, b1 = sizeof(float) * px;
+    const struct { const char* name; const void* p; size_t bytes; } ins[] = {
+        { "d_color_f3", d_color, b3 }, { "d_vectors_f3", d_vectors, b3 }, { "d_history_f3", d_history, b3 }, { "d_history_len", d_history_len, b1 } };
+    const struct { const char* name; const void* p; size_t bytes; } outs[] = {
+        { "d_out_f3", d_out, b3 }, { "d_out_len", d_out_len, b1 }, { "d_out_display", d_out_display, b1 } };
+    for (const auto& w : outs) {
+        for (const auto& r : ins)
+            if (byte_ranges_overlap(w.p, w.bytes, r.p, r.bytes)) return fail(c, VPT_ERR_INVALID, f + ": " + w.name + " overlaps " + r.name);
+        for (const auto& w2 : outs)
+            if (&w2 != &w && byte_ranges_overlap(w.p, w.bytes, w2.p, w2.bytes))
+                return fail(c, VPT_ERR_INVALID, f + ": " + w.name + " overlaps " + w2.name);
+    }
+    vpt::TemporalArgs a;
+    a.width = (int)width; a.height = (int)height; a.max_history = o.max_history; a.clip_sigma = o.clip_sigma; a.exposure_scale = exposure_scale;
+    a.a_origin = current->origin; a.a_llc = current->lower_left_corner; a.a_horizontal = current->horizontal; a.a_vertical = current->vertical;
+    a.b_origin = previous->origin; a.b_llc = previous->lower_left_corner; a.b_horizontal = previous->horizontal; a.b_vertical = previous->vertical;
+    a.color = d_color; a.vectors = d_vectors; a.history = d_history; a.history_len = d_history_len;
+    a.out = d_out; a.out_len = d_out_len; a.out_display = d_out_display;
+    VPT_CUDA(c, vpt::launch_temporal(a, (cudaStream_t)stream));
+    c->launches++;
+    return VPT_OK;
+}
+
 // Statistics accumulated since the last call (needs option "count_stats"): out[0..4] = volume lookups, lane-steps,
 // warp step iterations, lane transitions, warp transition rounds; out[5] = rays taken from the queue; out[6] = bricks
 // fetched (k_trace_brick only).  Synchronises the device.
@@ -1318,7 +1387,8 @@ int vpt_debug_ods_cameras(vpt_context* c, void* const params[VPT_NUM_ARGS], floa
     return rc;
 }
 
-// The camera of every local pixel's first sample of the next render call under camera motion (motion_req at iteration 0, else motion_cur):
+// The camera of every local pixel's first sample of the next render call under camera motion (motion_req at iteration 0, else motion_cur,
+// on the stream the sample offset selects):
 // its shutter draw and motion_camera of it, on the default stream.  Reads the camera and Kernel_params; writes d_out only.
 int vpt_debug_motion_cameras(vpt_context* c, void* const params[VPT_NUM_ARGS], float* d_out) {
     if (!c || !params || !d_out || !params[VPT_ARG_CAMERA] || !params[VPT_ARG_KERNEL_PARAMS])
@@ -1329,8 +1399,9 @@ int vpt_debug_motion_cameras(vpt_context* c, void* const params[VPT_NUM_ARGS], f
     if (kp.resolution.x == 0 || kp.resolution.y == 0) return fail(c, VPT_ERR_INVALID, "vpt_debug_motion_cameras: resolution is zero");
     const bool motion = kp.iteration == 0 ? c->motion_req : c->motion_cur;
     if (!motion) return fail(c, VPT_ERR_INVALID, "vpt_debug_motion_cameras: the next call has no camera motion (vpt_set_camera_motion)");
+    const uint32_t stream = (kp.iteration == 0 ? c->sample_offset_req : c->sample_offset_cur) + kp.iteration;   // the sample offset's stream
     VPT_CUDA(c, vpt::launch_motion_cameras(cam, kp.iteration == 0 ? c->motion_close_req : c->motion_close_cur,
-                                           make_geom(c, kp.resolution.x, kp.resolution.y), kp.iteration, d_out, 0));
+                                           make_geom(c, kp.resolution.x, kp.resolution.y), stream, d_out, 0));
     c->launches++;
     return VPT_OK;
 }

@@ -155,6 +155,93 @@ class Renderer:
         out = out.view(H, W, 3)
         return (out, words) if display else out
 
+    def set_sample_offset(self, offset):
+        """Draw pass p of a render call at kp.iteration = i from the Philox stream of iteration offset + i + p (vpt_set_sample_offset),
+        from the next call with kp.iteration == 0 on.  Every other use of the iteration keeps kp.iteration.  0 is the reference stream."""
+        check(lib.vpt_set_sample_offset(self.ctx, int(offset) & 0xFFFFFFFF), self.ctx, "vpt_set_sample_offset")
+
+    def temporal(self, previous_cam: N.camera, color=None, vectors=None, history=None, history_len=None, max_history=None, clip_sigma=None,
+                 display=False, out=None, out_len=None, stream=None):
+        """Temporal accumulation of a full frame (vpt_temporal), enqueued on `stream`: blends `color` into the history carried along each
+        pixel's motion from this renderer's camera to `previous_cam`.  Returns (out (H, W, 3), out_len (H, W)) float32, plus the display
+        words (H, W) int32 with display=True (packed with kp.exposure_scale).  color: None = this renderer's accumulator; vectors: None =
+        buffers.motion (rendered with target = previous_cam); history / history_len: the previous call's out / out_len, both None = no
+        history.  max_history / clip_sigma: None = the library's defaults (clip_sigma = inf: no clip).  out / out_len: None = new
+        tensors, or tensors to write (they may not overlap any input).  On a partitioned renderer pass full frames."""
+        H, W = self.height, self.width
+        if color is None:
+            if self.n_ranks > 1:
+                raise N.VptError("Renderer.temporal: a partitioned renderer holds no full frame; pass `color` and `vectors`")
+            color = self.buffers.accum
+        if vectors is None:
+            if self.buffers.motion is None or self.n_ranks > 1:
+                raise N.VptError("Renderer.temporal: no motion vectors (Renderer.enable_motion_vectors(previous_cam)) and none passed")
+            vectors = self.buffers.motion
+        dev = color.device
+        color = _frame_tensor(color, H * W * 3, "color", dev)
+        vectors = _frame_tensor(vectors, H * W * 3, "vectors", dev)
+        history = _frame_tensor(history, H * W * 3, "history", dev)
+        history_len = _frame_tensor(history_len, H * W, "history_len", dev)
+        out = torch.empty(H, W, 3, dtype=torch.float32, device=dev) if out is None else _frame_tensor(out, H * W * 3, "out", dev)
+        out_len = torch.empty(H, W, dtype=torch.float32, device=dev) if out_len is None else _frame_tensor(out_len, H * W, "out_len", dev)
+        words = torch.empty(H, W, dtype=torch.int32, device=dev) if display else None
+        opt = N.temporal_options()
+        lib.vpt_temporal_options_defaults(C.byref(opt))
+        if max_history is not None: opt.max_history = int(max_history)
+        if clip_sigma is not None: opt.clip_sigma = float(clip_sigma)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        check(lib.vpt_temporal(self.ctx, W, H, ptr(color), ptr(vectors), C.byref(self.cam), C.byref(previous_cam), ptr(history), ptr(history_len),
+                               C.byref(opt), float(self.kp.exposure_scale), ptr(out), ptr(out_len), ptr(words), C.c_void_p(stream or 0)),
+              self.ctx, "vpt_temporal")
+        out, out_len = out.view(H, W, 3), out_len.view(H, W)
+        return (out, out_len, words) if display else (out, out_len)
+
+    def enable_temporal(self, max_history=None, clip_sigma=None):
+        """Start temporal accumulation for render_temporal(): a viewer loop that restarts every frame at kp.iteration = 0 keeps converging
+        while the camera moves.  Allocates the motion vectors and two history buffers; the next render_temporal() has no history.
+        max_history / clip_sigma: vpt_temporal's options (None = the library's defaults).  One context only (n_ranks == 1)."""
+        if self.n_ranks > 1:
+            raise N.VptError("Renderer.enable_temporal: one context only; a partitioned frame calls Renderer.temporal on full frames")
+        dev = self.buffers.accum.device
+        self.buffers.motion = torch.zeros(self.n_local, 3, dtype=torch.float32, device=dev)
+        n = self.width * self.height
+        self._temporal = {"max_history": max_history, "clip_sigma": clip_sigma, "passes": 0, "prev_cam": None, "size": None, "k": 0,
+                          "out": [torch.empty(n * 3, dtype=torch.float32, device=dev) for _ in range(2)],
+                          "len": [torch.empty(n, dtype=torch.float32, device=dev) for _ in range(2)]}
+
+    def render_temporal(self, cam: N.camera, n_passes, display=False):
+        """One frame of a moving camera: n_passes passes from kp.iteration = 0 with camera `cam`, filtered against the previous frame's
+        output (Renderer.temporal).  In order: the motion vectors target the previous frame's camera, the sample offset is the number of
+        passes rendered since enable_temporal() (so every frame draws new samples), the frame renders, the filter blends it into the
+        history, and the output becomes the next frame's history.  The first frame after enable_temporal() has no history, and neither
+        has one after a change of resolution.  Returns Renderer.temporal's result; buffers.accum holds the unfiltered frame."""
+        st = getattr(self, "_temporal", None)
+        if st is None:
+            raise N.VptError("Renderer.render_temporal: temporal accumulation is not enabled (Renderer.enable_temporal())")
+        size = (self.width, self.height)
+        have = st["prev_cam"] is not None and st["size"] == size
+        prev = st["prev_cam"] if have else cam
+        check(lib.vpt_set_motion_vectors(self.ctx, C.c_void_p(self.buffers.motion.data_ptr()), C.byref(prev)), self.ctx, "vpt_set_motion_vectors")
+        self.set_sample_offset(st["passes"])
+        C.memmove(C.byref(self.cam), C.byref(cam), C.sizeof(self.cam))
+        self.kp.iteration = 0
+        self.render(n_passes)
+        k = st["k"]
+        res = self.temporal(prev, history=st["out"][k ^ 1] if have else None, history_len=st["len"][k ^ 1] if have else None,
+                            max_history=st["max_history"], clip_sigma=st["clip_sigma"], display=display, out=st["out"][k], out_len=st["len"][k])
+        st["passes"] += int(n_passes)
+        st["prev_cam"] = type(cam).from_buffer_copy(cam)
+        st["size"] = size
+        st["k"] = k ^ 1
+        return res
+
+    def disable_temporal(self):
+        """Stop temporal accumulation: drops the history, turns the motion vectors off and sets the sample offset back to 0 (from the next
+        call with kp.iteration == 0 on)."""
+        self._temporal = None
+        self.disable_motion_vectors()
+        self.set_sample_offset(0)
+
     def denoise_layers(self, layers, color=None, depth=True, rel_error=None, iterations=5, sigma_luminance=4.0, sigma_depth=0.2,
                        stream=None, display=False):
         """Renderer.denoise of `color` together with layers filtered by the beauty's own weights (vpt_denoise_layers), so the denoised
@@ -758,6 +845,11 @@ class DistributedRenderer:
 
     def disable_motion_vectors(self):
         self.r.disable_motion_vectors()
+
+    def set_sample_offset(self, offset):
+        """Renderer.set_sample_offset on this rank; every rank sets the same offset, so the sharded frame draws the streams a single
+        context draws."""
+        self.r.set_sample_offset(offset)
 
     def full_motion_vectors(self):
         """(H, W, 3) float32 motion-vector buffer (c vx, c vy, c) of the whole frame (see full_depth); unpremultiply_vectors() of it gives
