@@ -512,6 +512,41 @@ int  vpt_debug_motion_cameras(vpt_context* ctx, void* const params[VPT_NUM_ARGS]
  *     (VPT_ERR_INVALID, naming the buffer). */
 int  vpt_set_motion_vectors(vpt_context* ctx, float* d_vectors_f3, const vpt_camera* target);
 
+/* ---- collision AOVs: world position, normal and albedo at each sample's first collision -------------------------------------------
+ * The utility passes a compositor and a denoiser expect next to the beauty: world position P (relighting, position masks, fog, a
+ * disocclusion test), the normal N (relighting, a denoiser guide) and the albedo (the second guide of OIDN and the OptiX denoiser).
+ *
+ *   Definition.  For each pass a pixel takes, let c = (depth > 0) as for the alpha AOV (a NaN depth counts as false).  If c holds:
+ *     P = org + depth * dir, with (org, dir) the sample's camera ray exactly as the generator built it (as for vpt_set_motion_vectors:
+ *     pinhole, thin lens, the camera of the shutter draw under camera motion, keyed by the sample offset + iteration).  The depth pass's own
+ *     test on that ray (nearest of the octree root box and the sphere) tells what P lies on:
+ *     - Sphere: n = normalize(P - centre), albedo = the sphere's colour, the reflectance the integrators' sphere branch multiplies the
+ *       throughput by.
+ *     - Volume: rho(X) is the density the frame's tracker reads -- volume 0 through the frame's sampler (texture, brick pool or cell table)
+ *       in a single-volume scene, else the sum over the leaf list of the octree leaf that contains X (0 in no populated leaf).
+ *       g_i = (rho(P + h e_i) - rho(P - h e_i)) / (2h) with h = gradient_step in world units; n = -g / |g|, or (0, 0, 0) when g . g is 0
+ *       or not finite in float32.  albedo = Kernel_params.albedo * Cd(P) * density_color[index(rho(P))] / Kernel_params.extinction *
+ *       energy_inject: the throughput factor an accepted collision at P applies, with Cd the leaf colour (volume 0's colour grid, clamped
+ *       at 0, for one volume) and index = floor(clamp(rho / max_extinction * 255 / emission_pivot, 0, 255)).  Where P lies in no populated
+ *       leaf rho and Cd are 0 and the expression is evaluated as written.
+ *     Non-finite results are stored as they come (not guarded, as the motion vectors).
+ *   Buffers.  Per pixel the running means in accum's rule and arithmetic (iteration == 0 assigns, iteration < max_interactions updates
+ *     x + (s - x) / (iteration + 1), later passes change nothing) of: position float4 (c Px, c Py, c Pz, c) -- w is the alpha AOV bit for bit
+ *     and a one-pass frame holds P exactly; normal float3 c n (premultiplied: callers normalise); albedo float3 c a (premultiplied by the
+ *     coverage).  A miss or a pass that samples nothing adds exact zeros.  Caller-owned device memory of vpt_local_pixels() entries each
+ *     (rank-local order on a partitioned context).  Any buffer may be NULL; all three NULL turns the layers off at once.
+ *   Activation.  As for the AOVs: buffers set here take over at the next render call whose Kernel_params.iteration is 0.
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update the active layers (an adaptive frame's stopped pixels keep theirs; a render
+ *     region writes nothing outside it).  Works with camera motion, thin lens, both integrators, all three environments, instanced scenes,
+ *     brick and cell mode, partitioned contexts and vpt_set_sample_offset.  Every other output is bit for bit what the same call gives
+ *     without them: a kernel of its own reads each sample's depth word next to the frame's resolve, and runs the look-ups (seven density
+ *     and one colour fetch) only for covered samples.  Neither exchange carries the layers.  Level (A) has none.
+ *   Refused when set (VPT_ERR_INVALID; the layers are left as they were): a normal buffer with a gradient_step that is not finite or <= 0.
+ *     Refused at render time: VPT_PROJECTION_EQUIRECT and VPT_PROJECTION_ODS (VPT_ERR_UNSUPPORTED); a buffer that overlaps accum, depth,
+ *     cost, raw, display, an AOV, light-group, deep-slice, matte or motion-vector buffer, or another of the three (VPT_ERR_INVALID, naming
+ *     the buffers). */
+int  vpt_set_collision_aovs(vpt_context* ctx, float* d_position_f4, float* d_normal_f3, float* d_albedo_f3, float gradient_step);
+
 /* ---- sample-stream offset: a fresh Philox stream for every frame of a restarted accumulation ----------------------------------------
  * Pass p of a render call at Kernel_params.iteration = i draws the Philox stream the reference draws at iteration offset + i + p (32-bit
  * unsigned arithmetic, wrapping as iteration * 4096 does).  Everything else keyed by the iteration keeps the caller's i: the running-mean

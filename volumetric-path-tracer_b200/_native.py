@@ -167,6 +167,7 @@ EXPORTED_SYMBOLS = [
     "vpt_set_instance_mattes",
     "vpt_comm_p2p_export_binned", "vpt_comm_p2p_binned", "vpt_comm_p2p_block_bytes_binned",
     "vpt_set_motion_vectors", "vpt_set_sample_offset", "vpt_temporal_options_defaults", "vpt_temporal",
+    "vpt_set_collision_aovs",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -341,6 +342,7 @@ lib.vpt_set_camera_motion.argtypes = [_vp, C.POINTER(camera)]; lib.vpt_set_camer
 lib.vpt_debug_motion_cameras.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debug_motion_cameras.restype = C.c_int
 lib.vpt_set_motion_vectors.argtypes = [_vp, _vp, C.POINTER(camera)]; lib.vpt_set_motion_vectors.restype = C.c_int
 lib.vpt_set_sample_offset.argtypes = [_vp, C.c_uint32]; lib.vpt_set_sample_offset.restype = C.c_int
+lib.vpt_set_collision_aovs.argtypes = [_vp, _vp, _vp, _vp, C.c_float]; lib.vpt_set_collision_aovs.restype = C.c_int
 
 
 class temporal_options(C.Structure):

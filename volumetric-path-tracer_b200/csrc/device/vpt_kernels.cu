@@ -33,6 +33,8 @@
 //                     sample's camera on its eye's viewing circle (ods_camera); k_ods_cameras: vpt_debug_ods_cameras, and the ODS camera rays
 //   k_motion_vectors, k_motion_vectors_region, k_motion_vectors_adaptive (and their _motion forms) : motion vectors (vpt_set_motion_vectors)
 //                     -- each sample's first collision projected through the frame camera and a second pose, next to the frame's resolve
+//   k_collision_aovs, k_collision_aovs_region, k_collision_aovs_adaptive (and their _motion forms) : collision AOVs (vpt_set_collision_aovs)
+//                     -- the world position, density normal and albedo at each sample's first collision, next to the frame's resolve
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -1228,9 +1230,32 @@ __device__ __forceinline__ void sample_camera_ray(const FrameArgs& fa, const Cam
     dir = normalize(f3(psub(b0.x, offset.x), psub(b0.y, offset.y), psub(b0.z, offset.z)));
 }
 
-// One pixel (local pixel lp, local row lr, global row y) over the chunk's passes.  Reads only each record's depth word (A.w of a compact
-// record, B.w of a wide one; a miss, or a pixel k_miss_cull removed, has none: c = 0), rebuilds the camera ray of the samples with c and keeps
-// the running means in accum's rule and arithmetic, written as the alpha AOV's, so z is alpha bit for bit.
+// The depth word of pass p's record of local pixel lp (A.w of a compact record, B.w of a wide one); 0 for a miss and where `records` is false
+// (a pixel k_miss_cull removed, or a pass that samples nothing: no record)
+__device__ __forceinline__ float record_depth(const FrameArgs& fa, const int p, const uint32_t lp, const bool records, const bool compact)
+{
+    float depth = 0.0f;
+    if (records) {
+        const size_t s = (size_t)p * fa.geom.n_local + lp;
+        const float4 a = fa.planeA[s];
+        if (__float_as_uint(a.w) != kMissSentinel) depth = compact ? a.w : fa.planeB[s].w;
+    }
+    return depth;
+}
+
+// the camera ray of pixel (x, global row y)'s sample in pass p of the chunk (iteration = kp.iteration + p): the pass's jitter, the Philox
+// stream of the sample offset + iteration
+template <bool kMotion>
+__device__ __forceinline__ void pass_camera_ray(const FrameArgs& fa, const CameraMotion* mo, const int x, const int y, const int p,
+                                                const uint32_t iteration, float3& org, float3& dir)
+{
+    const float2 j = __ldg(fa.bn_table + (size_t)p * 65536 + (y % 256) * 256 + x % 256);
+    sample_camera_ray<kMotion>(fa, mo, x, y, fa.sample_offset + iteration, j, org, dir);
+}
+
+// One pixel (local pixel lp, local row lr, global row y) over the chunk's passes.  Reads only each record's depth word (a miss, or a pixel
+// k_miss_cull removed, has none: c = 0), rebuilds the camera ray of the samples with c and keeps the running means in accum's rule and
+// arithmetic, written as the alpha AOV's, so z is alpha bit for bit.
 template <bool kMotion>
 __device__ __forceinline__ void motion_vectors_pixel(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
                                                      const int sampled, const uint32_t lp, const int lr, const int y)
@@ -1245,12 +1270,7 @@ __device__ __forceinline__ void motion_vectors_pixel(const FrameArgs& fa, const 
     const bool compact = !fa.planeB;
     for (int p = 0; p < n_passes; ++p) {
         const uint32_t iteration = kp.iteration + (uint32_t)p;
-        float depth = 0.0f;
-        if (records) {
-            const size_t s = (size_t)p * g.n_local + lp;
-            const float4 a = fa.planeA[s];
-            if (__float_as_uint(a.w) != kMissSentinel) depth = compact ? a.w : fa.planeB[s].w;
-        }
+        const float depth = record_depth(fa, p, lp, records, compact);
         const bool c = depth > 0.0f;
         float vx = 0.0f, vy = 0.0f;
         if (c) {
@@ -1272,72 +1292,213 @@ __device__ __forceinline__ void motion_vectors_pixel(const FrameArgs& fa, const 
     mv.out[lp] = m;
 }
 
-// every local pixel of the frame (padding rows are skipped)
-template <bool kMotion>
-__device__ __forceinline__ void motion_vectors_frame(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
-                                                     const int sampled)
+// The pixel walkers of the per-pixel layer kernels (k_motion_vectors*, k_collision_aovs*): each calls f(lp, lr, y) for one pixel of the
+// thread.  frame: every local pixel (padding rows are skipped); region: R's pixels on this rank, row by row as k_resolve_region walks them;
+// adaptive: the pixels of the active tiles that have not stopped, as k_resolve_adaptive visits them.
+template <class F>
+__device__ __forceinline__ void frame_pixel(const FrameGeom& g, F&& f)
 {
-    const FrameGeom& g = fa.geom;
     const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
     if (lp >= (uint32_t)g.n_local) return;
     const int lr = lp / g.width;
     const int y = global_row(g, lr);
     if (y >= g.height) return;
-    motion_vectors_pixel<kMotion>(fa, mv, mo, n_passes, sampled, lp, lr, y);
+    f(lp, lr, y);
 }
 
-// R's pixels on this rank, row by row as k_resolve_region walks them
-template <bool kMotion>
-__device__ __forceinline__ void motion_vectors_region(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
-                                                      const int sampled, const RenderRegion& rg)
+template <class F>
+__device__ __forceinline__ void region_pixel(const FrameGeom& g, const RenderRegion& rg, F&& f)
 {
-    const FrameGeom& g = fa.geom;
     const uint32_t w = (uint32_t)(rg.x1 - rg.x0);
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= w * (uint32_t)(rg.lr1 - rg.lr0)) return;
     const uint32_t r = i / w;
     const int lr = rg.lr0 + (int)r;
     const uint32_t lp = (uint32_t)lr * (uint32_t)g.width + (uint32_t)rg.x0 + (i - r * w);
-    motion_vectors_pixel<kMotion>(fa, mv, mo, n_passes, sampled, lp, lr, global_row(g, lr));
+    f(lp, lr, global_row(g, lr));
 }
 
-// the pixels of the active tiles that have not stopped, as k_resolve_adaptive visits them
-template <bool kMotion>
-__device__ __forceinline__ void motion_vectors_adaptive(const FrameArgs& fa, const MotionVectors& mv, const CameraMotion* mo, const int n_passes,
-                                                        const AdaptArgs& ad)
+template <class F>
+__device__ __forceinline__ void adaptive_pixel(const FrameGeom& g, const AdaptArgs& ad, F&& f)
 {
-    const FrameGeom& g = fa.geom;
     const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
     if (!t.inside) return;
     const uint32_t lp = (uint32_t)t.lr * (uint32_t)g.width + (uint32_t)t.x;
     if (ad.stopped[lp]) return;
-    motion_vectors_pixel<kMotion>(fa, mv, mo, n_passes, 1, lp, t.lr, global_row(g, t.lr));
+    f(lp, t.lr, global_row(g, t.lr));
 }
 
 __global__ void __launch_bounds__(256)
 k_motion_vectors(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled)
-{ motion_vectors_frame<false>(fa, mv, nullptr, n_passes, sampled); }
+{ frame_pixel(fa.geom, [&](uint32_t lp, int lr, int y) { motion_vectors_pixel<false>(fa, mv, nullptr, n_passes, sampled, lp, lr, y); }); }
 
 __global__ void __launch_bounds__(256)
 k_motion_vectors_region(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled, const RenderRegion rg)
-{ motion_vectors_region<false>(fa, mv, nullptr, n_passes, sampled, rg); }
+{ region_pixel(fa.geom, rg, [&](uint32_t lp, int lr, int y) { motion_vectors_pixel<false>(fa, mv, nullptr, n_passes, sampled, lp, lr, y); }); }
 
 __global__ void __launch_bounds__(128)
 k_motion_vectors_adaptive(const FrameArgs fa, const MotionVectors mv, const int n_passes, const AdaptArgs ad)
-{ motion_vectors_adaptive<false>(fa, mv, nullptr, n_passes, ad); }
+{ adaptive_pixel(fa.geom, ad, [&](uint32_t lp, int lr, int y) { motion_vectors_pixel<false>(fa, mv, nullptr, n_passes, 1, lp, lr, y); }); }
 
 __global__ void __launch_bounds__(256)
 k_motion_vectors_motion(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled, const CameraMotion mo)
-{ motion_vectors_frame<true>(fa, mv, &mo, n_passes, sampled); }
+{ frame_pixel(fa.geom, [&](uint32_t lp, int lr, int y) { motion_vectors_pixel<true>(fa, mv, &mo, n_passes, sampled, lp, lr, y); }); }
 
 __global__ void __launch_bounds__(256)
 k_motion_vectors_region_motion(const FrameArgs fa, const MotionVectors mv, const int n_passes, const int sampled, const RenderRegion rg,
                                const CameraMotion mo)
-{ motion_vectors_region<true>(fa, mv, &mo, n_passes, sampled, rg); }
+{ region_pixel(fa.geom, rg, [&](uint32_t lp, int lr, int y) { motion_vectors_pixel<true>(fa, mv, &mo, n_passes, sampled, lp, lr, y); }); }
 
 __global__ void __launch_bounds__(128)
 k_motion_vectors_adaptive_motion(const FrameArgs fa, const MotionVectors mv, const int n_passes, const AdaptArgs ad, const CameraMotion mo)
-{ motion_vectors_adaptive<true>(fa, mv, &mo, n_passes, ad); }
+{ adaptive_pixel(fa.geom, ad, [&](uint32_t lp, int lr, int y) { motion_vectors_pixel<true>(fa, mv, &mo, n_passes, 1, lp, lr, y); }); }
+
+// =====================================================================================================
+// k_collision_aovs: world position, density normal and albedo at each sample's first collision (DESIGN.md section 8q)
+// =====================================================================================================
+// The leaf of the octree that contains X (the descent oct_locate_or_skip takes, read from the flat tables), or -1 when X lies outside the
+// root box or in an empty node
+__device__ __forceinline__ int collision_leaf(const SceneTables& sc, const float3 X)
+{
+    if (!aabb_contains(sc.root_pmin, sc.root_pmax, X)) return -1;
+    const OctInternal r = sc.internal[0];
+    const int c1 = oct_child(r, X);
+    if ((r.child_empty >> c1) & 1u) return -1;
+    const OctInternal n1 = sc.internal[1 + c1];
+    const int c2 = oct_child(n1, X);
+    if ((n1.child_empty >> c2) & 1u) return -1;
+    const OctInternal n2 = sc.internal[9 + c1 * 8 + c2];
+    const int c3 = oct_child(n2, X);
+    if ((n2.child_empty >> c3) & 1u) return -1;
+    return c1 * 64 + c2 * 8 + c3;
+}
+
+// rho(X), the density the frame's tracker reads at X: volume 0 through the frame's sampler (brick pool, cell table or texture) in a
+// single-volume scene, else the sum over the leaf list of the leaf that contains X (0 in no populated leaf)
+__device__ __forceinline__ float collision_density(const FrameArgs& fa, const CollisionAovs& ca, const SceneTables& sc, const VolumeRec& vol0,
+                                                   const float3 X)
+{
+    if (ca.brick_pool) {
+        BrickArgs ba;
+        ba.pool = ca.brick_pool; ba.dimx = ca.brick_dims[0]; ba.dimy = ca.brick_dims[1]; ba.dimz = ca.brick_dims[2];
+        ba.nbx = (ba.dimx + 3) / 4; ba.nby = (ba.dimy + 3) / 4; ba.nbz = (ba.dimz + 3) / 4;
+        float3 uvw;
+        if (!volume_coord(vol0, X, uvw)) return 0.0f;
+        return 0.0f + brick_sample_global<kBrickWeightMode>(uvw, ba);
+    }
+    if (fa.cell_table) return 0.0f + cell_density(fa, vol0, X);
+    if (sc.single_volume) return 0.0f + volume_density(vol0, X);
+    const int leaf = collision_leaf(sc, X);
+    return leaf < 0 ? 0.0f : leaf_density(sc, vol0, leaf, X);
+}
+
+// The normal and albedo of a covered sample whose camera ray (org, dir) first collided at P.  The depth pass's own test on the ray tells the
+// sphere from the volume: the sphere gives normalize(P - centre) and its colour (the reflectance the integrators' sphere branch multiplies
+// the throughput by); the volume gives -grad rho / |grad rho| by central differences of step h (0 where |grad rho| is 0 or not finite) and
+// the throughput factor scatter_event applies at an accepted collision at P.
+__device__ __forceinline__ void collision_surface(const FrameArgs& fa, const CollisionAovs& ca, const float3 org, const float3 dir, const float3 P,
+                                                  float3& n, float3& a)
+{
+    const vpt_kernel_params& kp = fa.kp;
+    const SceneTables& sc = *fa.scene;
+    const SphereRec sph = load_sphere(fa.sphere);
+    float t_min;
+    if (closest_object(sc, sph, org, dir, t_min) == 2) {
+        n = normalize(P - sph.center);
+        a = sph.color;
+        return;
+    }
+    const VolumeRec& vol0 = sc.volumes[0];
+    const float rho = collision_density(fa, ca, sc, vol0, P);
+    if (ca.normal) {
+        const float h = ca.step, inv2h = 1.0f / padd(h, h);
+        const float gx = pmul(psub(collision_density(fa, ca, sc, vol0, f3(padd(P.x, h), P.y, P.z)),
+                                   collision_density(fa, ca, sc, vol0, f3(psub(P.x, h), P.y, P.z))), inv2h);
+        const float gy = pmul(psub(collision_density(fa, ca, sc, vol0, f3(P.x, padd(P.y, h), P.z)),
+                                   collision_density(fa, ca, sc, vol0, f3(P.x, psub(P.y, h), P.z))), inv2h);
+        const float gz = pmul(psub(collision_density(fa, ca, sc, vol0, f3(P.x, P.y, padd(P.z, h))),
+                                   collision_density(fa, ca, sc, vol0, f3(P.x, P.y, psub(P.z, h)))), inv2h);
+        const float g2 = pfma(gx, gx, pfma(gy, gy, pmul(gz, gz)));
+        if (g2 > 0.0f && g2 <= VPT_M_INF) {                      // positive and finite
+            const float r = -rsqrtf(g2);
+            n = f3(pmul(gx, r), pmul(gy, r), pmul(gz, r));
+        }
+    }
+    if (ca.albedo) {
+        float3 Cd;
+        if (sc.single_volume) Cd = fmax3(f3(0.0f), volume_color(vol0, P));
+        else { const int leaf = collision_leaf(sc, P); Cd = leaf < 0 ? f3(0.0f) : leaf_color(sc, vol0, leaf, P); }
+        const int index = int(floorf(fminf(fmaxf((rho * (1.0f / sc.max_extinction) * 255.0f / kp.emission_pivot), 0.0f), 255.0f)));
+        const float3 density_color = reinterpret_cast<const float3*>(kp.density_color_texture)[index];
+        a = (ld3(kp.albedo) * Cd * density_color / ld3(kp.extinction)) * float(kp.energy_inject);
+    }
+}
+
+// One pixel over the chunk's passes, as motion_vectors_pixel: every record's depth word, the camera ray and the look-ups only for samples
+// with c, the running means in accum's rule with the alpha AOV's expressions (so position.w is alpha bit for bit; a sample without c adds
+// exact zeros)
+template <bool kMotion>
+__device__ __forceinline__ void collision_aovs_pixel(const FrameArgs& fa, const CollisionAovs& ca, const CameraMotion* mo, const int n_passes,
+                                                     const int sampled, const uint32_t lp, const int lr, const int y)
+{
+    const FrameGeom& g = fa.geom;
+    const vpt_kernel_params& kp = fa.kp;
+    const int x = (int)(lp - (uint32_t)lr * (uint32_t)g.width);
+    const bool prev = kp.iteration > 0;
+    float4 mp = prev && ca.position ? ca.position[lp] : make_float4(0.f, 0.f, 0.f, 0.f);
+    float3 mn = prev && ca.normal ? ca.normal[lp] : f3(0.f);
+    float3 ma = prev && ca.albedo ? ca.albedo[lp] : f3(0.f);
+    const bool records = sampled && !(fa.miss_mask && fa.miss_mask[lp]);
+    const bool compact = !fa.planeB;
+    for (int p = 0; p < n_passes; ++p) {
+        const uint32_t iteration = kp.iteration + (uint32_t)p;
+        const float depth = record_depth(fa, p, lp, records, compact);
+        const bool c = depth > 0.0f;
+        float3 P = f3(0.f), n = f3(0.f), a = f3(0.f);
+        if (c) {
+            float3 org, dir;
+            pass_camera_ray<kMotion>(fa, mo, x, y, p, iteration, org, dir);
+            P = madd3(org, dir, depth);
+            if (ca.normal || ca.albedo) collision_surface(fa, ca, org, dir, P, n, a);
+        }
+        const float cs = c ? 1.0f : 0.0f;
+        if (iteration == 0) { mp = make_float4(P.x, P.y, P.z, cs); mn = n; ma = a; }
+        else if (iteration < kp.max_interactions) {
+            const float k = (float)(iteration + 1);
+            mp.x = mp.x + (P.x - mp.x) / k; mp.y = mp.y + (P.y - mp.y) / k; mp.z = mp.z + (P.z - mp.z) / k; mp.w = mp.w + (cs - mp.w) / k;
+            mn.x = mn.x + (n.x - mn.x) / k; mn.y = mn.y + (n.y - mn.y) / k; mn.z = mn.z + (n.z - mn.z) / k;
+            ma.x = ma.x + (a.x - ma.x) / k; ma.y = ma.y + (a.y - ma.y) / k; ma.z = ma.z + (a.z - ma.z) / k;
+        }
+    }
+    if (ca.position) ca.position[lp] = mp;
+    if (ca.normal) ca.normal[lp] = mn;
+    if (ca.albedo) ca.albedo[lp] = ma;
+}
+
+__global__ void __launch_bounds__(256)
+k_collision_aovs(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const int sampled)
+{ frame_pixel(fa.geom, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<false>(fa, ca, nullptr, n_passes, sampled, lp, lr, y); }); }
+
+__global__ void __launch_bounds__(256)
+k_collision_aovs_region(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const int sampled, const RenderRegion rg)
+{ region_pixel(fa.geom, rg, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<false>(fa, ca, nullptr, n_passes, sampled, lp, lr, y); }); }
+
+__global__ void __launch_bounds__(128)
+k_collision_aovs_adaptive(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const AdaptArgs ad)
+{ adaptive_pixel(fa.geom, ad, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<false>(fa, ca, nullptr, n_passes, 1, lp, lr, y); }); }
+
+__global__ void __launch_bounds__(256)
+k_collision_aovs_motion(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const int sampled, const CameraMotion mo)
+{ frame_pixel(fa.geom, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<true>(fa, ca, &mo, n_passes, sampled, lp, lr, y); }); }
+
+__global__ void __launch_bounds__(256)
+k_collision_aovs_region_motion(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const int sampled, const RenderRegion rg,
+                               const CameraMotion mo)
+{ region_pixel(fa.geom, rg, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<true>(fa, ca, &mo, n_passes, sampled, lp, lr, y); }); }
+
+__global__ void __launch_bounds__(128)
+k_collision_aovs_adaptive_motion(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const AdaptArgs ad, const CameraMotion mo)
+{ adaptive_pixel(fa.geom, ad, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<true>(fa, ca, &mo, n_passes, 1, lp, lr, y); }); }
 
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
 // clipped at the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A neighbour row this
@@ -1993,7 +2154,9 @@ cudaError_t exchange_kernels_preload()
                 k_miss_cull_equirect, k_miss_cull_region_equirect, k_layers_publish, k_generate_motion, k_generate_adaptive_motion,
                 k_generate_region_motion, k_generate_ods, k_generate_adaptive_ods, k_generate_region_ods, k_miss_cull_ods, k_miss_cull_region_ods,
                 k_binned_publish, k_empty_ahead, k_motion_vectors, k_motion_vectors_region, k_motion_vectors_adaptive,
-                k_motion_vectors_motion, k_motion_vectors_region_motion, k_motion_vectors_adaptive_motion);
+                k_motion_vectors_motion, k_motion_vectors_region_motion, k_motion_vectors_adaptive_motion, k_collision_aovs,
+                k_collision_aovs_region, k_collision_aovs_adaptive, k_collision_aovs_motion, k_collision_aovs_region_motion,
+                k_collision_aovs_adaptive_motion);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -2149,6 +2312,28 @@ cudaError_t launch_motion_vectors(const FrameArgs& fa, const MotionVectors& mv, 
         const unsigned blocks = (unsigned)((fa.geom.n_local + 255) / 256);
         if (mo) k_motion_vectors_motion<<<blocks, 256, 0, s>>>(fa, mv, n_passes, sampled, *mo);
         else k_motion_vectors<<<blocks, 256, 0, s>>>(fa, mv, n_passes, sampled);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_collision_aovs(const FrameArgs& fa, const CollisionAovs& ca, int n_passes, int sampled, const RenderRegion* rg,
+                                  const AdaptArgs* ad, const CameraMotion* mo, cudaStream_t s)
+{
+    if (ad) {
+        if (ad->n_tiles <= 0) return cudaSuccess;
+        if (mo) k_collision_aovs_adaptive_motion<<<ad->n_tiles, 128, 0, s>>>(fa, ca, n_passes, *ad, *mo);
+        else k_collision_aovs_adaptive<<<ad->n_tiles, 128, 0, s>>>(fa, ca, n_passes, *ad);
+    } else if (rg) {
+        const long long n = region_pixels(*rg);
+        if (n <= 0) return cudaSuccess;
+        const unsigned blocks = (unsigned)((n + 255) / 256);
+        if (mo) k_collision_aovs_region_motion<<<blocks, 256, 0, s>>>(fa, ca, n_passes, sampled, *rg, *mo);
+        else k_collision_aovs_region<<<blocks, 256, 0, s>>>(fa, ca, n_passes, sampled, *rg);
+    } else {
+        if (fa.geom.n_local <= 0) return cudaSuccess;
+        const unsigned blocks = (unsigned)((fa.geom.n_local + 255) / 256);
+        if (mo) k_collision_aovs_motion<<<blocks, 256, 0, s>>>(fa, ca, n_passes, sampled, *mo);
+        else k_collision_aovs<<<blocks, 256, 0, s>>>(fa, ca, n_passes, sampled);
     }
     return cudaGetLastError();
 }

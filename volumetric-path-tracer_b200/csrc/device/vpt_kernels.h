@@ -243,6 +243,16 @@ struct MotionVectors { float3* out = nullptr; vpt_f3 origin, lower_left_corner, 
 // motion_camera's at its shutter draw).  At most one of rg and ad.
 cudaError_t launch_motion_vectors(const FrameArgs& fa, const MotionVectors& mv, int n_passes, int sampled, const RenderRegion* rg,
                                   const AdaptArgs* ad, const CameraMotion* mo, cudaStream_t s);
+// Collision AOVs (vpt_set_collision_aovs): position[local pixel] = running means of (c Px, c Py, c Pz, c), normal and albedo those of c n and
+// c a, c = [depth > 0] of the pass sample and P = org + depth dir its first collision on its camera ray; n and a the sphere's or the volume's
+// there (collision_surface in vpt_kernels.cu).  Any output may be null.  step: the central differences' world step h (normal only).
+// brick_pool / brick_dims: volume 0's brick pool in brick mode (null otherwise; the cell table comes with FrameArgs).  Kept by
+// k_collision_aovs* in a launch of their own next to the frame's resolve (launch_collision_aovs), so no other kernel's parameter block changes.
+struct CollisionAovs { float4* position = nullptr; float3* normal = nullptr; float3* albedo = nullptr; float step = 0.f;
+                       const float* brick_pool = nullptr; int brick_dims[3] = {}; };
+// as launch_motion_vectors: one chunk of n_passes passes (sampled 0: every sample c = 0), rg / ad / mo as there
+cudaError_t launch_collision_aovs(const FrameArgs& fa, const CollisionAovs& ca, int n_passes, int sampled, const RenderRegion* rg,
+                                  const AdaptArgs* ad, const CameraMotion* mo, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);

@@ -325,6 +325,18 @@ int vpt_set_motion_vectors(vpt_context* c, float* d_vectors_f3, const vpt_camera
     return VPT_OK;
 }
 
+int vpt_set_collision_aovs(vpt_context* c, float* d_position_f4, float* d_normal_f3, float* d_albedo_f3, float gradient_step) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_collision_aovs: null context");
+    if (d_normal_f3 && !(std::isfinite(gradient_step) && gradient_step > 0.0f))
+        return fail(c, VPT_ERR_INVALID, "vpt_set_collision_aovs: gradient_step must be finite and > 0 with a normal buffer (got " + std::to_string(gradient_step) + ")");
+    vpt::CollisionAovs a;
+    a.position = reinterpret_cast<float4*>(d_position_f4); a.normal = reinterpret_cast<float3*>(d_normal_f3); a.albedo = reinterpret_cast<float3*>(d_albedo_f3);
+    a.step = gradient_step;
+    c->ca_req = a;
+    c->ca_active = false;           // all null: off from now on; otherwise the buffers take over at the next call with iteration == 0
+    return VPT_OK;
+}
+
 int vpt_set_sample_offset(vpt_context* c, uint32_t offset) {
     if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_sample_offset: null context");
     c->sample_offset_req = offset;  // taken at the next iteration-0 call
@@ -407,6 +419,8 @@ struct FramePlan {
     vpt::Mattes mattes;                   // the active instance mattes (out null: off)
     vpt::MatteIds matte_ids;              // their id plane, for the trace kernel
     vpt::MotionVectors mv;                // the active motion vectors (out null: off)
+    vpt::CollisionAovs ca;                // the active collision AOVs (all three outputs null: off)
+    bool collisions() const { return ca.position || ca.normal || ca.albedo; }
     bool region = false;                  // a render region is active: the region kernels over rg
     vpt::RenderRegion rg;
     vpt::Projection proj;                 // the frame's projection: the equirectangular kernels when equirect(proj)
@@ -522,6 +536,33 @@ static int check_motion_vector_buffer(vpt_context* c, const vpt_kernel_params& k
     return VPT_OK;
 }
 
+// The collision-AOV buffers may not share a byte with a Kernel_params output buffer, an AOV, light-group, deep-slice, matte or motion-vector
+// buffer, or with each other (n = local pixels).
+static int check_collision_aov_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    const vpt::CollisionAovs& ca = c->ca_req;
+    const struct { const char* name; const void* p; size_t bytes; } others[] = {
+        { "Kernel_params.accum_buffer", (const void*)(uintptr_t)kp.accum_buffer, 12 * n }, { "Kernel_params.depth_buffer", (const void*)(uintptr_t)kp.depth_buffer, 4 * n },
+        { "Kernel_params.cost_buffer", (const void*)(uintptr_t)kp.cost_buffer, 12 * n }, { "Kernel_params.raw_buffer", (const void*)(uintptr_t)kp.raw_buffer, 16 * n },
+        { "Kernel_params.display_buffer", (const void*)(uintptr_t)kp.display_buffer, 4 * n },
+        { "the alpha AOV buffer", c->aov_alpha, 4 * n }, { "the volume AOV buffer", c->aov_volume, 12 * n },
+        { "the sun light-group buffer", c->lg_out[0], 12 * n }, { "the point light-group buffer", c->lg_out[1], 12 * n },
+        { "the emission light-group buffer", c->lg_out[2], 12 * n }, { "the environment light-group buffer", c->lg_out[3], 12 * n },
+        { "the deep slice buffer", c->deep_req.out, 16 * n * (size_t)c->deep_req.n },
+        { "the matte buffer", c->matte_req.out, 16 * n * (size_t)c->matte_req.n },
+        { "the motion-vector buffer", c->mv_req.out, 12 * n } };
+    const struct { const char* name; const void* p; size_t bytes; } mine[3] = {
+        { "position", ca.position, 16 * n }, { "normal", ca.normal, 12 * n }, { "albedo", ca.albedo, 12 * n } };
+    for (int k = 0; k < 3; ++k) {
+        for (const auto& o : others)
+            if (byte_ranges_overlap(mine[k].p, mine[k].bytes, o.p, o.bytes))
+                return fail(c, VPT_ERR_INVALID, std::string("vpt_set_collision_aovs: the ") + mine[k].name + " buffer overlaps " + o.name);
+        for (int j = 0; j < k; ++j)
+            if (byte_ranges_overlap(mine[k].p, mine[k].bytes, mine[j].p, mine[j].bytes))
+                return fail(c, VPT_ERR_INVALID, std::string("vpt_set_collision_aovs: the ") + mine[j].name + " buffer and the " + mine[k].name + " buffer overlap");
+    }
+    return VPT_OK;
+}
+
 // The preamble of a render call of n_passes passes: validation, scene-table refresh, trace-kernel choice, chunk size and scratch buffers.
 static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned n_passes, cudaStream_t stream, FramePlan& plan) {
     vpt::FrameArgs& fa = plan.fa;
@@ -584,6 +625,10 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     const bool vectors = c->mv_active || (kp.iteration == 0 && c->mv_req.out);
     if (vectors && (vpt::equirect(proj) || vpt::ods(proj)))
         return fail(c, VPT_ERR_UNSUPPORTED, "motion vectors (vpt_set_motion_vectors) are not supported with the equirectangular or ODS projection");
+    // collision AOVs: the same rule
+    const bool collisions = c->ca_active || (kp.iteration == 0 && (c->ca_req.position || c->ca_req.normal || c->ca_req.albedo));
+    if (collisions && (vpt::equirect(proj) || vpt::ods(proj)))
+        return fail(c, VPT_ERR_UNSUPPORTED, "collision AOVs (vpt_set_collision_aovs) are not supported with the equirectangular or ODS projection");
 
     if (c->brick_pool || c->cell_table) {
         // brick / cell mode read volume 0 from their own copy of the grid: only the lean case of the direct integrator is built for them,
@@ -800,6 +845,14 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         c->mv_active = true;
         plan.mv = c->mv_req;
     }
+    if (collisions) {
+        int rc = check_collision_aov_buffers(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+        c->ca_active = true;
+        plan.ca = c->ca_req;
+        plan.ca.brick_pool = c->brick_pool;
+        for (int a = 0; a < 3; ++a) plan.ca.brick_dims[a] = c->brick_dims[a];
+    }
     // instance mattes: the map goes to the device when they take over
     if (mattes) {
         if (!c->matte_active) {
@@ -911,6 +964,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_motion_vectors(fa, plan.mv, (int)np, 1, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream); }));
             c->launches++;
         }
+        if (plan.collisions()) {
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_collision_aovs(fa, plan.ca, (int)np, 1, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream); }));
+            c->launches++;
+        }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
             return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
                                                        plan.proj, stream, plan.ods_arg())
@@ -927,6 +984,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         { int rc = vpt::comm_p2p_peers(c, stream, &peers); if (rc != VPT_OK) return rc; }
         if (plan.mv.out) {
             VPT_CUDA(c, vpt::launch_motion_vectors(fa, plan.mv, (int)(n_passes - n_sampled), 0, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream));
+            c->launches++;
+        }
+        if (plan.collisions()) {
+            VPT_CUDA(c, vpt::launch_collision_aovs(fa, plan.ca, (int)(n_passes - n_sampled), 0, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream));
             c->launches++;
         }
         if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
@@ -1062,6 +1123,10 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
             VPT_CUDA(c, timed(c, stream, 1, [&] { return launch_trace_of(c, plan, np, stream); }));
             if (plan.mv.out) {
                 VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_motion_vectors(fa, plan.mv, (int)np, 1, nullptr, &ad, plan.motion_arg(), stream); }));
+                c->launches++;
+            }
+            if (plan.collisions()) {
+                VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_collision_aovs(fa, plan.ca, (int)np, 1, nullptr, &ad, plan.motion_arg(), stream); }));
                 c->launches++;
             }
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.mattes, plan.proj, stream, plan.ods_arg()); }));

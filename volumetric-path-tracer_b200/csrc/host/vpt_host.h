@@ -133,6 +133,10 @@ struct vpt_context {
     // null: off) and activated like the AOVs, so a frame in progress keeps the target it started with (setting clears mv_active)
     vpt::MotionVectors mv_req;
     bool      mv_active = false;
+    // collision AOVs (vpt_set_collision_aovs): caller-owned [local pixel] position / normal / albedo buffers and the gradient step, checked when
+    // set (all three null: off) and activated like the AOVs
+    vpt::CollisionAovs ca_req;
+    bool      ca_active = false;
     // sample-stream offset (vpt_set_sample_offset): the one set last becomes sample_offset_cur at the next render call with iteration == 0,
     // so the passes of one frame draw consecutive streams
     uint32_t  sample_offset_req = 0, sample_offset_cur = 0;

@@ -26,7 +26,9 @@ class FrameBuffers:
     tensor, LIGHT_GROUPS order), once Renderer.enable_light_groups() has allocated them (None until then); `deep`, the deep slices
     ((K, n, 4) float32), once Renderer.enable_deep() has allocated them (None until then); `mattes`, the instance mattes ((K, n, 4) float32),
     once Renderer.enable_mattes() has allocated them (None until then); `motion`, the motion vectors ((n, 3) float32: the means of c vx,
-    c vy and c), once Renderer.enable_motion_vectors() has allocated them (None until then)."""
+    c vy and c), once Renderer.enable_motion_vectors() has allocated them (None until then); `position` ((n, 4): the means of c P and c),
+    `normal` and `albedo` ((n, 3): the means of c n and c a), the collision AOVs, once Renderer.enable_collision_aovs() has allocated them
+    (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -41,9 +43,13 @@ class FrameBuffers:
         self.deep = None
         self.mattes = None
         self.motion = None
+        self.position = None
+        self.normal = None
+        self.albedo = None
 
     def zero_(self):
         for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep, self.mattes, self.motion,
+                  self.position, self.normal, self.albedo,
                   *(self.groups.values() if self.groups else ())):
             if t is not None:
                 t.zero_()
@@ -448,6 +454,48 @@ class Renderer:
             raise N.VptError("Renderer.motion_vector_image: motion vectors are not enabled (Renderer.enable_motion_vectors(target_cam))")
         return unpremultiply_vectors(self.buffers.motion.view(self.n_local // self.width, self.width, 3))
 
+    def voxel_edge(self):
+        """The shortest world-space edge of one voxel of volume 0 (the length of the shortest of its xform's three index-axis columns)."""
+        g = self.scene.instances[0]
+        X = np.array([[g.xform[a][b] for b in range(4)] for a in range(4)], dtype=np.float64)
+        return float(np.linalg.norm(X[:3, :3], axis=0).min())
+
+    def enable_collision_aovs(self, position=True, normal=True, albedo=True, step=None):
+        """Allocate and register the collision AOVs (vpt_set_collision_aovs): buffers.position (n, 4) float32 holds per pixel the running
+        means of (c Px, c Py, c Pz, c), buffers.normal and buffers.albedo (n, 3) those of c n and c a, c the coverage [depth > 0] and P, n,
+        a the world position, normal and albedo at each sample's first collision (DESIGN.md section 8q).  A layer passed as False stays None
+        and is not kept.  step: the world step h of the density gradient's central differences; None = one voxel edge of volume 0 in world
+        units (voxel_edge()).  They take over at the next render call with kp.iteration == 0.  A step that is not finite or <= 0 with the
+        normal raises VptError and leaves the layers as they were.  n is the renderer's local pixel count."""
+        dev = self.buffers.accum.device
+        h = self.voxel_edge() if step is None else float(step)
+        pos = torch.zeros(self.n_local, 4, dtype=torch.float32, device=dev) if position else None
+        nrm = torch.zeros(self.n_local, 3, dtype=torch.float32, device=dev) if normal else None
+        alb = torch.zeros(self.n_local, 3, dtype=torch.float32, device=dev) if albedo else None
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        check(lib.vpt_set_collision_aovs(self.ctx, ptr(pos), ptr(nrm), ptr(alb), h), self.ctx, "vpt_set_collision_aovs")
+        self.buffers.position, self.buffers.normal, self.buffers.albedo = pos, nrm, alb
+
+    def disable_collision_aovs(self):
+        """Turn the collision AOVs off at once; the buffers keep what they hold."""
+        check(lib.vpt_set_collision_aovs(self.ctx, None, None, None, 0.0), self.ctx, "vpt_set_collision_aovs")
+
+    def collision_images(self):
+        """(P, n, albedo, coverage): the (H, W, 3) float32 unpremultiplied world position, normal and albedo (each divided by the coverage,
+        0 where it is 0; None for a layer not enabled) and the (H, W) coverage, which is the alpha AOV ((local rows, ...) on a partitioned
+        renderer).  The normal is the mean of unit normals: normalise it for a unit vector."""
+        b = self.buffers
+        if b.position is None:
+            raise N.VptError("Renderer.collision_images: no position layer, which holds the coverage (Renderer.enable_collision_aovs())")
+        rows = self.n_local // self.width
+        z = b.position[:, 3]
+        cov = z > 0
+        den = torch.where(cov, z, torch.ones_like(z)).unsqueeze(-1)
+        def unpre(t, k):
+            if t is None: return None
+            return torch.where(cov.unsqueeze(-1), t[:, :k] / den, torch.zeros_like(t[:, :k])).view(rows, self.width, k)
+        return unpre(b.position, 3), unpre(b.normal, 3), unpre(b.albedo, 3), z.view(rows, self.width)
+
     def set_region(self, x0, y0, x1, y1):
         """Render only the full-frame pixels [x0, x1) x [y0, y1) (vpt_set_render_region) from the next call with kp.iteration == 0 on:
         inside it every buffer gets what a full-frame render gives there, bit for bit; outside it nothing is written, so the display keeps
@@ -845,6 +893,14 @@ class DistributedRenderer:
 
     def disable_motion_vectors(self):
         self.r.disable_motion_vectors()
+
+    def enable_collision_aovs(self, position=True, normal=True, albedo=True, step=None):
+        """Renderer.enable_collision_aovs on this rank: the buffers stay rank-local (no exchange carries them); every rank passes the same
+        step (None: one voxel edge of volume 0, the same on every rank)."""
+        self.r.enable_collision_aovs(position, normal, albedo, step)
+
+    def disable_collision_aovs(self):
+        self.r.disable_collision_aovs()
 
     def set_sample_offset(self, offset):
         """Renderer.set_sample_offset on this rank; every rank sets the same offset, so the sharded frame draws the streams a single
