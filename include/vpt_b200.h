@@ -858,8 +858,9 @@ void vpt_volume_bounds(const vpt_gpu_vdb* h_volume, float out6[6]);
  * complete block (scalars + texture objects; scratch buffer pointers null); free with vpt_atmosphere_destroy(handle).
  * The tables reproduce the reference's build of the model, including the places where it departs from Bruneton's paper (later
  * orders overwrite instead of accumulate because the host passes a float4 where its kernels read an int: quirk Q17; mie_extinction
- * taken from the Mie scattering spectrum), except that table look-ups past the last texel are clamped where the reference reads
- * beyond its buffers (atmosphere_kernels.cu:366-372): the outermost texels of orders >= 2 differ by construction. */
+ * taken from the Mie scattering spectrum), except that a table look-up whose linear index leaves the table is clamped to it where
+ * the reference reads outside its buffers (atmosphere_kernels.cu:161-171, 375-395): before the delta scattering-density buffer
+ * for rays just below the horizon near the ground, one past the transmittance table's end (vpt_bruneton.cu). */
 typedef struct vpt_atmosphere_options {
     int   use_constant_solar_spectrum;   /* main.cpp:1433 default 1 */
     int   use_ozone;                     /* default 1 */
@@ -875,6 +876,20 @@ int  vpt_atmosphere_destroy(void* handle);
 int  vpt_texture_read_f4(vpt_tex_t tex, int w, int h, int d, float* host_out);
 /* Diagnostic: tex3D<float> at n arbitrary normalised coordinates (uvw: 3 floats per point). */
 int  vpt_debug_texture_sample(vpt_tex_t tex, const float* uvw, int n, float* out);
+/* Diagnostic: ONE launch of one of the six precompute kernels -- the launch vpt_atmosphere_precompute makes for that stage -- on
+ * caller-owned device tables, then a device synchronisation.  tables[9]: float4 device buffers in the order of the reference's
+ * AtmosphereParameters (definitions.h:82-90): delta irradiance, delta Rayleigh, delta Mie, delta scattering density, delta multiple
+ * scattering (256x128x32 except the irradiance ones), transmittance (256x64), irradiance (256x64), scattering, single Mie.  P's own
+ * buffer pointers are not read.  lfr: the luminance-from-radiance matrix, row-major (y_r = sum_c lfr[r*3+c] x_c).  blend (0 or 1) goes
+ * to the kernels that take it (single scattering: both of its flags); order (2..16) to the three kernels of the later orders.
+ * Anything else is refused with VPT_ERR_INVALID and nothing is launched. */
+#define VPT_BRUNETON_TRANSMITTANCE        0
+#define VPT_BRUNETON_DIRECT_IRRADIANCE    1
+#define VPT_BRUNETON_SINGLE_SCATTERING    2
+#define VPT_BRUNETON_SCATTERING_DENSITY   3
+#define VPT_BRUNETON_INDIRECT_IRRADIANCE  4
+#define VPT_BRUNETON_MULTIPLE_SCATTERING  5
+int  vpt_debug_bruneton_stage(int stage, const vpt_atmosphere* P, const vpt_devptr_t tables[9], const float lfr[9], int blend, int order);
 
 /* Thin-lens camera set-up (camera::update_camera, camera.h:110-129). */
 void vpt_camera_look_at(vpt_camera* cam, const float lookfrom[3], const float lookat[3], const float vup[3],

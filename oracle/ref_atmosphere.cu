@@ -10,6 +10,10 @@
  *                            switches of main.cpp:1433-1436 passed in by the caller.  The reference loads
  *                            "atmosphere_kernels.ptx" from the working directory (atmosphere.cpp:1190), so the
  *                            call runs with the cwd switched to `module_dir` (oracle/_ref/atmo).
+ *   vptref_atmosphere_stage: ONE launch of one of the six `calculate_*` kernels of that cubin, with the launch shape and the
+ *                            argument bytes of atmosphere::precompute (atmosphere.cpp:923-1083), on a caller-owned parameter
+ *                            block whose nine buffer pointers the caller chose.  Lets a test drive the reference chain one
+ *                            stage at a time and hand both implementations identical inputs.
  *
  * The reference's util/fileIO.cpp (OpenEXR/stb) and util/logger.cpp are not built; the five functions of
  * theirs that atmosphere.cpp links against are stubbed below: loaders report "no cached textures" (which makes
@@ -83,5 +87,55 @@ extern "C" int vptref_atmosphere_init(const char* module_dir, int use_constant_s
     if (cudaDeviceSynchronize() != cudaSuccess) return -4;
     g_atmo->update_model();                          // main.cpp:1733-1738 (exposure / white balance refresh)
     memcpy(out_params, &g_atmo->atmosphere_parameters, sizeof(AtmosphereParameters));
+    return 0;
+}
+
+/* Stage numbers are those of vpt_debug_bruneton_stage (include/vpt_b200.h).  Arguments as atmosphere::precompute passes them:
+ *   direct irradiance        int BLEND                                                  (:953)
+ *   single scattering        float4 (0, 0, B, B), mat3                                  (:982-984)
+ *   scattering density       float4 (0, 0, 0, 0), order                                 (:1027-1029)
+ *   indirect irradiance,     float4 (0, 1, 0, 0) where the kernels declare `int blend`: the int they read is the bit pattern of
+ *   multiple scattering      0.0f = 0 (quirk Q17, :1056-1082); mat3; order.  blend = 1 passes an int 1 instead (the reference never
+ *                            does; the test drives both implementations' blend paths with it).
+ * lfr9 is the luminance-from-radiance array row-major, as the host builds it (:1247-1252); the kernels receive it through
+ * mat3::toMatrix, whose storage is the transpose (matrix_math.h:686-692).  Grid: size / 8 + 1 blocks of 8x8 (x 8), as :923-980.
+ * The buffers of params464 must stay readable wherever the reference's look-ups stray (the caller surrounds them with guards). */
+static CUmodule g_stage_mod = nullptr;
+static CUfunction g_stage_fn[6] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
+
+extern "C" int vptref_atmosphere_stage(const char* module_dir, int stage, const void* params464, int blend, const float* lfr9, int order)
+{
+    static const char* names[6] = { "calculate_transmittance", "calculate_direct_irradiance", "calculate_single_scattering",
+                                    "calculate_scattering_density", "calculate_indirect_irradiance", "calculate_multiple_scattering" };
+    if (stage < 0 || stage > 5 || !params464 || !lfr9 || !module_dir) return -1;
+    cudaFree(0);
+    if (!g_stage_mod) {
+        const std::string path = std::string(module_dir) + "/atmosphere_kernels.ptx";
+        if (cuModuleLoad(&g_stage_mod, path.c_str()) != CUDA_SUCCESS) { g_stage_mod = nullptr; return -2; }
+    }
+    if (!g_stage_fn[stage] && cuModuleGetFunction(&g_stage_fn[stage], g_stage_mod, names[stage]) != CUDA_SUCCESS) return -3;
+    alignas(16) unsigned char params[464];
+    memcpy(params, params464, sizeof params);
+    float mat[9];
+    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) mat[c * 3 + r] = lfr9[r * 3 + c];
+    const int blend_int = blend;
+    const float4 blend_single = make_float4(0.0f, 0.0f, (float)blend, (float)blend);
+    const float4 blend_zero = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    const float4 blend_later = make_float4(0.0f, 1.0f, 0.0f, 0.0f);
+    const void* blend_later_arg = blend ? (const void*)&blend_int : (const void*)&blend_later;
+    int ord = order;
+    void* args[4] = { params, nullptr, nullptr, nullptr };
+    unsigned gx = SCATTERING_TEXTURE_WIDTH / 8 + 1, gy = SCATTERING_TEXTURE_HEIGHT / 8 + 1, gz = SCATTERING_TEXTURE_DEPTH / 8 + 1, bz = 8;
+    if (stage == 0) { gx = TRANSMITTANCE_TEXTURE_WIDTH / 8 + 1; gy = TRANSMITTANCE_TEXTURE_HEIGHT / 8 + 1; gz = 1; bz = 1; }
+    if (stage == 1 || stage == 4) { gx = IRRADIANCE_TEXTURE_WIDTH / 8 + 1; gy = IRRADIANCE_TEXTURE_HEIGHT / 8 + 1; gz = 1; bz = 1; }
+    switch (stage) {
+    case 1: args[1] = (void*)&blend_int; break;
+    case 2: args[1] = (void*)&blend_single; args[2] = mat; break;
+    case 3: args[1] = (void*)&blend_zero; args[2] = &ord; break;
+    case 4: case 5: args[1] = (void*)blend_later_arg; args[2] = mat; args[3] = &ord; break;
+    default: break;
+    }
+    if (cuLaunchKernel(g_stage_fn[stage], gx, gy, gz, 8, 8, bz, 0, NULL, args, NULL) != CUDA_SUCCESS) return -4;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -5;
     return 0;
 }

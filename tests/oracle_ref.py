@@ -216,6 +216,8 @@ class RefOracle:
         L.vptref_instance_xform.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.POINTER(C.c_float)]
         L.vptref_atmosphere_init.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
         L.vptref_atmosphere_init.restype = C.c_int
+        L.vptref_atmosphere_stage.argtypes = [C.c_char_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_float), C.c_int]
+        L.vptref_atmosphere_stage.restype = C.c_int
         self._loaded = False
 
     def atmosphere_init(self, atmos, use_constant_solar_spectrum=True, use_ozone=True, luminance=0, white_balance=True, exposure=1.0):
@@ -249,6 +251,16 @@ class RefOracle:
         for name in _ATMO_TABLES + ("scratch_buffers",):
             f = getattr(type(atmos), name); C.memset(C.addressof(params) + f.offset, 0, f.size)
         _store(skey, dict(digest=np.array(digest), params=np.frombuffer(bytes(params), dtype=np.uint8)))
+
+    def atmosphere_stage(self, stage, atmos, blend=0, lfr=(1, 0, 0, 0, 1, 0, 0, 0, 1), order=0):
+        """One launch of the reference's own precompute kernel for `stage` (VPT_BRUNETON_* numbering) on the buffers that
+        `atmos.scratch_buffers` points to, with atmosphere::precompute's launch shape and argument bytes.  `lfr`: the
+        luminance-from-radiance matrix, row-major.  Needs the reference build (no stored outputs: the inputs are device tables)."""
+        assert C.sizeof(atmos) == 464
+        m = (C.c_float * 9)(*[float(v) for v in lfr])
+        rc = self.lib.vptref_atmosphere_stage(os.path.join(REF_DIR, "atmo").encode(), int(stage), C.cast(C.byref(atmos), C.c_void_p),
+                                              int(blend), m, int(order))
+        if rc: raise RuntimeError(f"vptref_atmosphere_stage({stage}) -> {rc}")
 
     def fill_volume(self, d_buffer_ptr, dims, scale=0.1, noise_type=0):
         """The reference's fill_volume_buffer into a device buffer of dims[0]*dims[1]*dims[2] floats."""

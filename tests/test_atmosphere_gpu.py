@@ -2,10 +2,13 @@
 atmosphere::init (compiled unmodified into oracle/_ref), and the sky-lit render paths running on the library's own tables --
 no reference code involved in producing their inputs.
 
-Tables: compared texel for texel.  The reference's precompute indexes its scattering buffers one row / slice past the end for
-coordinates that reach 1 (atmosphere_kernels.cu:366-372) and reads whatever memory follows (zeros in the oracle harness's padded
-slab); this build clamps.  Texels whose look-ups touch that rim therefore differ BY CONSTRUCTION; the test reports how many and
-requires the rest (the interior) to agree within 2e-3 relative (fp32 quadratures of 50..500 steps, fast-math on both sides).
+Tables: compared texel for texel in all four channels, for the default options, a non-constant solar spectrum without ozone, and
+luminance mode PRECOMPUTED (five wavelength triples blended through non-identity luminance-from-radiance matrices).  The reference
+reads outside its buffers in two places (tests/test_bruneton_stages_gpu.py attributes them with guard canaries): before the start
+of its delta scattering-density buffer in multiple scattering, and one texel past the transmittance table in single scattering;
+this build clamps those look-ups to the table, and both leave no trace in the final tables.  Measured on an H100 (sm_90a):
+transmittance bit for bit; no texel of single Mie, irradiance or scattering off by more than 2e-3 relative in any option set
+(99.9 % quantiles: single Mie <= 4.8e-7, irradiance <= 1.4e-5, scattering <= 1.8e-5), so none is allowed.
 """
 import ctypes as C
 import os
@@ -68,24 +71,34 @@ def test_parameter_block_equals_reference(opts):
     a.destroy()
 
 
+TABLE_OPTION_SETS = {"default": dict(), "solar_no_ozone": dict(use_constant_solar_spectrum=False, use_ozone=False), "luminance2": dict(luminance=2)}
+# fraction of the texels with any channel off by more than 2e-3 relative: measured 0 everywhere (docstring)
+TABLE_BAD_FRACTION = {name: dict(single_mie=0.0, irradiance=0.0, scattering=0.0) for name in TABLE_OPTION_SETS}
+
+
 @needs_atmo_build
-def test_tables_against_reference_precompute(mine_default):
+@pytest.mark.parametrize("opts", list(TABLE_OPTION_SETS))
+def test_tables_against_reference_precompute(opts):
+    o = TABLE_OPTION_SETS[opts]
+    mine = V.Atmosphere(**o)
     ref = V.AtmosphereParameters()
-    oracle_ref.RefOracle().atmosphere_init(ref)
-    T_ref = V.read_atmosphere_tables(ref); T = V.read_atmosphere_tables(mine_default.params)
+    oracle_ref.RefOracle().atmosphere_init(ref, use_constant_solar_spectrum=o.get("use_constant_solar_spectrum", True), use_ozone=o.get("use_ozone", True),
+                                           luminance=o.get("luminance", 0))
+    T_ref = V.read_atmosphere_tables(ref); T = V.read_atmosphere_tables(mine.params)
     report = {}
     for name in ("transmittance", "single_mie", "irradiance", "scattering"):
-        a, b = T[name][..., :3].astype(np.float64), T_ref[name][..., :3].astype(np.float64)
-        floor = 1e-6 * max(np.abs(b).max(), 1e-30)
-        e = rel_err(a, b, floor)
+        a, b = T[name].astype(np.float64), T_ref[name].astype(np.float64)
+        floor = np.maximum(1e-6 * np.abs(b).reshape(-1, 4).max(axis=0), 1e-30)
+        e = rel_err(a, b, floor).max(axis=-1)
         bad = e > 2e-3
-        report[name] = (float(np.median(e)), float(np.quantile(e, 0.999)), float(bad.mean()), float(np.abs(b).max()))
-        print(f"{name:14s}: median rel err {report[name][0]:.3g}, 99.9 % quantile {report[name][1]:.3g}, texels off by > 2e-3: {100 * report[name][2]:.3f} %, max |ref| {report[name][3]:.3g}")
-    # first-order tables have no look-up into a scattering table: everything must agree
-    assert report["transmittance"][2] == 0.0 and report["single_mie"][2] <= 1e-4
-    # later orders: interior agrees, the rim (look-ups the reference takes beyond its buffers) is reported above
-    assert report["scattering"][2] <= 0.05 and report["irradiance"][2] <= 0.05
+        report[name] = (float(np.median(e)), float(np.quantile(e, 0.999)), float(bad.mean()), float(np.abs(b).max()), bool((a == b).all()))
+        print(f"[{opts}] {name:14s}: median rel err {report[name][0]:.3g}, 99.9 % quantile {report[name][1]:.3g}, texels off by > 2e-3: "
+              f"{100 * report[name][2]:.4f} % ({int(bad.sum())}), max |ref| {report[name][3]:.3g}{', bit for bit' if report[name][4] else ''}")
+    assert report["transmittance"][4]
+    for name, frac in TABLE_BAD_FRACTION[opts].items():
+        assert report[name][2] <= frac, (name, report[name][2], frac)
     assert np.isfinite(T["scattering"]).all() and float(np.abs(T["scattering"]).max()) > 0
+    mine.destroy()
 
 
 @needs_ref

@@ -155,7 +155,7 @@ EXPORTED_SYMBOLS = [
     "vpt_octree_info", "vpt_octree_read_flat", "vpt_bvh_build", "vpt_bvh_read", "vpt_bvh_destroy", "vpt_env_tables_compute",
     "vpt_comm_get_unique_id", "vpt_comm_init", "vpt_comm_set_gather", "vpt_comm_wait", "vpt_comm_info", "vpt_comm_destroy",
     "vpt_texture_create_3d_from_device", "vpt_procedural_fill", "vpt_bricks_create", "vpt_bricks_destroy", "vpt_set_brick_volume", "vpt_bricks_read", "vpt_debug_sampler_compare", "vpt_debug_software_sample", "vpt_atmosphere_options_defaults", "vpt_atmosphere_precompute", "vpt_atmosphere_destroy",
-    "vpt_texture_read_f4", "vpt_debug_texture_sample",
+    "vpt_texture_read_f4", "vpt_debug_texture_sample", "vpt_debug_bruneton_stage",
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
     "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
@@ -308,6 +308,11 @@ lib.vpt_atmosphere_precompute.argtypes = [C.POINTER(atmosphere_options), C.POINT
 lib.vpt_atmosphere_destroy.argtypes = [_vp]; lib.vpt_atmosphere_destroy.restype = C.c_int
 lib.vpt_texture_read_f4.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]; lib.vpt_texture_read_f4.restype = C.c_int
 lib.vpt_debug_texture_sample.argtypes = [C.c_uint64, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_float)]; lib.vpt_debug_texture_sample.restype = C.c_int
+# vpt_debug_bruneton_stage: stage numbers (VPT_BRUNETON_*)
+BRUNETON_TRANSMITTANCE, BRUNETON_DIRECT_IRRADIANCE, BRUNETON_SINGLE_SCATTERING = 0, 1, 2
+BRUNETON_SCATTERING_DENSITY, BRUNETON_INDIRECT_IRRADIANCE, BRUNETON_MULTIPLE_SCATTERING = 3, 4, 5
+lib.vpt_debug_bruneton_stage.argtypes = [C.c_int, C.POINTER(AtmosphereParameters), C.POINTER(C.c_uint64), C.POINTER(C.c_float), C.c_int, C.c_int]
+lib.vpt_debug_bruneton_stage.restype = C.c_int
 
 
 class ins_header(C.Structure):

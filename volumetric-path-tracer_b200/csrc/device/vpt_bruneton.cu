@@ -12,10 +12,14 @@
 //     atmosphere_kernels.cu:654,676: quirk Q17), so `blend` is the bit pattern of 0.0f = 0: orders 2..4 OVERWRITE the scattering
 //     and irradiance tables instead of accumulating.  The final scattering table is the 4th order alone, the single-Mie table the
 //     first order, the irradiance table the 4th order's indirect term;
-//   * the scattering look-up indexes its buffers with UNCLAMPED texel coordinates (:366-372): u = 1 addresses texel `size`, one
-//     row / slice beyond the table.  The reference reads whatever memory follows its buffers there; this build clamps the three
-//     indices to the table (the value a bounds-respecting reader would get).  The outermost texels of orders >= 2 therefore
-//     differ from the reference's by construction (tests compare the interior and report the rim).
+//   * the scattering look-up indexes its buffers with UNCLAMPED texel coordinates (:375-395): a coordinate one below 0 or at the
+//     table size addresses the neighbouring row / slice through the linear index, and this build does the same; the transmittance
+//     look-up clamps its linear index to one texel past the end (:161-171).  Where such an index leaves the buffer the reference
+//     reads whatever lies there; this build clamps the LINEAR index to the table.  Which texels read outside was measured
+//     (tests/test_bruneton_stages_gpu.py, each reference stage run with the guards around its buffers holding 0 and then 3.0): in
+//     multiple scattering, 2048 texels per order -- the first five mu rows (rays just below the horizon) of the 2nd-5th r layers
+//     -- whose look-ups near r = Rg take a negative mu coordinate in the lowest r slice and read BEFORE the delta scattering-
+//     density buffer; in single scattering, the transmittance reads one past that table's end (sun below the horizon).
 // Arithmetic keeps the reference's operand types: its double literals promote the neighbouring float products (see
 // vpt_atmosphere.cuh for why that matters 6.4e6 m from the planet centre), compiled with the same --use_fast_math.
 #include <cuda_runtime.h>
@@ -222,19 +226,23 @@ struct Model {
         const float frag_mu_s = fmodf(fx, float(kSMuS));
         const float4 uvwz = make_float4(frag_nu / float(kSNu - 1), frag_mu_s / float(kSMuS), fy / float(kSMu), fz / float(kSR));
         scattering_params(uvwz, r, mu, mu_s, nu, ground);
-        const float s = sqrt((1.0 - mu * mu) * (1.0 - mu_s * mu_s));
+        const double s = sqrt((1.0 - mu * mu) * (1.0 - mu_s * mu_s));     // the bounds are formed in double and rounded once (:362)
         nu = clampf(nu, mu * mu_s - s, mu * mu_s + s);
     }
-    // nearest-texel read of a scattering table at the two nu slices around the coordinate (:359-376), indices clamped to the table
+    // nearest-texel read of a scattering table at the two nu slices around the coordinate (:375-395).  The texel coordinates are
+    // NOT clamped per axis: like the reference, a coordinate one below 0 or at the table size addresses the neighbouring row /
+    // slice through the linear index; only a linear index outside the table (where the reference reads beyond its buffer) is
+    // clamped to the table's first / last texel.
     __device__ V3 scattering_lookup(const float4* table, float r, float mu, float mu_s, float nu, bool ground) const {
         const float4 uvwz = scattering_uvwz(r, mu, mu_s, nu, ground);
         const float tex_coord_x = uvwz.x * float(kSNu - 1);
         const float tex_x = floor(tex_coord_x);
         const float lerp = tex_coord_x - tex_x;
         const float u0 = (tex_x + uvwz.y) / float(kSNu), u1 = (tex_x + 1.0 + uvwz.y) / float(kSNu);
-        const int x0 = min(max(int(u0 * kSW), 0), kSW - 1), x1 = min(max(int(u1 * kSW), 0), kSW - 1);
-        const int y = min(max(int(uvwz.z * kSH), 0), kSH - 1), z = min(max(int(uvwz.w * kSD), 0), kSD - 1);
-        const float4 v0 = table[x0 + kSW * (y + kSH * z)], v1 = table[x1 + kSW * (y + kSH * z)];
+        const int x0 = int(u0 * kSW), x1 = int(u1 * kSW), y = int(uvwz.z * kSH), z = int(uvwz.w * kSD);
+        const int n = kSW * kSH * kSD;
+        const int i0 = min(max(x0 + kSW * (y + kSH * z), 0), n - 1), i1 = min(max(x1 + kSW * (y + kSH * z), 0), n - 1);
+        const float4 v0 = table[i0], v1 = table[i1];
         return v3(v0) * (1.0 - lerp) + v3(v1) * lerp;
     }
     __device__ V3 scattering_of_order(float r, float mu, float mu_s, float nu, bool ground, int order) const {
@@ -431,11 +439,9 @@ __global__ void k_multiple_scattering(const vpt_atmosphere atm, const Tables t, 
 
 } // namespace bru
 
-// One precompute iteration = atmosphere::precompute (atmosphere.cpp:888-1114): transmittance, direct irradiance, single scattering,
-// then for every further order {scattering density, indirect irradiance, multiple scattering}.  `blend` is the host's BLEND flag
-// (accumulate over wavelength triples, luminance mode PRECOMPUTED); the later kernels of the reference receive 0 whatever it is
-// (quirk Q17) and so do these.  `transmittance_only`: atmosphere::compute_transmittance.
-cudaError_t bruneton_iteration(const vpt_atmosphere& atm, float4* const tables[9], const float lfr9[9], int blend, int orders, int transmittance_only, cudaStream_t s)
+// One launch of one of the six table kernels (stage = VPT_BRUNETON_*, vpt_b200.h) on the nine tables in the order of definitions.h:82-90.
+// `blend` goes to every kernel that takes it (single scattering: both flags); `order` to the three kernels of the later orders.
+cudaError_t bruneton_stage(int stage, const vpt_atmosphere& atm, float4* const tables[9], const float lfr9[9], int blend, int order, cudaStream_t s)
 {
     bru::Tables t;
     t.delta_irradiance = tables[0]; t.delta_rayleigh = tables[1]; t.delta_mie = tables[2]; t.delta_density = tables[3]; t.delta_multiple = tables[4];
@@ -444,17 +450,31 @@ cudaError_t bruneton_iteration(const vpt_atmosphere& atm, float4* const tables[9
     const dim3 b2(8, 8, 1), b3(8, 8, 8);
     const dim3 gt((bru::kTW + 7) / 8, (bru::kTH + 7) / 8, 1), gi((bru::kIW + 7) / 8, (bru::kIH + 7) / 8, 1);
     const dim3 gs((bru::kSW + 7) / 8, (bru::kSH + 7) / 8, (bru::kSD + 7) / 8);
-    bru::k_transmittance<<<gt, b2, 0, s>>>(atm, t);
-    if (!transmittance_only) {
-        bru::k_direct_irradiance<<<gi, b2, 0, s>>>(atm, t, blend);
-        bru::k_single_scattering<<<gs, b3, 0, s>>>(atm, t, blend, blend, M);
-        for (int order = 2; order <= orders; ++order) {
-            bru::k_scattering_density<<<gs, b3, 0, s>>>(atm, t, order);
-            bru::k_indirect_irradiance<<<gi, b2, 0, s>>>(atm, t, 0, M, order);
-            bru::k_multiple_scattering<<<gs, b3, 0, s>>>(atm, t, 0, M);
-        }
+    switch (stage) {
+    case 0: bru::k_transmittance<<<gt, b2, 0, s>>>(atm, t); break;
+    case 1: bru::k_direct_irradiance<<<gi, b2, 0, s>>>(atm, t, blend); break;
+    case 2: bru::k_single_scattering<<<gs, b3, 0, s>>>(atm, t, blend, blend, M); break;
+    case 3: bru::k_scattering_density<<<gs, b3, 0, s>>>(atm, t, order); break;
+    case 4: bru::k_indirect_irradiance<<<gi, b2, 0, s>>>(atm, t, blend, M, order); break;
+    case 5: bru::k_multiple_scattering<<<gs, b3, 0, s>>>(atm, t, blend, M); break;
+    default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();
+}
+
+// One precompute iteration = atmosphere::precompute (atmosphere.cpp:888-1114): transmittance, direct irradiance, single scattering,
+// then for every further order {scattering density, indirect irradiance, multiple scattering}.  `blend` is the host's BLEND flag
+// (accumulate over wavelength triples, luminance mode PRECOMPUTED); the later kernels of the reference receive 0 whatever it is
+// (quirk Q17) and so do these.  `transmittance_only`: atmosphere::compute_transmittance.
+cudaError_t bruneton_iteration(const vpt_atmosphere& atm, float4* const tables[9], const float lfr9[9], int blend, int orders, int transmittance_only, cudaStream_t s)
+{
+    cudaError_t e = bruneton_stage(0, atm, tables, lfr9, 0, 0, s);
+    if (transmittance_only) return e;
+    if (e == cudaSuccess) e = bruneton_stage(1, atm, tables, lfr9, blend, 0, s);
+    if (e == cudaSuccess) e = bruneton_stage(2, atm, tables, lfr9, blend, 0, s);
+    for (int order = 2; order <= orders && e == cudaSuccess; ++order)
+        for (int stage = 3; stage <= 5 && e == cudaSuccess; ++stage) e = bruneton_stage(stage, atm, tables, lfr9, 0, order, s);
+    return e;
 }
 
 // texel centres of a float4 texture (linear filtering returns the texel itself there): tests read LUTs back through this

@@ -17,6 +17,7 @@
 
 namespace vpt {
 cudaError_t bruneton_iteration(const vpt_atmosphere& atm, float4* const tables[9], const float lfr9[9], int blend, int orders, int transmittance_only, cudaStream_t s);
+cudaError_t bruneton_stage(int stage, const vpt_atmosphere& atm, float4* const tables[9], const float lfr9[9], int blend, int order, cudaStream_t s);
 cudaError_t launch_texture_readback(unsigned long long tex, int w, int h, int d, float4* d_out, cudaStream_t s);
 cudaError_t launch_texture_sample_f1(unsigned long long tex, const float* d_uvw, int n, float* d_out, cudaStream_t s);
 }
@@ -248,6 +249,21 @@ int vpt_atmosphere_destroy(void* handle) {
     for (int i = 0; i < 4; ++i) { if (h->tex[i]) cudaDestroyTextureObject(h->tex[i]); if (h->arrays[i]) cudaFreeArray(h->arrays[i]); }
     cudaFree(h->slab);
     delete h;
+    return VPT_OK;
+}
+
+int vpt_debug_bruneton_stage(int stage, const vpt_atmosphere* P, const vpt_devptr_t tables[9], const float lfr[9], int blend, int order) {
+    if (!P || !tables || !lfr || stage < VPT_BRUNETON_TRANSMITTANCE || stage > VPT_BRUNETON_MULTIPLE_SCATTERING || blend < 0 || blend > 1 ||
+        (stage >= VPT_BRUNETON_SCATTERING_DENSITY && (order < 2 || order > 16)))
+        return vpt::fail_global(VPT_ERR_INVALID, "vpt_debug_bruneton_stage: bad arguments");
+    float4* t[9];
+    for (int i = 0; i < 9; ++i) {
+        if (!tables[i] || tables[i] % 16) return vpt::fail_global(VPT_ERR_INVALID, "vpt_debug_bruneton_stage: null or misaligned table");
+        t[i] = reinterpret_cast<float4*>(tables[i]);
+    }
+    cudaError_t e = vpt::bruneton_stage(stage, *P, t, lfr, blend, order, 0);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) return vpt::fail_global(VPT_ERR_CUDA, std::string("vpt_debug_bruneton_stage: ") + cudaGetErrorString(e));
     return VPT_OK;
 }
 
