@@ -27,6 +27,7 @@ constexpr int kSkyIrrW = 256, kSkyIrrH = 64;
 //     c*c - (pdp - pdv*pdv)          in path: FMUL, FADD            tail: FFMA(c, c, .)
 //     (rmu*rmu - r*r) + Rt*Rt        sky_radiance, both sites: FMUL, FMUL, FADD, then FADD + FMUL(Rt*Rt)
 //                                    radiance_to_point, both sites: FFMA(rmu, rmu, -r*r), then FADD + FMUL(Rt*Rt)
+//     sc*ph_r + mie*ph_m             radiance_to_point, every site: FMUL(sc, ph_r), then FFMA(mie, ph_m, .)
 // With r ~ 6.36e6 m a product rounded to fp32 is off by up to 2e6 m^2, so the forms give visibly different look-up coordinates.
 template <bool kInPath>
 struct Sky {
@@ -211,7 +212,9 @@ struct Sky {
         mie = mie - transmittance * mie_p;
         mie = mie * smooth01(0.0f, 0.01f, mu_s);      // sun-below-horizon fade
 
-        const float3 rad = sc * rayleigh_phase(nu) + mie * mie_phase(a.mie_phase_function_g, nu);
+        // the reference rounds the Rayleigh product and fuses the Mie one, at all four call sites: fma(mie, ph_m, sc * ph_r)
+        const float pr = rayleigh_phase(nu), pm = mie_phase(a.mie_phase_function_g, nu);
+        const float3 rad = f3(pfma(mie.x, pm, pmul(sc.x, pr)), pfma(mie.y, pm, pmul(sc.y, pr)), pfma(mie.z, pm, pmul(sc.z, pr)));
         return apply_luminance(rad, a.sky_spectral_radiance_to_luminance);
     }
 
