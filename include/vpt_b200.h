@@ -53,7 +53,8 @@ int  vpt_abi_sizes(size_t* out, int n);
  * lights under the direct integrator, or when the density grid is larger than twice the L2 or the scene has 64 or more instances, else 3;
  * 2 or 3 to force it),
  * "l2_sector_fetch" (0|1: while a cell table is set, ask the L2 for 32-byte DRAM fetches -- a device-wide hint, see vpt_set_cell_volume),
- * "ctas_per_sm" (0 = occupancy maximum), "generic_kernel" (1: never pick the lean instantiation), "debug_flags" (development),
+ * "ctas_per_sm" (trace CTAs per SM, each of the trace kernel's own size: 256 threads for the lean kernel at 2 rays per lane, whose
+ * maximum is 3, and 128 for the others; 0 = occupancy maximum), "generic_kernel" (1: never pick the lean instantiation), "debug_flags" (development),
  * "miss_cull" (1, the default: a pinhole HDRI frame first marks the pixels whose every jitter misses the volume's root box and the sphere,
  * and writes and reads no sample records for them -- the miss samples are rebuilt from the camera and the jitter, the frame is bit for
  * bit the same; 0: off),

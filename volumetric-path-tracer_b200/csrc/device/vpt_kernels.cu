@@ -1923,8 +1923,6 @@ cudaError_t launch_empty_ahead(SceneTables* scene, int enable, cudaStream_t s)
     return cudaGetLastError();
 }
 
-static size_t trace_smem_bytes(int slots) { return (size_t)kTraceWarps * kRayWords * 32 * slots * sizeof(float); }
-
 static BrickArgs brick_args(const float* pool, const int dims[3])
 {
     BrickArgs ba;
@@ -1940,22 +1938,22 @@ template <class F>
 static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const LightGroups& lg, const MatteIds& mi, const BrickArgs& ba, F&& f)
 {
     switch (k) {
-    case TK_LEAN_3_MATTES:           return f(+k_trace<0, true, 3, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, mi);
-    case TK_LEAN_2_MATTES:           return f(+k_trace<0, true, 2, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(2), NoAtmo{}, mi);
-    case TK_GENERIC_3_MATTES:        return f(+k_trace<0, false, 3, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, mi);
-    case TK_GENERIC_2_MATTES:        return f(+k_trace<0, false, 2, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(2), NoAtmo{}, mi);
-    case TK_VOL_3_MATTES:            return f(+k_trace<1, false, 3, false, false, MatteIds>, kTraceThreads, trace_smem_bytes(3), atm, mi);
-    case TK_GENERIC_3_GROUPS_MATTES: return f(+k_trace<0, false, 3, false, true, LightGroups, MatteIds>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, lg, mi);
-    case TK_VOL_3_GROUPS_MATTES:     return f(+k_trace<1, false, 3, false, true, LightGroups, MatteIds>, kTraceThreads, trace_smem_bytes(3), atm, lg, mi);
-    case TK_GENERIC_3:        return f(k_trace<0, false, 3>, kTraceThreads, trace_smem_bytes(3), NoAtmo{});
-    case TK_LEAN_3:           return f(k_trace<0, true, 3>, kTraceThreads, trace_smem_bytes(3), NoAtmo{});
-    case TK_VOL_3:            return f(k_trace<1, false, 3>, kTraceThreads, trace_smem_bytes(3), atm);
+    case TK_LEAN_3_MATTES:           return f(+k_trace<0, true, 3, false, false, MatteIds>, trace_threads(true, 3), trace_smem_bytes(true, 3), NoAtmo{}, mi);
+    case TK_LEAN_2_MATTES:           return f(+k_trace<0, true, 2, false, false, MatteIds>, trace_threads(true, 2), trace_smem_bytes(true, 2), NoAtmo{}, mi);
+    case TK_GENERIC_3_MATTES:        return f(+k_trace<0, false, 3, false, false, MatteIds>, trace_threads(false, 3), trace_smem_bytes(false, 3), NoAtmo{}, mi);
+    case TK_GENERIC_2_MATTES:        return f(+k_trace<0, false, 2, false, false, MatteIds>, trace_threads(false, 2), trace_smem_bytes(false, 2), NoAtmo{}, mi);
+    case TK_VOL_3_MATTES:            return f(+k_trace<1, false, 3, false, false, MatteIds>, trace_threads(false, 3), trace_smem_bytes(false, 3), atm, mi);
+    case TK_GENERIC_3_GROUPS_MATTES: return f(+k_trace<0, false, 3, false, true, LightGroups, MatteIds>, trace_threads(false, 3), trace_smem_bytes(false, 3), NoAtmo{}, lg, mi);
+    case TK_VOL_3_GROUPS_MATTES:     return f(+k_trace<1, false, 3, false, true, LightGroups, MatteIds>, trace_threads(false, 3), trace_smem_bytes(false, 3), atm, lg, mi);
+    case TK_GENERIC_3:        return f(k_trace<0, false, 3>, trace_threads(false, 3), trace_smem_bytes(false, 3), NoAtmo{});
+    case TK_LEAN_3:           return f(k_trace<0, true, 3>, trace_threads(true, 3), trace_smem_bytes(true, 3), NoAtmo{});
+    case TK_VOL_3:            return f(k_trace<1, false, 3>, trace_threads(false, 3), trace_smem_bytes(false, 3), atm);
     case TK_BRICK:            return f(k_trace_brick, kBrickThreads, (size_t)kBrickThreads * kBrickBytes, ba);
-    case TK_GENERIC_2:        return f(k_trace<0, false, 2>, kTraceThreads, trace_smem_bytes(2), NoAtmo{});
-    case TK_LEAN_2:           return f(k_trace<0, true, 2>, kTraceThreads, trace_smem_bytes(2), NoAtmo{});
-    case TK_LEAN_2_CELLS:     return f(k_trace<0, true, 2, true>, kTraceThreads, trace_smem_bytes(2), NoAtmo{});
-    case TK_GENERIC_3_GROUPS: return f(+k_trace<0, false, 3, false, true, LightGroups>, kTraceThreads, trace_smem_bytes(3), NoAtmo{}, lg);
-    case TK_VOL_3_GROUPS:     return f(+k_trace<1, false, 3, false, true, LightGroups>, kTraceThreads, trace_smem_bytes(3), atm, lg);
+    case TK_GENERIC_2:        return f(k_trace<0, false, 2>, trace_threads(false, 2), trace_smem_bytes(false, 2), NoAtmo{});
+    case TK_LEAN_2:           return f(k_trace<0, true, 2>, trace_threads(true, 2), trace_smem_bytes(true, 2), NoAtmo{});
+    case TK_LEAN_2_CELLS:     return f(k_trace<0, true, 2, true>, trace_threads(true, 2), trace_smem_bytes(true, 2), NoAtmo{});
+    case TK_GENERIC_3_GROUPS: return f(+k_trace<0, false, 3, false, true, LightGroups>, trace_threads(false, 3), trace_smem_bytes(false, 3), NoAtmo{}, lg);
+    case TK_VOL_3_GROUPS:     return f(+k_trace<1, false, 3, false, true, LightGroups>, trace_threads(false, 3), trace_smem_bytes(false, 3), atm, lg);
     default:                  return cudaErrorInvalidValue;
     }
 }

@@ -7,7 +7,7 @@
 
 namespace vpt {
 
-constexpr int kTraceThreads = 128;
+constexpr int kTraceThreads = 128;                    // CTA size of the trace kernels but the lean ones at 2 rays per lane (trace_threads)
 #ifndef VPT_TRACE_MIN_CTAS
 #define VPT_TRACE_MIN_CTAS 4
 #endif

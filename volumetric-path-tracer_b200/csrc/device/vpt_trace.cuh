@@ -38,11 +38,15 @@ enum Phase : int {
 enum ExitReason : int { EX_NONE = 0, EX_OUTSIDE, EX_DISTANCE, EX_SCATTER, EX_TR_DONE };
 enum TrKind : int { TR_SUN = 0, TR_POINT = 1, TR_SPHERE = 2 };
 
-// rays per lane: 3 (4 CTAs per SM, <= 128 registers) or 2 (5 CTAs per SM, <= 96 registers: more warps in flight, the better
-// trade when every look-up misses all caches; slower when the look-ups hit L2)
-constexpr int trace_min_ctas(int slots) { return slots == 2 ? 5 : kTraceMinCtas; }
+// rays per lane: 3 (4 CTAs of 128 threads per SM, <= 128 registers) or 2: more warps in flight, the better trade when every look-up
+// misses all caches; slower when the look-ups hit L2.  The generic kernels at 2 run 5 CTAs of 128 threads (<= 96 registers); the lean
+// ones, whose stepping loop is bound by the latency of its look-ups, run 3 CTAs of 256 threads (<= 80 registers): 24 warps per SM instead
+// of 20, because the frame tables and the hardware's per-CTA reserve are paid once per 8 warps instead of once per 4 (DESIGN.md section 4).
+constexpr int trace_threads(bool lean, int slots) { return lean && slots == 2 ? 256 : kTraceThreads; }
+constexpr int trace_min_ctas(bool lean, int slots) { return slots != 2 ? kTraceMinCtas : lean ? 3 : 5; }
 constexpr int kRayWords = 34;             // 32-bit words per ray in shared memory
-constexpr int kTraceWarps = kTraceThreads / 32;
+// the opt-in dynamic shared memory of an instantiation: its warps' parked rays
+constexpr size_t trace_smem_bytes(bool lean, int slots) { return (size_t)(trace_threads(lean, slots) / 32) * kRayWords * 32 * slots * sizeof(float); }
 
 struct PathState {
     float3 pos, dir;      // the integrator's ray
@@ -711,7 +715,7 @@ struct NoAtmo { int pad[4]; };
 // pack, not a template flag, that selects them, so every kernel without mattes keeps its name as well.
 template <class... Lg> constexpr bool has_matte_ids = (std::is_same<Lg, MatteIds>::value || ... || false);
 template <int kInteg, bool kLean, int kSlots, bool kCells = false, bool kGroups = false, class... Lg>
-__global__ void __launch_bounds__(kTraceThreads, trace_min_ctas(kSlots))
+__global__ void __launch_bounds__(trace_threads(kLean, kSlots), trace_min_ctas(kLean, kSlots))
 k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atmosphere, NoAtmo>::type atm, const Lg... lgs)
 {
     static_assert(sizeof...(Lg) == (kGroups ? 1 : 0) + (has_matte_ids<Lg...> ? 1 : 0),
@@ -721,7 +725,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     // (the LightGroups are reached through lg_of(lgs...) where they are used: a pointer variable in every instantiation, even unused,
     // moved two stack stores of k_trace<1, false, 3>)
     __shared__ FrameShared fs;
-    extern __shared__ float pool_smem[];                         // kTraceWarps x kRayWords x kPool words (opt-in dynamic shared memory)
+    extern __shared__ float pool_smem[];                         // warps x kRayWords x kPool words (opt-in dynamic shared memory)
     __shared__ EmptyAhead ea;
     // the lean kernels end walks at "empty ahead" (the render call's table, staged with the octree); the generic ones keep their hot loop
     // as it was (on the fireball, config 3, the extra code of the shortcut cost more in the fetch-bound loop than its hops saved)

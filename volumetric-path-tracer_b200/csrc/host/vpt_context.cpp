@@ -791,7 +791,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         fa.miss_mask = c->d_miss_mask;
     }
 
-    // rays per lane: 3 by default; 2 (one more CTA per SM) when warps in flight matter more than rays per warp -- a lean frame, whose
+    // rays per lane: 3 by default; 2 (more warps per SM) when warps in flight matter more than rays per warp -- a lean frame, whose
     // stepping loop is bound by the latency of its look-ups even when they hit L2, or a look-up that is a chain of cache misses: a density
     // grid that cannot live in L2 (every look-up a DRAM round trip) or long per-leaf instance lists (dependent loads) (DESIGN.md section 4).
     int slots = 3;
