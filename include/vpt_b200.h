@@ -680,6 +680,47 @@ int  vpt_temporal(vpt_context* ctx, unsigned width, unsigned height,
                   unsigned* d_out_display,        /* [H][W] BGRA words as k_resolve writes them, may be NULL */
                   void* stream);
 
+/* vpt_temporal_layers accumulates the beauty exactly as vpt_temporal does and blends further layers (the compositing AOVs, light groups,
+ * collision AOVs, deep slices, mattes, or any other full-frame planes) with the beauty's taps and history length, so additive identities
+ * between the layers and the beauty (volume + (1 - alpha) k, the sum of the light groups, the sum of the deep slices) still hold in the
+ * filtered frames, up to rounding (DESIGN.md section 8r; tests/temporal_layers_ref.py restates it).
+ *   Beauty.  d_out_f3, d_out_len and d_out_display are vpt_temporal's outputs for the same arguments, bit for bit; n_layers == 0 is
+ *     vpt_temporal.
+ *   Layers.  Each pixel uses the beauty's motion (step 1) and taps (step 2): the same taps in the same order with the same weights, and a
+ *     tap the beauty drops is dropped for every layer -- also one dropped for a non-finite beauty history colour where the layer's value
+ *     is finite.  Each channel x of each plane becomes
+ *         h_x = sum(w H_x) / sum(w)   (fmaf in tap order, divided as the beauty divides)
+ *         out_x = h_x + (x - h_x) / (float)L_new   (the beauty's L_new, accum's expression with k_resolve's flags).
+ *     Where the beauty has no history (no history buffers, v not finite, q outside the frame, no tap left, a non-finite C) out_x = x bit
+ *     for bit.  The clip (step 3) belongs to the beauty: layers are blended unclipped, so with a finite clip_sigma the identities hold
+ *     only where the clip did not move the beauty's history (the default is no clip).  A layer carries no history length and guides
+ *     nothing; a non-finite layer value in a tap that is used spreads to the pixel.  A layer whose src is d_color_f3 and whose history
+ *     is d_history_f3 comes out equal to d_out_f3 bit for bit when there is no clip, and so does each of its channels passed as a
+ *     1-channel layer.
+ *   Guarantee.  vpt_temporal's still-camera case (B == A, no clip, max_history >= F, F one-pass frames at sample offsets 0 .. F-1): every
+ *     layer k_resolve keeps with accum's running-mean rule -- alpha, volume, the light groups, the deep and matte bins, position, normal
+ *     and albedo -- equals that layer of one F-pass progressive render bit for bit, with the beauty's exceptions (a sample replaced by the
+ *     NaN / Inf guard) and the max_interactions gate.
+ *   Contract.  As vpt_temporal's: asynchronous on `stream`, deterministic, no scratch, one launch.  The fetch reads neighbours, so
+ *     nothing works in place: the caller ping-pongs each layer's two buffers as it does the beauty's.
+ *   Refused (VPT_ERR_INVALID, nothing enqueued): everything vpt_temporal refuses; n_layers > 0 with a NULL layers; n_layers above
+ *     VPT_TEMPORAL_MAX_LAYERS; a NULL src or dst; a layer history that is NULL while d_history_f3 is set, or set while it is NULL;
+ *     channels outside 1..4; count 0; any byte overlap of a dst with any input (the beauty's or a layer's), with d_out_f3, d_out_len or
+ *     d_out_display, or with another dst; any overlap of the beauty's outputs with a layer's src or history. */
+#define VPT_TEMPORAL_MAX_LAYERS 16
+typedef struct vpt_temporal_layer {
+    const float* src;       /* [count][H][W][channels] float, this frame's layer (e.g. the alpha AOV), full row-major frames */
+    const float* history;   /* same shape: the previous call's dst; NULL exactly when d_history_f3 is NULL */
+    float*       dst;       /* same shape; overlaps nothing else */
+    unsigned     channels;  /* 1..4 */
+    unsigned     count;     /* >= 1 planes of H*W pixels (K for deep slices / mattes, 1 otherwise) */
+} vpt_temporal_layer;
+int  vpt_temporal_layers(vpt_context* ctx, unsigned width, unsigned height,
+                         const float* d_color_f3, const float* d_vectors_f3, const vpt_camera* current, const vpt_camera* previous,
+                         const float* d_history_f3, const float* d_history_len, const vpt_temporal_options* opt, float exposure_scale,
+                         float* d_out_f3, float* d_out_len, unsigned* d_out_display,
+                         const vpt_temporal_layer* layers, unsigned n_layers, void* stream);
+
 /* The flattened scene tables are cached per (volumes pointer, octree root pointer, build generation of a vpt_octree_build
  * octree) and refreshed whenever a call arrives with Kernel_params.iteration == 0 (the reference application resets the
  * iteration on every scene edit, main.cpp:1667-1780).  Call this only if the GPU_VDB[] array or a foreign octree was

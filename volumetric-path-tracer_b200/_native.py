@@ -166,7 +166,7 @@ EXPORTED_SYMBOLS = [
     "vpt_ods_options_defaults", "vpt_set_projection_ods", "vpt_debug_ods_cameras",
     "vpt_set_instance_mattes",
     "vpt_comm_p2p_export_binned", "vpt_comm_p2p_binned", "vpt_comm_p2p_block_bytes_binned",
-    "vpt_set_motion_vectors", "vpt_set_sample_offset", "vpt_temporal_options_defaults", "vpt_temporal",
+    "vpt_set_motion_vectors", "vpt_set_sample_offset", "vpt_temporal_options_defaults", "vpt_temporal", "vpt_temporal_layers",
     "vpt_set_collision_aovs",
 ]
 
@@ -358,6 +358,16 @@ lib.vpt_temporal_options_defaults.argtypes = [C.POINTER(temporal_options)]; lib.
 lib.vpt_temporal.argtypes = [_vp, C.c_uint, C.c_uint, _vp, _vp, C.POINTER(camera), C.POINTER(camera), _vp, _vp, C.POINTER(temporal_options),
                              C.c_float, _vp, _vp, _vp, _vp]
 lib.vpt_temporal.restype = C.c_int
+VPT_TEMPORAL_MAX_LAYERS = 16
+
+
+class temporal_layer(C.Structure):
+    _fields_ = [("src", _vp), ("history", _vp), ("dst", _vp), ("channels", C.c_uint), ("count", C.c_uint)]
+
+
+lib.vpt_temporal_layers.argtypes = [_vp, C.c_uint, C.c_uint, _vp, _vp, C.POINTER(camera), C.POINTER(camera), _vp, _vp,
+                                    C.POINTER(temporal_options), C.c_float, _vp, _vp, _vp, C.POINTER(temporal_layer), C.c_uint, _vp]
+lib.vpt_temporal_layers.restype = C.c_int
 
 
 def temporal_defaults():

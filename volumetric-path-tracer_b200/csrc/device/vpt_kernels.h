@@ -365,6 +365,15 @@ cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t s);
 
 // Temporal filter (vpt_temporal, csrc/device/vpt_temporal.cu): k_temporal, one thread per pixel of full [H][W] frames.  history and
 // history_len are both null (no history) or both set; out_display may be null; no output overlaps an input or another output.
+// vpt_temporal_layers adds up to kTemporalMaxLayers layers, carried in the parameter block and blended with the beauty's taps and L_new;
+// a layer's history is null exactly when `history` is.
+constexpr int kTemporalMaxLayers = 16;                // VPT_TEMPORAL_MAX_LAYERS of vpt_b200.h
+struct TemporalLayer {
+    const float* src;                    // [count][H][W][channels]
+    const float* history;                // same shape
+    float*       dst;                    // same shape
+    unsigned     channels, count;        // 1..4, >= 1
+};
 struct TemporalArgs {
     int          width, height;
     unsigned     max_history;
@@ -378,6 +387,8 @@ struct TemporalArgs {
     float*       out;                    // [H][W] float3
     float*       out_len;                // [H][W]
     unsigned*    out_display;            // [H][W]
+    int          n_layers = 0;
+    TemporalLayer layers[kTemporalMaxLayers] = {};
 };
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s);
 

@@ -3,7 +3,7 @@
 // 3x3 neighbourhood and blended with accum's own running-mean arithmetic.  tests/temporal_ref.py restates it in NumPy.
 //
 //   k_temporal : one thread per pixel: motion (vectors + the environment's motion at infinity), bilinear history fetch, clip, blend,
-//                display word
+//                display word; then the layers of vpt_temporal_layers (section 8r), blended with the beauty's taps and L_new
 //
 // Deterministic: every pixel is one thread reading its taps in a fixed order, no atomics.  Compiled with vpt_kernels.cu's flags
 // (--use_fast_math), so the blend's division and the display words are k_resolve's own.  Includes neither vpt_math.cuh nor the trace
@@ -39,25 +39,43 @@ __device__ __forceinline__ bool pixel_motion(const TemporalArgs& a, const int x,
     return true;
 }
 
-// The history at q = (x + 1/2, y + 1/2) + v: the bilinear taps around q - 1/2 that lie in the frame, weigh more than 0 and hold a finite
-// colour, renormalised; *len the least history length among them.  False: no history.
-__device__ __forceinline__ bool fetch_history(const TemporalArgs& a, const int x, const int y, const float2 v, float3* h, float* len)
+// The bilinear footprint of q - 1/2, q = (x + 1/2, y + 1/2) + v: the first tap (x0, y0) and the fractions (fx, fy); tap k = 2 j + i is
+// (x0 + i, y0 + j) with weight tap_weight(fx, fy, i, j).  False: no history (v not finite, or q outside [0, W] x [0, H]).
+__device__ __forceinline__ bool footprint(const TemporalArgs& a, const int x, const int y, const float2 v, int* x0, int* y0, float* fx, float* fy)
 {
     if (!isfinite(v.x) || !isfinite(v.y)) return false;
     const float qx = __fadd_rn(__fadd_rn((float)x, 0.5f), v.x), qy = __fadd_rn(__fadd_rn((float)y, 0.5f), v.y);
     if (!(qx >= 0.0f && qx <= (float)a.width && qy >= 0.0f && qy <= (float)a.height)) return false;
     const float px = __fsub_rn(qx, 0.5f), py = __fsub_rn(qy, 0.5f);
     const float fx0 = floorf(px), fy0 = floorf(py);
-    const float fx = __fsub_rn(px, fx0), fy = __fsub_rn(py, fy0);
-    const int x0 = (int)fx0, y0 = (int)fy0;
+    *fx = __fsub_rn(px, fx0); *fy = __fsub_rn(py, fy0);
+    *x0 = (int)fx0; *y0 = (int)fy0;
+    return true;
+}
+
+__device__ __forceinline__ float tap_weight(const float fx, const float fy, const int i, const int j)
+{
+    return __fmul_rn(i ? fx : __fsub_rn(1.0f, fx), j ? fy : __fsub_rn(1.0f, fy));
+}
+
+// The history at q: the footprint's taps that lie in the frame, weigh more than 0 and hold a finite colour, renormalised; *len the least
+// history length among them; *used the taps used (bit k = 2 j + i), *sw their weights' sum in tap order.  The layers are blended with
+// exactly these taps (tap_mean).  False: no history.
+__device__ __forceinline__ bool fetch_history(const TemporalArgs& a, const int x, const int y, const float2 v, float3* h, float* len,
+                                              unsigned* used, float* sw_out)
+{
+    int x0, y0;
+    float fx, fy;
+    if (!footprint(a, x, y, v, &x0, &y0, &fx, &fy)) return false;
     float sw = 0.0f, l = 0.0f;
     float3 sh = make_float3(0.0f, 0.0f, 0.0f);
+    unsigned u = 0u;
     #pragma unroll
     for (int j = 0; j < 2; ++j) {
         #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const int tx = x0 + i, ty = y0 + j;
-            const float w = __fmul_rn(i ? fx : __fsub_rn(1.0f, fx), j ? fy : __fsub_rn(1.0f, fy));
+            const float w = tap_weight(fx, fy, i, j);
             if (!(w > 0.0f) || tx < 0 || ty < 0 || tx >= a.width || ty >= a.height) continue;
             const size_t tp = (size_t)ty * a.width + tx;
             const float3 c = ldg3(a.history, tp);
@@ -66,13 +84,40 @@ __device__ __forceinline__ bool fetch_history(const TemporalArgs& a, const int x
             l = sw > 0.0f ? fminf(l, tl) : tl;
             sw = __fadd_rn(sw, w);
             sh = make_float3(__fmaf_rn(w, c.x, sh.x), __fmaf_rn(w, c.y, sh.y), __fmaf_rn(w, c.z, sh.z));
+            u |= 1u << (2 * j + i);
         }
     }
     if (!(sw > 0.0f)) return false;
     *h = make_float3(__fdiv_rn(sh.x, sw), __fdiv_rn(sh.y, sw), __fdiv_rn(sh.z, sw));
     *len = l;
+    *used = u; *sw_out = sw;
     return true;
 }
+
+// The taps fetch_history used, for the layers: footprint, used mask and weight sum
+struct Taps {
+    int      x0, y0;
+    unsigned used;
+    float    fx, fy, sw;
+};
+
+// Channel ch of an nc-channel history plane at the beauty's taps: sum(w H) / sum(w) in the beauty's order and arithmetic
+__device__ __forceinline__ float tap_mean(const TemporalArgs& a, const Taps& t, const float* plane, const unsigned nc, const unsigned ch)
+{
+    const float* q = plane + ((ptrdiff_t)t.y0 * a.width + t.x0) * (ptrdiff_t)nc + ch;   // tap 0, which may lie outside the frame
+    const unsigned row = (unsigned)a.width * nc;
+    float s = 0.0f;
+    #pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (!((t.used >> k) & 1u)) continue;
+        const int i = k & 1, j = k >> 1;
+        s = __fmaf_rn(tap_weight(t.fx, t.fy, i, j), __ldg(q + (j * row + i * nc)), s);
+    }
+    return __fdiv_rn(s, t.sw);
+}
+
+// accum's running mean as resolve_pixel writes it, accum + (value - accum) / (float)(iteration + 1), with len for iteration + 1
+__device__ __forceinline__ float blend(const float h, const float c, const float len) { return h + (c - h) / len; }
 
 // h clamped per channel to mu +- gamma sigma of the current frame's finite colours in the 3x3 window (clipped at the frame edge)
 __device__ __forceinline__ float3 clip_history(const TemporalArgs& a, const int x, const int y, const float3 h)
@@ -111,7 +156,7 @@ __device__ __forceinline__ float3 clip_history(const TemporalArgs& a, const int 
 
 } // namespace
 
-__global__ void __launch_bounds__(256) k_temporal(const TemporalArgs a)
+__global__ void __launch_bounds__(256) k_temporal(const __grid_constant__ TemporalArgs a)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= a.width || y >= a.height) return;
@@ -122,15 +167,34 @@ __global__ void __launch_bounds__(256) k_temporal(const TemporalArgs a)
     float2 v;
     float3 h;
     float lh;
-    if (a.history && finite3(c) && pixel_motion(a, x, y, ldg3(a.vectors, p), &v) && fetch_history(a, x, y, v, &h, &lh)) {
+    Taps t;
+    t.used = 0u;
+    if (a.history && finite3(c) && pixel_motion(a, x, y, ldg3(a.vectors, p), &v) && fetch_history(a, x, y, v, &h, &lh, &t.used, &t.sw)) {
         if (isfinite(a.clip_sigma)) h = clip_history(a, x, y, h);
         len = fminf(lh + 1.0f, (float)a.max_history);
-        // accum's running mean as resolve_pixel writes it: accum + (value - accum) / (float)(iteration + 1)
-        out = make_float3(h.x + (c.x - h.x) / len, h.y + (c.y - h.y) / len, h.z + (c.z - h.z) / len);
+        out = make_float3(blend(h.x, c.x, len), blend(h.y, c.y, len), blend(h.z, c.z, len));
     }
     a.out[3 * p] = out.x; a.out[3 * p + 1] = out.y; a.out[3 * p + 2] = out.z;
     a.out_len[p] = len;
     if (a.out_display) a.out_display[p] = tonemap_display(out, a.exposure_scale).word;
+    if (a.n_layers == 0) return;
+    // the layers: every channel of every plane with the beauty's taps and L_new, unclipped; no history (t.used == 0): the value itself.
+    // The footprint is recomputed from v rather than kept across the clip, whose 3x3 window needs the registers.
+    const bool have = t.used != 0u;
+    if (have) footprint(a, x, y, v, &t.x0, &t.y0, &t.fx, &t.fy);
+    const size_t n = (size_t)a.width * a.height;
+    for (int l = 0; l < a.n_layers; ++l) {
+        const TemporalLayer& L = a.layers[l];
+        const unsigned nc = L.channels;
+        for (unsigned k = 0; k < L.count; ++k) {
+            const size_t base = (size_t)k * n * nc;
+            for (unsigned ch = 0; ch < nc; ++ch) {
+                const size_t i = base + p * nc + ch;
+                const float xv = __ldg(L.src + i);
+                L.dst[i] = have ? blend(tap_mean(a, t, L.history + base, nc, ch), xv, len) : xv;
+            }
+        }
+    }
 }
 
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s)

@@ -1302,12 +1302,16 @@ void vpt_temporal_options_defaults(vpt_temporal_options* opt) {
     opt->max_history = 16; opt->clip_sigma = INFINITY;   // DESIGN.md section 8p: the sweep
 }
 
-// Temporal filter: one k_temporal launch on `stream` (csrc/device/vpt_temporal.cu), no synchronisation, no scratch.  The fetch reads
-// neighbouring pixels of the history and the clip those of the colour, so no output may share a byte with any input.
-int vpt_temporal(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_vectors, const vpt_camera* current,
-                 const vpt_camera* previous, const float* d_history, const float* d_history_len, const vpt_temporal_options* opt,
-                 float exposure_scale, float* d_out, float* d_out_len, unsigned* d_out_display, void* stream) {
-    const std::string f("vpt_temporal");
+static_assert(vpt::kTemporalMaxLayers == VPT_TEMPORAL_MAX_LAYERS, "temporal layer limit");
+
+// Temporal filter: one k_temporal launch on `stream` (csrc/device/vpt_temporal.cu), no synchronisation, no scratch, for vpt_temporal (no
+// layers) and vpt_temporal_layers (`fn` names the caller in the messages).  The fetch reads neighbouring pixels of the histories and the
+// clip those of the colour, so no output may share a byte with any input or with another output.
+static int temporal(vpt_context* c, const char* fn, unsigned width, unsigned height, const float* d_color, const float* d_vectors,
+                    const vpt_camera* current, const vpt_camera* previous, const float* d_history, const float* d_history_len,
+                    const vpt_temporal_options* opt, float exposure_scale, float* d_out, float* d_out_len, unsigned* d_out_display,
+                    const vpt_temporal_layer* layers, unsigned n_layers, void* stream) {
+    const std::string f(fn);
     if (!c || !d_color || !d_vectors || !current || !previous || !d_out || !d_out_len)
         return fail(c, VPT_ERR_INVALID, f + ": null context, colour, vectors, camera or output");
     if (width == 0 || height == 0) return fail(c, VPT_ERR_INVALID, f + ": width and height must be >= 1");
@@ -1326,12 +1330,30 @@ int vpt_temporal(vpt_context* c, unsigned width, unsigned height, const float* d
             if (!std::isfinite(fl.v.x) || !std::isfinite(fl.v.y) || !std::isfinite(fl.v.z))
                 return fail(c, VPT_ERR_INVALID, f + ": " + k.cam + "." + fl.name + " is not finite");
     }
+    if (n_layers > 0 && !layers) return fail(c, VPT_ERR_INVALID, f + ": n_layers > 0 with a null layers array");
+    if (n_layers > VPT_TEMPORAL_MAX_LAYERS)
+        return fail(c, VPT_ERR_INVALID, f + ": at most " + std::to_string(VPT_TEMPORAL_MAX_LAYERS) + " layers");
+    for (unsigned l = 0; l < n_layers; ++l) {
+        const vpt_temporal_layer& L = layers[l];
+        const std::string at = f + ": layer " + std::to_string(l);
+        if (!L.src || !L.dst) return fail(c, VPT_ERR_INVALID, at + " has a null src or dst");
+        if (!L.history != !d_history) return fail(c, VPT_ERR_INVALID, at + ": history must be set exactly when d_history_f3 is");
+        if (L.channels < 1 || L.channels > 4) return fail(c, VPT_ERR_INVALID, at + ": channels must be 1..4");
+        if (L.count == 0) return fail(c, VPT_ERR_INVALID, at + ": count must be >= 1");
+    }
     const size_t px = (size_t)width * height;
     const size_t b3 = 3 * sizeof(float) * px, b1 = sizeof(float) * px;
-    const struct { const char* name; const void* p; size_t bytes; } ins[] = {
-        { "d_color_f3", d_color, b3 }, { "d_vectors_f3", d_vectors, b3 }, { "d_history_f3", d_history, b3 }, { "d_history_len", d_history_len, b1 } };
-    const struct { const char* name; const void* p; size_t bytes; } outs[] = {
-        { "d_out_f3", d_out, b3 }, { "d_out_len", d_out_len, b1 }, { "d_out_display", d_out_display, b1 } };
+    struct Range { std::string name; const void* p; size_t bytes; };
+    std::vector<Range> ins = { { "d_color_f3", d_color, b3 }, { "d_vectors_f3", d_vectors, b3 }, { "d_history_f3", d_history, b3 },
+                               { "d_history_len", d_history_len, b1 } };
+    std::vector<Range> outs = { { "d_out_f3", d_out, b3 }, { "d_out_len", d_out_len, b1 }, { "d_out_display", d_out_display, b1 } };
+    for (unsigned l = 0; l < n_layers; ++l) {
+        const size_t n = (size_t)layers[l].count * layers[l].channels * sizeof(float) * px;
+        const std::string at = "layer " + std::to_string(l);
+        ins.push_back({ at + " src", layers[l].src, n });
+        ins.push_back({ at + " history", layers[l].history, n });
+        outs.push_back({ at + " dst", layers[l].dst, n });
+    }
     for (const auto& w : outs) {
         for (const auto& r : ins)
             if (byte_ranges_overlap(w.p, w.bytes, r.p, r.bytes)) return fail(c, VPT_ERR_INVALID, f + ": " + w.name + " overlaps " + r.name);
@@ -1345,9 +1367,27 @@ int vpt_temporal(vpt_context* c, unsigned width, unsigned height, const float* d
     a.b_origin = previous->origin; a.b_llc = previous->lower_left_corner; a.b_horizontal = previous->horizontal; a.b_vertical = previous->vertical;
     a.color = d_color; a.vectors = d_vectors; a.history = d_history; a.history_len = d_history_len;
     a.out = d_out; a.out_len = d_out_len; a.out_display = d_out_display;
+    a.n_layers = (int)n_layers;
+    for (unsigned l = 0; l < n_layers; ++l)
+        a.layers[l] = vpt::TemporalLayer{ layers[l].src, layers[l].history, layers[l].dst, layers[l].channels, layers[l].count };
     VPT_CUDA(c, vpt::launch_temporal(a, (cudaStream_t)stream));
     c->launches++;
     return VPT_OK;
+}
+
+int vpt_temporal(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_vectors, const vpt_camera* current,
+                 const vpt_camera* previous, const float* d_history, const float* d_history_len, const vpt_temporal_options* opt,
+                 float exposure_scale, float* d_out, float* d_out_len, unsigned* d_out_display, void* stream) {
+    return temporal(c, "vpt_temporal", width, height, d_color, d_vectors, current, previous, d_history, d_history_len, opt, exposure_scale,
+                    d_out, d_out_len, d_out_display, nullptr, 0, stream);
+}
+
+int vpt_temporal_layers(vpt_context* c, unsigned width, unsigned height, const float* d_color, const float* d_vectors,
+                        const vpt_camera* current, const vpt_camera* previous, const float* d_history, const float* d_history_len,
+                        const vpt_temporal_options* opt, float exposure_scale, float* d_out, float* d_out_len, unsigned* d_out_display,
+                        const vpt_temporal_layer* layers, unsigned n_layers, void* stream) {
+    return temporal(c, "vpt_temporal_layers", width, height, d_color, d_vectors, current, previous, d_history, d_history_len, opt,
+                    exposure_scale, d_out, d_out_len, d_out_display, layers, n_layers, stream);
 }
 
 // Statistics accumulated since the last call (needs option "count_stats"): out[0..4] = volume lookups, lane-steps,

@@ -202,18 +202,27 @@ class Renderer:
         out, out_len = out.view(H, W, 3), out_len.view(H, W)
         return (out, out_len, words) if display else (out, out_len)
 
-    def enable_temporal(self, max_history=None, clip_sigma=None):
+    def enable_temporal(self, max_history=None, clip_sigma=None, layers=()):
         """Start temporal accumulation for render_temporal(): a viewer loop that restarts every frame at kp.iteration = 0 keeps converging
         while the camera moves.  Allocates the motion vectors and two history buffers; the next render_temporal() has no history.
-        max_history / clip_sigma: vpt_temporal's options (None = the library's defaults).  One context only (n_ranks == 1)."""
+        max_history / clip_sigma: vpt_temporal's options (None = the library's defaults).  layers: names of Renderer.temporal_layers
+        (e.g. ("alpha", "volume", *LIGHT_GROUPS)), each of which must be enabled; every frame then blends them with the beauty's taps
+        (vpt_temporal_layers) into two history buffers of their own, read by temporal_layer_images().  One context only (n_ranks == 1)."""
         if self.n_ranks > 1:
             raise N.VptError("Renderer.enable_temporal: one context only; a partitioned frame calls Renderer.temporal on full frames")
+        names = tuple(layers)
+        for name in names:
+            if name not in _TEMPORAL_LAYERS:
+                raise N.VptError(f"Renderer.enable_temporal: unknown layer {name!r} (one of {', '.join(_TEMPORAL_LAYERS)})")
+            self._layer_buffer(name, "Renderer.enable_temporal")
         dev = self.buffers.accum.device
         self.buffers.motion = torch.zeros(self.n_local, 3, dtype=torch.float32, device=dev)
         n = self.width * self.height
         self._temporal = {"max_history": max_history, "clip_sigma": clip_sigma, "passes": 0, "prev_cam": None, "size": None, "k": 0,
                           "out": [torch.empty(n * 3, dtype=torch.float32, device=dev) for _ in range(2)],
-                          "len": [torch.empty(n, dtype=torch.float32, device=dev) for _ in range(2)]}
+                          "len": [torch.empty(n, dtype=torch.float32, device=dev) for _ in range(2)],
+                          "layers": {name: [torch.empty(self._temporal_layer_shape(name), dtype=torch.float32, device=dev) for _ in range(2)]
+                                     for name in names}}
 
     def render_temporal(self, cam: N.camera, n_passes, display=False):
         """One frame of a moving camera: n_passes passes from kp.iteration = 0 with camera `cam`, filtered against the previous frame's
@@ -233,13 +242,29 @@ class Renderer:
         self.kp.iteration = 0
         self.render(n_passes)
         k = st["k"]
-        res = self.temporal(prev, history=st["out"][k ^ 1] if have else None, history_len=st["len"][k ^ 1] if have else None,
-                            max_history=st["max_history"], clip_sigma=st["clip_sigma"], display=display, out=st["out"][k], out_len=st["len"][k])
+        kw = dict(history=st["out"][k ^ 1] if have else None, history_len=st["len"][k ^ 1] if have else None, max_history=st["max_history"],
+                  clip_sigma=st["clip_sigma"], display=display)
+        if st["layers"]:
+            lay = self.temporal_layers(prev, tuple(st["layers"]), layer_history={n: b[k ^ 1] for n, b in st["layers"].items()} if have else None,
+                                       out={"beauty": st["out"][k], "len": st["len"][k], **{n: b[k] for n, b in st["layers"].items()}}, **kw)
+            res = (lay["beauty"], lay["len"], lay["display"]) if display else (lay["beauty"], lay["len"])
+        else:
+            res = self.temporal(prev, out=st["out"][k], out_len=st["len"][k], **kw)
         st["passes"] += int(n_passes)
         st["prev_cam"] = type(cam).from_buffer_copy(cam)
         st["size"] = size
         st["k"] = k ^ 1
         return res
+
+    def temporal_layer_images(self):
+        """The layers enable_temporal(layers=...) named, as the last render_temporal() filtered them: a dict of views of the history
+        buffers in Renderer.temporal_layers' shapes (the next render_temporal() overwrites the other buffer, not these)."""
+        st = getattr(self, "_temporal", None)
+        if st is None:
+            raise N.VptError("Renderer.temporal_layer_images: temporal accumulation is not enabled (Renderer.enable_temporal())")
+        if st["prev_cam"] is None:
+            raise N.VptError("Renderer.temporal_layer_images: no frame rendered since enable_temporal()")
+        return {name: b[st["k"] ^ 1] for name, b in st["layers"].items()}
 
     def disable_temporal(self):
         """Stop temporal accumulation: drops the history, turns the motion vectors off and sets the sample offset back to 0 (from the next
@@ -247,6 +272,84 @@ class Renderer:
         self._temporal = None
         self.disable_motion_vectors()
         self.set_sample_offset(0)
+
+    def temporal_layers(self, previous_cam: N.camera, layers, layer_history=None, color=None, vectors=None, history=None, history_len=None,
+                        max_history=None, clip_sigma=None, display=False, stream=None, out=None):
+        """Renderer.temporal of `color` together with layers blended with the beauty's own taps and history length (vpt_temporal_layers),
+        so the filtered layers still add up to the filtered frame (DESIGN.md section 8r).  Returns a dict: "beauty" (H, W, 3) and "len"
+        (H, W), equal bit for bit to Renderer.temporal with the same arguments, "display" with display=True, and one entry per layer:
+        "alpha" (H, W); "volume", each name of LIGHT_GROUPS, "normal" and "albedo" (H, W, 3); "position" (H, W, 4); "deep" and "mattes"
+        (K, H, W, 4).
+        layers: an iterable of those names, taken from this renderer's buffers (they must be enabled), or a dict mapping names to full-frame
+        tensors of those shapes (a partitioned renderer must pass a dict).  layer_history: a dict of the previous call's layer outputs by
+        name, given exactly when `history` is.  The other arguments are Renderer.temporal's.  out: None = new tensors, or a dict of tensors
+        to write for "beauty", "len" and every layer (none may overlap an input or another output)."""
+        H, W = self.height, self.width
+        if color is None:
+            if self.n_ranks > 1:
+                raise N.VptError("Renderer.temporal_layers: a partitioned renderer holds no full frame; pass `color` and `vectors`")
+            color = self.buffers.accum
+        if vectors is None:
+            if self.buffers.motion is None or self.n_ranks > 1:
+                raise N.VptError("Renderer.temporal_layers: no motion vectors (Renderer.enable_motion_vectors(previous_cam)) and none passed")
+            vectors = self.buffers.motion
+        if (layer_history is None) != (history is None):
+            raise N.VptError("Renderer.temporal_layers: layer_history must be given exactly when history is")
+        dev = color.device
+        color = _frame_tensor(color, H * W * 3, "color", dev)
+        vectors = _frame_tensor(vectors, H * W * 3, "vectors", dev)
+        history = _frame_tensor(history, H * W * 3, "history", dev)
+        history_len = _frame_tensor(history_len, H * W, "history_len", dev)
+        named = dict(layers) if isinstance(layers, dict) else {name: None for name in layers}
+        if len(named) > N.VPT_TEMPORAL_MAX_LAYERS:
+            raise N.VptError(f"Renderer.temporal_layers: {len(named)} layers (at most {N.VPT_TEMPORAL_MAX_LAYERS})")
+        out = dict(out or {})
+        res = {"beauty": out.get("beauty"), "len": out.get("len")}
+        res["beauty"] = torch.empty(H, W, 3, dtype=torch.float32, device=dev) if res["beauty"] is None else \
+            _frame_tensor(res["beauty"], H * W * 3, "out beauty", dev)
+        res["len"] = torch.empty(H, W, dtype=torch.float32, device=dev) if res["len"] is None else _frame_tensor(res["len"], H * W, "out len", dev)
+        if display:
+            res["display"] = torch.empty(H, W, dtype=torch.int32, device=dev)
+        descs = (N.temporal_layer * max(1, len(named)))()
+        for i, (name, t) in enumerate(named.items()):
+            if name not in _TEMPORAL_LAYERS:
+                raise N.VptError(f"Renderer.temporal_layers: unknown layer {name!r} (one of {', '.join(_TEMPORAL_LAYERS)})")
+            if t is None:
+                if self.n_ranks > 1:
+                    raise N.VptError(f"Renderer.temporal_layers: a partitioned renderer holds no full frame of {name!r}; pass a dict of "
+                                     "full-frame tensors")
+                t = self._layer_buffer(name, "Renderer.temporal_layers")
+            k = t.shape[0] if name in ("deep", "mattes") else 1
+            ch = _TEMPORAL_LAYERS[name]
+            t = _frame_tensor(t, k * H * W * ch, name, dev)
+            hist = None
+            if layer_history is not None:
+                if name not in layer_history:
+                    raise N.VptError(f"Renderer.temporal_layers: layer_history has no {name!r}")
+                hist = _frame_tensor(layer_history[name], k * H * W * ch, f"{name} history", dev)
+            shape = self._temporal_layer_shape(name, k)
+            dst = torch.empty(shape, dtype=torch.float32, device=dev) if out.get(name) is None else \
+                _frame_tensor(out[name], k * H * W * ch, f"out {name}", dev).view(shape)
+            res[name] = dst
+            descs[i] = N.temporal_layer(t.data_ptr(), hist.data_ptr() if hist is not None else None, dst.data_ptr(), ch, k)
+        opt = N.temporal_options()
+        lib.vpt_temporal_options_defaults(C.byref(opt))
+        if max_history is not None: opt.max_history = int(max_history)
+        if clip_sigma is not None: opt.clip_sigma = float(clip_sigma)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        check(lib.vpt_temporal_layers(self.ctx, W, H, ptr(color), ptr(vectors), C.byref(self.cam), C.byref(previous_cam), ptr(history),
+                                      ptr(history_len), C.byref(opt), float(self.kp.exposure_scale), ptr(res["beauty"]), ptr(res["len"]),
+                                      ptr(res.get("display")), descs, len(named), C.c_void_p(stream or 0)), self.ctx, "vpt_temporal_layers")
+        res["beauty"], res["len"] = res["beauty"].view(H, W, 3), res["len"].view(H, W)
+        return res
+
+    def _temporal_layer_shape(self, name, k=None):
+        """The full-frame shape of layer `name` as Renderer.temporal_layers returns it (k: the planes of deep / mattes; None = this
+        renderer's own)."""
+        H, W, ch = self.height, self.width, _TEMPORAL_LAYERS[name]
+        if name in ("deep", "mattes"):
+            return (self._layer_buffer(name).shape[0] if k is None else k, H, W, ch)
+        return (H, W) if ch == 1 else (H, W, ch)
 
     def denoise_layers(self, layers, color=None, depth=True, rel_error=None, iterations=5, sigma_luminance=4.0, sigma_depth=0.2,
                        stream=None, display=False):
@@ -302,23 +405,27 @@ class Renderer:
                                      ptr(out), ptr(words), descs, len(srcs), C.c_void_p(stream or 0)), self.ctx, "vpt_denoise_layers")
         return res
 
-    def _layer_buffer(self, name):
-        """This renderer's own buffer of denoise layer `name`, or VptError when it is not enabled."""
+    def _layer_buffer(self, name, caller="Renderer.denoise_layers"):
+        """This renderer's own buffer of layer `name`, or VptError (naming `caller`) when it is not enabled."""
         b = self.buffers
         if name in ("alpha", "volume"):
             if getattr(b, name) is None:
-                raise N.VptError(f"Renderer.denoise_layers: layer {name!r} needs the AOVs (Renderer.enable_aovs())")
+                raise N.VptError(f"{caller}: layer {name!r} needs the AOVs (Renderer.enable_aovs())")
             return getattr(b, name)
         if name in LIGHT_GROUPS:
             if b.groups is None:
-                raise N.VptError(f"Renderer.denoise_layers: layer {name!r} needs the light groups (Renderer.enable_light_groups())")
+                raise N.VptError(f"{caller}: layer {name!r} needs the light groups (Renderer.enable_light_groups())")
             return b.groups[name]
+        if name in ("position", "normal", "albedo"):
+            if getattr(b, name) is None:
+                raise N.VptError(f"{caller}: layer {name!r} needs the collision AOVs (Renderer.enable_collision_aovs())")
+            return getattr(b, name)
         if name == "deep":
             if b.deep is None:
-                raise N.VptError("Renderer.denoise_layers: layer 'deep' needs the deep slices (Renderer.enable_deep(bounds))")
+                raise N.VptError(f"{caller}: layer 'deep' needs the deep slices (Renderer.enable_deep(bounds))")
             return b.deep
         if b.mattes is None:
-            raise N.VptError("Renderer.denoise_layers: layer 'mattes' needs the instance mattes (Renderer.enable_mattes(sets))")
+            raise N.VptError(f"{caller}: layer 'mattes' needs the instance mattes (Renderer.enable_mattes(sets))")
         return b.mattes
 
     def enable_aovs(self):
@@ -661,6 +768,9 @@ _EXCHANGE_LAYERS = {**N.LAYER_BITS, "motion": N.VPT_LAYER_MOTION}
 
 # the layers Renderer.denoise_layers takes by name, and their channels per pixel
 _DENOISE_LAYERS = {"alpha": 1, "volume": 3, **{g: 3 for g in LIGHT_GROUPS}, "deep": 4, "mattes": 4}
+# the layers Renderer.temporal_layers takes by name: the denoise layers and the collision AOVs (the motion vectors and depth are the
+# filter's inputs, not its layers)
+_TEMPORAL_LAYERS = {**_DENOISE_LAYERS, "position": 4, "normal": 3, "albedo": 3}
 
 
 def _layer_names(layers):
