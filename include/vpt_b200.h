@@ -574,6 +574,10 @@ int  vpt_set_sample_offset(vpt_context* ctx, uint32_t offset);
  *         w = exp(-|Y_p - Y_q| / (sigma_luminance sqrt(g) + 1e-10) - |z_p - z_q| / (sigma_depth max(|z_p|, |z_q|) + 1e-6))
  *     (no depth term when d_depth is NULL; the centre tap weighs 1), and c' = sum(h w c_q) / sum(h w), v' = sum((h w)^2 v_q) / sum(h w)^2.
  *   Non-finite pixels.  A pixel whose colour (or luminance) is not finite is copied unchanged and has weight 0 as a neighbour.
+ *   Float32.  The filter computes in float32 with denormals flushed to zero: a v below 2^-126 is 0 (a pixel whose 3x3 window of v is all
+ *     below it is copied), an h w below 2^-126 drops out and one whose square is below it adds 0 to v' (against an infinite v_q that makes
+ *     v' NaN, and a pixel whose g then sees the NaN is copied); |Y_p - Y_q| is formed in float32, so luminances near FLT_MAX of opposite
+ *     sign are inf apart and drop each other as taps, even where g is infinite.
  *   Outputs.  The last level writes d_out_f3 and, if d_out_display is given, the display word of each pixel exactly as k_resolve packs it
  *     (ACES, exposure_scale, gamma 2.2, BGRA).  A zero error map therefore reproduces the colour and k_resolve's display words bit for bit.
  *   Contract.  The work is enqueued asynchronously on `stream` (a cudaStream_t), with no synchronisation.  All buffers are full row-major

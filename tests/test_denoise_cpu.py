@@ -1,8 +1,9 @@
-"""The denoiser without a GPU: the NumPy restatement of vpt_denoise (tests/denoise_ref.py) on synthetic frames, and the host-only parts
-of the C entry points."""
+"""The denoiser without a GPU: the NumPy restatement of vpt_denoise (tests/denoise_ref.py) on synthetic frames, its float32 rules (the
+flush to zero and the float32 luminance difference), its pass rule, and the host-only parts of the C entry points."""
 import ctypes as C
 
 import numpy as np
+import pytest
 
 import denoise_ref as D
 
@@ -10,6 +11,17 @@ import denoise_ref as D
 def grey(a):
     """(H, W) -> (H, W, 3) with r = g = b, so Y equals the value (the luminance weights sum to 1)."""
     return np.repeat(np.asarray(a, np.float32)[..., None], 3, axis=-1)
+
+
+def noisy_ramp(h, w, seed, noise=0.1):
+    """A tinted ramp along x and y with `noise` relative Gaussian noise per channel -> (colour, depth, error map), float32."""
+    rng = np.random.RandomState(seed)
+    x = np.arange(w)[None, :] / max(w - 1, 1); y = np.arange(h)[:, None] / max(h - 1, 1)
+    base = 0.5 + 1.0 * x + 0.5 * y
+    c = (base[..., None] * np.array([0.8, 1.0, 1.2]) * (1 + noise * rng.randn(h, w, 3))).astype(np.float32)
+    z = (2 + 3 * x + 0.5 * y + 0.05 * rng.randn(h, w)).astype(np.float32)
+    err = (noise * (0.5 + rng.rand(h, w))).astype(np.float32)
+    return c, z, err
 
 
 def test_zero_error_map_is_the_identity_bit_for_bit():
@@ -112,3 +124,88 @@ def test_options_defaults_and_null_context_fail_loudly():
     assert C.sizeof(N.denoise_options) == 12
     rc = N.lib.vpt_denoise(None, 4, 4, C.c_void_p(16), None, None, None, 1.0, C.c_void_p(64), None, None)
     assert rc == -1 and b"vpt_denoise" in N.lib.vpt_last_error(None)
+
+
+def test_a_denormal_variance_is_flushed_and_its_window_copied():
+    """err = 1e-20 at Y ~ 0.5 gives v ~ 2.5e-41, a float32 denormal the device flushes to 0: a pixel whose whole 3x3 window is like that
+    has g == 0 and is copied.  Without the flush the restatement filters it."""
+    rng = np.random.RandomState(11)
+    c = grey(0.5 + 0.01 * rng.rand(3, 3))
+    err = np.full((3, 3), 1e-20, np.float32)
+    assert (D.noise_variance(c, err) == 0).all()
+    assert 0 < D.noise_variance(c, err, ftz=False).min() < D.FLT_MIN
+    out, copied = D.denoise_and_copies(c, rel_error=err)
+    assert copied.all() and np.array_equal(out.view(np.uint32), c.view(np.uint32))
+    out64, copied64 = D.denoise_and_copies(c, rel_error=err, ftz=False)
+    assert not copied64.any()
+    # one normal v in the window: every pixel next to it is filtered again
+    err[1, 1] = 0.05
+    assert not D.copied_pixels(c, rel_error=err).any()
+    assert D.flush(np.array([1e-40, -1e-40, 2e-38, np.nan, -np.inf], np.float32)).tolist()[:3] == [0.0, 0.0, np.float32(2e-38)]
+    assert np.signbit(D.flush(np.float32(-1e-40)))
+
+
+def test_the_luminance_difference_overflows_in_float32():
+    """Grey +-3e38 side by side in a 5x1 frame with an infinite error map: g = inf makes inv_l 0, |Y_p - Y_q| is inf in float32, and
+    inf * 0 = NaN drops the tap, so each sign averages only with itself.  In float64 the difference is finite and every tap weighs 1."""
+    c = grey(np.array([[3e38, 3e38, -3e38, -3e38, 3e38]], np.float32))
+    err = np.full((1, 5), np.inf, np.float32)
+    out = D.denoise(c, rel_error=err, iterations=1)[0, :, 0]
+    assert np.isinf(D.noise_variance(c, err)).all()
+    assert (np.sign(out) == np.sign(c[0, :, 0])).all() and (np.abs(out) > 2.9e38).all(), out
+    mixed = D.denoise(c, rel_error=err, iterations=1, ftz=False)[0, :, 0]   # the float32 difference in either mode
+    assert np.array_equal(mixed, out)
+    # the same frame at 1e37: no overflow, every tap weighs 1, so the two signs mix
+    small = D.denoise(c * np.float32(1 / 30), rel_error=err, iterations=1)[0, :, 0]
+    assert abs(small[1]) < 1e37 and abs(small[2]) < 1e37
+
+
+def test_an_infinite_variance_behind_a_tiny_tap_weight_turns_nan():
+    """A tap whose h w squares below 2^-126 weighs 0 in the variance on the device; against an infinite v that is 0 * inf = NaN, and a
+    pixel whose g sees a NaN v is copied.  Pixel 6 (Y 2, finite g, inv_l 12.5) reaches pixel 8 (Y 7, v = inf) with e = 62.5."""
+    c = grey(np.array([[2.0] * 8 + [7.0]], np.float32))
+    err = np.array([[0.01] * 8 + [np.inf]], np.float32)
+    v, ok = D.noise_variance(c, err), D.finite_pixels(c)
+    filt, taps = D.level_taps(v, D.luminance(c), np.zeros(v.shape, np.float32), ok, 1, 4.0, 0.2, False)
+    hw = {dx: t[0, 6] for dy, dx, t, _ in taps if dy == 0}
+    assert D.FLT_MIN < hw[2] and hw[2] ** 2 < D.FLT_MIN, hw
+    v1, v1_64 = D.next_variance(v, filt, taps), D.next_variance(v, filt, taps, ftz=False)
+    assert np.isnan(v1[0, 6]) and np.isinf(v1_64[0, 6])
+    assert np.isinf(v1[0, 7]) and np.isinf(v1[0, 8]) and np.isfinite(v1[0, :6]).all()
+    # at the next level every pixel whose 3x3 window holds that NaN is copied
+    nxt = list(D.filter_levels(c, rel_error=err, iterations=2))[1][1]
+    assert not nxt[0, 5:8].any() and nxt[0, :4].all()
+
+
+@pytest.mark.parametrize("option", ["iterations", "sigma_luminance", "sigma_depth"])
+def test_every_option_changes_the_output_on_a_noisy_ramp(option):
+    """Each value the GPU tests give an option moves the restatement's output away from the default-option output by far more than the
+    GPU tolerance, so an option the device ignored could not pass them."""
+    values = {"iterations": (1, 2, 3, 6, 10), "sigma_luminance": (0.25, 64.0), "sigma_depth": (0.01, 5.0)}[option]
+    for w, h in ((67, 45), (1100, 7), (1, 300), (300, 1)):
+        c, z, err = noisy_ramp(h, w, 1)
+        base = D.denoise(c, z, err)
+        for v in values:
+            out = D.denoise(c, z, err, **{option: v})
+            moved = float((np.abs(out.astype(np.float64) - base).max(axis=-1) / D.tolerance(c, max(5, v if option == "iterations" else 5), 1e-4)).max())
+            assert moved > 5, (w, h, option, v, moved)
+
+
+def test_the_pass_rule():
+    """compare(): the bound scales with the largest input value within reach, copied pixels must be bit for bit, kinds must match."""
+    c, z, err = noisy_ramp(9, 40, 2)
+    assert D.reach_max(c, 1).shape == (9, 40)
+    spike = np.zeros((9, 40), np.float32); spike[4, 20] = 100.0; spike[0, 0] = np.nan
+    M = D.reach_max(spike, 2)                                        # reach 6
+    assert M[4, 26] == 100 and M[4, 27] == 0 and M[0, 0] == 0 and M[0, 14] == 100
+    want, copied = D.denoise_and_copies(c, z, err)
+    assert not copied.any()
+    fails, stats = D.compare(want, want, c, copied, 5, 1e-4)
+    assert not fails and stats["worst"] == 0 and stats["bit_equal"] == 1
+    got = want.copy(); got[3, 7, 1] += np.float32(1e-3)                 # M ~ 2.2: 1e-3 is ~4x the bound
+    fails, stats = D.compare(got, want, c, copied, 5, 1e-4)
+    assert len(fails) == 1 and "outside" in fails[0] and 3 < stats["worst"] < 6
+    got = want.copy(); got[0, 0, 2] = np.inf
+    assert "kind" in D.compare(got, want, c, copied, 5, 1e-4)[0][0]
+    cp = copied.copy(); cp[5, 5] = True                               # a copied pixel must equal its input, not the restatement
+    assert "copied" in D.compare(want, want, c, cp, 5, 1e-4)[0][0]

@@ -14,7 +14,6 @@ from test_adaptive_gpu import make_case
 from test_parity_gpu import make_kp
 
 pytestmark = pytest.mark.gpu
-RTOL, ATOL, MIN_MATCH = 1e-4, 1e-5, 0.999
 
 
 @pytest.fixture(scope="module")
@@ -32,17 +31,19 @@ def noisy_frame(scene, r, passes=16, min_passes=8):
 
 
 def assert_matches_restatement(r, color, depth, err, label):
+    """Every pixel against the restatement (denoise_ref.compare) and every display word within 1 LSB of the packing of the device's colour."""
     got, words = r.denoise(color=color, depth=depth, rel_error=err, display=True)
     torch.cuda.synchronize()
     got = got.cpu().numpy(); words = words.cpu().numpy().view(np.uint32)
-    want = D.denoise(color.cpu().numpy(), None if depth is None else depth.cpu().numpy(), None if err is None else err.cpu().numpy())
-    ok = (np.abs(got.astype(np.float64) - want) <= ATOL + RTOL * np.abs(want.astype(np.float64))).all(axis=-1)
-    frac = float(ok.mean())
+    src = color.cpu().numpy()
+    want, copied = D.denoise_and_copies(src, None if depth is None else depth.cpu().numpy(), None if err is None else err.cpu().numpy())
+    fails, st = D.compare(got, want, src, copied, 5, D.RTOL)
     want_words = D.display_words(got, float(r.kp.exposure_scale))   # the words of the device's own colour: the packing alone
     lsb = max(int(np.max(np.abs(((words >> s) & 0xff).astype(int) - ((want_words >> s) & 0xff).astype(int)))) for s in (0, 8, 16))
-    moved = float(np.mean(np.any(got != color.cpu().numpy(), axis=-1)))
-    print(f"{label}: {100 * frac:.4f} % of the pixels within tolerance, display words within {lsb} LSB, {100 * moved:.1f} % of the pixels changed")
-    assert frac >= MIN_MATCH, f"{label}: {100 * (1 - frac):.3f} % of the pixels outside {ATOL} + {RTOL}*|ref|"
+    moved = float(np.mean(np.any(got != src, axis=-1)))
+    print(f"{label}: worst |d|/bound {st['worst']:.3g}, |d|/(1e-5 + M) {st['ratio']:.3g}, {100 * st['bit_equal']:.2f} % bit-equal, "
+          f"{st['copied']} copied, display words within {lsb} LSB, {100 * moved:.1f} % of the pixels changed")
+    assert not fails, f"{label}: " + "; ".join(fails)
     assert lsb <= 1 and (words >> 24 == 0xff).all()
     assert moved > 0 or color.numel() <= 3 * 21
 

@@ -10,6 +10,7 @@ import torch
 import vpt_b200 as V
 from vpt_b200.scene import synthetic_env
 import denoise_layers_ref as DL
+import denoise_ref as D
 from test_adaptive_gpu import make_case
 from test_aov_gpu import constant_env_renderer
 from test_denoise_gpu import MODES, noisy_frame
@@ -17,7 +18,6 @@ from test_exchange_binned_gpu import ALL, Case, Shards, atmosphere, dragon, emis
 from test_parity_gpu import make_kp
 
 pytestmark = pytest.mark.gpu
-RTOL, ATOL, MIN_MATCH = 1e-4, 1e-5, 0.999
 NAMES = ("alpha", "volume", *V.LIGHT_GROUPS, "deep", "mattes")
 
 
@@ -93,14 +93,16 @@ def test_layers_against_the_restatement(dragon, emissive, atmosphere):
     for g in V.LIGHT_GROUPS:
         assert float(srcs[g].abs().max()) > 0, f"light group {g} is empty"
     flat = [srcs[n].cpu().numpy() for n in srcs] + list(r.deep_image().cpu().numpy()) + list(r.matte_image().cpu().numpy())
-    beauty, want = DL.denoise_layers(color.cpu().numpy(), flat, depth.cpu().numpy(), err.cpu().numpy())
+    args = (color.cpu().numpy(), depth.cpu().numpy(), err.cpu().numpy())
+    beauty, want = DL.denoise_layers(args[0], flat, *args[1:])
+    _, copied = D.denoise_and_copies(*args)
     got = [out[n].cpu().numpy() for n in srcs] + list(out["deep"].cpu().numpy()) + list(out["mattes"].cpu().numpy())
     labels = list(srcs) + [f"deep {k}" for k in range(8)] + [f"matte {k}" for k in range(3)]
-    for label, g, w in zip(labels, got, want):
-        ok = np.abs(g.astype(np.float64) - w) <= ATOL + RTOL * np.abs(w.astype(np.float64))
-        frac = float((ok.all(axis=-1) if ok.ndim == 3 else ok).mean())
-        print(f"{label}: {100 * frac:.4f} % of the pixels within tolerance")
-        assert frac >= MIN_MATCH, label
+    for label, g, w, s in zip(labels, got, want, flat):
+        fails, st = D.compare(g, w, s, copied, 5, D.RTOL)
+        print(f"{label}: worst |d|/bound {st['worst']:.3g}, |d|/(1e-5 + M) {st['ratio']:.3g}, {100 * st['bit_equal']:.2f} % bit-equal, "
+              f"{st['copied']} copied")
+        assert not fails, f"{label}: " + "; ".join(fails)
 
 
 def test_identities_survive_denoising(dragon, emissive, atmosphere):
