@@ -653,6 +653,18 @@ int  vpt_denoise_layers(vpt_context* ctx, unsigned width, unsigned height,
  *   4. Blend.  L_new = min(L_hist + 1, max_history) and out = h' + (C - h') / (float)L_new, accum's running-mean expression of k_resolve
  *      (the reference's render_kernel.cu:2284).  With no history, no history buffers, or a non-finite C: out = C bit for bit, L_new = 1.
  *      d_out_display, if given, gets the display word of out exactly as k_resolve packs it (ACES, exposure_scale, gamma 2.2, BGRA).
+ *   Float32.  The footprint is float32: q = (float)x + 1/2 + v rounded, so a q that rounds onto 0, W or H keeps its history; px = q - 1/2
+ *     and x0 = floorf(px) (q = 0 gives x0 = -1, fx = 1/2); a tap's weight is (1 - fx)(1 - fy) etc. each rounded, and an integer px gives
+ *     weight-0 taps, which are dropped.  Lengths: the first used tap's L, then fminf with each further one, so a NaN length is ignored
+ *     while another used tap has a number, and L_hist is NaN only when every used tap's is; L_new = fminf(L_hist + 1, max_history) in
+ *     float32, so a NaN or +inf L_hist gives max_history, -inf gives -inf (out = h'), L_hist = -1 gives L_new = 0 (out = +-inf, or NaN
+ *     where C = h'), fractional and negative lengths divide as written and L_hist + 1 rounds (2^24 + 1 is 2^24).  The library's own
+ *     d_out_len is always finite and >= 1; these cases only come from caller buffers.  C - h' is formed in float32: +-inf when C and h'
+ *     lie near +-FLT_MAX with opposite signs.  The weighted history sum and its division by sum(w) are float32 and can round past
+ *     FLT_MAX.  The clip's window sum, mean and deviation are float32: a window sum that overflows gives mu = +-inf and mu - r NaN, which
+ *     fmaxf / fminf drop, so the clip does nothing on that channel; a deviation that overflows gives r = inf and no clip either.  Denormals
+ *     are flushed to zero in arithmetic (--use_fast_math): a denormal C, H, layer value or clip_sigma counts as 0 (a denormal clip_sigma
+ *     clamps h to mu), and a denormal result is stored as 0; a pixel without history keeps its input bits, denormals included.
  *   Guarantee.  A still camera, clip_sigma = +inf, max_history >= F and F one-pass frames rendered at iteration 0 with sample offsets
  *     0 .. F-1 (vpt_set_sample_offset), each filtered against the previous call's outputs: out is accum of one F-pass progressive render
  *     bit for bit, and so is the display word -- unless a sample of those frames was replaced by the reference's NaN / Inf guard, which at

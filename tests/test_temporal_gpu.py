@@ -25,7 +25,6 @@ from test_parity_gpu import make_kp
 from test_aov_gpu import make_aov_case
 from test_adaptive_gpu import make_case
 from test_exchange_layers_gpu import Case as LayerCase, Shards as LayerShards, enable_all
-import denoise_ref as D
 import temporal_ref as T
 
 pytestmark = pytest.mark.gpu
@@ -250,17 +249,16 @@ def test_the_kernel_matches_the_restatement(dragon, w, h, motion, clip):
     out, L, words = r.temporal(b, color=t(c), vectors=t(m), history=t(hist), history_len=t(ln), max_history=8, clip_sigma=clip, display=True)
     torch.cuda.synchronize()
     out, L, words = out.cpu().numpy().reshape(-1, 3), L.cpu().numpy().reshape(-1), words.cpu().numpy().reshape(-1).view(np.uint32)
-    # the history is white noise, so a rounding of the motion by 1e-4 pixels moves out by 1e-4: the motion in the kernel's float32 order
-    ref = T.temporal(w, h, c, m, a, b, hist, ln, max_history=8, clip_sigma=clip, motion_dt=np.float32)
-    assert np.array_equal(L, ref["L"]), "history lengths"
+    # the history is white noise, so a rounding of the motion by 1e-4 pixels moves out by 1e-4: the motion and the footprint in the
+    # kernel's float32 order
+    ref = T.temporal(w, h, c, m, a, b, hist, ln, max_history=8, clip_sigma=clip, motion_dt=np.float32, footprint_dt=np.float32)
+    assert np.array_equal(L.view(np.uint32), ref["L"].astype(np.float32).view(np.uint32)), "history lengths"
     used = ref["used"]
-    assert np.array_equal(out[~used].view(np.uint32), c[~used].view(np.uint32)), "no history: out = C bit for bit"
-    fin = np.isfinite(ref["out"]).all(1)
-    err = np.abs(out[fin] - ref["out"][fin])
-    assert (err <= 1e-5 + 1e-4 * np.abs(ref["out"][fin])).all(), float(err.max())
-    want = D.display_words(np.where(np.isfinite(out), out, 0.0)[fin], float(r.kp.exposure_scale))
+    fails, _ = T.compare(out, ref["out"], c, ~used, ref["M"])       # every pixel: no history => out = C bit for bit
+    assert not fails, "; ".join(fails)
+    want = T.display_words(out, float(r.kp.exposure_scale))
     for s in (0, 8, 16):
-        d = np.abs(((words[fin] >> s) & 0xFF).astype(int) - ((want >> s) & 0xFF).astype(int))
+        d = np.abs(((words >> s) & 0xFF).astype(int) - ((want >> s) & 0xFF).astype(int))
         assert d.max() <= 1, s
     if w * h > 100:
         assert used.any() and (~used).any()

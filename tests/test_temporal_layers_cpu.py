@@ -53,7 +53,7 @@ def test_the_blend_is_linear_in_float64():
     f64 = lambda t: t.astype(np.float64)
     Z, HZ = ka * f64(X) + kb * f64(Y), ka * f64(HX) + kb * f64(HY)
     # blend_layer reads float32 planes, so the combination (not float32) is blended here with the same taps
-    out_x, out_y = TL.blend_layer(bt, X, HX, 4, 2), TL.blend_layer(bt, Y, HY, 4, 2)
+    out_x, out_y = TL.blend_layer(bt, X, HX, 4, 2, diff32=False), TL.blend_layer(bt, Y, HY, 4, 2, diff32=False)
     used = bt["used"]
     fma, _ = T._ops(np.float64)
     out_z = Z.copy()
@@ -120,3 +120,32 @@ def test_refusals_that_need_no_device():
     r = V.Renderer.__new__(V.Renderer)
     with pytest.raises(V.VptError, match="not enabled"):
         r.temporal_layer_images()
+
+
+@pytest.mark.parametrize("wh", [(1, 1), (2, 1), (1, 2), (23, 17)])
+def test_the_vectorised_blend_equals_the_loop(wh):
+    from test_temporal_cpu import hostile
+    w, h = wh
+    n = w * h
+    a, b = camera((0.0, 0.0, 0.0), w=w, h=h), camera((0.02, 0.0, 0.01), yaw=0.01, w=w, h=h)
+    c, m, hist, ln = hostile(w, h, 3 * w + h)
+    rng = np.random.default_rng(w + h)
+    for fdt in (None, np.float32):
+        bt = TL.beauty_taps(w, h, c, m, a, b, hist, ln, max_history=5, footprint_dt=fdt)
+        for ch, k in ((1, 1), (2, 3), (4, 2)):
+            src, lh = (rng.uniform(-3, 3, (k, n, ch)).astype(np.float32) for _ in range(2))
+            lh[rng.random((k, n, ch)) < 0.05] = np.nan
+            want = TL.blend_layer_loop(bt, src, lh, ch, k)
+            assert np.array_equal(TL.blend_layer(bt, src, lh, ch, k, diff32=False, ftz=False), want, equal_nan=True), (wh, ch, k)
+
+
+def test_the_layer_reach_is_the_src_and_the_used_taps():
+    w, h = 4, 1
+    m = np.tile(np.array([0.5, 0.0, 1.0], np.float32), (4, 1))
+    c, hist = np.ones((4, 3), np.float32), np.ones((4, 3), np.float32)
+    hist[2] = np.nan                                             # pixel 2's tap dropped for every layer
+    bt = TL.beauty_taps(w, h, c, m, None, None, hist, np.ones(4, np.float32))
+    src = np.array([[1, -2], [0, 0], [0.5, 0], [7, np.inf]], np.float32)
+    lh = np.array([[3, 0], [-4, 1], [100, 0], [0, -6]], np.float32)
+    M = TL.layer_reach(bt, src, lh, 2)[0]
+    assert list(M) == [4, 4, 6, 7]                               # taps (0, 1), (1, -), (-, 3), (3, -)

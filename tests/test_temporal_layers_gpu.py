@@ -22,6 +22,7 @@ from test_parity_gpu import make_kp
 from test_aov_gpu import constant_env_renderer
 from test_temporal_gpu import bits, same, copy_cam, pan_cameras, look_at, synthetic, dragon  # noqa: F401 (fixture)
 import temporal_layers_ref as TL
+import temporal_ref as T
 
 pytestmark = pytest.mark.gpu
 INF = float("inf")
@@ -130,22 +131,19 @@ def test_the_layers_match_the_restatement(dragon, w, h, motion, clip):
                                  clip, max_history=8)
     torch.cuda.synchronize()
     assert rc == 0, msg
-    bt = TL.beauty_taps(w, h, c, m, a, b, hist, ln, max_history=8, motion_dt=np.float32)
-    assert np.array_equal(out_len.cpu().numpy().reshape(-1), bt["L"]), "history lengths"
+    bt = TL.beauty_taps(w, h, c, m, a, b, hist, ln, max_history=8, motion_dt=np.float32, footprint_dt=np.float32)
+    assert np.array_equal(out_len.cpu().numpy().reshape(-1).view(np.uint32), bt["L"].astype(np.float32).view(np.uint32)), "history lengths"
     used = bt["used"]
     if n > 100:
         assert used.any() and (~used).any()
     for i, (ch, k) in enumerate(specs):
         got = dsts[i].cpu().numpy().reshape(k, n, ch)
         want = TL.blend_layer(bt, srcs[i], hists[i], ch, k)
-        label = f"{ch} channels x {k}"
-        assert np.array_equal(got[:, ~used].view(np.uint32), srcs[i][:, ~used].view(np.uint32)), f"{label}: no history is the value"
-        assert np.array_equal(np.isnan(got), np.isnan(want)), f"{label}: NaNs"
-        fin = np.isfinite(want)
-        err = np.abs(got[fin] - want[fin])
-        # test_temporal_gpu's bound for the beauty, taken relative to the layers' range [-2, 2]: the values are signed, so an output can
-        # be near 0 while its taps are not
-        assert (err <= 1e-5 + 1e-4 * np.maximum(np.abs(want[fin]), 2.0)).all(), (label, float(err.max()))
+        M = TL.layer_reach(bt, srcs[i], hists[i], ch, k)
+        for p in range(k):
+            # every value: no history => the value bit for bit, non-finite in kind, finite within 1e-5 + 1e-4 M
+            fails, _ = T.compare(got[p], want[p], srcs[i][p], ~used, M[p])
+            assert not fails, f"{ch} channels x {k}, plane {p}: " + "; ".join(fails)
     if n > 100:
         assert np.isnan(dsts[2].cpu().numpy()).any(), "a NaN in a used tap spreads"
     r.close()
