@@ -1951,7 +1951,7 @@ static cudaError_t trace_kernel(TraceKernel k, const vpt_atmosphere& atm, const 
     case TK_BRICK:            return f(k_trace_brick, kBrickThreads, (size_t)kBrickThreads * kBrickBytes, ba);
     case TK_GENERIC_2:        return f(k_trace<0, false, 2>, trace_threads(false, 2), trace_smem_bytes(false, 2), NoAtmo{});
     case TK_LEAN_2:           return f(k_trace<0, true, 2>, trace_threads(true, 2), trace_smem_bytes(true, 2), NoAtmo{});
-    case TK_LEAN_2_CELLS:     return f(k_trace<0, true, 2, true>, trace_threads(true, 2), trace_smem_bytes(true, 2), NoAtmo{});
+    case TK_LEAN_2_CELLS:     return f(k_trace<0, true, 2, true>, trace_threads(true, 2, true), trace_smem_bytes(true, 2, true), NoAtmo{});
     case TK_GENERIC_3_GROUPS: return f(+k_trace<0, false, 3, false, true, LightGroups>, trace_threads(false, 3), trace_smem_bytes(false, 3), NoAtmo{}, lg);
     case TK_VOL_3_GROUPS:     return f(+k_trace<1, false, 3, false, true, LightGroups>, trace_threads(false, 3), trace_smem_bytes(false, 3), atm, lg);
     default:                  return cudaErrorInvalidValue;
@@ -2099,14 +2099,24 @@ cudaError_t launch_trace(const FrameArgs& fa, TraceKernel k, const vpt_atmospher
     });
 }
 
+static_assert(sizeof(FrameShared) + sizeof(EmptyAhead) <= kTraceTablesBytes, "k_trace's static shared memory outgrew kTraceTablesBytes");
+static_assert(trace_sm_smem_bytes(true, 2) <= kSmemPerSm && trace_sm_smem_bytes(true, 2, true) <= kSmemPerSm && trace_sm_smem_bytes(false, 2) <= kSmemPerSm,
+              "trace CTAs do not fit an SM");
+
 // Once per context (= per device): opt the trace kernels into their dynamic shared memory and record how many CTAs of each fit
-// on an SM.  The attribute is a per-device property of the function, so this must not be a process-wide static.
+// on an SM.  The attribute is a per-device property of the function, so this must not be a process-wide static.  The lean kernels at
+// 2 rays per lane must fit trace_min_ctas CTAs; under VPT_LEAN2_SHAPE 1 they ask for the least shared-memory carveout that holds them
+// (the rest of the 256 KB is L1).
 cudaError_t trace_kernels_init(int max_ctas[kTraceKernelsAll])
 {
     for (int k = 0; k < kTraceKernelsAll; ++k) {
+        const bool lean2 = k == TK_LEAN_2 || k == TK_LEAN_2_MATTES || k == TK_LEAN_2_CELLS, cells = k == TK_LEAN_2_CELLS;
         const cudaError_t e = trace_kernel((TraceKernel)k, {}, {}, {}, {}, [&](auto kernel, int threads, size_t smem, const auto&...) {
-            const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            return r != cudaSuccess ? r : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[k], kernel, threads, smem);
+            cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (r == cudaSuccess && lean2 && VPT_LEAN2_SHAPE == 1) r = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, trace_carveout_percent(true, 2, cells));
+            if (r == cudaSuccess) r = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas[k], kernel, threads, smem);
+            if (r == cudaSuccess && lean2 && max_ctas[k] < trace_min_ctas(true, 2, cells)) r = cudaErrorInvalidConfiguration;
+            return r;
         });
         if (e != cudaSuccess) return e;
     }

@@ -13,6 +13,31 @@ constexpr int kTraceThreads = 128;                    // CTA size of the trace k
 #endif
 constexpr int kTraceMinCtas = VPT_TRACE_MIN_CTAS;     // __launch_bounds__ hint: 4 CTAs x (51 KB ray slots + 4 KB tables) and <= 128 registers per thread
 
+// The shape of a k_trace instantiation (DESIGN.md section 4): CTA size, CTAs per SM (the __launch_bounds__ minimum, which sets the
+// register budget) and the words each parked ray takes in shared memory.  The lean kernels at 2 rays per lane park a 29-word record
+// (vpt_trace.cuh, PoolLean) and run one of three shapes, VPT_LEAN2_SHAPE (DESIGN.md section 4 has the timings): 2, the default = 4 CTAs
+// of 224 threads (28 warps, <= 72 registers); 0 = 3 CTAs of 256 threads (24 warps, <= 80 registers) under the driver's carveout (228 KB:
+// 28 KB of L1); 1 = the same CTAs under the 196 KB carveout, which leaves the L1 60 KB.  The cell-table kernel keeps 3 CTAs of 256 threads
+// in every shape: at 72 registers its stepping loop spills.
+#ifndef VPT_LEAN2_SHAPE
+#define VPT_LEAN2_SHAPE 2
+#endif
+constexpr int kRayWords = 34;                         // 32-bit words per parked ray (every kernel but the lean ones at 2 rays per lane)
+constexpr int kLeanRayWords = 29;                     // ... and in the lean kernels at 2 rays per lane
+constexpr int kTraceTablesBytes = 4352;               // static shared memory of k_trace: FrameShared and the empty-ahead table (asserted)
+constexpr int kSmemPerSm = 233472;                    // shared memory an SM offers to its CTAs (228 KB), and the 1 KB reserved per CTA
+constexpr int kSmemReservePerCta = 1024;
+constexpr bool trace_28_warps(bool lean, int slots, bool cells) { return lean && slots == 2 && !cells && VPT_LEAN2_SHAPE == 2; }
+constexpr int trace_threads(bool lean, int slots, bool cells = false) { return lean && slots == 2 ? (trace_28_warps(lean, slots, cells) ? 224 : 256) : kTraceThreads; }
+constexpr int trace_min_ctas(bool lean, int slots, bool cells = false) { return slots != 2 ? kTraceMinCtas : lean ? (trace_28_warps(lean, slots, cells) ? 4 : 3) : 5; }
+constexpr int trace_ray_words(bool lean, int slots) { return lean && slots == 2 ? kLeanRayWords : kRayWords; }
+// the opt-in dynamic shared memory of an instantiation: its warps' parked rays
+constexpr size_t trace_smem_bytes(bool lean, int slots, bool cells = false) { return (size_t)(trace_threads(lean, slots, cells) / 32) * trace_ray_words(lean, slots) * 32 * slots * sizeof(float); }
+// the shared memory trace_min_ctas CTAs take on an SM, and the carveout (percent of kSmemPerSm) the lean kernels at 2 rays per lane ask
+// for under VPT_LEAN2_SHAPE 1: the least that holds them.  The driver rounds a carveout up to the next capacity the SM supports (..., 164, 196, 228 KB).
+constexpr size_t trace_sm_smem_bytes(bool lean, int slots, bool cells = false) { return (size_t)trace_min_ctas(lean, slots, cells) * (trace_smem_bytes(lean, slots, cells) + kTraceTablesBytes + kSmemReservePerCta); }
+constexpr int trace_carveout_percent(bool lean, int slots, bool cells = false) { return (int)((trace_sm_smem_bytes(lean, slots, cells) * 100 + kSmemPerSm - 1) / kSmemPerSm); }
+
 // Which pixels this rank renders: rows are dealt to ranks in interleaved stripes of `stripe_h` rows
 // (rank r owns stripes r, r+R, r+2R, ...).  One rank: identity mapping, local == global indices.
 struct FrameGeom {

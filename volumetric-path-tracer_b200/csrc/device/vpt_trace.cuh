@@ -40,13 +40,8 @@ enum TrKind : int { TR_SUN = 0, TR_POINT = 1, TR_SPHERE = 2 };
 
 // rays per lane: 3 (4 CTAs of 128 threads per SM, <= 128 registers) or 2: more warps in flight, the better trade when every look-up
 // misses all caches; slower when the look-ups hit L2.  The generic kernels at 2 run 5 CTAs of 128 threads (<= 96 registers); the lean
-// ones, whose stepping loop is bound by the latency of its look-ups, run 3 CTAs of 256 threads (<= 80 registers): 24 warps per SM instead
-// of 20, because the frame tables and the hardware's per-CTA reserve are paid once per 8 warps instead of once per 4 (DESIGN.md section 4).
-constexpr int trace_threads(bool lean, int slots) { return lean && slots == 2 ? 256 : kTraceThreads; }
-constexpr int trace_min_ctas(bool lean, int slots) { return slots != 2 ? kTraceMinCtas : lean ? 3 : 5; }
-constexpr int kRayWords = 34;             // 32-bit words per ray in shared memory
-// the opt-in dynamic shared memory of an instantiation: its warps' parked rays
-constexpr size_t trace_smem_bytes(bool lean, int slots) { return (size_t)(trace_threads(lean, slots) / 32) * kRayWords * 32 * slots * sizeof(float); }
+// ones, whose stepping loop is bound by the latency of its look-ups, park a 29-word record and run the shape of VPT_LEAN2_SHAPE
+// (trace_threads, trace_min_ctas, trace_smem_bytes in vpt_kernels.h; DESIGN.md section 4).
 
 struct PathState {
     float3 pos, dir;      // the integrator's ray
@@ -309,6 +304,95 @@ VPT_DEV void store_walk(const PoolGroups<kSlots>& pv, int s, const PathState& st
     pv.g(G_AUX, s) = f4(st.aux, st.alpha);
     pv.g(G_WALK, s) = make_float4(st.trv, __uint_as_float(st.rng.k), __uint_as_float(st.lp),
                                   __uint_as_float((st.packed & ~kExitMask) | ((uint32_t)st.exit_reason << 6)));
+}
+
+// The lean kernels at 2 rays per lane park 29 words, word-major as PoolView (DESIGN.md section 4): six words of the 34 hold nothing a
+// lean path needs across a park, so they are not stored, and one word is added (word 28, below).  The frame stays bit for bit what the
+// 34-word record gives:
+//   wdir     a lean walk is either the delta walk along the path's dir (PH_VOL_ITER, start_path) or a transmittance walk along
+//            tc.sun_dir (PH_VOL_DONE, PH_SPHERE; begin_ratio_walk reads wdir and never writes it): load_walk takes it from `mode`.  A
+//            service round needs none (advance assigns wdir before each walk, and begin_ratio_walk runs in the round that asked for it).
+//   light    no point lights: light_budget and light_index stay 0.
+//   T_c      live from begin_ratio_walk to PH_AFTER_TR only, where it is 1 or expf(-sigma_c * distance) of the walk's unchanged distance:
+//            bit 24 of the packed word says which, and load_ray recomputes it (the same expression on the same inputs).
+//   tmin_c   read only in the service round of the closest-object test that computed it, or in a fresh path's first round (parked at
+//            PH_BOUNCE_TOP with k_generate's test); trv is dead there (begin_ratio_walk sets it before any read), so the two share word 22.
+// pass < 64 (start_path) leaves bits 24..31 of the packed word free; rd and vd keep their 16 bits each.
+//   0-2 pos   3-5 dir   6-8 L   9-11 beta   12-14 wpos   15-17 aux   18 alpha   19 depth   20 t   21 distance   22 trv | tmin_c
+//   23 rng.k   24 lp   25 packed word   26 rd | vd   27 qslot   28 rng.key
+// Word 28, the ray's Philox key (its global pixel), is the one word more than the 34-word record needs: a walk swap keys the stream from
+// it instead of from the pixel word, so the stepping loop holds no multi-rank row arithmetic (which spilled at 72 registers).
+template <int kPool>
+struct PoolLean {
+    float* w;                                                    // this warp's kLeanRayWords * kPool words, already offset by the lane
+    float3 sun_dir;                                              // TraceConsts: a transmittance walk's direction
+    float sigma_c;                                               // ... and the control variate's extinction of T_c
+    VPT_DEV float& f(int word, int slot) const { return w[word * kPool + slot * 32]; }
+    VPT_DEV uint32_t& u(int word, int slot) const { return reinterpret_cast<uint32_t*>(w)[word * kPool + slot * 32]; }
+};
+constexpr uint32_t kTcBit = 1u << 24;                            // packed word of PoolLean: T_c is expf(-sigma_c * distance), not 1
+
+template <int kPool>
+VPT_DEV void store_ray(const PoolLean<kPool>& pv, int s, const PathState& st)
+{
+    pv.f(0, s) = st.pos.x;  pv.f(1, s) = st.pos.y;  pv.f(2, s) = st.pos.z;
+    pv.f(3, s) = st.dir.x;  pv.f(4, s) = st.dir.y;  pv.f(5, s) = st.dir.z;
+    pv.f(6, s) = st.L.x;    pv.f(7, s) = st.L.y;    pv.f(8, s) = st.L.z;
+    pv.f(9, s) = st.beta.x; pv.f(10, s) = st.beta.y; pv.f(11, s) = st.beta.z;
+    pv.f(12, s) = st.wpos.x; pv.f(13, s) = st.wpos.y; pv.f(14, s) = st.wpos.z;
+    pv.f(15, s) = st.aux.x; pv.f(16, s) = st.aux.y; pv.f(17, s) = st.aux.z;
+    pv.f(18, s) = st.alpha; pv.f(19, s) = st.depth; pv.f(20, s) = st.t; pv.f(21, s) = st.distance;
+    pv.f(22, s) = st.phase == PH_BOUNCE_TOP ? st.tmin_c : st.trv;
+    pv.u(23, s) = st.rng.k; pv.u(24, s) = st.lp;
+    pv.u(25, s) = (uint32_t)st.phase | ((uint32_t)st.mode << 4) | ((uint32_t)st.exit_reason << 6) | ((uint32_t)st.tr_kind << 9) |
+                  ((uint32_t)st.obj_c << 11) | ((uint32_t)st.mi << 13) | ((uint32_t)st.first_walk << 14) | ((uint32_t)st.have_closest << 15) |
+                  ((uint32_t)st.sphere_bounced << 16) | ((uint32_t)st.sphere_free << 17) | (st.pass << 18) | (st.T_c != 1.0f ? kTcBit : 0u);
+    pv.u(26, s) = (uint32_t)(st.rd & 0xffff) | ((uint32_t)(st.vd & 0xffff) << 16);
+    pv.u(27, s) = st.qslot; pv.u(28, s) = st.rng.key;
+}
+
+template <int kPool>
+VPT_DEV void load_ray(const PoolLean<kPool>& pv, int s, PathState& st, const FrameArgs& fa)
+{
+    st.pos = f3(pv.f(0, s), pv.f(1, s), pv.f(2, s));    st.dir = f3(pv.f(3, s), pv.f(4, s), pv.f(5, s));
+    st.L = f3(pv.f(6, s), pv.f(7, s), pv.f(8, s));      st.beta = f3(pv.f(9, s), pv.f(10, s), pv.f(11, s));
+    st.wpos = f3(pv.f(12, s), pv.f(13, s), pv.f(14, s)); st.aux = f3(pv.f(15, s), pv.f(16, s), pv.f(17, s));
+    st.alpha = pv.f(18, s); st.depth = pv.f(19, s); st.t = pv.f(20, s); st.distance = pv.f(21, s);
+    st.trv = pv.f(22, s); st.tmin_c = st.trv;
+    const uint32_t k = pv.u(23, s); st.lp = pv.u(24, s);
+    const uint32_t a = pv.u(25, s), b = pv.u(26, s);
+    st.phase = a & 15; st.mode = (a >> 4) & 3; st.exit_reason = (a >> 6) & 7; st.tr_kind = (a >> 9) & 3; st.obj_c = (a >> 11) & 3;
+    st.mi = (a >> 13) & 1; st.first_walk = (a >> 14) & 1; st.have_closest = (a >> 15) & 1; st.sphere_bounced = (a >> 16) & 1; st.sphere_free = (a >> 17) & 1;
+    st.pass = (a >> 18) & 63u;
+    st.T_c = (a & kTcBit) ? expf(-pv.sigma_c * st.distance) : 1.0f;   // begin_ratio_walk's expression
+    st.rd = b & 0xffff; st.vd = b >> 16;
+    st.light_budget = 0; st.light_index = 0;
+    st.qslot = pv.u(27, s);
+    st.org = ray_origin(fa, st.qslot);
+    st.rng.init(pv.u(28, s), fa.kp.iteration + st.pass, k);
+}
+
+// a walk loads 13 words (wpos, dir unless it is a transmittance walk, alpha, t, distance, trv, rng.k, rng.key, packed) and stores 8: the lean
+// walk changes no aux, and its T_c bit rides in the packed word
+template <int kPool>
+VPT_DEV void load_walk(const PoolLean<kPool>& pv, int s, PathState& st, const FrameArgs& fa)
+{
+    const uint32_t a = pv.u(25, s);
+    st.packed = a;
+    st.mode = (a >> 4) & 3; st.exit_reason = (a >> 6) & 7; st.sphere_free = (a >> 17) & 1; st.pass = (a >> 18) & 63u;
+    st.wpos = f3(pv.f(12, s), pv.f(13, s), pv.f(14, s));
+    st.wdir = st.mode == W_DELTA ? f3(pv.f(3, s), pv.f(4, s), pv.f(5, s)) : pv.sun_dir;
+    st.alpha = pv.f(18, s); st.t = pv.f(20, s); st.distance = pv.f(21, s); st.trv = pv.f(22, s);
+    st.rng.init(pv.u(28, s), fa.kp.iteration + st.pass, pv.u(23, s));   // (a walk reads no pixel word)
+}
+
+template <int kPool>
+VPT_DEV void store_walk(const PoolLean<kPool>& pv, int s, const PathState& st)
+{
+    pv.f(12, s) = st.wpos.x; pv.f(13, s) = st.wpos.y; pv.f(14, s) = st.wpos.z;
+    pv.f(18, s) = st.alpha; pv.f(20, s) = st.t; pv.f(22, s) = st.trv;
+    pv.u(23, s) = st.rng.k;
+    pv.u(25, s) = (st.packed & ~kExitMask) | ((uint32_t)st.exit_reason << 6);
 }
 
 // Density of volume 0 from its cell table (vpt_cells_create): the eight corner texels of the cell under the point are 32 contiguous,
@@ -715,7 +799,7 @@ struct NoAtmo { int pad[4]; };
 // pack, not a template flag, that selects them, so every kernel without mattes keeps its name as well.
 template <class... Lg> constexpr bool has_matte_ids = (std::is_same<Lg, MatteIds>::value || ... || false);
 template <int kInteg, bool kLean, int kSlots, bool kCells = false, bool kGroups = false, class... Lg>
-__global__ void __launch_bounds__(trace_threads(kLean, kSlots), trace_min_ctas(kLean, kSlots))
+__global__ void __launch_bounds__(trace_threads(kLean, kSlots, kCells), trace_min_ctas(kLean, kSlots, kCells))
 k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atmosphere, NoAtmo>::type atm, const Lg... lgs)
 {
     static_assert(sizeof...(Lg) == (kGroups ? 1 : 0) + (has_matte_ids<Lg...> ? 1 : 0),
@@ -725,7 +809,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
     // (the LightGroups are reached through lg_of(lgs...) where they are used: a pointer variable in every instantiation, even unused,
     // moved two stack stores of k_trace<1, false, 3>)
     __shared__ FrameShared fs;
-    extern __shared__ float pool_smem[];                         // warps x kRayWords x kPool words (opt-in dynamic shared memory)
+    extern __shared__ float pool_smem[];                         // warps x kWords x kPool words (opt-in dynamic shared memory)
     __shared__ EmptyAhead ea;
     // the lean kernels end walks at "empty ahead" (the render call's table, staged with the octree); the generic ones keep their hot loop
     // as it was (on the fireball, config 3, the extra code of the shortcut cost more in the fetch-bound loop than its hops saved)
@@ -739,12 +823,15 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
 
     constexpr int kPool = 32 * kSlots;
     constexpr bool kGroups16 = kLean && kSlots == 3;             // the headline kernels park their rays in 16-byte groups
-    typename std::conditional<kGroups16, PoolGroups<kSlots>, PoolView<kPool>>::type pv;
-    float* const pool_warp = pool_smem + (size_t)warp * kRayWords * kPool;   // this warp's kRayWords * kPool words
+    constexpr bool kLean28 = kLean && kSlots == 2;               // ... the lean ones at 2 rays per lane in 29 words
+    constexpr int kWords = kLean28 ? kLeanRayWords : kRayWords;
+    typename std::conditional<kGroups16, PoolGroups<kSlots>, typename std::conditional<kLean28, PoolLean<kPool>, PoolView<kPool>>::type>::type pv;
+    float* const pool_warp = pool_smem + (size_t)warp * kWords * kPool;   // this warp's kWords * kPool words
     if constexpr (kGroups16) {
         pv.q = reinterpret_cast<float4*>(pool_warp) + lane;
         pv.h = reinterpret_cast<float2*>(pool_warp + kRayGroups4 * 4 * kPool) + lane;
     } else pv.w = pool_warp + lane;
+    if constexpr (kLean28) { pv.sun_dir = tc.sun_dir; pv.sigma_c = tc.sigma_c; }
     constexpr int OP_NOSLOT = 15;                                 // third slot disabled when kSlots == 2
     int tag0 = OP_IDLE, tag1 = OP_IDLE, tag2 = (kSlots > 2) ? OP_IDLE : OP_NOSLOT;   // operation each of my rays waits for
 
@@ -768,6 +855,7 @@ k_trace(const FrameArgs fa, const typename std::conditional<kInteg != 0, vpt_atm
             if (has_idle && slot < q_count) {
                 const int j = (tag0 == OP_IDLE) ? 0 : (tag1 == OP_IDLE) ? 1 : 2;
                 start_path<kInteg>(st, fa, slot);
+                if constexpr (kLean28) st.rng.key = ray_global_pixel(fa.geom, st.lp);   // the record keeps the stream's key
                 if constexpr (kGroups) {                          // the sample slot's group sums start at 0 (integrator 0 keeps no environment sum)
                     const size_t s = group_slot(st, fa);
                     #pragma unroll
