@@ -548,6 +548,58 @@ int  vpt_set_motion_vectors(vpt_context* ctx, float* d_vectors_f3, const vpt_cam
  *     the buffers). */
 int  vpt_set_collision_aovs(vpt_context* ctx, float* d_position_f4, float* d_normal_f3, float* d_albedo_f3, float gradient_step);
 
+/* ---- Cryptomatte: per-pixel instance coverage ranked by id, keyed after the render ----------------------------------------------
+ * The industry's ID matte (Nuke, Fusion, Houdini and Resolve key it natively): each pixel keeps how many of its camera rays collided first
+ * with each volume instance (or the sphere), and the user picks the ids afterwards.  Unlike the instance mattes nothing is declared before
+ * the render and there is no plane per set.
+ *
+ *   State.  Caller-owned device memory of uint32, 2 + 2 S planes of vpt_local_pixels() entries each, plane-major (rank-local order on a
+ *     partitioned context), S = capacity in 1..VPT_CRYPTO_MAX_ENTRIES: plane 0 n (the passes counted), plane 1 overflow, plane 2 + 2j id_j,
+ *     plane 3 + 2j count_j.  4-byte aligned.
+ *   Per pass.  For pass p of a call at Kernel_params.iteration = i, with it = i + p, in this order:
+ *     1. it >= max_interactions: nothing changes (accum's gate);
+ *     2. it == 0: the pixel is cleared first (n, overflow and every id_j and count_j set to 0; accum's "iteration 0 assigns");
+ *     3. n += 1;
+ *     4. if c = depth > 0 (the alpha AOV's decision; a NaN depth is false), the sample's id -- the instance of its camera ray's first
+ *        collision, or 0xffffffff for the sphere, exactly the id of the instance mattes -- goes to the entry that holds it (count_j > 0 and
+ *        id_j == id: count_j += 1), otherwise to the first entry with count_j == 0 (it takes (id, 1)), otherwise overflow += 1.
+ *     So a pass that samples nothing (Kernel_params.render == 0, a pixel the miss cull removed) counts in n and adds no id; entries fill in
+ *     first-seen order and stay a prefix of the table; the state is exact integer arithmetic, so chunks, fused passes, single passes and a
+ *     continued call give the same bits, and an adaptive frame's pixel holds the state of a fixed-count frame of its own pass count.  For any
+ *     set of ids, sum(count_j over the set) / n estimates the coverage that set's instance matte keeps (exactly: n * matte.w rounds to it).
+ *     The rules assume a state this library wrote since an iteration-0 call (as accum does).
+ *   Activation.  A NULL state turns the Cryptomatte off at once (capacity is then ignored).  Otherwise state and capacity take over at the
+ *     next render call whose Kernel_params.iteration is 0; calls before that leave the state untouched.
+ *   Calls.  vpt_render_pass(es) and vpt_render_adaptive update it (an adaptive frame's stopped pixels keep their state; a render region
+ *     writes nothing outside it; panoramas and the miss cull as the mattes).  The trace kernel writes the id plane of the instance mattes
+ *     (the mattes' trace kernels, one plane shared by both); a kernel of its own reads the depth words and the ids next to the frame's
+ *     resolve.  Every other output is bit for bit what the same call gives without it.  On a partitioned context the state is rank-local;
+ *     neither exchange carries it.  Level (A) has none.
+ *   Refused when set (VPT_ERR_INVALID; the Cryptomatte is left as it was): a non-NULL state with capacity outside 1..VPT_CRYPTO_MAX_ENTRIES
+ *     or not 4-byte aligned.  Refused at render time: a state that overlaps accum, depth, cost, raw, display, an AOV, light-group, deep-slice,
+ *     matte, motion-vector or collision-AOV buffer (VPT_ERR_INVALID, naming the buffer); brick or cell mode (VPT_ERR_UNSUPPORTED). */
+#define VPT_CRYPTO_MAX_ENTRIES 32
+int  vpt_set_cryptomatte(vpt_context* ctx, uint32_t* d_state, unsigned capacity);
+
+/* The Cryptomatte ranks of a state (width * rows pixels, capacity S, as vpt_set_cryptomatte), for an EXR writer.  Per pixel the non-empty
+ * entries (count_j > 0) are sorted by count descending, then by id ascending (instance index; the sphere, 0xffffffff, last).  Rank r goes
+ * to float4 plane r / 2 of d_out_f4 ([n_ranks / 2][pixel], 16-byte aligned), components 2 (r % 2) and 2 (r % 2) + 1, as (id float,
+ * coverage): id float = d_id_of_instance[id] for id < n_instances, sphere_id for the sphere, 0.0f otherwise; coverage = count / n, the
+ * float32 division rounded to nearest of the two converted counts.  Ranks past the last entry, and every rank where n == 0, are (0, 0),
+ * Cryptomatte's empty rank.  d_out_overflow (may be NULL): overflow / n the same way (0 where n == 0).  The kernel never hashes: the id
+ * table holds the floats of vpt_cryptomatte_hash.  Asynchronous on `stream`, deterministic, no scratch.
+ *   Refused (VPT_ERR_INVALID): a NULL state or output, a NULL table with n_instances > 0, capacity outside 1..VPT_CRYPTO_MAX_ENTRIES,
+ *   n_ranks odd or outside 2..32, width or rows 0, more than 2^31 pixels, a misaligned buffer, an output that overlaps the state, the
+ *   table or the other output. */
+int  vpt_cryptomatte_rank(vpt_context* ctx, unsigned width, unsigned rows, const uint32_t* d_state, unsigned capacity,
+                          const float* d_id_of_instance, unsigned n_instances, float sphere_id, unsigned n_ranks, float* d_out_f4,
+                          float* d_out_overflow, void* stream);
+
+/* MurmurHash3_x86_32 of the len bytes at name (seed 0; NULL with len 0 is the empty name), as Cryptomatte hashes its names.  id_out (may
+ * be NULL): the Cryptomatte float of the name, the hash with bit 23 flipped where its exponent (h >> 23) & 0xff is 0 or 255 (so no id is a
+ * denormal, an infinity or a NaN), read as float bits.  The manifest entry of a name is "%08x" of those float bits. */
+uint32_t vpt_cryptomatte_hash(const char* name, size_t len, float* id_out);
+
 /* ---- sample-stream offset: a fresh Philox stream for every frame of a restarted accumulation ----------------------------------------
  * Pass p of a render call at Kernel_params.iteration = i draws the Philox stream the reference draws at iteration offset + i + p (32-bit
  * unsigned arithmetic, wrapping as iteration * 4096 does).  Everything else keyed by the iteration keeps the caller's i: the running-mean

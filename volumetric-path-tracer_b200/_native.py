@@ -167,7 +167,7 @@ EXPORTED_SYMBOLS = [
     "vpt_set_instance_mattes",
     "vpt_comm_p2p_export_binned", "vpt_comm_p2p_binned", "vpt_comm_p2p_block_bytes_binned",
     "vpt_set_motion_vectors", "vpt_set_sample_offset", "vpt_temporal_options_defaults", "vpt_temporal", "vpt_temporal_layers",
-    "vpt_set_collision_aovs",
+    "vpt_set_collision_aovs", "vpt_set_cryptomatte", "vpt_cryptomatte_rank", "vpt_cryptomatte_hash",
 ]
 
 # exchange layers of vpt_comm_p2p_export_layers: name -> VPT_LAYER_* bit (bit order = plane order in the block)
@@ -348,6 +348,12 @@ lib.vpt_debug_motion_cameras.argtypes = [_vp, C.POINTER(_vp), _vp]; lib.vpt_debu
 lib.vpt_set_motion_vectors.argtypes = [_vp, _vp, C.POINTER(camera)]; lib.vpt_set_motion_vectors.restype = C.c_int
 lib.vpt_set_sample_offset.argtypes = [_vp, C.c_uint32]; lib.vpt_set_sample_offset.restype = C.c_int
 lib.vpt_set_collision_aovs.argtypes = [_vp, _vp, _vp, _vp, C.c_float]; lib.vpt_set_collision_aovs.restype = C.c_int
+VPT_CRYPTO_MAX_ENTRIES = 32                                         # vpt_set_cryptomatte: most entries per pixel
+VPT_CRYPTO_SPHERE = 0xFFFFFFFF                                      # the sphere's id in the Cryptomatte state (and the mattes' id plane)
+lib.vpt_set_cryptomatte.argtypes = [_vp, _vp, C.c_uint]; lib.vpt_set_cryptomatte.restype = C.c_int
+lib.vpt_cryptomatte_rank.argtypes = [_vp, C.c_uint, C.c_uint, _vp, C.c_uint, _vp, C.c_uint, C.c_float, C.c_uint, _vp, _vp, _vp]
+lib.vpt_cryptomatte_rank.restype = C.c_int
+lib.vpt_cryptomatte_hash.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_float)]; lib.vpt_cryptomatte_hash.restype = C.c_uint32
 
 
 class temporal_options(C.Structure):

@@ -35,6 +35,8 @@
 //                     -- each sample's first collision projected through the frame camera and a second pose, next to the frame's resolve
 //   k_collision_aovs, k_collision_aovs_region, k_collision_aovs_adaptive (and their _motion forms) : collision AOVs (vpt_set_collision_aovs)
 //                     -- the world position, density normal and albedo at each sample's first collision, next to the frame's resolve
+//   k_cryptomatte, k_cryptomatte_region, k_cryptomatte_adaptive : the Cryptomatte (vpt_set_cryptomatte) -- each pixel's collided samples
+//                     counted by instance id, next to the frame's resolve; k_cryptomatte_rank : its ranks (vpt_cryptomatte_rank)
 //
 // Numerics: compiled with the reference's flags (--use_fast_math); decision-relevant expressions keep the reference
 // build's operation order (read off its SASS) so a pixel's path is reproduced sample for sample (see vpt_math.cuh).
@@ -1500,6 +1502,133 @@ __global__ void __launch_bounds__(128)
 k_collision_aovs_adaptive_motion(const FrameArgs fa, const CollisionAovs ca, const int n_passes, const AdaptArgs ad, const CameraMotion mo)
 { adaptive_pixel(fa.geom, ad, [&](uint32_t lp, int lr, int y) { collision_aovs_pixel<true>(fa, ca, &mo, n_passes, 1, lp, lr, y); }); }
 
+// =====================================================================================================
+// k_cryptomatte: per-pixel instance coverage counted by id; k_cryptomatte_rank: the ranks (DESIGN.md section 8s)
+// =====================================================================================================
+// A table of up to kCryptoRegEntries entries is kept in registers over the chunk (the loops over it are unrolled, so it never goes to local
+// memory); a larger one is searched and counted in its state rows, which a warp reads coalesced and L1 keeps.
+constexpr int kCryptoRegEntries = 8;
+
+// One pixel over the chunk's passes.  Entries fill in first-seen order and are never emptied, so the entries with count > 0 are a prefix of
+// the table (`used` of them) in every state the kernels write: the search for an id ends at the first empty entry, which is the one a new
+// id takes.  The id plane is read only where c holds, where the trace kernel wrote it.
+template <bool kRegs>
+__device__ __forceinline__ void cryptomatte_pixel(const FrameArgs& fa, const Cryptomatte& cm, const int n_passes, const int sampled, const uint32_t lp)
+{
+    const vpt_kernel_params& kp = fa.kp;
+    const uint32_t it0 = kp.iteration;
+    if (it0 >= kp.max_interactions) return;                       // accum's gate: no pass of the chunk changes the state
+    const uint32_t left = kp.max_interactions - it0;
+    const int n_upd = (uint32_t)n_passes < left ? n_passes : (int)left;
+    const size_t n = (size_t)fa.geom.n_local;
+    uint32_t* st = cm.state + lp;                                  // plane k of the pixel at st[k * n]
+    const int cap = cm.cap;
+    const bool clear = it0 == 0;                                   // iteration 0 assigns: the pixel starts empty
+    uint32_t count_n = clear ? 0u : st[0];
+    uint32_t overflow = clear ? 0u : st[n];
+    const bool records = sampled && !(fa.miss_mask && fa.miss_mask[lp]);
+    const bool compact = !fa.planeB;
+    if constexpr (kRegs) {
+        uint32_t ids[kCryptoRegEntries], counts[kCryptoRegEntries];
+        int used = 0;
+#pragma unroll
+        for (int j = 0; j < kCryptoRegEntries; ++j) {
+            ids[j] = 0u; counts[j] = 0u;
+            if (!clear && j < cap) { ids[j] = st[(size_t)(2 + 2 * j) * n]; counts[j] = st[(size_t)(3 + 2 * j) * n]; }
+            if (j == used && counts[j] != 0u) used = j + 1;
+        }
+        for (int p = 0; p < n_upd; ++p) {
+            ++count_n;
+            if (!(record_depth(fa, p, lp, records, compact) > 0.0f)) continue;
+            const uint32_t id = cm.id[(size_t)p * n + lp];
+            bool found = false;
+#pragma unroll
+            for (int j = 0; j < kCryptoRegEntries; ++j)
+                if (j < used && ids[j] == id) { ++counts[j]; found = true; }
+            if (found) continue;
+            if (used < cap) {
+#pragma unroll
+                for (int j = 0; j < kCryptoRegEntries; ++j)
+                    if (j == used) { ids[j] = id; counts[j] = 1u; }
+                ++used;
+            } else {
+                ++overflow;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kCryptoRegEntries; ++j)
+            if (j < cap && (clear || j < used)) { st[(size_t)(2 + 2 * j) * n] = ids[j]; st[(size_t)(3 + 2 * j) * n] = counts[j]; }
+    } else {
+        int used = 0;
+        if (clear) {
+            for (int j = 0; j < cap; ++j) { st[(size_t)(2 + 2 * j) * n] = 0u; st[(size_t)(3 + 2 * j) * n] = 0u; }
+        } else {
+            while (used < cap && st[(size_t)(3 + 2 * used) * n] != 0u) ++used;
+        }
+        for (int p = 0; p < n_upd; ++p) {
+            ++count_n;
+            if (!(record_depth(fa, p, lp, records, compact) > 0.0f)) continue;
+            const uint32_t id = cm.id[(size_t)p * n + lp];
+            int j = 0;
+            while (j < used && st[(size_t)(2 + 2 * j) * n] != id) ++j;
+            if (j < used) {
+                st[(size_t)(3 + 2 * j) * n] += 1u;
+            } else if (used < cap) {
+                st[(size_t)(2 + 2 * used) * n] = id; st[(size_t)(3 + 2 * used) * n] = 1u;
+                ++used;
+            } else {
+                ++overflow;
+            }
+        }
+    }
+    st[0] = count_n;
+    st[n] = overflow;
+}
+
+template <bool kRegs>
+__global__ void __launch_bounds__(256)
+k_cryptomatte(const FrameArgs fa, const Cryptomatte cm, const int n_passes, const int sampled)
+{ frame_pixel(fa.geom, [&](uint32_t lp, int, int) { cryptomatte_pixel<kRegs>(fa, cm, n_passes, sampled, lp); }); }
+
+template <bool kRegs>
+__global__ void __launch_bounds__(256)
+k_cryptomatte_region(const FrameArgs fa, const Cryptomatte cm, const int n_passes, const int sampled, const RenderRegion rg)
+{ region_pixel(fa.geom, rg, [&](uint32_t lp, int, int) { cryptomatte_pixel<kRegs>(fa, cm, n_passes, sampled, lp); }); }
+
+template <bool kRegs>
+__global__ void __launch_bounds__(128)
+k_cryptomatte_adaptive(const FrameArgs fa, const Cryptomatte cm, const int n_passes, const AdaptArgs ad)
+{ adaptive_pixel(fa.geom, ad, [&](uint32_t lp, int, int) { cryptomatte_pixel<kRegs>(fa, cm, n_passes, 1, lp); }); }
+
+// One thread per pixel.  The non-empty entries are copied to the thread's own arrays; each entry's rank is the number of non-empty entries
+// ahead of it (count greater, or equal count and smaller id: the sphere's id is the largest uint32, so it comes last among equals).
+__global__ void __launch_bounds__(256)
+k_cryptomatte_rank(const CryptoRank a)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n_px) return;
+    const size_t n_px = (size_t)a.n_px;
+    const uint32_t n = a.state[i];
+    uint32_t ids[kCryptoMaxEntries], counts[kCryptoMaxEntries];
+    int m = 0;
+    if (n != 0u)
+        for (int j = 0; j < a.cap; ++j) {
+            const uint32_t c = a.state[(size_t)(3 + 2 * j) * n_px + i];
+            if (c != 0u) { ids[m] = a.state[(size_t)(2 + 2 * j) * n_px + i]; counts[m] = c; ++m; }
+        }
+    const float fn = (float)n;
+    for (int k = 0; k < m; ++k) {
+        int r = 0;
+        for (int q = 0; q < m; ++q) r += (counts[q] > counts[k] || (counts[q] == counts[k] && ids[q] < ids[k])) ? 1 : 0;
+        if (r >= a.n_ranks) continue;
+        const uint32_t id = ids[k];
+        const float idf = id == kMatteSphereId ? a.sphere_id : id < a.n_instances ? __ldg(a.id_of_instance + id) : 0.0f;
+        a.out[((size_t)(r >> 1) * n_px + i) * 2 + (r & 1)] = make_float2(idf, __fdiv_rn((float)counts[k], fn));
+    }
+    for (int r = m; r < a.n_ranks; ++r) a.out[((size_t)(r >> 1) * n_px + i) * 2 + (r & 1)] = make_float2(0.0f, 0.0f);
+    if (a.out_overflow) a.out_overflow[i] = n == 0u ? 0.0f : __fdiv_rn((float)a.state[n_px + i], fn);
+}
+
 // Convergence test, one block of 128 per active tile: an active pixel stops when the largest err over its 3x3 neighbourhood (global rows,
 // clipped at the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A neighbour row this
 // rank owns is read from ad.stat, a row of another rank from `halo` (the local exchange block's full-frame err plane, which k_adapt_halo of
@@ -2164,7 +2293,8 @@ cudaError_t exchange_kernels_preload()
                 k_binned_publish, k_empty_ahead, k_motion_vectors, k_motion_vectors_region, k_motion_vectors_adaptive,
                 k_motion_vectors_motion, k_motion_vectors_region_motion, k_motion_vectors_adaptive_motion, k_collision_aovs,
                 k_collision_aovs_region, k_collision_aovs_adaptive, k_collision_aovs_motion, k_collision_aovs_region_motion,
-                k_collision_aovs_adaptive_motion);
+                k_collision_aovs_adaptive_motion, k_cryptomatte<true>, k_cryptomatte<false>, k_cryptomatte_region<true>,
+                k_cryptomatte_region<false>, k_cryptomatte_adaptive<true>, k_cryptomatte_adaptive<false>, k_cryptomatte_rank);
 }
 
 cudaError_t launch_sampler_compare(unsigned long long tex, const float* pool, const int dims[3], int n, unsigned seed, double* d_out12, cudaStream_t s)
@@ -2343,6 +2473,37 @@ cudaError_t launch_collision_aovs(const FrameArgs& fa, const CollisionAovs& ca, 
         if (mo) k_collision_aovs_motion<<<blocks, 256, 0, s>>>(fa, ca, n_passes, sampled, *mo);
         else k_collision_aovs<<<blocks, 256, 0, s>>>(fa, ca, n_passes, sampled);
     }
+    return cudaGetLastError();
+}
+
+// the table in registers when it fits there (kCryptoRegEntries), else in the state rows
+cudaError_t launch_cryptomatte(const FrameArgs& fa, const Cryptomatte& cm, int n_passes, int sampled, const RenderRegion* rg, const AdaptArgs* ad,
+                               cudaStream_t s)
+{
+    const bool regs = cm.cap <= kCryptoRegEntries;
+    if (ad) {
+        if (ad->n_tiles <= 0) return cudaSuccess;
+        if (regs) k_cryptomatte_adaptive<true><<<ad->n_tiles, 128, 0, s>>>(fa, cm, n_passes, *ad);
+        else k_cryptomatte_adaptive<false><<<ad->n_tiles, 128, 0, s>>>(fa, cm, n_passes, *ad);
+    } else if (rg) {
+        const long long n = region_pixels(*rg);
+        if (n <= 0) return cudaSuccess;
+        const unsigned blocks = (unsigned)((n + 255) / 256);
+        if (regs) k_cryptomatte_region<true><<<blocks, 256, 0, s>>>(fa, cm, n_passes, sampled, *rg);
+        else k_cryptomatte_region<false><<<blocks, 256, 0, s>>>(fa, cm, n_passes, sampled, *rg);
+    } else {
+        if (fa.geom.n_local <= 0) return cudaSuccess;
+        const unsigned blocks = (unsigned)((fa.geom.n_local + 255) / 256);
+        if (regs) k_cryptomatte<true><<<blocks, 256, 0, s>>>(fa, cm, n_passes, sampled);
+        else k_cryptomatte<false><<<blocks, 256, 0, s>>>(fa, cm, n_passes, sampled);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_cryptomatte_rank(const CryptoRank& a, cudaStream_t s)
+{
+    if (a.n_px <= 0) return cudaSuccess;
+    k_cryptomatte_rank<<<(unsigned)((a.n_px + 255) / 256), 256, 0, s>>>(a);
     return cudaGetLastError();
 }
 

@@ -179,7 +179,7 @@ cudaError_t launch_miss_cull(const FrameArgs& fa, uint8_t* mask, const Projectio
 struct LightGroups;
 // The trace kernels, with their instantiations in trace_kernel (vpt_kernels.cu): generic / lean / volumetric path at 3 rays per lane,
 // k_trace_brick, generic / lean at 2, lean at 2 on the cell table, generic / volumetric path keeping the light-group planes.
-// kTraceKernels counts those; the *_MATTES kernels after them are the same with the instance mattes' id plane (MatteIds, below), and
+// kTraceKernels counts those; the *_MATTES kernels after them are the same with the id plane of the instance mattes and the Cryptomatte (MatteIds, below), and
 // kTraceKernelsAll counts every trace kernel.
 enum TraceKernel : int { TK_GENERIC_3, TK_LEAN_3, TK_VOL_3, TK_BRICK, TK_GENERIC_2, TK_LEAN_2, TK_LEAN_2_CELLS, TK_GENERIC_3_GROUPS,
                          TK_VOL_3_GROUPS, kTraceKernels,
@@ -278,6 +278,22 @@ struct CollisionAovs { float4* position = nullptr; float3* normal = nullptr; flo
 // as launch_motion_vectors: one chunk of n_passes passes (sampled 0: every sample c = 0), rg / ad / mo as there
 cudaError_t launch_collision_aovs(const FrameArgs& fa, const CollisionAovs& ca, int n_passes, int sampled, const RenderRegion* rg,
                                   const AdaptArgs* ad, const CameraMotion* mo, cudaStream_t s);
+// Cryptomatte (vpt_set_cryptomatte): the uint32 state of 2 + 2 cap planes of n_local words, plane-major: n (passes counted), overflow, then
+// (id_j, count_j) for j < cap.  Per pass under accum's gate (iteration < max_interactions; iteration 0 clears the pixel first): n += 1, and a
+// sample with c = [depth > 0] adds its id (the trace's id plane, MatteIds) to the entry that holds it, else to the first entry with count 0,
+// else to overflow.  Kept by k_cryptomatte* in a launch of their own next to the frame's resolve, so no other kernel's parameter block changes.
+constexpr int kCryptoMaxEntries = 32;                 // VPT_CRYPTO_MAX_ENTRIES of vpt_b200.h
+struct Cryptomatte { uint32_t* state = nullptr; int cap = 0; const uint32_t* id = nullptr; };
+// as launch_motion_vectors: one chunk of n_passes passes (sampled 0: every sample c = 0), rg / ad as there (no camera ray is rebuilt)
+cudaError_t launch_cryptomatte(const FrameArgs& fa, const Cryptomatte& cm, int n_passes, int sampled, const RenderRegion* rg, const AdaptArgs* ad,
+                               cudaStream_t s);
+// vpt_cryptomatte_rank: per pixel of n_px, the non-empty entries of the state by count descending, then id ascending (the sphere,
+// kMatteSphereId, last); rank r = (id float, count / n) in float4 plane r / 2 of out, components 2 (r % 2) and 2 (r % 2) + 1; (0, 0) past the
+// last entry and where n == 0.  id float: id_of_instance[id] (id < n_instances), sphere_id (the sphere), else 0.  out_overflow (may be null):
+// overflow / n.
+struct CryptoRank { const uint32_t* state = nullptr; int cap = 0; long long n_px = 0; const float* id_of_instance = nullptr; uint32_t n_instances = 0;
+                    float sphere_id = 0.f; int n_ranks = 0; float2* out = nullptr; float* out_overflow = nullptr; };
+cudaError_t launch_cryptomatte_rank(const CryptoRank& a, cudaStream_t s);
 // flags: 64-bit epoch counters in peer-mapped memory.  signal: store `epoch` into slot `rank` of flag array `which` (0 ready, 1 done) of every
 // peer; wait: spin until slots 0..n-1 of the LOCAL array have all reached `epoch` (gives up after ~10 s and raises the block's error word).
 cudaError_t launch_peer_signal(unsigned long long* const peer_flags[kMaxPeers], int n, int rank, int which, unsigned long long epoch, cudaStream_t s);

@@ -337,6 +337,54 @@ int vpt_set_collision_aovs(vpt_context* c, float* d_position_f4, float* d_normal
     return VPT_OK;
 }
 
+static_assert(vpt::kCryptoMaxEntries == VPT_CRYPTO_MAX_ENTRIES, "Cryptomatte capacity");
+
+int vpt_set_cryptomatte(vpt_context* c, uint32_t* d_state, unsigned capacity) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_cryptomatte: null context");
+    vpt::Cryptomatte m;
+    if (d_state) {
+        if (capacity < 1 || capacity > VPT_CRYPTO_MAX_ENTRIES)
+            return fail(c, VPT_ERR_INVALID, "vpt_set_cryptomatte: capacity must be in 1.." + std::to_string(VPT_CRYPTO_MAX_ENTRIES) + ", got " + std::to_string(capacity));
+        if ((uintptr_t)d_state % 4 != 0) return fail(c, VPT_ERR_INVALID, "vpt_set_cryptomatte: the state buffer must be 4-byte aligned (the kernels move uint32)");
+        m.state = d_state;
+        m.cap = (int)capacity;
+    }
+    c->crypto_req = m;
+    c->crypto_active = false;       // null: off from now on; otherwise the state takes over at the next call with iteration == 0
+    return VPT_OK;
+}
+
+// MurmurHash3_x86_32 (Austin Appleby's public-domain hash) of the bytes with seed 0
+uint32_t vpt_cryptomatte_hash(const char* name, size_t len, float* id_out) {
+    const uint8_t* data = reinterpret_cast<const uint8_t*>(name);
+    if (!data) len = 0;
+    const uint32_t c1 = 0xcc9e2d51u, c2 = 0x1b873593u;
+    auto rotl = [](uint32_t x, int r) { return (x << r) | (x >> (32 - r)); };
+    uint32_t h = 0u;
+    const size_t n4 = len / 4;
+    for (size_t i = 0; i < n4; ++i) {
+        uint32_t k = (uint32_t)data[4 * i] | (uint32_t)data[4 * i + 1] << 8 | (uint32_t)data[4 * i + 2] << 16 | (uint32_t)data[4 * i + 3] << 24;
+        k *= c1; k = rotl(k, 15); k *= c2;
+        h ^= k; h = rotl(h, 13); h = h * 5u + 0xe6546b64u;
+    }
+    const uint8_t* tail = data + 4 * n4;
+    uint32_t k = 0u;
+    switch (len & 3u) {
+    case 3: k ^= (uint32_t)tail[2] << 16; [[fallthrough]];
+    case 2: k ^= (uint32_t)tail[1] << 8; [[fallthrough]];
+    case 1: k ^= tail[0]; k *= c1; k = rotl(k, 15); k *= c2; h ^= k;
+    }
+    h ^= (uint32_t)len;
+    h ^= h >> 16; h *= 0x85ebca6bu; h ^= h >> 13; h *= 0xc2b2ae35u; h ^= h >> 16;
+    if (id_out) {
+        // the Cryptomatte float: no denormal, infinity or NaN (bit 23 flipped where the exponent is 0 or 255)
+        const uint32_t e = (h >> 23) & 0xffu;
+        const uint32_t bits = (e == 0u || e == 255u) ? h ^ (1u << 23) : h;
+        memcpy(id_out, &bits, sizeof(bits));
+    }
+    return h;
+}
+
 int vpt_set_sample_offset(vpt_context* c, uint32_t offset) {
     if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_set_sample_offset: null context");
     c->sample_offset_req = offset;  // taken at the next iteration-0 call
@@ -417,7 +465,8 @@ struct FramePlan {
     vpt::LightGroups lg;                  // the active light groups (every output null: off; planes null: a lean kernel traces the frame)
     vpt::DeepSlices deep;                 // the active deep slices (out null: off)
     vpt::Mattes mattes;                   // the active instance mattes (out null: off)
-    vpt::MatteIds matte_ids;              // their id plane, for the trace kernel
+    vpt::MatteIds matte_ids;              // their id plane, for the trace kernel (the mattes' and the Cryptomatte's)
+    vpt::Cryptomatte crypto;              // the active Cryptomatte (state null: off)
     vpt::MotionVectors mv;                // the active motion vectors (out null: off)
     vpt::CollisionAovs ca;                // the active collision AOVs (all three outputs null: off)
     bool collisions() const { return ca.position || ca.normal || ca.albedo; }
@@ -538,6 +587,28 @@ static int check_motion_vector_buffer(vpt_context* c, const vpt_kernel_params& k
 
 // The collision-AOV buffers may not share a byte with a Kernel_params output buffer, an AOV, light-group, deep-slice, matte or motion-vector
 // buffer, or with each other (n = local pixels).
+// The Cryptomatte state may not share a byte with a Kernel_params output buffer or any layer buffer (n = local pixels).
+static int check_cryptomatte_buffer(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
+    const vpt::CollisionAovs& ca = c->ca_req;
+    const struct { const char* name; const void* p; size_t bytes; } others[] = {
+        { "Kernel_params.accum_buffer", (const void*)(uintptr_t)kp.accum_buffer, 12 * n }, { "Kernel_params.depth_buffer", (const void*)(uintptr_t)kp.depth_buffer, 4 * n },
+        { "Kernel_params.cost_buffer", (const void*)(uintptr_t)kp.cost_buffer, 12 * n }, { "Kernel_params.raw_buffer", (const void*)(uintptr_t)kp.raw_buffer, 16 * n },
+        { "Kernel_params.display_buffer", (const void*)(uintptr_t)kp.display_buffer, 4 * n },
+        { "the alpha AOV buffer", c->aov_alpha, 4 * n }, { "the volume AOV buffer", c->aov_volume, 12 * n },
+        { "the sun light-group buffer", c->lg_out[0], 12 * n }, { "the point light-group buffer", c->lg_out[1], 12 * n },
+        { "the emission light-group buffer", c->lg_out[2], 12 * n }, { "the environment light-group buffer", c->lg_out[3], 12 * n },
+        { "the deep slice buffer", c->deep_req.out, 16 * n * (size_t)c->deep_req.n },
+        { "the matte buffer", c->matte_req.out, 16 * n * (size_t)c->matte_req.n },
+        { "the motion-vector buffer", c->mv_req.out, 12 * n },
+        { "the collision position buffer", ca.position, 16 * n }, { "the collision normal buffer", ca.normal, 12 * n },
+        { "the collision albedo buffer", ca.albedo, 12 * n } };
+    const size_t bytes = 4 * n * (2 + 2 * (size_t)c->crypto_req.cap);
+    for (const auto& o : others)
+        if (byte_ranges_overlap(c->crypto_req.state, bytes, o.p, o.bytes))
+            return fail(c, VPT_ERR_INVALID, std::string("vpt_set_cryptomatte: the state buffer overlaps ") + o.name);
+    return VPT_OK;
+}
+
 static int check_collision_aov_buffers(vpt_context* c, const vpt_kernel_params& kp, size_t n) {
     const vpt::CollisionAovs& ca = c->ca_req;
     const struct { const char* name; const void* p; size_t bytes; } others[] = {
@@ -739,6 +810,14 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         int rc = check_matte_buffers(c, kp, (size_t)fa.geom.n_local);
         if (rc != VPT_OK) return rc;
     }
+    // the Cryptomatte: the same rule, and the same id plane (`ids`: the trace kernel writes it for either)
+    const bool crypto = c->crypto_active || (kp.iteration == 0 && c->crypto_req.state);
+    if (crypto) {
+        if (c->brick_pool || c->cell_table) return fail(c, VPT_ERR_UNSUPPORTED, "the Cryptomatte (vpt_set_cryptomatte) is not supported in brick or cell mode");
+        int rc = check_cryptomatte_buffer(c, kp, (size_t)fa.geom.n_local);
+        if (rc != VPT_OK) return rc;
+    }
+    const bool ids = mattes || crypto;
     const bool deep = c->deep_active || (kp.iteration == 0 && c->deep_req.out);
     // an active exchange whose block carries deep slices or mattes: this call's count must be the exported one, or k_binned_publish would
     // store another layout.  Checked before any state changes and before the call enqueues its first flag signal
@@ -757,13 +836,13 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     int chunk = c->passes_per_chunk;
     if (c->chunk_auto) chunk = (size_t)fa.geom.n_local <= ((size_t)1 << 20) ? 64 : 32;
     {
-        const size_t per_sample = (wide ? 88 + (planeD ? 16 : 0) : 56) + (group_planes ? 48 : 0) + (mattes ? 4 : 0);
+        const size_t per_sample = (wide ? 88 + (planeD ? 16 : 0) : 56) + (group_planes ? 48 : 0) + (ids ? 4 : 0);
         const size_t fit = c->max_scratch_bytes / (per_sample * (size_t)(fa.geom.n_local > 0 ? fa.geom.n_local : 1));
         if ((size_t)chunk > fit) chunk = fit < 1 ? 1 : (int)fit;
     }
     if (n_sampled) {
         const size_t per_chunk = (size_t)fa.geom.n_local * (size_t)(n_sampled < (unsigned)chunk ? n_sampled : (unsigned)chunk);
-        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD, group_planes, mattes);
+        int rc = ensure_frame_buffers(c, per_chunk, (size_t)fa.geom.n_local, wide, planeD, group_planes, ids);
         if (rc != VPT_OK) return rc;
     }
     if (c->cap_chunk < chunk) {
@@ -804,7 +883,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
             if (vpt::scene_registry_find(d_root, &ent) && (ent.max_grid_bytes > 2ull * c->l2_bytes || ent.n >= 64)) slots = 2;
         }
     }
-    const vpt::TraceKernel trace = vpt::pick_trace_kernel(c->brick_pool != nullptr, c->cell_table != nullptr, vol_integ, lean, group_planes, slots, mattes);
+    const vpt::TraceKernel trace = vpt::pick_trace_kernel(c->brick_pool != nullptr, c->cell_table != nullptr, vol_integ, lean, group_planes, slots, ids);
     fa.sched_min_lanes = c->sched_min_lanes > 0 ? c->sched_min_lanes : vpt::trace_sched_min_lanes(trace);
     int ctas_per_sm = c->ctas_per_sm > 0 ? c->ctas_per_sm : c->max_ctas[trace];
     if (ctas_per_sm < 1) ctas_per_sm = 1;
@@ -868,8 +947,13 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
         plan.mattes = c->matte_req;
         plan.mattes.map = c->d_matte_map;
         plan.mattes.id = c->d_matte_ids;
-        plan.matte_ids.id = c->d_matte_ids;
     }
+    if (crypto) {
+        c->crypto_active = true;
+        plan.crypto = c->crypto_req;
+        plan.crypto.id = c->d_matte_ids;
+    }
+    if (ids) plan.matte_ids.id = c->d_matte_ids;
     plan.resolve.mattes = mattes;
     plan.proj = proj;
     plan.ods = ods;
@@ -968,6 +1052,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_collision_aovs(fa, plan.ca, (int)np, 1, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream); }));
             c->launches++;
         }
+        if (plan.crypto.state) {
+            VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_cryptomatte(fa, plan.crypto, (int)np, 1, region ? &rg : nullptr, nullptr, stream); }));
+            c->launches++;
+        }
         VPT_CUDA(c, timed(c, stream, 2, [&] {
             return region ? vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)np, 1, last ? 1 : 0, last ? &peers : nullptr, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
                                                        plan.proj, stream, plan.ods_arg())
@@ -988,6 +1076,10 @@ int vpt_render_passes(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigned
         }
         if (plan.collisions()) {
             VPT_CUDA(c, vpt::launch_collision_aovs(fa, plan.ca, (int)(n_passes - n_sampled), 0, region ? &rg : nullptr, nullptr, plan.motion_arg(), stream));
+            c->launches++;
+        }
+        if (plan.crypto.state) {
+            VPT_CUDA(c, vpt::launch_cryptomatte(fa, plan.crypto, (int)(n_passes - n_sampled), 0, region ? &rg : nullptr, nullptr, stream));
             c->launches++;
         }
         if (region) VPT_CUDA(c, vpt::launch_resolve_region(fa, plan.resolve, plan.atmo, (int)(n_passes - n_sampled), 0, 1, &peers, plan.aov, plan.lg, plan.deep, plan.mattes, rg,
@@ -1129,6 +1221,10 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
                 VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_collision_aovs(fa, plan.ca, (int)np, 1, nullptr, &ad, plan.motion_arg(), stream); }));
                 c->launches++;
             }
+            if (plan.crypto.state) {
+                VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_cryptomatte(fa, plan.crypto, (int)np, 1, nullptr, &ad, stream); }));
+                c->launches++;
+            }
             VPT_CUDA(c, timed(c, stream, 2, [&] { return vpt::launch_resolve_adaptive(fa, plan.resolve, plan.atmo, (int)np, ad, plan.aov, plan.lg, plan.deep, plan.mattes, plan.proj, stream, plan.ods_arg()); }));
             c->launches += 3 + (plan.resolve.deep ? 1 : 0) + (plan.resolve.mattes ? 1 : 0);
         }
@@ -1173,6 +1269,36 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }
     if (passes_run) *passes_run = done;
+    return VPT_OK;
+}
+
+int vpt_cryptomatte_rank(vpt_context* c, unsigned width, unsigned rows, const uint32_t* d_state, unsigned capacity, const float* d_id_of_instance,
+                         unsigned n_instances, float sphere_id, unsigned n_ranks, float* d_out_f4, float* d_out_overflow, void* stream) {
+    if (!c) return fail(nullptr, VPT_ERR_INVALID, "vpt_cryptomatte_rank: null context");
+    if (!d_state || !d_out_f4) return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: null state or output");
+    if (n_instances > 0 && !d_id_of_instance) return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: null id table with n_instances > 0");
+    if (capacity < 1 || capacity > VPT_CRYPTO_MAX_ENTRIES)
+        return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: capacity must be in 1.." + std::to_string(VPT_CRYPTO_MAX_ENTRIES) + ", got " + std::to_string(capacity));
+    if (n_ranks < 2 || n_ranks > 32 || (n_ranks & 1u))
+        return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: n_ranks must be even and in 2..32, got " + std::to_string(n_ranks));
+    if (width == 0 || rows == 0) return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: width and rows must be >= 1");
+    const unsigned long long n_px = (unsigned long long)width * rows;
+    if (n_px > (1ull << 31)) return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: width * rows exceeds 2^31 pixels");
+    if ((uintptr_t)d_state % 4 != 0 || (uintptr_t)d_out_f4 % 16 != 0 || (uintptr_t)d_id_of_instance % 4 != 0 || (uintptr_t)d_out_overflow % 4 != 0)
+        return fail(c, VPT_ERR_INVALID, "vpt_cryptomatte_rank: the state, id table and overflow must be 4-byte aligned, the output 16-byte aligned");
+    const size_t n = (size_t)n_px;
+    const struct { const char* name; const void* p; size_t bytes; } bufs[] = {
+        { "the state", d_state, 4 * n * (2 + 2 * (size_t)capacity) }, { "the id table", d_id_of_instance, 4 * (size_t)n_instances },
+        { "the output", d_out_f4, 16 * n * (size_t)(n_ranks / 2) }, { "the overflow output", d_out_overflow, 4 * n } };
+    for (int k = 2; k < 4; ++k)
+        for (int j = 0; j < k; ++j)
+            if (byte_ranges_overlap(bufs[k].p, bufs[k].bytes, bufs[j].p, bufs[j].bytes))
+                return fail(c, VPT_ERR_INVALID, std::string("vpt_cryptomatte_rank: ") + bufs[k].name + " overlaps " + bufs[j].name);
+    vpt::CryptoRank a;
+    a.state = d_state; a.cap = (int)capacity; a.n_px = (long long)n_px; a.id_of_instance = d_id_of_instance; a.n_instances = n_instances;
+    a.sphere_id = sphere_id; a.n_ranks = (int)n_ranks; a.out = reinterpret_cast<float2*>(d_out_f4); a.out_overflow = d_out_overflow;
+    VPT_CUDA(c, vpt::launch_cryptomatte_rank(a, (cudaStream_t)stream));
+    c->launches++;
     return VPT_OK;
 }
 

@@ -137,6 +137,10 @@ struct vpt_context {
     // set (all three null: off) and activated like the AOVs
     vpt::CollisionAovs ca_req;
     bool      ca_active = false;
+    // Cryptomatte (vpt_set_cryptomatte): the caller-owned uint32 state and its capacity, checked when set (crypto_req.state null: off) and
+    // activated like the mattes; the trace kernel writes its ids into d_matte_ids, shared with the mattes
+    vpt::Cryptomatte crypto_req;
+    bool      crypto_active = false;
     // sample-stream offset (vpt_set_sample_offset): the one set last becomes sample_offset_cur at the next render call with iteration == 0,
     // so the passes of one frame draw consecutive streams
     uint32_t  sample_offset_req = 0, sample_offset_cur = 0;

@@ -7,6 +7,7 @@ ranks of a torch.distributed job, replicates the scene, and all-gathers the rank
 (one NCCL all-gather per call) before un-permuting them into a full frame.
 """
 import ctypes as C
+import json
 
 import numpy as np
 import torch
@@ -28,7 +29,8 @@ class FrameBuffers:
     once Renderer.enable_mattes() has allocated them (None until then); `motion`, the motion vectors ((n, 3) float32: the means of c vx,
     c vy and c), once Renderer.enable_motion_vectors() has allocated them (None until then); `position` ((n, 4): the means of c P and c),
     `normal` and `albedo` ((n, 3): the means of c n and c a), the collision AOVs, once Renderer.enable_collision_aovs() has allocated them
-    (None until then)."""
+    (None until then); `crypto`, the Cryptomatte state ((2 + 2 S) * n int32 words, plane-major), once Renderer.enable_cryptomatte() has
+    allocated it (None until then)."""
 
     def __init__(self, n_pixels, device):
         self.n = int(n_pixels)
@@ -46,10 +48,11 @@ class FrameBuffers:
         self.position = None
         self.normal = None
         self.albedo = None
+        self.crypto = None
 
     def zero_(self):
         for t in (self.accum, self.cost, self.depth, self.raw, self.display, self.alpha, self.volume, self.deep, self.mattes, self.motion,
-                  self.position, self.normal, self.albedo,
+                  self.position, self.normal, self.albedo, self.crypto,
                   *(self.groups.values() if self.groups else ())):
             if t is not None:
                 t.zero_()
@@ -603,6 +606,103 @@ class Renderer:
             return torch.where(cov.unsqueeze(-1), t[:, :k] / den, torch.zeros_like(t[:, :k])).view(rows, self.width, k)
         return unpre(b.position, 3), unpre(b.normal, 3), unpre(b.albedo, 3), z.view(rows, self.width)
 
+    def enable_cryptomatte(self, capacity=16, names=None, sphere="sphere"):
+        """Allocate and register the Cryptomatte (vpt_set_cryptomatte): buffers.crypto ((2 + 2 capacity) * n int32 words, read as uint32)
+        keeps per pixel the passes counted, the overflow and up to `capacity` (id, count) entries of the instances its camera rays collided
+        with first (DESIGN.md section 8s).  names: one per instance, the names the ids are hashed from (default: the scene's
+        instance_names, else "instance<i>"); sphere: the sphere's name.  Duplicate names raise VptError.  The state takes over at the next
+        render call with kp.iteration == 0.  n is the renderer's local pixel count (rank-local rows on a partitioned renderer)."""
+        cap = int(capacity)
+        if not 1 <= cap <= N.VPT_CRYPTO_MAX_ENTRIES:
+            raise N.VptError(f"Renderer.enable_cryptomatte: capacity {cap} (1..{N.VPT_CRYPTO_MAX_ENTRIES})")
+        n_inst = len(self.scene.instances)
+        if names is None:
+            names = getattr(self.scene, "instance_names", None) or [f"instance{i}" for i in range(n_inst)]
+        names = [str(x) for x in names]
+        if len(names) != n_inst:
+            raise N.VptError(f"Renderer.enable_cryptomatte: {len(names)} names for {n_inst} instances")
+        everything = names + [str(sphere)]
+        if len(set(everything)) != len(everything):
+            dup = sorted({x for x in everything if everything.count(x) > 1})
+            raise N.VptError(f"Renderer.enable_cryptomatte: duplicate names {dup}")
+        dev = self.buffers.accum.device
+        state = torch.zeros((2 + 2 * cap) * self.n_local, dtype=torch.int32, device=dev)
+        table = torch.tensor([cryptomatte_id(x)[0] for x in names], dtype=torch.float32, device=dev)
+        check(lib.vpt_set_cryptomatte(self.ctx, C.c_void_p(state.data_ptr()), cap), self.ctx, "vpt_set_cryptomatte")
+        self.buffers.crypto = state
+        self.crypto_capacity, self.crypto_names, self.crypto_sphere, self.crypto_table = cap, names, str(sphere), table
+
+    def disable_cryptomatte(self):
+        """Turn the Cryptomatte off at once; buffers.crypto keeps what it holds."""
+        check(lib.vpt_set_cryptomatte(self.ctx, None, 0), self.ctx, "vpt_set_cryptomatte")
+
+    def _crypto_state(self, caller):
+        if self.buffers.crypto is None:
+            raise N.VptError(f"{caller}: the Cryptomatte is not enabled (Renderer.enable_cryptomatte())")
+        return self.buffers.crypto
+
+    def cryptomatte_state(self):
+        """Views of buffers.crypto: {"n": (H, W), "overflow": (H, W), "ids": (S, H, W), "counts": (S, H, W)}, int32 holding the uint32 words
+        (the sphere's id 0xffffffff reads as -1); (local rows, W) on a partitioned renderer."""
+        s = self._crypto_state("Renderer.cryptomatte_state")
+        rows, S = self.n_local // self.width, self.crypto_capacity
+        planes = s.view(2 + 2 * S, rows, self.width)
+        return {"n": planes[0], "overflow": planes[1], "ids": planes[2::2], "counts": planes[3::2]}
+
+    def cryptomatte_image(self, ranks=6, overflow=False, stream=None):
+        """(ranks / 2, H, W, 4) float32: the Cryptomatte ranks (vpt_cryptomatte_rank), rank r in plane r // 2 as (id float, coverage) at
+        components 2 (r % 2), 2 (r % 2) + 1 -- the channels CryptoObject00.RGBA, CryptoObject01.RGBA, ... of the EXR layer.  overflow=True
+        also returns the (H, W) overflow / n."""
+        s = self._crypto_state("Renderer.cryptomatte_image")
+        ranks = int(ranks)
+        rows = self.n_local // self.width
+        out = torch.empty(max(ranks // 2, 1), self.n_local, 4, dtype=torch.float32, device=s.device)
+        ovf = torch.empty(self.n_local, dtype=torch.float32, device=s.device) if overflow else None
+        sphere_id = cryptomatte_id(self.crypto_sphere)[0]
+        check(lib.vpt_cryptomatte_rank(self.ctx, self.width, rows, C.c_void_p(s.data_ptr()), self.crypto_capacity,
+                                       C.c_void_p(self.crypto_table.data_ptr()) if len(self.crypto_names) else None, len(self.crypto_names),
+                                       sphere_id, ranks, C.c_void_p(out.data_ptr()), C.c_void_p(ovf.data_ptr()) if overflow else None,
+                                       C.c_void_p(stream or 0)), self.ctx, "vpt_cryptomatte_rank")
+        img = out.view(-1, rows, self.width, 4)
+        return (img, ovf.view(rows, self.width)) if overflow else img
+
+    def cryptomatte_manifest(self):
+        """{name: "%08x" of its Cryptomatte float's bits} for every instance and the sphere"""
+        if not hasattr(self, "crypto_names"):
+            raise N.VptError("Renderer.cryptomatte_manifest: the Cryptomatte is not enabled (Renderer.enable_cryptomatte())")
+        return {x: cryptomatte_id(x)[1] for x in self.crypto_names + [self.crypto_sphere]}
+
+    def cryptomatte_metadata(self, layer="CryptoObject"):
+        """The four EXR header attributes of the Cryptomatte layer `layer` (channels <layer>00.RGBA, <layer>01.RGBA, ... from
+        cryptomatte_image()): cryptomatte/<key>/name, hash, conversion and manifest, <key> the first 7 hex digits of the layer name's hash."""
+        key = "%08x" % int(lib.vpt_cryptomatte_hash(layer.encode("utf-8"), len(layer.encode("utf-8")), None))
+        pre = f"cryptomatte/{key[:7]}/"
+        return {pre + "name": layer, pre + "hash": "MurmurHash3_32", pre + "conversion": "uint32_to_float32",
+                pre + "manifest": json.dumps(self.cryptomatte_manifest(), sort_keys=True)}
+
+    def cryptomatte_matte(self, selection):
+        """(H, W) float32 coverage of the instances in `selection` (names or indices; the sphere by its name or by VPT_CRYPTO_SPHERE): the
+        sum of their counts over n, read from the full state (every entry, not the ranks); 0 where n == 0.  Entries lost to the overflow are
+        not in it."""
+        st = self.cryptomatte_state()
+        index = {x: i for i, x in enumerate(self.crypto_names)}
+        want = set()
+        for x in selection:
+            if isinstance(x, str):
+                if x == self.crypto_sphere: want.add(N.VPT_CRYPTO_SPHERE)
+                elif x in index: want.add(index[x])
+                else: raise N.VptError(f"Renderer.cryptomatte_matte: no instance named {x!r}")
+            else:
+                want.add(int(x) & 0xFFFFFFFF)
+        ids = st["ids"].long() & 0xFFFFFFFF
+        counts = st["counts"].long() & 0xFFFFFFFF
+        sel = torch.zeros_like(ids, dtype=torch.bool)
+        for i in want:
+            sel |= ids == i
+        total = torch.where(sel & (counts > 0), counts, torch.zeros_like(counts)).sum(0).double()
+        n = (st["n"].long() & 0xFFFFFFFF).double()
+        return torch.where(n > 0, total / torch.where(n > 0, n, torch.ones_like(n)), torch.zeros_like(n)).float()
+
     def set_region(self, x0, y0, x1, y1):
         """Render only the full-frame pixels [x0, x1) x [y0, y1) (vpt_set_render_region) from the next call with kp.iteration == 0 on:
         inside it every buffer gets what a full-frame render gives there, bit for bit; outside it nothing is written, so the display keeps
@@ -754,6 +854,15 @@ def _frame_tensor(t, numel, name, device):
         raise N.VptError(f"Renderer.denoise: `{name}` must be a contiguous float32 tensor of {numel} elements on {device} "
                          f"(got {t.dtype}, {tuple(t.shape)}, contiguous={t.is_contiguous()}, {t.device})")
     return t
+
+
+def cryptomatte_id(name):
+    """(id float, manifest hex) of a Cryptomatte name: the library's MurmurHash3_x86_32 of its UTF-8 bytes (vpt_cryptomatte_hash), bit 23
+    flipped where the exponent is 0 or 255, as float bits and as "%08x" of those bits"""
+    b = str(name).encode("utf-8")
+    f = C.c_float(0.0)
+    lib.vpt_cryptomatte_hash(b, len(b), C.byref(f))
+    return f.value, "%08x" % int.from_bytes(bytes(f), "little")
 
 
 def unpremultiply_vectors(m):
@@ -1011,6 +1120,28 @@ class DistributedRenderer:
 
     def disable_collision_aovs(self):
         self.r.disable_collision_aovs()
+
+    def enable_cryptomatte(self, capacity=16, names=None, sphere="sphere"):
+        """Renderer.enable_cryptomatte on this rank: the state stays rank-local (no exchange carries it)."""
+        self.r.enable_cryptomatte(capacity, names, sphere)
+
+    def disable_cryptomatte(self):
+        self.r.disable_cryptomatte()
+
+    def cryptomatte_state(self):
+        return self.r.cryptomatte_state()
+
+    def cryptomatte_image(self, ranks=6, overflow=False, stream=None):
+        return self.r.cryptomatte_image(ranks, overflow, stream)
+
+    def cryptomatte_manifest(self):
+        return self.r.cryptomatte_manifest()
+
+    def cryptomatte_metadata(self, layer="CryptoObject"):
+        return self.r.cryptomatte_metadata(layer)
+
+    def cryptomatte_matte(self, selection):
+        return self.r.cryptomatte_matte(selection)
 
     def set_sample_offset(self, offset):
         """Renderer.set_sample_offset on this rank; every rank sets the same offset, so the sharded frame draws the streams a single

@@ -321,15 +321,18 @@ def load_ins(path):
 def scene_from_ins(path, env=None, resolve=None, device="cuda:0"):
     """Build a Scene the way the reference does for an `.ins` argument (main.cpp:1040-1102): every listed .vdb is loaded once
     and instanced with its (position, quaternion, scale) records; a "light" file yields the point-light list instead.
-    `resolve(path) -> path` maps the verbatim paths of the file (the reference uses them relative to its CWD)."""
+    `resolve(path) -> path` maps the verbatim paths of the file (the reference uses them relative to its CWD).  The scene's
+    instance_names are "<vdb stem>.<k>", the k-th instance of that file (the names Renderer.enable_cryptomatte hashes)."""
     d = load_ins(path)
     if d["kind"] == "lights":
         return d["lights"]
-    instances = []
+    instances, names = [], []
     for f in d["files"]:
         vol = Volume.load_vdb(resolve(f["path"]) if resolve else f["path"])
         instances += [vol.instance(pos, quat, scale) for pos, quat, scale in f["instances"]]
-    return Scene(instances, env=env, device=device)
+        stem = os.path.splitext(os.path.basename(f["path"].replace("\\", "/")))[0]
+        names += [f"{stem}.{k}" for k in range(len(f["instances"]))]
+    return Scene(instances, env=env, device=device, instance_names=names)
 
 
 def synthetic_env(width=3000, height=1500):
@@ -351,8 +354,10 @@ def synthetic_blue_noise():
 class Scene:
     """Everything the nine launch parameters point at (main.cpp:1299-1313, 1378-1403, 1480-1502)."""
 
-    def __init__(self, instances, device="cuda:0", env="Barce_Rooftop_C_3k.hdr", lights=None, keep=None):
+    def __init__(self, instances, device="cuda:0", env="Barce_Rooftop_C_3k.hdr", lights=None, keep=None, instance_names=None):
         self.device = torch.device(device)
+        # one name per instance (Renderer.enable_cryptomatte's default names), or None
+        self.instance_names = [str(x) for x in instance_names] if instance_names is not None else None
         torch.cuda.set_device(self.device)
         self.keep = keep or []
         self.instances = list(instances)
