@@ -193,9 +193,12 @@ int  vpt_render_passes(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsig
  *     sample, taken exactly as the sample enters the running mean (after the NaN / Inf guard and the viz_dof tint):
  *         n += 1;  d = Y - mean;  mean += d / n;  M2 += d * (Y - mean)
  *     and its relative error is err = sqrt(M2 / (n (n-1))) / max(mean, 1e-3)  (the floor keeps dark pixels from never converging).
+ *     The arithmetic is fixed: Y = fma(0.0722, b, fma(0.2126, r, 0.7152 g)), every operation float32 round-to-nearest with subnormal
+ *     inputs and results flushed to zero, M2's update a product then a sum (DESIGN.md section 8a).
  *   Tests.  After min_passes passes, then every check_interval passes, a pixel that is still active stops if the largest err over its
  *     3x3 neighbourhood (clipped at the frame edge) is strictly below `threshold`; a neighbour that has already stopped counts with the
- *     last err it had.  threshold = 0: no pixel ever stops; threshold = FLT_MAX: every pixel stops at the first test.
+ *     last err it had, and a NaN err counts as +Inf, so a pixel with a NaN err and its neighbours never stop.  threshold = 0: no pixel
+ *     ever stops; threshold = FLT_MAX (or +Inf): every pixel whose neighbourhood holds only finite errors stops at the first test.
  *   Outputs.  d_pass_count[p] (W*H unsigned, device, required) = the passes pixel p took, and accum, depth, cost, raw and display of p
  *     are bit for bit what vpt_render_passes(d_pass_count[p]) would leave there: the Philox stream is keyed by (pixel, iteration) and
  *     the jitter of a pass does not depend on which pixels sample it.  d_rel_error (W*H float, device, may be NULL) = each pixel's last
@@ -215,7 +218,8 @@ int  vpt_render_passes(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsig
  *     pass counts and relative errors (vpt_comm_p2p_adaptive_frame).  Every convergence test waits for all peers, so each rank's call
  *     must be issued by its own host thread or process.  If a peer flag wait gives up (about 10 s), the call issues no further passes and
  *     fails with VPT_ERR_CUDA naming the barrier; the exchange is then out of step and must be set up again.
- *   Refused: render == 0, max_interactions < 2, min_passes < 2, check_interval == 0, a negative threshold, max_passes == 0, a frame size
+ *   Refused: render == 0, max_interactions < 2, min_passes < 2, check_interval == 0, a negative or NaN threshold, a subnormal threshold
+ *     (0 < threshold < FLT_MIN, which the device would flush to 0), max_passes == 0, a frame size
  *     other than the exported one (VPT_ERR_INVALID); a partitioned context without an active peer exchange -- vpt_set_partition alone, a
  *     suspended exchange -- and the NCCL exchange, whose adaptive frames are not built (VPT_ERR_UNSUPPORTED).  Brick mode and cell mode
  *     work.  opt == NULL takes the defaults. */
@@ -227,6 +231,16 @@ typedef struct vpt_adaptive_options {
 void vpt_adaptive_options_defaults(vpt_adaptive_options* opt);
 int  vpt_render_adaptive(vpt_context* ctx, void* const params[VPT_NUM_ARGS], unsigned max_passes, const vpt_adaptive_options* opt,
                          unsigned* d_pass_count, float* d_rel_error, unsigned* passes_run, void* stream);
+/* The stopping rule alone, on caller-given samples: d_samples (device, float3 [n_passes][height][width]) are the samples of each pass as
+ * they enter the running mean.  Runs vpt_render_adaptive's schedule of chunks and tests on one rank, with the same Welford arithmetic, tile
+ * lists and convergence-test kernels, and `region` (NULL, or {x0, y0, x1, y1}) as a render region.  Writes d_pass_count and d_rel_error
+ * (device [H][W], d_rel_error may be NULL) for the pixels that sample, as vpt_render_adaptive does, and at test t < max_tests every
+ * pixel's err as the test reads it into d_test_err[t] (device [max_tests][H][W]; NaN outside the region, so a test that read
+ * a pixel outside the region would hold its neighbours running).  *passes_run / *n_tests (host,
+ * may be NULL): the passes issued and the tests run.  Synchronises the device.  Options are refused as vpt_render_adaptive refuses them. */
+int  vpt_debug_adapt_rule(const float* d_samples, unsigned width, unsigned height, unsigned n_passes, const vpt_adaptive_options* opt,
+                          const unsigned* region, unsigned* d_pass_count, float* d_rel_error, float* d_test_err, unsigned max_tests,
+                          unsigned* passes_run, unsigned* n_tests);
 
 /* ---- compositing AOVs: how much of each pixel is volume, and the volume's colour without the background ----------------------
  * accum_buffer holds the volume over the environment.  With AOV buffers set, every render call also keeps, per pixel, two running
@@ -801,7 +815,9 @@ int  vpt_get_stats(vpt_context* ctx, unsigned long long* kernel_launches_total, 
 
 /* Instrumentation.  Option "count_stats" = 1 makes the trace kernel accumulate out[0] volume lookups,
  * out[1] lane-steps, out[2] warp step-loop iterations, out[3] rays serviced, out[4] warp service rounds, out[5] rays
- * fetched from the queue, out[6] bricks staged by TMA (brick mode) (SIMT efficiency of the step loop = out[1] / (32 * out[2])).  Option "profile" = 1 brackets every kernel with
+ * fetched from the queue, out[6] bricks staged by TMA (brick mode) (SIMT efficiency of the step loop = out[1] / (32 * out[2])), and
+ * out[7] the rays per lane of the last render call's trace kernel (2 or 3; 0 for k_trace_brick or before any render call), which
+ * unlike the warp totals out[2] and out[4] does not depend on how the warps were scheduled.  Option "profile" = 1 brackets every kernel with
  * CUDA events: ms/n[0..3] = generate, trace, resolve, blue-noise advance (in adaptive frames the convergence tests count as resolve;
  * the per-call miss cull of option "miss_cull" counts as generate).
  * Both calls synchronise the device. */

@@ -68,3 +68,4 @@ def test_two_and_three_rays_per_lane_give_the_same_frame(dragon, case):
         assert c2[k] == c3[k], k
     assert h2 == h3
     assert c2["warp_step_iters"] != c3["warp_step_iters"]           # a different kernel ran
+    assert (c2["rays_per_lane"], c3["rays_per_lane"]) == (2, 3)

@@ -158,7 +158,7 @@ EXPORTED_SYMBOLS = [
     "vpt_texture_read_f4", "vpt_debug_texture_sample", "vpt_debug_bruneton_stage",
     "vpt_cells_create", "vpt_cells_read", "vpt_cells_destroy", "vpt_set_cell_volume",
     "vpt_comm_p2p_export", "vpt_comm_p2p_import", "vpt_comm_p2p_import_local", "vpt_comm_p2p_block", "vpt_comm_p2p_frame", "vpt_comm_p2p_enable", "vpt_comm_p2p_status",
-    "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame",
+    "vpt_adaptive_options_defaults", "vpt_render_adaptive", "vpt_comm_p2p_adaptive_frame", "vpt_debug_adapt_rule",
     "vpt_denoise_options_defaults", "vpt_denoise", "vpt_denoise_layers",
     "vpt_set_aov_buffers", "vpt_set_light_group_buffers", "vpt_set_render_region", "vpt_set_projection", "vpt_debug_camera_rays",
     "vpt_comm_p2p_export_layers", "vpt_comm_p2p_layer", "vpt_comm_p2p_block_bytes",
@@ -197,6 +197,10 @@ class adaptive_options(C.Structure):
 lib.vpt_adaptive_options_defaults.argtypes = [C.POINTER(adaptive_options)]; lib.vpt_adaptive_options_defaults.restype = None
 lib.vpt_render_adaptive.argtypes = [_vp, C.POINTER(_vp), C.c_uint, C.POINTER(adaptive_options), _vp, _vp, C.POINTER(C.c_uint), _vp]
 lib.vpt_render_adaptive.restype = C.c_int
+# vpt_debug_adapt_rule(samples, width, height, n_passes, opt, region[4] or NULL, pass_count, rel_error, test_err, max_tests, passes_run, n_tests)
+lib.vpt_debug_adapt_rule.argtypes = [_vp, C.c_uint, C.c_uint, C.c_uint, C.POINTER(adaptive_options), C.POINTER(C.c_uint), _vp, _vp, _vp,
+                                     C.c_uint, C.POINTER(C.c_uint), C.POINTER(C.c_uint)]
+lib.vpt_debug_adapt_rule.restype = C.c_int
 lib.vpt_set_aov_buffers.argtypes = [_vp, _vp, _vp]; lib.vpt_set_aov_buffers.restype = C.c_int
 lib.vpt_set_light_group_buffers.argtypes = [_vp, _vp, _vp, _vp, _vp]; lib.vpt_set_light_group_buffers.restype = C.c_int
 VPT_DEEP_MAX_SLICES = 32                                            # vpt_set_deep_buffers: most slices

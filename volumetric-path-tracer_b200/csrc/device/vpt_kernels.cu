@@ -17,7 +17,8 @@
 //                     emission, environment).  Its twelve instantiations, and those of k_resolve_adaptive, are listed in resolve_kernels below.
 //   k_bn_advance, k_unpermute : blue-noise advance for non-sampling passes; stripe un-permutation after the multi-GPU gather
 //   k_generate_adaptive, k_resolve_adaptive<S, A, G>, k_adapt : adaptive frames (vpt_render_adaptive) -- the same per-pixel work over the tiles
-//                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test
+//                     that still hold an active pixel, a Welford state of the sample luminance, and the 3x3 convergence test;
+//                     k_debug_adapt_pass feeds the same Welford state from caller-given samples (vpt_debug_adapt_rule)
 //   k_adapt_halo, k_adapt_count_publish, k_adapt_tally, k_adapt_publish : the same frame sharded over the peer-memory exchange -- stripe-edge
 //                     errors, the agreement on when to stop, and the final full-frame stores
 //   k_layers_publish : depth, the compositing AOVs and the light groups into every rank's full-frame planes (vpt_comm_p2p_export_layers)
@@ -766,6 +767,26 @@ __device__ __forceinline__ void deep_end(const Bins& dp, const uint8_t* done, co
         if (done[k] < n_passes) dp.out[(size_t)k * px.n_local + px.lp] = deep_catch_up(dp, done, px, k, n_passes);
 }
 
+// The adaptive rule's arithmetic (DESIGN.md section 8a), one code site for every k_resolve_adaptive instantiation and
+// k_debug_adapt_pass.  Written in the round-to-nearest intrinsics of vpt_math.cuh in a fixed order, so that --use_fast_math neither
+// contracts it differently per instantiation nor turns the divisions and the root into approximations; they compile to .rn.ftz.
+// Welford step with the sample v as it entered the running mean:  Y = fma(0.0722, b, fma(0.2126, r, 0.7152 g));  n += 1;
+// d = Y - mean;  mean += d / n;  M2 += d (Y - mean)  (a product and a sum, not an fma).
+__device__ __forceinline__ void adapt_welford(float& wn, float& wmean, float& wm2, const float3 v)
+{
+    const float lum = pfma(0.0722f, v.z, pfma(0.2126f, v.x, pmul(0.7152f, v.y)));
+    wn = padd(wn, 1.0f);
+    const float d = psub(lum, wmean);
+    wmean = padd(wmean, __fdiv_rn(d, wn));
+    wm2 = padd(wm2, pmul(d, psub(lum, wmean)));
+}
+// err = sqrt(M2 / (n (n-1))) / max(mean, 1e-3), +Inf while n < 2 (a NaN mean takes the floor: fmaxf returns the other operand)
+__device__ __forceinline__ float adapt_err(const float wn, const float wmean, const float wm2)
+{
+    if (!(wn >= 2.0f)) return INFINITY;
+    return __fdiv_rn(__fsqrt_rn(__fdiv_rn(wm2, pmul(wn, psub(wn, 1.0f)))), fmaxf(wmean, kAdaptMeanFloor));
+}
+
 // One pixel of k_resolve (local pixel lp, local row lr, global row y).  kAdaptive (k_resolve_adaptive): the same running mean, plus the
 // pixel's Welford state of the sample luminance and its pass count / relative error; no peer exchange.  kAov: also the running means of
 // the compositing AOVs in `aov` (DESIGN.md section 8c).  kGroups: also the running means of the light groups in `lg` (section 8d).
@@ -936,13 +957,7 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
             }
         }
         if constexpr (kDeep) deep_pass(*dp, done, dpx, p, value, depth, guarded);
-        if constexpr (kAdaptive) {                              // the sample as it entered the mean (after the NaN guard and the tint)
-            const float lum = 0.2126f * value.x + 0.7152f * value.y + 0.0722f * value.z;
-            wn += 1.0f;
-            const float d = lum - wmean;
-            wmean += d / wn;
-            wm2 += d * (lum - wmean);
-        }
+        if constexpr (kAdaptive) adapt_welford(wn, wmean, wm2, value);   // the sample as it entered the mean (after the NaN guard and the tint)
     };
     const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
     if (culled) {
@@ -978,7 +993,7 @@ __device__ __forceinline__ void resolve_pixel(const FrameArgs& fa, const SkyArg<
         for (int k = 0; k < kLightGroups; ++k) if (lg->out[k]) lg->out[k][lp] = gm[k];
     }
     if constexpr (kAdaptive) {
-        const float err = wn >= 2.0f ? sqrtf(wm2 / (wn * (wn - 1.0f))) / fmaxf(wmean, kAdaptMeanFloor) : INFINITY;
+        const float err = adapt_err(wn, wmean, wm2);
         ad->stat[lp] = make_float4(wn, wmean, wm2, err);
         ad->pass_count[lp] = kp.iteration + (uint32_t)n_passes;
         if (ad->rel_error) ad->rel_error[lp] = err;
@@ -1633,7 +1648,8 @@ k_cryptomatte_rank(const CryptoRank a)
 // clipped at the frame edge; a stopped neighbour counts with the last err it had) is strictly below the threshold.  A neighbour row this
 // rank owns is read from ad.stat, a row of another rank from `halo` (the local exchange block's full-frame err plane, which k_adapt_halo of
 // every rank filled before the barrier ahead of this launch).  One rank owns every row: the neighbour set is the local one.  A tile with a
-// pixel still active is appended to the next list (one atomic per tile).
+// pixel still active is appended to the next list (one atomic per tile).  A NaN err counts as +Inf (fmaxf alone would drop it): such a
+// pixel and its neighbours never stop.
 // kRegion (k_adapt_region): the neighbourhood is clipped at R's edge instead, so the rule is the one above applied to R as if R were the frame.
 template <bool kRegion>
 __device__ __forceinline__ void adapt_body(const FrameGeom& g, const AdaptArgs& ad, const float* __restrict__ halo, const RenderRegion* rg)
@@ -1660,7 +1676,8 @@ __device__ __forceinline__ void adapt_body(const FrameGeom& g, const AdaptArgs& 
                 for (int dx = -1; dx <= 1; ++dx) {
                     const int c = t.x + dx;
                     if (c < xlo || c >= xhi) continue;
-                    worst = fmaxf(worst, own ? ad.stat[(size_t)r * g.width + c].w : halo[(size_t)gy * g.width + c]);
+                    const float e = own ? ad.stat[(size_t)r * g.width + c].w : halo[(size_t)gy * g.width + c];
+                    worst = fmaxf(worst, isnan(e) ? INFINITY : e);
                 }
             }
             if (worst < ad.threshold) ad.stopped[lp] = 1;
@@ -1675,6 +1692,24 @@ k_adapt(const FrameGeom g, const AdaptArgs ad, const float* __restrict__ halo) {
 
 __global__ void __launch_bounds__(128)
 k_adapt_region(const FrameGeom g, const AdaptArgs ad, const RenderRegion rg) { adapt_body<true>(g, ad, nullptr, &rg); }
+
+// vpt_debug_adapt_rule: the passes [p0, p0 + n_passes) of caller-given samples (float3 [pass][pixel], each as it enters the running mean)
+// through the pixel's Welford state, over the active tiles as k_resolve_adaptive visits them, and the same stores at the end of the chunk
+__global__ void __launch_bounds__(128)
+k_debug_adapt_pass(const FrameGeom g, const AdaptArgs ad, const float3* __restrict__ samples, const int p0, const int n_passes)
+{
+    const TilePixel t = tile_pixel(g, (int)__ldg(ad.tiles + blockIdx.x));
+    if (!t.inside) return;
+    const uint32_t lp = (uint32_t)t.lr * (uint32_t)g.width + (uint32_t)t.x;
+    if (ad.stopped[lp]) return;
+    float wn = 0.f, wmean = 0.f, wm2 = 0.f;
+    if (p0 > 0) { const float4 st = ad.stat[lp]; wn = st.x; wmean = st.y; wm2 = st.z; }
+    for (int p = 0; p < n_passes; ++p) adapt_welford(wn, wmean, wm2, samples[(size_t)(p0 + p) * g.n_local + lp]);
+    const float err = adapt_err(wn, wmean, wm2);
+    ad.stat[lp] = make_float4(wn, wmean, wm2, err);
+    ad.pass_count[lp] = (unsigned)(p0 + n_passes);
+    if (ad.rel_error) ad.rel_error[lp] = err;
+}
 
 __global__ void k_adapt_init(uint8_t* stopped, unsigned* tiles, int n_local, int n_tiles)
 {
@@ -2580,6 +2615,13 @@ cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const R
 {
     if (ad.n_tiles <= 0) return cudaSuccess;
     k_adapt_region<<<ad.n_tiles, 128, 0, s>>>(g, ad, rg);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_debug_adapt_pass(const FrameGeom& g, const AdaptArgs& ad, const float3* samples, int p0, int n_passes, cudaStream_t s)
+{
+    if (ad.n_tiles <= 0 || n_passes <= 0) return cudaSuccess;
+    k_debug_adapt_pass<<<ad.n_tiles, 128, 0, s>>>(g, ad, samples, p0, n_passes);
     return cudaGetLastError();
 }
 

@@ -204,6 +204,15 @@ inline TraceKernel pick_trace_kernel(bool brick, bool cells, bool vol_integ, boo
     if (slots == 2) return lean ? TK_LEAN_2 : TK_GENERIC_2;
     return lean ? TK_LEAN_3 : TK_GENERIC_3;
 }
+// rays per lane of a k_trace instantiation (2 or 3); 0 for k_trace_brick, which parks no rays per lane
+inline int trace_rays_per_lane(TraceKernel k)
+{
+    switch (k) {
+    case TK_BRICK: return 0;
+    case TK_GENERIC_2: case TK_LEAN_2: case TK_LEAN_2_CELLS: case TK_LEAN_2_MATTES: case TK_GENERIC_2_MATTES: return 2;
+    default: return 3;
+    }
+}
 // default of option "sched_min_lanes": lanes an operation must gather before it pre-empts stepping (26 helps only the lean kernel at 3)
 inline int trace_sched_min_lanes(TraceKernel k) { return k == TK_LEAN_3 || k == TK_LEAN_3_MATTES ? 26 : 20; }
 // per device: dynamic shared memory opt-in of every trace kernel, and how many CTAs of each fit on an SM
@@ -359,6 +368,9 @@ cudaError_t launch_resolve_region(const FrameArgs& fa, const ResolveKey& key, co
                                   const RenderRegion& rg, const Projection& pj, cudaStream_t s, const OdsParams* od = nullptr);
 cudaError_t launch_adapt_init_region(const FrameGeom& g, uint8_t* stopped, unsigned* tiles, const RenderRegion& rg, cudaStream_t s);
 cudaError_t launch_adapt_region(const FrameGeom& g, const AdaptArgs& ad, const RenderRegion& rg, cudaStream_t s);
+// vpt_debug_adapt_rule: passes [p0, p0 + n_passes) of `samples` ([pass][local pixel]) through the adaptive Welford state of the active
+// pixels of ad.tiles, ending with k_resolve_adaptive's stat / pass_count / rel_error stores
+cudaError_t launch_debug_adapt_pass(const FrameGeom& g, const AdaptArgs& ad, const float3* samples, int p0, int n_passes, cudaStream_t s);
 
 // Sharded adaptive frame over the peer-memory exchange: every rank's block as mapped here, full-frame planes [H][W] at global pixels.
 struct AdaptPeers {

@@ -892,6 +892,7 @@ static int frame_setup(vpt_context* c, void* const params[VPT_NUM_ARGS], unsigne
     fa.cell_table = c->cell_table; fa.cell_nx = c->cell_dims[0]; fa.cell_ny = c->cell_dims[1]; fa.cell_nz = c->cell_dims[2];
     const unsigned long long frame_px = (unsigned long long)kp.resolution.x * kp.resolution.y;
     plan.trace = trace; plan.trace_ctas = c->num_sms * ctas_per_sm;
+    c->last_trace_rays = vpt::trace_rays_per_lane(trace);
     plan.chunk = chunk; plan.n_sampled = n_sampled;
     plan.bn_limit = frame_px < 65536ull ? (int)frame_px : 65536;
 
@@ -1122,6 +1123,8 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
     if (o.min_passes < 2) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: min_passes must be >= 2 (the error estimate needs two samples)");
     if (o.check_interval < 1) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: check_interval must be >= 1");
     if (!(o.threshold >= 0.0f)) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: threshold must be >= 0");
+    if (o.threshold > 0.0f && o.threshold < FLT_MIN)
+        return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: threshold must be 0 or >= FLT_MIN (the device flushes a subnormal threshold to 0)");
     if (max_passes == 0) return fail(c, VPT_ERR_INVALID, "vpt_render_adaptive: max_passes must be >= 1");
     // a partitioned frame needs the peer-memory exchange: the 3x3 test reads across stripe boundaries and the ranks must agree on when to stop
     if (c->nccl_comm || (c->p2p_block && !c->p2p_on) || (c->n_ranks > 1 && !c->p2p_on))
@@ -1269,6 +1272,72 @@ int vpt_render_adaptive(vpt_context* c, void* const params[VPT_NUM_ARGS], unsign
         { int rc = vpt::comm_p2p_end(c, stream); if (rc != VPT_OK) return rc; }
     }
     if (passes_run) *passes_run = done;
+    return VPT_OK;
+}
+
+// The stopping rule alone: vpt_render_adaptive's schedule of chunks and tests on one rank, with k_debug_adapt_pass in place of the
+// sample, trace and resolve kernels.  The tile lists, k_adapt / k_adapt_region and the Welford arithmetic are the production ones.
+int vpt_debug_adapt_rule(const float* d_samples, unsigned width, unsigned height, unsigned n_passes, const vpt_adaptive_options* opt,
+                         const unsigned* region, unsigned* d_pass_count, float* d_rel_error, float* d_test_err, unsigned max_tests,
+                         unsigned* passes_run, unsigned* n_tests) {
+    const char* me = "vpt_debug_adapt_rule: ";
+    if (!d_samples || !d_pass_count) return vpt::fail_global(VPT_ERR_INVALID, std::string(me) + "null samples or pass counts");
+    if (width == 0 || height == 0 || n_passes == 0) return vpt::fail_global(VPT_ERR_INVALID, std::string(me) + "width, height and n_passes must be >= 1");
+    if ((unsigned long long)width * height > (1ull << 30)) return vpt::fail_global(VPT_ERR_INVALID, std::string(me) + "frame too large");
+    if (max_tests > 0 && !d_test_err) return vpt::fail_global(VPT_ERR_INVALID, std::string(me) + "max_tests > 0 needs d_test_err");
+    vpt_adaptive_options o;
+    vpt_adaptive_options_defaults(&o);
+    if (opt) o = *opt;
+    if (o.min_passes < 2 || o.check_interval < 1 || !(o.threshold >= 0.0f) || (o.threshold > 0.0f && o.threshold < FLT_MIN))
+        return vpt::fail_global(VPT_ERR_INVALID, std::string(me) + "options refused as vpt_render_adaptive refuses them");
+    vpt::FrameGeom g;                                      // a single-rank frame of width x height
+    g.width = (int)width; g.height = (int)height; g.local_rows = (int)height; g.n_local = (int)(width * height);
+    g.stripe_h = (int)height; g.n_ranks = 1; g.rank = 0;
+    vpt::RenderRegion rg;
+    if (region) {
+        if (region[0] >= region[2] || region[1] >= region[3] || region[2] > width || region[3] > height)
+            return vpt::fail_global(VPT_ERR_INVALID, std::string(me) + "the region must satisfy x0 < x1 <= width and y0 < y1 <= height");
+        rg = vpt::region_geometry(g, (int)region[0], (int)region[1], (int)region[2], (int)region[3]);
+    }
+    const int n_tiles = ((g.width + 31) / 32) * ((g.local_rows + 3) / 4);
+    float4* stat = nullptr; uint8_t* stopped = nullptr; unsigned* lists = nullptr;
+    cudaError_t e = cudaMalloc(&stat, sizeof(float4) * (size_t)g.n_local);
+    if (e == cudaSuccess) e = cudaMalloc(&stopped, (size_t)g.n_local);
+    if (e == cudaSuccess) e = cudaMalloc(&lists, sizeof(unsigned) * (2 * (size_t)n_tiles + 1));
+    // NaN state (all bits set): a pixel that never samples -- outside the region -- holds its neighbours running if a test reads it
+    if (e == cudaSuccess) e = cudaMemset(stat, 0xff, sizeof(float4) * (size_t)g.n_local);
+    unsigned* list[2] = { lists, lists + n_tiles };
+    int cur = 0;
+    vpt::AdaptArgs ad;
+    ad.tiles = list[0]; ad.n_tiles = region ? (int)vpt::region_tiles(rg) : n_tiles; ad.stopped = stopped; ad.stat = stat;
+    ad.pass_count = d_pass_count; ad.rel_error = d_rel_error;
+    ad.next_tiles = list[1]; ad.next_count = lists + 2 * (size_t)n_tiles; ad.threshold = o.threshold;
+    if (e == cudaSuccess) e = region ? vpt::launch_adapt_init_region(g, stopped, lists, rg, 0) : vpt::launch_adapt_init(g, stopped, lists, n_tiles, 0);
+    const float3* samples = reinterpret_cast<const float3*>(d_samples);
+    unsigned done = 0, next_test = o.min_passes, tests = 0;
+    while (e == cudaSuccess && done < n_passes && ad.n_tiles > 0) {
+        const unsigned np = (next_test < n_passes ? next_test : n_passes) - done;
+        e = vpt::launch_debug_adapt_pass(g, ad, samples, (int)done, (int)np, 0);
+        done += np;
+        if (e != cudaSuccess || done != next_test || done >= n_passes) continue;
+        e = cudaMemset(ad.next_count, 0, sizeof(unsigned));
+        if (e == cudaSuccess && tests < max_tests)          // every pixel's err as the test reads it: the .w plane of the state
+            e = cudaMemcpy2D(d_test_err + (size_t)tests * g.n_local, sizeof(float), reinterpret_cast<const char*>(stat) + 3 * sizeof(float),
+                             sizeof(float4), sizeof(float), (size_t)g.n_local, cudaMemcpyDeviceToDevice);
+        if (e == cudaSuccess) e = region ? vpt::launch_adapt_region(g, ad, rg, 0) : vpt::launch_adapt(g, ad, nullptr, 0);
+        unsigned active = 0;
+        if (e == cudaSuccess) e = cudaMemcpy(&active, ad.next_count, sizeof(unsigned), cudaMemcpyDeviceToHost);
+        cur ^= 1;
+        ad.tiles = list[cur]; ad.next_tiles = list[cur ^ 1];
+        ad.n_tiles = (int)active;
+        ++tests;
+        next_test = o.check_interval > 0xffffffffu - next_test ? 0xffffffffu : next_test + o.check_interval;
+    }
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    cudaFree(stat); cudaFree(stopped); cudaFree(lists);
+    if (e != cudaSuccess) return vpt::fail_global(VPT_ERR_CUDA, std::string(me) + cudaGetErrorString(e));
+    if (passes_run) *passes_run = done;
+    if (n_tests) *n_tests = tests;
     return VPT_OK;
 }
 
@@ -1523,6 +1592,7 @@ int vpt_get_counters(vpt_context* c, unsigned long long out[8], int reset) {
     if (!c || !out) return VPT_ERR_INVALID;
     VPT_CUDA(c, cudaDeviceSynchronize());
     VPT_CUDA(c, cudaMemcpy(out, c->d_stats, sizeof(unsigned long long) * 8, cudaMemcpyDeviceToHost));
+    out[7] = (unsigned long long)c->last_trace_rays;              // no kernel counts into slot 7
     if (reset) VPT_CUDA(c, cudaMemset(c->d_stats, 0, sizeof(unsigned long long) * 16));
     return VPT_OK;
 }

@@ -55,6 +55,7 @@ struct vpt_context {
     int count_stats = 0;              // option "count_stats": accumulate trace counters
     int empty_ahead = 1;              // option "empty_ahead": walks end at the first empty node with no populated leaf ahead (same result)
     unsigned long long* d_stats = nullptr;   // 16 counters (vpt_kernels.h FrameArgs::counters)
+    int    last_trace_rays = 0;              // rays per lane of the last render call's trace kernel (vpt_get_counters out[7])
     int profile = 0;                  // option "profile": CUDA-event timing of every kernel (debug / bench breakdown)
     struct Ev { int kind; cudaEvent_t a, b; };
     std::vector<Ev> events;

@@ -808,7 +808,8 @@ class Renderer:
         out = (C.c_ulonglong * 8)()
         check(lib.vpt_get_counters(self.ctx, out, 1 if reset else 0), self.ctx, "vpt_get_counters")
         v = list(out)
-        return dict(lookups=v[0], lane_steps=v[1], warp_step_iters=v[2], lane_services=v[3], warp_service_rounds=v[4], rays=v[5], brick_fetches=v[6])
+        return dict(lookups=v[0], lane_steps=v[1], warp_step_iters=v[2], lane_services=v[3], warp_service_rounds=v[4], rays=v[5], brick_fetches=v[6],
+                    rays_per_lane=v[7])
 
     def hop_counters(self, reset=True):
         """Hop statistics (option "count_stats"); read them before counters(reset=True), which clears them too."""
